@@ -221,6 +221,44 @@ int ssp_aug_batch_plan(const ssp_aug_item* items_host, int n, int out_w, int out
                        long long table_bytes, int* stage_dims_host20);
 int ssp_aug_batch_run(const void* table_dev, int n, const int* stage_dims_host20, void* stream);
 
+/* ---- multi-object training-image pipeline (multi_obj_pose_estimation/image_multi.py load_data_detection), byte-exact with the
+ *      Pillow routines it calls.  Per sample the caller owns four network-size (out_w x out_h x 3 bytes) device images --
+ *      main_img, main_mask, total_img, total_mask -- and counts[4] (unsigned): [S, I, accepted, unused].  luts = posmask | negmask
+ *      (2 x 256 bytes, as in ssp_aug_sample).  Every item needs its own 16-B aligned work buffer of
+ *      ssp_augm_work_bytes(in_w, in_h, out_w, out_h) bytes, with (in_w, in_h) = the crop window (cw, ch) for begin / attempt
+ *      and the background size for finish.  The plan calls only write HOST memory (no allocation, no device access, no
+ *      synchronisation); ssp_augm_run launches the planned stages of one phase (<= 16 launches for the whole batch) on
+ *      `stream`, reading the device copy of the table.
+ *  ssp_augm_plan_begin: main object of each sample -- crop (pleft, ptop, cw, ch) of img / mask (src_w x src_h), resize,
+ *      ImageChops.offset(shift_x, shift_y), FLIP_LEFT_RIGHT if flip, mask_background (image_multi.py:184-228, 38-50); sets
+ *      main_* and initialises total_* (:316-322).
+ *  ssp_augm_plan_attempt: one candidate object per item (n = samples still placing objects).  img / mask = the candidate at
+ *      source resolution; mask_bg = 1 masks img IN PLACE first (mask_background, :338), 0 = img is already masked.  Crop,
+ *      resize, flip (:230-263); S = bytes > 200 of the candidate mask, I = those also > 200 in total_mask; accepted =
+ *      S != 0 && (double)I / S < 0.2, computed on the device and written to counts[2]; if accepted, superimpose_masks and
+ *      superimpose_masked_imgs (:265-297) update total_mask / total_img.  Nothing waits for the host; it reads counts after
+ *      the round to decide what to draw next.
+ *  ssp_augm_plan_finish: img = background (src_w x src_h), resized to out_w x out_h; main object on top (:363),
+ *      change_background (:380), then out_u8 (HWC) and / or out_chw (float32 CHW, byte / 255, ToTensor). ---- */
+typedef struct ssp_augm_item {
+  void* img; const void* mask; int src_w, src_h;
+  int pleft, ptop, cw, ch;
+  int flip, shift_x, shift_y, mask_bg;
+  void* main_img; void* main_mask; void* total_img; void* total_mask;
+  unsigned* counts;
+  const void* luts;
+  void* work; long long work_bytes; void* out_u8; float* out_chw;
+} ssp_augm_item;
+long long ssp_augm_work_bytes(int in_w, int in_h, int out_w, int out_h, int resample);
+long long ssp_augm_table_bytes(int n);
+int ssp_augm_plan_begin(const ssp_augm_item* items_host, int n, int out_w, int out_h, int resample, void* table_host,
+                        long long table_bytes, int* stage_dims_host32);
+int ssp_augm_plan_attempt(const ssp_augm_item* items_host, int n, int out_w, int out_h, int resample, void* table_host,
+                          long long table_bytes, int* stage_dims_host32);
+int ssp_augm_plan_finish(const ssp_augm_item* items_host, int n, int out_w, int out_h, int resample, void* table_host,
+                         long long table_bytes, int* stage_dims_host32);
+int ssp_augm_run(const void* table_dev, int n, const int* stage_dims_host32, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

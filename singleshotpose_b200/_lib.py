@@ -63,9 +63,16 @@ SIGNATURES = {
     "ssp_aug_batch_run": [_p, _i, _p, _p],
     "ssp_aug_sample_work_bytes": [_i, _i, _i, _i, _i, _i, _i, _i, _i],
     "ssp_aug_sample": [_p, _p, _i, _i, _p, _i, _i, _p, _i, _i, _i, _i, _i, _i, _i, _p, _ll, _p, _p, _p],
+    "ssp_augm_work_bytes": [_i, _i, _i, _i, _i],
+    "ssp_augm_table_bytes": [_i],
+    "ssp_augm_plan_begin": [_p, _i, _i, _i, _i, _p, _ll, _p],
+    "ssp_augm_plan_attempt": [_p, _i, _i, _i, _i, _p, _ll, _p],
+    "ssp_augm_plan_finish": [_p, _i, _i, _i, _i, _p, _ll, _p],
+    "ssp_augm_run": [_p, _i, _p, _p],
 }
 _RESTYPE = {"ssp_last_error": C.c_char_p, "ssp_flat_alloc_rows": _ll, "ssp_flat_row": _ll,
-            "ssp_aug_resize_work_bytes": _ll, "ssp_aug_sample_work_bytes": _ll, "ssp_aug_batch_table_bytes": _ll}
+            "ssp_aug_resize_work_bytes": _ll, "ssp_aug_sample_work_bytes": _ll, "ssp_aug_batch_table_bytes": _ll,
+            "ssp_augm_work_bytes": _ll, "ssp_augm_table_bytes": _ll}
 
 _lib = None
 

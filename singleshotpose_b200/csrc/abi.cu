@@ -60,6 +60,10 @@ int aug_to_tensor_u8(const uint8_t*, long long, float*, cudaStream_t);
 long long aug_batch_table_bytes(int);
 int aug_batch_plan(const ssp_aug_item*, int, int, int, int, void*, long long, int*);
 int aug_batch_run(const void*, int, const int*, cudaStream_t);
+long long augm_work_bytes(int, int, int, int, int);
+long long augm_table_bytes(int);
+int augm_plan(int, const ssp_augm_item*, int, int, int, int, void*, long long, int*);
+int augm_run(const void*, int, const int*, cudaStream_t);
 int aug_sample(const uint8_t*, const uint8_t*, int, int, const uint8_t*, int, int, const uint8_t*, int, int, int, int, int, int, int, uint8_t*,
                long long, uint8_t*, float*, cudaStream_t);
 }  // namespace ssp
@@ -209,6 +213,18 @@ int ssp_aug_batch_plan(const ssp_aug_item* items, int n, int out_w, int out_h, i
   return aug_batch_plan(items, n, out_w, out_h, resample, table_host, table_bytes, stage_dims);
 }
 int ssp_aug_batch_run(const void* table_dev, int n, const int* stage_dims, void* s) { return aug_batch_run(table_dev, n, stage_dims, ST(s)); }
+long long ssp_augm_work_bytes(int in_w, int in_h, int out_w, int out_h, int resample) { return augm_work_bytes(in_w, in_h, out_w, out_h, resample); }
+long long ssp_augm_table_bytes(int n) { return augm_table_bytes(n); }
+int ssp_augm_plan_begin(const ssp_augm_item* items, int n, int out_w, int out_h, int resample, void* table_host, long long table_bytes, int* dims) {
+  return augm_plan(0, items, n, out_w, out_h, resample, table_host, table_bytes, dims);
+}
+int ssp_augm_plan_attempt(const ssp_augm_item* items, int n, int out_w, int out_h, int resample, void* table_host, long long table_bytes, int* dims) {
+  return augm_plan(1, items, n, out_w, out_h, resample, table_host, table_bytes, dims);
+}
+int ssp_augm_plan_finish(const ssp_augm_item* items, int n, int out_w, int out_h, int resample, void* table_host, long long table_bytes, int* dims) {
+  return augm_plan(2, items, n, out_w, out_h, resample, table_host, table_bytes, dims);
+}
+int ssp_augm_run(const void* table_dev, int n, const int* stage_dims, void* s) { return augm_run(table_dev, n, stage_dims, ST(s)); }
 long long ssp_aug_sample_work_bytes(int ow, int oh, int bw, int bh, int cw, int ch, int out_w, int out_h, int resample) {
   return aug_sample_work_bytes(ow, oh, bw, bh, cw, ch, out_w, out_h, resample);
 }

@@ -74,8 +74,22 @@ __global__ void aug_to_tensor_kernel(const uint8_t* __restrict__ src, long long 
 // one STAGE of a batch: op table column per sample (blockIdx.z), one thread per element of the op's (nx, ny) extent
 __global__ void __launch_bounds__(256) aug_stage_kernel(const AugOp* __restrict__ ops) {
   const AugOp& op = ops[blockIdx.z];
-  if (op.kind == OP_NONE) return;
-  op_element(op, blockIdx.x * 32 + (threadIdx.x & 31), blockIdx.y * 8 + (threadIdx.x >> 5));
+  if (op.kind == OP_NONE) return;                  // uniform per block: the whole block works on one sample's op
+  const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = blockIdx.y * 8 + (threadIdx.x >> 5);
+  if (op.kind == OP_COUNT) {
+    // overlap counts of a multi-object candidate: warp sums, then one integer atomic per warp with a non-zero sum, so the
+    // per-sample totals do not depend on the order of the additions
+    unsigned s = 0, i = 0;
+    if (x < op.nx && y < op.ny) count_px(op, x, y, &s, &i);
+    s = __reduce_add_sync(0xffffffffu, s);
+    i = __reduce_add_sync(0xffffffffu, i);
+    if ((threadIdx.x & 31) == 0) {
+      if (s) atomicAdd(op.counts, s);
+      if (i) atomicAdd(op.counts + 1, i);
+    }
+    return;
+  }
+  op_element(op, x, y);
 }
 
 namespace {
@@ -169,6 +183,45 @@ int aug_batch_run(const void* table_dev, int n, const int* stage_dims, cudaStrea
   if (!table_dev || !stage_dims || n <= 0 || n > 65535) return fail_msg(SSP_ERR_ARG, "ssp_aug_batch_run: bad argument");
   const AugOp* ops = (const AugOp*)table_dev;
   for (int st = 0; st < kMaxStages; st++) {
+    const int nx = stage_dims[2 * st], ny = stage_dims[2 * st + 1];
+    if (nx <= 0 || ny <= 0) continue;
+    dim3 grid((nx + 31) / 32, (ny + 7) / 8, n);
+    aug_stage_kernel<<<grid, 256, 0, s>>>(ops + (long long)st * n);
+  }
+  SSP_CHECK_LAUNCH();
+  return SSP_OK;
+}
+
+// ---- multi-object pipeline: three planned phases over the same stage kernel
+long long augm_work_bytes(int in_w, int in_h, int out_w, int out_h, int resample) {
+  if (in_w <= 0 || in_h <= 0 || out_w <= 0 || out_h <= 0) return SSP_ERR_ARG;
+  return multi_work_bytes(in_w, in_h, out_w, out_h, resample);
+}
+long long augm_table_bytes(int n) { return n > 0 ? (long long)kMaxMultiStages * n * (long long)sizeof(AugOp) : SSP_ERR_ARG; }
+
+int augm_plan(int phase, const ssp_augm_item* items, int n, int out_w, int out_h, int resample, void* table_host, long long table_bytes,
+              int* stage_dims) {
+  static_assert(sizeof(ssp_augm_item) == sizeof(AugMultiItem), "ssp_augm_item (include/ssp_b200.h) must mirror AugMultiItem (augment_core.h)");
+  static const char* who[3] = {"ssp_augm_plan_begin", "ssp_augm_plan_attempt", "ssp_augm_plan_finish"};
+  if (!items || !table_host || !stage_dims || n <= 0 || table_bytes < augm_table_bytes(n)) return fail_msg(SSP_ERR_ARG, "ssp_augm_plan_*: bad argument");
+  for (int i = 0; i < n; i++) {
+    const ssp_augm_item& it = items[i];
+    const bool common = it.img && it.luts && it.work && it.main_img && it.main_mask && it.total_img && it.total_mask && (uintptr_t)it.work % 16 == 0;
+    const bool phase_ok = phase == MULTI_BEGIN ? it.mask != nullptr
+                        : phase == MULTI_ATTEMPT ? it.mask && it.counts
+                        : (it.out_u8 || it.out_chw);
+    if (!common || !phase_ok || it.src_w <= 0 || it.src_h <= 0)
+      return fail_msg(SSP_ERR_ARG, "ssp_augm_plan_*: null pointer, misaligned work buffer or empty source in an item");
+  }
+  const int rc = multi_batch_plan(phase, reinterpret_cast<const AugMultiItem*>(items), n, out_w, out_h, resample, (AugOp*)table_host, stage_dims);
+  if (rc) return driver_rc(rc, who[phase]);
+  return SSP_OK;
+}
+
+int augm_run(const void* table_dev, int n, const int* stage_dims, cudaStream_t s) {
+  if (!table_dev || !stage_dims || n <= 0 || n > 65535) return fail_msg(SSP_ERR_ARG, "ssp_augm_run: bad argument");
+  const AugOp* ops = (const AugOp*)table_dev;
+  for (int st = 0; st < kMaxMultiStages; st++) {
     const int nx = stage_dims[2 * st], ny = stage_dims[2 * st + 1];
     if (nx <= 0 || ny <= 0) continue;
     dim3 grid((nx + 31) / 32, (ny + 7) / 8, n);

@@ -265,7 +265,9 @@ int augment_sample_driver(Backend& be, const uint8_t* img, const uint8_t* mask, 
 // stages are then executed in order (the only dependencies are between consecutive calls of ONE sample), every op by
 // op_element() per element of its (nx, ny) extent -- on the GPU one thread per element with blockIdx.z = sample
 // (augment.cu), in the host harness plain loops.  The table holds device pointers and is copied with the batch's bytes.
-enum { OP_NONE = 0, OP_COEFFS = 1, OP_PASS = 2, OP_NEAREST = 3, OP_COMPOSITE = 4, OP_DISTORT = 5 };
+enum { OP_NONE = 0, OP_COEFFS = 1, OP_PASS = 2, OP_NEAREST = 3, OP_COMPOSITE = 4, OP_DISTORT = 5,
+       // multi-object pipeline (image_multi.py), see the drivers further down
+       OP_MASKBG = 6, OP_PLACE_MAIN = 7, OP_ZERO_COUNTS = 8, OP_COUNT = 9, OP_SUPERIMPOSE = 10, OP_FINISH = 11 };
 static constexpr int kMaxStages = 10;       // 2 x (2 coefficient tables + 2 passes) + composite + distort
 struct AugOp {
   int kind, nx, ny, pad_;
@@ -273,7 +275,62 @@ struct AugOp {
   int in_size, in0, in1, out_size, resample, ksize; int* bounds; int* kk;  // OP_COEFFS
   const uint8_t* img; const uint8_t* bg; const uint8_t* mask; const uint8_t* lut_pos; const uint8_t* lut_neg; uint8_t* comp_out;   // OP_COMPOSITE (nx = bytes per row)
   const uint8_t* src; const uint8_t* luts; uint8_t* out_u8; float* out_chw;   // OP_DISTORT (nx x ny pixels)
+  // multi-object ops: network-size object (img, mask above: unshifted, unflipped), per-sample totals and counters
+  uint8_t* main_img; uint8_t* main_mask; uint8_t* total_img; uint8_t* total_mask; unsigned* counts;
+  int flip, shift_x, shift_y, pad2_;
 };
+
+SSP_HD int wrap_index(int v, int n) { const int r = v % n; return r < 0 ? r + n : r; }
+
+// shifted_data_augmentation_with_mask's ImageChops.offset(dx, dy) then FLIP_LEFT_RIGHT, followed by mask_background
+// (image_multi.py:218-223, 38-50), as one index mapping from the network-size resize outputs; initialises the totals
+// (:321-322).  out[y][x] = sized[(y - dy) mod H][(x' - dx) mod W] with x' = W-1-x when flipped.
+SSP_HD void place_main_px(const AugOp& op, int x, int y) {
+  const int W = op.nx, H = op.ny;
+  const long long s = ((long long)wrap_index(y - op.shift_y, H) * W + wrap_index((op.flip ? W - 1 - x : x) - op.shift_x, W)) * 3;
+  const long long d = ((long long)y * W + x) * 3;
+  for (int c = 0; c < 3; c++) {
+    const uint8_t m = op.mask[s + c];
+    const uint8_t a = clip8((int)op.img[s + c] * (int)op.lut_pos[m]);
+    op.main_img[d + c] = a; op.total_img[d + c] = a;
+    op.main_mask[d + c] = m; op.total_mask[d + c] = m;
+  }
+}
+// the overlap test of augment_objects (image_multi.py:344-352) for one pixel of the (flipped) candidate mask:
+// s = bytes > 200 of the candidate, i = those that are also > 200 in the total mask
+SSP_HD void count_px(const AugOp& op, int x, int y, unsigned* s, unsigned* i) {
+  const long long src = ((long long)y * op.nx + (op.flip ? op.nx - 1 - x : x)) * 3, d = ((long long)y * op.nx + x) * 3;
+  for (int c = 0; c < 3; c++) {
+    const unsigned xx = op.mask[src + c] > 200;
+    *s += xx; *i += xx & (unsigned)(op.total_mask[d + c] > 200);
+  }
+}
+// accept iff float(I) / float(S) < 0.2 with S != 0 (image_multi.py:349-353): a double division, as in Python
+SSP_HD bool accept_counts(const unsigned* counts) { return counts[0] != 0 && (double)counts[1] / (double)counts[0] < 0.2; }
+// superimpose_masks + superimpose_masked_imgs (image_multi.py:355-356, 265-297) of one pixel, predicated on the accept decision
+SSP_HD void superimpose_px(const AugOp& op, int x, int y) {
+  const bool acc = accept_counts(op.counts);
+  if (x == 0 && y == 0) op.counts[2] = acc;
+  if (!acc) return;
+  const long long src = ((long long)y * op.nx + (op.flip ? op.nx - 1 - x : x)) * 3, d = ((long long)y * op.nx + x) * 3;
+  for (int c = 0; c < 3; c++) {
+    const uint8_t m = op.mask[src + c];
+    op.total_mask[d + c] = clip8((int)m + (int)op.total_mask[d + c] * (int)op.lut_neg[m]);
+    op.total_img[d + c] = composite_px(op.img[src + c], op.total_img[d + c], m, op.lut_pos, op.lut_neg);
+  }
+}
+// main object on top (image_multi.py:363), change_background with the network-size background (:380), ToTensor
+SSP_HD void finish_px(const AugOp& op, int x, int y) {
+  const long long n = (long long)op.nx * op.ny, i = (long long)y * op.nx + x;
+  for (int c = 0; c < 3; c++) {
+    const long long k = 3 * i + c;
+    const uint8_t t = composite_px(op.main_img[k], op.total_img[k], op.main_mask[k], op.lut_pos, op.lut_neg);
+    const uint8_t v = composite_px(t, op.bg[k], op.total_mask[k], op.lut_pos, op.lut_neg);
+    if (op.out_u8) op.out_u8[k] = v;
+    if (op.out_chw) op.out_chw[c * n + i] = (float)v / 255.0f;
+  }
+}
+
 SSP_HD void op_element(const AugOp& op, int x, int y) {
   if (x >= op.nx || y >= op.ny) return;
   switch (op.kind) {
@@ -288,6 +345,12 @@ SSP_HD void op_element(const AugOp& op, int x, int y) {
       if (op.out_u8) { op.out_u8[3 * i] = o[0]; op.out_u8[3 * i + 1] = o[1]; op.out_u8[3 * i + 2] = o[2]; }
       if (op.out_chw) { op.out_chw[i] = (float)o[0] / 255.0f; op.out_chw[n + i] = (float)o[1] / 255.0f; op.out_chw[2 * n + i] = (float)o[2] / 255.0f; }
     } break;
+    case OP_MASKBG: { const long long i = (long long)y * op.nx + x; op.comp_out[i] = clip8((int)op.img[i] * (int)op.lut_pos[op.mask[i]]); } break;
+    case OP_PLACE_MAIN: place_main_px(op, x, y); break;
+    case OP_ZERO_COUNTS: op.counts[0] = op.counts[1] = op.counts[2] = 0; break;
+    case OP_COUNT: break;             // a per-sample reduction: done by the executor (aug_stage_kernel, host harness) with count_px
+    case OP_SUPERIMPOSE: superimpose_px(op, x, y); break;
+    case OP_FINISH: finish_px(op, x, y); break;
     default: break;
   }
 }
@@ -295,7 +358,7 @@ SSP_HD void op_element(const AugOp& op, int x, int y) {
 struct PlanBackend {
   AugOp* table; int n_samples, sample, call; bool overflow;
   AugOp* next() {
-    if (call >= kMaxStages) { overflow = true; return nullptr; }
+    if (call >= max_stages) { overflow = true; return nullptr; }
     AugOp* o = table + (long long)call * n_samples + sample;
     call++;
     return o;
@@ -314,6 +377,16 @@ struct PlanBackend {
     if (AugOp* o = next()) { o->kind = OP_DISTORT; o->nx = w; o->ny = h; o->src = src; o->luts = luts; o->out_u8 = out_u8; o->out_chw = out_chw; }
   }
   int row_bytes;      // 3 * ow of the sample being planned (composite is a flat byte op; rows give it a 2-D extent)
+  int max_stages = kMaxStages;
+  // multi-object ops: one op per network-size image (nx x ny pixels) unless stated
+  AugOp* multi(int kind, int w, int h) {
+    AugOp* o = next();
+    if (o) { o->kind = kind; o->nx = w; o->ny = h; }
+    return o;
+  }
+  void mask_bg(uint8_t* img, const uint8_t* mask, int w, int h, const uint8_t* lp) {      // in place, flat bytes
+    if (AugOp* o = multi(OP_MASKBG, 3 * w, h)) { o->img = img; o->mask = mask; o->comp_out = img; o->lut_pos = lp; }
+  }
 };
 struct AugItem {      // one sample of a batch: the arguments of augment_sample_driver (device pointers)
   const uint8_t* img; const uint8_t* mask; int ow, oh; const uint8_t* bg; int bw, bh; const uint8_t* luts; int pleft, ptop, cw, ch;
@@ -328,6 +401,88 @@ static inline int augment_batch_plan(const AugItem* items, int n, int out_w, int
     PlanBackend be{table, n, i, 0, false, 3 * it.ow};
     const int rc = augment_sample_driver(be, it.img, it.mask, it.ow, it.oh, it.bg, it.bw, it.bh, it.luts, it.pleft, it.ptop, it.cw, it.ch, out_w, out_h,
                                          resample, it.work, it.work_bytes, it.out_u8, it.out_chw);
+    if (rc) return rc;
+    if (be.overflow) return -3;
+    for (int s = 0; s < be.call; s++) {
+      const AugOp& o = table[(long long)s * n + i];
+      if (o.nx > stage_dims[2 * s]) stage_dims[2 * s] = o.nx;
+      if (o.ny > stage_dims[2 * s + 1]) stage_dims[2 * s + 1] = o.ny;
+    }
+  }
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------------------------------
+// Multi-object pipeline (multi_obj_pose_estimation/image_multi.py load_data_detection / augment_objects), batched in three
+// phases over per-sample network-size state (main object, total image, total mask: W x H x 3 bytes each):
+//   begin   - jitter crop + resize of the main object's image and mask (the resize driver above), then offset + flip +
+//             mask_background in one index mapping (OP_PLACE_MAIN), which also initialises the totals;
+//   attempt - one candidate per sample: mask_background at source resolution (in place, only for a candidate that is not yet
+//             masked), zero the counters, crop + resize image and mask, count (> 200 bytes of the flipped candidate and their
+//             overlap with the total mask; a per-sample integer reduction), then the accept decision on the device and the
+//             predicated superimpose of mask and image (OP_SUPERIMPOSE writes the decision to counts[2]);
+//   finish  - resize of the background, main object on top, change_background, ToTensor (OP_FINISH).
+// Flip is folded into the index mapping of the op that reads the resized candidate.  All resizing is resize_u8_driver.
+static constexpr int kMaxMultiStages = 16;  // attempt: mask_bg + zero + 2 x (2 coefficient tables + 2 passes) + count + superimpose
+struct AugMultiItem {   // one sample of one phase (device pointers); fields a phase does not read may be null
+  uint8_t* img; const uint8_t* mask; int src_w, src_h;   // begin: main object; attempt: candidate; finish: background (img)
+  int pleft, ptop, cw, ch;                                  // crop window (cw = swidth - 1, image_multi.py:203,248)
+  int flip, shift_x, shift_y, mask_bg;                      // mask_bg: attempt masks `img` in place first
+  uint8_t* main_img; uint8_t* main_mask; uint8_t* total_img; uint8_t* total_mask;
+  unsigned* counts;                                         // [S, I, accepted, unused]
+  const uint8_t* luts;                                      // posmask | negmask, 2 x 256 bytes
+  uint8_t* work; long long work_bytes; uint8_t* out_u8; float* out_chw;
+};
+static inline long long multi_work_bytes(int in_w, int in_h, int out_w, int out_h, int resample) {
+  return 2 * align16(3LL * out_w * out_h) + align16(resize_work_bytes(in_w, in_h, out_w, out_h, resample));
+}
+enum { MULTI_BEGIN = 0, MULTI_ATTEMPT = 1, MULTI_FINISH = 2 };
+
+static inline int multi_sample_plan(PlanBackend& be, int phase, const AugMultiItem& it, int W, int H, int resample) {
+  const uint8_t* lp = it.luts;
+  const uint8_t* ln = it.luts + 256;
+  uint8_t* sized_img = it.work;
+  uint8_t* sized_mask = it.work + align16(3LL * W * H);
+  uint8_t* rest = sized_mask + align16(3LL * W * H);
+  const long long rest_bytes = it.work_bytes - (rest - it.work);
+  if (phase == MULTI_FINISH) {
+    if (it.work_bytes < multi_work_bytes(it.src_w, it.src_h, W, H, resample)) return -2;
+    int rc = resize_u8_driver(be, it.img, it.src_w, it.src_h, 0, 0, it.src_w, it.src_h, sized_img, W, H, resample, rest, rest_bytes);
+    if (rc) return rc;
+    if (AugOp* o = be.multi(OP_FINISH, W, H)) {
+      o->main_img = it.main_img; o->main_mask = it.main_mask; o->total_img = it.total_img; o->total_mask = it.total_mask;
+      o->bg = sized_img; o->lut_pos = lp; o->lut_neg = ln; o->out_u8 = it.out_u8; o->out_chw = it.out_chw;
+    }
+    return 0;
+  }
+  if (it.cw <= 0 || it.ch <= 0) return -1;
+  if (it.work_bytes < multi_work_bytes(it.cw, it.ch, W, H, resample)) return -2;
+  if (phase == MULTI_ATTEMPT) {
+    if (it.mask_bg) be.mask_bg(it.img, it.mask, it.src_w, it.src_h, lp);
+    if (AugOp* o = be.multi(OP_ZERO_COUNTS, 1, 1)) o->counts = it.counts;
+  }
+  int rc = resize_u8_driver(be, it.img, it.src_w, it.src_h, it.pleft, it.ptop, it.cw, it.ch, sized_img, W, H, resample, rest, rest_bytes);
+  if (rc) return rc;
+  rc = resize_u8_driver(be, it.mask, it.src_w, it.src_h, it.pleft, it.ptop, it.cw, it.ch, sized_mask, W, H, resample, rest, rest_bytes);
+  if (rc) return rc;
+  const int kinds[2] = {phase == MULTI_BEGIN ? OP_PLACE_MAIN : OP_COUNT, phase == MULTI_BEGIN ? OP_NONE : OP_SUPERIMPOSE};
+  for (int k = 0; k < 2 && kinds[k] != OP_NONE; k++)
+    if (AugOp* o = be.multi(kinds[k], W, H)) {
+      o->img = sized_img; o->mask = sized_mask; o->lut_pos = lp; o->lut_neg = ln; o->flip = it.flip; o->shift_x = it.shift_x; o->shift_y = it.shift_y;
+      o->main_img = it.main_img; o->main_mask = it.main_mask; o->total_img = it.total_img; o->total_mask = it.total_mask; o->counts = it.counts;
+    }
+  return 0;
+}
+
+// fills table[kMaxMultiStages][n] and stage_dims[kMaxMultiStages][2] for one phase of a batch; 0 ok, < 0 error
+static inline int multi_batch_plan(int phase, const AugMultiItem* items, int n, int out_w, int out_h, int resample, AugOp* table, int* stage_dims) {
+  if (phase < MULTI_BEGIN || phase > MULTI_FINISH || out_w <= 0 || out_h <= 0) return -1;
+  for (long long i = 0; i < (long long)kMaxMultiStages * n; i++) { AugOp z = AugOp(); table[i] = z; }
+  for (int s = 0; s < 2 * kMaxMultiStages; s++) stage_dims[s] = 0;
+  for (int i = 0; i < n; i++) {
+    PlanBackend be{table, n, i, 0, false, 3 * out_w};
+    be.max_stages = kMaxMultiStages;
+    const int rc = multi_sample_plan(be, phase, items[i], out_w, out_h, resample);
     if (rc) return rc;
     if (be.overflow) return -3;
     for (int s = 0; s < be.call; s++) {

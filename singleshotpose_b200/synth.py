@@ -160,3 +160,70 @@ def write_linemod_like(root, n=4, ow=160, oh=120, num_bg=3):
     with open(listfile, "w") as f:
         f.write("\n".join(lines) + "\n")
     return listfile, bgs
+
+
+LINEMOD_OBJECTS = ("ape", "benchvise", "cam", "can", "cat", "driller", "duck", "eggbox", "glue", "holepuncher", "iron", "lamp", "phone")
+
+
+def object_sample(seed, ow, oh, empty=False, spread=False):
+    """One LINEMOD-like object view: (image, mask), uint8 HxWx3.  The mask is a SMALL ellipse (about 3 % of the frame, like the
+    LINEMOD objects) near the centre, so that pasted objects overlap often enough to be rejected now and then but a scene of 8
+    objects still fits; `empty=True` gives an all-zero mask.  `spread=True` places the object anywhere in the central 3/4 of the
+    frame instead of the central 2/5 (fewer rejections; used for throughput runs on many samples).  Integer arithmetic only."""
+    rng = np.random.default_rng(3000 + seed)
+    yy, xx = np.mgrid[0:oh, 0:ow]
+    base = np.stack([(xx * 7 + seed * 31) % 256, (yy * 5 + seed * 17) % 256, ((xx + yy) * 3) % 256], -1)
+    img = np.clip(base + rng.integers(-40, 41, (oh, ow, 3)), 0, 255).astype(np.uint8)
+    if spread:
+        cx, cy = int(rng.integers(ow // 8, 7 * ow // 8)), int(rng.integers(oh // 8, 7 * oh // 8))
+    else:
+        cx, cy = int(rng.integers(3 * ow // 10, 7 * ow // 10)), int(rng.integers(3 * oh // 10, 7 * oh // 10))
+    ax, ay = int(rng.integers(ow // 14, ow // 8)), int(rng.integers(oh // 14, oh // 8))
+    d = ((xx - cx) * ay) ** 2 + ((yy - cy) * ax) ** 2
+    r2 = (ax * ay) ** 2
+    m = np.where(d < r2 * 8 // 10, 255, np.where(d < r2, rng.integers(0, 256, (oh, ow)), 0)).astype(np.uint8)
+    if empty:
+        m[:] = 0
+    return np.ascontiguousarray(img), np.ascontiguousarray(np.repeat(m[:, :, None], 3, 2))
+
+
+def write_linemod_multi_like(root, n=3, ow=160, oh=120, num_bg=2, spread=False):
+    """All 13 LINEMOD object folders with the paths the multi-object pipeline reads (image_multi.py: LINEMOD/<obj>/train.txt
+    listing LINEMOD/<obj>/JPEGImages/00000i.png relative to `root`, mask/000i.png, labels/00000i.txt), the test-mode labels of
+    dataset_multi.py (labels_occlusion/00000i.txt, several objects per file, every 5th file empty), plus backgrounds under bg/.
+    PNG throughout.  The mask of cat's image 1 is empty (the "no object pixels" rejection); every 4th label file is empty.
+    Returns the background paths."""
+    from PIL import Image
+    for k, obj in enumerate(LINEMOD_OBJECTS):
+        base = os.path.join(root, "LINEMOD", obj)
+        for d in ("JPEGImages", "mask", "labels", "labels_occlusion"):
+            os.makedirs(os.path.join(base, d), exist_ok=True)
+        lines = []
+        for i in range(n):
+            seed = 100 * k + i
+            img, mask = object_sample(seed, ow, oh, empty=(obj == "cat" and i == 1), spread=spread)
+            name = "%06d" % i
+            Image.fromarray(img).save(os.path.join(base, "JPEGImages", name + ".png"))
+            Image.fromarray(mask).save(os.path.join(base, "mask", "%04d.png" % i))
+            rows = label_rows(seed, n=1 + i % 2)
+            rows[:, 0] = k
+            with open(os.path.join(base, "labels", name + ".txt"), "w") as f:
+                if (k * n + i) % 4 != 3:
+                    np.savetxt(f, rows)
+            with open(os.path.join(base, "labels_occlusion", name + ".txt"), "w") as f:      # the test-mode labels of dataset_multi
+                if (k * n + i) % 5 != 4:
+                    occ = label_rows(500 + seed, n=1 + (k + i) % 3)
+                    occ[:, 0] = [(k + j) % 13 for j in range(len(occ))]
+                    np.savetxt(f, occ)
+            lines.append("LINEMOD/%s/JPEGImages/%s.png" % (obj, name))
+        with open(os.path.join(base, "train.txt"), "w") as f:
+            f.write("\n".join(lines) + "\n")
+    bgdir = os.path.join(root, "bg")
+    os.makedirs(bgdir, exist_ok=True)
+    bgs = []
+    for j in range(num_bg):
+        _i, _m, bg = photo_sample(90 + j, 8, 8, ow * 5 // 4 + 13 * j, oh * 5 // 4 + 7 * j)
+        pth = os.path.join(bgdir, "bg%d.png" % j)
+        Image.fromarray(bg).save(pth)
+        bgs.append(pth)
+    return bgs
