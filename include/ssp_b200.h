@@ -169,6 +169,16 @@ int ssp_region_decode_multi(const float* out_nchw, int B, int num_keypoints, int
                             int W, int only_objectness, int correspondingclass, float* boxes, float* conf_sel,
                             float* det_conf, float* cls_corr, long long* max_ind, float* max_conf, float* max_cls,
                             void* stream);
+/* ---- multi-object evaluation (valid_multi.py:97-132, train_multi.py:196-240): per image, as the reference's batch-1 call, the
+ *      box list of get_multi_region_boxes(..., int(target[b][0]), only_objectness=0) and the box chosen for each ground truth.
+ *      target (B, target_stride) fp32 device, rows [cls, x0, y0, ..., x8, y8, w, h]; gt_offset (B+1) device: prefix sums of the
+ *      number of ground truths per image (G = gt_offset[B]).  Out: boxes [G][2K+3] the chosen box; flags [G] bit 0 = fallback box,
+ *      bit 1 = carried over from the previous ground truth of the image; uv [2G][K][2] pixels, the G ground truths after
+ *      fix_corner_order, then the G predictions: the points of ssp_pnp_batched.  num_keypoints must be 9 and
+ *      H*W*num_anchors at most 4096 (SSP_ERR_ARG otherwise). ---- */
+int ssp_eval_multi_select(const float* out_nchw, int B, int num_keypoints, int num_classes, int num_anchors, int H, int W,
+                          const float* target, int target_stride, const int* gt_offset, float conf_thresh, float im_width,
+                          float im_height, float* boxes, int* flags, float* uv, void* stream);
 
 /* ---- pnp (utils.py:86-100 -> cv2.solvePnP ITERATIVE + Rodrigues), compute_projection (utils.py:40-45) ---- */
 int ssp_pnp_batched(const float* points3d, int points3d_shared, const float* points2d, const float* K3x3,

@@ -50,6 +50,8 @@ int region_decode_argmax(const float*, int, int, int, int, int, int, float*, flo
 int region_loss_multi_fwd_bwd(const float*, const float*, float*, double*, int, int, int, int, int, int, const float*, int, float, float, float,
                               float, float, int, float, cudaStream_t);
 int region_decode_multi(const float*, int, int, int, int, int, int, int, int, float*, float*, float*, float*, long long*, float*, float*, cudaStream_t);
+int eval_multi_select(const float*, int, int, int, int, int, int, const float*, int, const int*, float, float, float, float*, int*, float*,
+                      cudaStream_t);
 int pnp_batched(const float*, int, const float*, const float*, int, long long, int, double*, double*, int*, int*, cudaStream_t);
 int project_points(const float*, int, int, const double*, const double*, long long, float*, cudaStream_t);
 long long aug_resize_work_bytes(int, int, int, int, int);
@@ -189,6 +191,11 @@ int ssp_region_loss_multi_fwd_bwd(const float* out, const float* target, float* 
 int ssp_region_decode_multi(const float* out, int B, int K, int nC, int nA, int H, int W, int only_objectness, int corr, float* boxes, float* conf_sel,
                             float* det, float* cls_corr, long long* max_ind, float* max_conf, float* max_cls, void* s) {
   return region_decode_multi(out, B, K, nC, nA, H, W, only_objectness, corr, boxes, conf_sel, det, cls_corr, max_ind, max_conf, max_cls, ST(s));
+}
+int ssp_eval_multi_select(const float* out, int B, int K, int nC, int nA, int H, int W, const float* target, int target_stride,
+                          const int* gt_offset, float conf_thresh, float im_width, float im_height, float* boxes, int* flags, float* uv,
+                          void* s) {
+  return eval_multi_select(out, B, K, nC, nA, H, W, target, target_stride, gt_offset, conf_thresh, im_width, im_height, boxes, flags, uv, ST(s));
 }
 int ssp_pnp_batched(const float* P3, int shared, const float* uv, const float* K, int np, long long n, int max_iter, double* R, double* t, int* iters, void* s) {
   return pnp_batched(P3, shared, uv, K, np, n, max_iter, R, t, iters, nullptr, ST(s));

@@ -4,6 +4,7 @@
 // The reference's "best_n = -1" read (region_loss_multi.py:51,63: tconf is computed from the LAST anchor of the
 // PREVIOUS image at the ground-truth cell, wrapping to the last image for b = 0) is reproduced on purpose.
 #include "ssp_common.cuh"
+#include "eval_multi_core.h"
 
 namespace ssp {
 
@@ -154,6 +155,7 @@ __global__ void __launch_bounds__(256) region_loss_multi_kernel(const RegionMult
 // ------------------------------------------------------------------------------------------------ decode
 // dense pass: for every (image, cell, anchor) -- cell-major, anchor fastest, the reference's visiting order -- the box
 // [x0/w, y0/h, ..., det_conf, cls_max_conf, cls_max_id], the selection confidence and softmax[correspondingclass]
+// (ssp_evm::decode_entry, the arithmetic eval_multi_select_kernel shares)
 __global__ void __launch_bounds__(256) region_decode_multi_kernel(const float* __restrict__ out, int B, int K, int nC, int nA, int H, int W,
                                                                   int only_objectness, int corr, float* __restrict__ boxes,
                                                                   float* __restrict__ conf_sel, float* __restrict__ det, float* __restrict__ cls_corr) {
@@ -164,21 +166,11 @@ __global__ void __launch_bounds__(256) region_decode_multi_kernel(const float* _
   const int cy = cell / W, cx = cell % W;
   const float* o = out + ((long long)b * nA + a) * nch * HW + cell;
   float* bx = boxes + idx * (2 * K + 3);
-  for (int k = 0; k < K; k++) {
-    float vx = o[(2 * k) * HW], vy = o[(2 * k + 1) * HW];
-    if (k == 0) { vx = sigmoidm_(vx); vy = sigmoidm_(vy); }
-    bx[2 * k] = (vx + (float)cx) / (float)W; bx[2 * k + 1] = (vy + (float)cy) / (float)H;
-  }
-  const float dc = sigmoidm_(o[(2 * K) * HW]);
-  float mx = -INFINITY; int id = 0;
-  for (int c = 0; c < nC; c++) { const float v = o[(2 * K + 1 + c) * HW]; if (v > mx) { mx = v; id = c; } }
-  float den = 0.f;
-  for (int c = 0; c < nC; c++) den += expf(o[(2 * K + 1 + c) * HW] - mx);
-  const float cmax = 1.f / den;
-  bx[2 * K] = dc; bx[2 * K + 1] = cmax; bx[2 * K + 2] = (float)id;
-  conf_sel[idx] = only_objectness ? dc : dc * cmax;
-  det[idx] = dc;
-  cls_corr[idx] = (corr >= 0 && corr < nC) ? expf(o[(2 * K + 1 + corr) * HW] - mx) / den : 0.f;
+  const ssp_evm::Decoded d = ssp_evm::decode_entry(o, HW, K, nC, cx, cy, W, H, corr, bx);
+  bx[2 * K] = d.det; bx[2 * K + 1] = d.cmax; bx[2 * K + 2] = (float)d.id;
+  conf_sel[idx] = only_objectness ? d.det : d.det * d.cmax;
+  det[idx] = d.det;
+  cls_corr[idx] = d.corr;
 }
 
 // the reference's running maxima (max_conf reset per image, max_cls_conf and max_ind never reset): inherently sequential
@@ -194,6 +186,82 @@ __global__ void region_decode_multi_fallback_kernel(const float* __restrict__ de
     }
     max_ind[b] = mind; max_conf[b] = mconf; max_cls[b] = mcls;
   }
+}
+
+// ------------------------------------------------------------------------------------------------ evaluation selection
+// valid_multi.py:97-132 for every image of a batch, each as the reference's own batch-1 call (rules: eval_multi_core.h).
+// One CTA per image: the decode of every (cell, anchor) and the per-class best listed box in parallel (a 64-bit shared
+// atomicMax over pick_key, so the result does not depend on the order of the atomics), then thread 0 runs the fallback's
+// running maxima (only when needed) and the per-ground-truth choice, then one thread per ground truth writes its box and
+// PnP inputs.  Ground truths are taken ssp_evm::kMaxGt at a time; the carried-over choice lives in thread 0's registers.
+__global__ void __launch_bounds__(256) eval_multi_select_kernel(const float* __restrict__ out, int B, int K, int nC, int nA, int H, int W,
+                                                                const float* __restrict__ target, int stride, const int* __restrict__ gt_offset,
+                                                                float thr, float imw, float imh, float* __restrict__ boxes,
+                                                                int* __restrict__ flags, float* __restrict__ uv) {
+  using namespace ssp_evm;
+  const int b = blockIdx.x;
+  const int g0 = gt_offset[b], ng = gt_offset[b + 1] - g0, G = gt_offset[B];
+  if (ng <= 0) return;
+  __shared__ float s_det[kMaxEntries], s_corr[kMaxEntries];
+  __shared__ unsigned long long s_best[kMaxClasses];
+  __shared__ int s_src[kMaxGt], s_flags[kMaxGt];
+  __shared__ Fallback s_fb;
+  const int HW = H * W, n = HW * nA, nl = 2 * K + 3;
+  const float* t = target + (long long)b * stride;
+  const int corr = (int)t[0];
+  const float* o = out + (long long)b * nA * (2 * K + 1 + nC) * HW;
+  for (int c = threadIdx.x; c < nC; c += blockDim.x) s_best[c] = 0ull;
+  __syncthreads();
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    int cx, cy;
+    const float* oi = entry_ptr(o, i, nA, K, nC, W, HW, &cx, &cy);
+    const Decoded d = decode_entry(oi, HW, K, nC, cx, cy, W, H, corr, nullptr);
+    s_det[i] = d.det; s_corr[i] = d.corr;
+    if (listed(d, thr)) atomicMax(&s_best[d.id], pick_key(d.det, i));
+  }
+  __syncthreads();
+  const bool has_corr = corr >= 0 && corr < nC && s_best[corr] != 0ull;
+  if (threadIdx.x == 0) {
+    Fallback fb = fallback_init();
+    if (!has_corr)
+      for (int i = 0; i < n; i++) fallback_update(fb, s_det[i], s_corr[i], i);
+    s_fb = fb;
+  }
+  int src = 0, fl = 0;                                     // thread 0: the previous ground truth's choice
+  for (int base = 0; base < ng; base += kMaxGt) {
+    const int m = min(kMaxGt, ng - base);
+    if (threadIdx.x == 0)
+      for (int g = 0; g < m; g++) {
+        src = select_box(s_best, nC, corr, has_corr, (int)t[(base + g) * nl], src, fl, &fl);
+        s_src[g] = src; s_flags[g] = fl;
+      }
+    __syncthreads();
+    for (int g = threadIdx.x; g < m; g += blockDim.x) {
+      const long long gi = g0 + base + g;
+      float box[2 * kKeypoints + 3];
+      write_box(o, s_src[g], s_fb, corr, nA, K, nC, W, H, box);
+      for (int j = 0; j < nl; j++) boxes[gi * nl + j] = box[j];
+      flags[gi] = s_flags[g];
+      write_uv(t + (base + g) * nl, box, imw, imh, uv + gi * 2 * K, uv + (G + gi) * 2 * K);
+    }
+    __syncthreads();
+  }
+}
+
+int eval_multi_select(const float* out, int B, int K, int nC, int nA, int H, int W, const float* target, int target_stride,
+                      const int* gt_offset, float conf_thresh, float im_width, float im_height, float* boxes, int* flags, float* uv,
+                      cudaStream_t s) {
+  if (K != ssp_evm::kKeypoints)
+    return fail_msg(SSP_ERR_ARG, "eval_multi_select: num_keypoints must be 9 (fix_corner_order is defined for the 9 keypoints of a box)");
+  if (!out || !target || !gt_offset || !boxes || !flags || !uv || B < 0 || nC < 1 || nA < 1 || H < 1 || W < 1 || target_stride < 2 * K + 3)
+    return fail_msg(SSP_ERR_ARG, "eval_multi_select: bad argument");
+  if ((long long)H * W * nA > ssp_evm::kMaxEntries)
+    return fail_msg(SSP_ERR_ARG, "eval_multi_select: grid too large (H*W*num_anchors must be at most 4096, e.g. 26x26x5)");
+  if (nC > ssp_evm::kMaxClasses) return fail_msg(SSP_ERR_ARG, "eval_multi_select: at most 256 classes");
+  if (B == 0) return SSP_OK;
+  eval_multi_select_kernel<<<B, 256, 0, s>>>(out, B, K, nC, nA, H, W, target, target_stride, gt_offset, conf_thresh, im_width, im_height,
+                                             boxes, flags, uv);
+  SSP_CHECK_LAUNCH(); return SSP_OK;
 }
 
 int region_loss_multi_fwd_bwd(const float* out, const float* target, float* grad, double* acc, int B, int K, int nC, int nA, int H, int W,

@@ -3,6 +3,7 @@ The dense per-(cell, anchor) arithmetic and the reference's sequential fallback 
 applies the confidence mask (one device->host copy).  The pose helpers are shared with utils.py."""
 from __future__ import annotations
 
+import numpy as np
 import torch
 
 from ._lib import call, ptr, stream_ptr, SspError
@@ -115,3 +116,98 @@ def get_multi_region_boxes(output, conf_thresh, num_classes, num_keypoints, anch
             cur.append([float(v) for v in src[:2 * K]] + [float(max_conf[b]), float(max_cls[b]), int(correspondingclass)])
         all_boxes.append(cur)
     return all_boxes
+
+
+# ------------------------------------------------------------------------------------------ batched evaluation tail
+ACCURACY_THRESHOLDS = (5, 10, 15, 20, 25, 30, 35, 40, 45, 50)
+
+
+def truths_lengths(target, num_keypoints=9, max_num_gt=50):
+    """valid_multi.py:20-23 per image of a (B, rows*(2K+3)) label: the rows before the first with x0 == 0 -> int64 numpy (B,).
+    A label whose max_num_gt rows are all filled counts them all (the reference's truths_length returns None there)."""
+    nl = 2 * num_keypoints + 3
+    t = (target.detach().cpu().float().numpy() if torch.is_tensor(target) else np.asarray(target, np.float32))
+    t = t.reshape(t.shape[0], -1, nl)[:, :max_num_gt]
+    empty = t[:, :, 1] == 0
+    return np.where(empty.any(1), empty.argmax(1), t.shape[1]).astype(np.int64)
+
+
+def projection_accuracy(pixel_err, thresholds=ACCURACY_THRESHOLDS):
+    """valid_multi.py:154-158 over the accumulated per-object 2-D projection errors: [% of errors <= px for px in thresholds],
+    computed as the reference does, len(where(err <= px)) * 100 / (n + 1e-5)."""
+    if torch.is_tensor(pixel_err):
+        pixel_err = pixel_err.detach().cpu().numpy()
+    err = np.asarray(pixel_err, dtype=np.float64).reshape(-1)
+    return [len(np.where(err <= px)[0]) * 100. / (len(err) + 1e-5) for px in thresholds]
+
+
+def evaluate_multi_poses_batched(output, target, conf_thresh, num_classes, num_keypoints, num_anchors, vertices, corners3D,
+                                 internal_calibration, im_width=640, im_height=480):
+    """GPU version of the multi-object evaluation loop (valid_multi.py:97-149, train_multi.py:196-240) for a whole batch.
+
+    output (B, (2K+1+C)*A, H, W) CUDA network output; target (B, 50*(2K+3)) label of dataset_multi.listDataset in test mode, host
+    or device; vertices (3|4, Nv) mesh; corners3D (3|4, 8) from get_3D_corners; internal_calibration (3, 3).
+
+    Per image, exactly as one iteration of the reference's batch-1 loop: the box list of get_multi_region_boxes(output, conf_thresh,
+    ..., int(target[0]), only_objectness=0); for each ground truth the first box of its class with the largest det_conf, else the
+    previous ground truth's box; PnP of the fix_corner_order'ed ground truth and of the prediction against [0; corners3D]; the
+    mean 2-D distance of all vertices projected with both poses.  One launch selects (ssp_eval_multi_select), one PnP launch
+    solves all 2G problems, one projects all vertices for the 2G poses.  The object counts come from a host copy of the target
+    (one device->host copy when it lives on the device), so nothing waits on the GPU.
+
+    Returns a dict of CUDA tensors with leading dimension G (all ground truths of the batch, image-major): image, gt_index, cls,
+    box (the chosen box [x0/w, y0/h, ..., det_conf, cls_conf, cls_id]), fallback and carried (bool), R_gt, t_gt, R_pr, t_pr (fp64),
+    pixel_err.  Accumulate pixel_err over batches and pass it to projection_accuracy.
+
+    Deliberate departures: with B > 1 every image is evaluated as the reference's own batch-1 call (the reference takes
+    correspondingclass from image 0 and keeps its fallback maxima across the batch); a label with all 50 rows filled is evaluated
+    in full, where the reference raises TypeError from range(None).  The reference's per-object corner_confidence and projected
+    corners are never used by it and are not computed."""
+    if output.dim() == 3:
+        output = output.unsqueeze(0)
+    if not output.is_cuda:
+        raise SspError("evaluate_multi_poses_batched runs on CUDA tensors only")
+    out = output.detach().contiguous().float()
+    dev = out.device
+    B, C, H, W = out.shape
+    K, nC, nA = num_keypoints, num_classes, num_anchors
+    assert C == (2 * K + 1 + nC) * nA
+    nl = 2 * K + 3
+    tgt = target.detach() if torch.is_tensor(target) else torch.as_tensor(np.asarray(target))
+    tgt = tgt.reshape(B, -1)
+    if tgt.shape[1] < nl:
+        raise SspError("target rows hold %d values, need at least 2K+3 = %d" % (tgt.shape[1], nl))
+    counts = truths_lengths(tgt, K)
+    offsets = np.concatenate([[0], np.cumsum(counts)]).astype(np.int32)
+    G = int(offsets[-1])
+    image = torch.from_numpy(np.repeat(np.arange(B), counts)).to(dev)
+    gt_index = torch.from_numpy(np.arange(G) - np.repeat(offsets[:-1].astype(np.int64), counts)).to(dev)
+    tgt_d = tgt.to(dev, torch.float32).contiguous()
+    off_d = torch.from_numpy(offsets).to(dev)
+    box = torch.empty(G, nl, dtype=torch.float32, device=dev)
+    flags = torch.empty(G, dtype=torch.int32, device=dev)
+    uv = torch.empty(2 * G, K, 2, dtype=torch.float32, device=dev)
+    if G:
+        call("ssp_eval_multi_select", ptr(out), B, K, nC, nA, H, W, ptr(tgt_d), tgt_d.shape[1], ptr(off_d), float(conf_thresh),
+             float(im_width), float(im_height), ptr(box), ptr(flags), ptr(uv), stream_ptr())
+    rows = tgt_d.shape[1] // nl
+    cls = tgt_d[:, :rows * nl].reshape(B, rows, nl)[image, gt_index, 0].long()
+    res = dict(image=image, gt_index=gt_index, cls=cls, box=box, fallback=(flags & 1) != 0, carried=(flags & 2) != 0)
+    if G == 0:                                                  # nothing to solve: empty poses and errors
+        R0 = torch.zeros(0, 3, 3, dtype=torch.float64, device=dev)
+        t0 = torch.zeros(0, 3, dtype=torch.float64, device=dev)
+        return dict(res, R_gt=R0, t_gt=t0, R_pr=R0.clone(), t_pr=t0.clone(), pixel_err=torch.zeros(0, dtype=torch.float32, device=dev))
+    c3 = np.asarray(corners3D, dtype=np.float64)[:3]
+    P3 = np.array(np.transpose(np.concatenate((np.zeros((3, 1)), c3), axis=1)), dtype="float32")          # valid_multi.py:135
+    Kc = torch.as_tensor(np.asarray(internal_calibration, dtype=np.float32)).to(dev)
+    R, t = pnp_batched(torch.from_numpy(P3).to(dev), uv, Kc)                                                 # 2G problems, one launch
+    Rt = torch.cat([R, t.unsqueeze(2)], 2)
+    V = torch.as_tensor(np.asarray(vertices, dtype=np.float32)).to(dev)
+    if V.shape[0] == 3:
+        V = torch.cat([V, torch.ones(1, V.shape[1], device=dev)], 0)
+    proj = project_points_batched(V, Rt, torch.as_tensor(np.asarray(internal_calibration, dtype=np.float64)).to(dev))   # (2G, 2, Nv)
+    d = proj[:G] - proj[G:]
+    # valid_multi.py:143-149.  Elementwise distances, then an fp64 mean: the result of one object does not depend on how many
+    # objects the batch holds (a batched fp32 reduction may change its summation order with the shape)
+    pixel_err = torch.hypot(d[:, 0], d[:, 1]).double().mean(dim=1).float()
+    return dict(res, R_gt=R[:G], t_gt=t[:G], R_pr=R[G:], t_pr=t[G:], pixel_err=pixel_err)
