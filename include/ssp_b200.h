@@ -192,6 +192,21 @@ int ssp_pnp_batched_work(const float* points3d, int points3d_shared, const float
 int ssp_project_points(const float* X, int rows, int nv, const double* Rt, const double* K3x3, long long n,
                        float* out, void* stream);
 
+/* ---- pose errors over the mesh (utils.py:50-64, valid.py:69-72, 173-177), fp64 throughout (csrc/adds.cu, csrc/adds_core.h).
+ *      X [nv][3] fp64 vertices; Rt_est, Rt_gt [n][3][4] fp64 poses [R | t].
+ *  ssp_adds_batched: adds_out[p] = mean_i min_j |Rt_gt[p] x_i - Rt_est[p] x_j|, the reference's adi(pts_est, pts_gt) (ADD-S, for
+ *      symmetric objects); add_out[p] (optional) = mean_i |Rt_gt[p] x_i - Rt_est[p] x_i| (ADD).  Each pose's result is computed in
+ *      a fixed order: bit-identical on every launch, whatever n and the pose's position in the batch.  work: device scratch of at
+ *      least ssp_adds_work_bytes(nv, n) bytes (8-B aligned).  n = 0 does nothing.
+ *  ssp_mesh_diameter: *diam_out = the largest distance between two vertices, bit-identical to calc_pts_diameter on float64.
+ *  SSP_ERR_ARG for a null pointer, nv < 1, nv > SSP_ADDS_MAX_VERTICES, n < 0 or n > 2^31 - 1 (ssp_adds_work_bytes returns
+ *  SSP_ERR_ARG for these sizes too). ---- */
+#define SSP_ADDS_MAX_VERTICES (1 << 20)
+long long ssp_adds_work_bytes(int nv, long long n);
+int ssp_adds_batched(const double* X, int nv, const double* Rt_est, const double* Rt_gt, long long n, double* adds_out,
+                     double* add_out_or_null, void* work, long long work_bytes, void* stream);
+int ssp_mesh_diameter(const double* X, int nv, double* diam_out, void* stream);
+
 /* ---- training-image pipeline (SURVEY 8f.3): byte-exact with the Pillow routines image.py calls.  Images are device
  *      uint8 HWC RGB, dense.  resample = PIL.Image.Resampling value (0 NEAREST, 2 BILINEAR, 3 BICUBIC = resize()'s default
  *      in Pillow >= 7).  `work` is caller-provided device scratch (16-B aligned) of at least *_work_bytes() bytes.

@@ -54,6 +54,9 @@ int eval_multi_select(const float*, int, int, int, int, int, int, const float*, 
                       cudaStream_t);
 int pnp_batched(const float*, int, const float*, const float*, int, long long, int, double*, double*, int*, int*, cudaStream_t);
 int project_points(const float*, int, int, const double*, const double*, long long, float*, cudaStream_t);
+long long adds_work_bytes(int, long long);
+int adds_batched(const double*, int, const double*, const double*, long long, double*, double*, void*, long long, cudaStream_t);
+int mesh_diameter(const double*, int, double*, cudaStream_t);
 long long aug_resize_work_bytes(int, int, int, int, int);
 long long aug_sample_work_bytes(int, int, int, int, int, int, int, int, int);
 int aug_resize_u8(const uint8_t*, int, int, int, int, int, int, uint8_t*, int, int, int, uint8_t*, long long, cudaStream_t);
@@ -207,6 +210,12 @@ int ssp_pnp_batched_work(const float* P3, int shared, const float* uv, const flo
 int ssp_project_points(const float* X, int rows, int nv, const double* Rt, const double* K, long long n, float* out, void* s) {
   return project_points(X, rows, nv, Rt, K, n, out, ST(s));
 }
+long long ssp_adds_work_bytes(int nv, long long n) { return adds_work_bytes(nv, n); }
+int ssp_adds_batched(const double* X, int nv, const double* Rt_est, const double* Rt_gt, long long n, double* adds_out, double* add_out,
+                     void* work, long long work_bytes, void* s) {
+  return adds_batched(X, nv, Rt_est, Rt_gt, n, adds_out, add_out, work, work_bytes, ST(s));
+}
+int ssp_mesh_diameter(const double* X, int nv, double* diam_out, void* s) { return mesh_diameter(X, nv, diam_out, ST(s)); }
 long long ssp_aug_resize_work_bytes(int in_w, int in_h, int out_w, int out_h, int resample) { return aug_resize_work_bytes(in_w, in_h, out_w, out_h, resample); }
 int ssp_aug_resize_u8(const void* src, int src_w, int src_h, int x0, int y0, int in_w, int in_h, void* dst, int out_w, int out_h, int resample,
                       void* work, long long work_bytes, void* s) {

@@ -10,7 +10,7 @@ from __future__ import annotations
 import numpy as np
 import torch
 
-from ._lib import call, ptr, stream_ptr, SspError
+from ._lib import call, load, ptr, stream_ptr, SspError
 from .utils_host import (makedirs, get_all_files, calc_pts_diameter, adi, get_2d_bb, compute_2d_bb, compute_2d_bb_from_orig_pix,  # noqa: F401
                          corner_confidences, corner_confidence, sigmoid, softmax, fix_corner_order, read_truths, read_truths_args,
                          read_pose, load_class_names, image2torch, read_data_cfg, scale_bboxes, file_lines, get_image_size, logging)
@@ -129,15 +129,75 @@ def project_points_batched(points_3D, Rt, internal_calibration):
     return out
 
 
+# ------------------------------------------------------------------------------------------ pose errors over the mesh
+def _mesh_rows(vertices, dev):
+    """(3|4, Nv) or (Nv, 3), any float dtype -> (Nv, 3) fp64 contiguous on `dev` (converted there).  An array with 3 or 4 rows
+    is read as (3|4, Nv), the layout of valid.py's `vertices`."""
+    V = vertices if torch.is_tensor(vertices) else torch.as_tensor(np.asarray(vertices))
+    if V.dim() != 2 or not (V.shape[0] in (3, 4) or V.shape[1] == 3):
+        raise SspError("vertices must be (3|4, Nv) or (Nv, 3), got %s" % (tuple(V.shape),))
+    V = V.to(dev)
+    V = V[:3].t() if V.shape[0] in (3, 4) else V
+    return V.double().contiguous()
+
+
+def _pose_stack(Rt, dev):
+    T = (Rt if torch.is_tensor(Rt) else torch.as_tensor(np.asarray(Rt))).to(dev, torch.float64)
+    T = T.unsqueeze(0) if T.dim() == 2 else T
+    if T.dim() != 3 or tuple(T.shape[1:]) != (3, 4):
+        raise SspError("poses must be (n, 3, 4), got %s" % (tuple(T.shape),))
+    return T.contiguous()
+
+
+def adi_batched(vertices, Rt_est, Rt_gt, with_add=False):
+    """adi(pts_est, pts_gt) of utils.py:60-64 for n pose pairs: for each vertex under Rt_gt[p], the distance to the nearest
+    vertex under Rt_est[p], averaged over the mesh (ADD-S, the LINEMOD error of the symmetric eggbox and glue).
+    vertices (3|4, Nv) or (Nv, 3), any float dtype (converted to fp64 on the device); Rt_est, Rt_gt (n, 3, 4).
+    -> (n,) fp64 CUDA tensor; with with_add=True (adds, add), add[p] = mean_i |Rt_gt[p] x_i - Rt_est[p] x_i| (ADD) from the
+    same launch.  Brute force on the GPU (n * Nv^2 fp64 pair distances, ssp_adds_batched) where the reference builds a k-d
+    tree; each pose's value is computed in a fixed order, the same in any batch."""
+    dev = _dev()
+    X = _mesh_rows(vertices, dev)
+    E, G = _pose_stack(Rt_est, dev), _pose_stack(Rt_gt, dev)
+    if E.shape[0] != G.shape[0]:
+        raise SspError("Rt_est and Rt_gt hold %d and %d poses" % (E.shape[0], G.shape[0]))
+    n, nv = E.shape[0], X.shape[0]
+    adds = torch.empty(n, dtype=torch.float64, device=dev)
+    add = torch.empty(n, dtype=torch.float64, device=dev) if with_add else None
+    if n:
+        wb = int(load().ssp_adds_work_bytes(nv, n))
+        if wb < 0:
+            raise SspError("ssp_adds_work_bytes: bad size (Nv = %d, n = %d)" % (nv, n))
+        work = torch.empty(wb // 8, dtype=torch.float64, device=dev)
+        call("ssp_adds_batched", ptr(X), nv, ptr(E), ptr(G), n, ptr(adds), ptr(add), ptr(work), wb, stream_ptr())
+    return (adds, add) if with_add else adds
+
+
+def mesh_diameter(pts):
+    """calc_pts_diameter (utils.py:50-58) on the GPU: the largest distance between two of the (Nv, 3) points -> Python float,
+    bit-identical to calc_pts_diameter on float64 points.  Waits for the result."""
+    dev = _dev()
+    P = pts if torch.is_tensor(pts) else torch.as_tensor(np.asarray(pts))
+    if P.dim() != 2 or P.shape[1] != 3:
+        raise SspError("mesh_diameter takes (Nv, 3) points, got %s" % (tuple(P.shape),))
+    P = P.to(dev).double().contiguous()
+    out = torch.empty(1, dtype=torch.float64, device=dev)
+    call("ssp_mesh_diameter", ptr(P), P.shape[0], ptr(out), stream_ptr())
+    return float(out.item())
+
+
 # ------------------------------------------------------------------------------------------ batched evaluation tail
 def evaluate_poses_batched(output, target, vertices, points_3D, internal_calibration, num_classes=1, num_keypoints=9,
-                           im_width=640, im_height=480):
+                           im_width=640, im_height=480, adds=False):
     """GPU-resident version of the per-image evaluation loop of reference valid.py:123-183 (SURVEY 8f.1): per-image decode
     (arg-max cell of EACH image, not the whole batch), PnP of the ground-truth and the predicted keypoints, reprojection of
     all mesh vertices, pixel / 3-D / angular / translation errors -- no Python loop over images.
 
     output (B, 2K+1+C, h, w) CUDA; target (B, >= 2K+1) rows [cls, x0, y0, ..., x8, y8, ...] (first object);
-    vertices (3|4, Nv); points_3D (K, 3); internal_calibration (3, 3).  Returns a dict of CUDA tensors with leading dim B."""
+    vertices (3|4, Nv); points_3D (K, 3); internal_calibration (3, 3).  Returns a dict of CUDA tensors with leading dim B.
+    adds=True adds `adds_dist` (B,) fp64, adi(pts_pr, pts_gt) over the mesh as given in fp64 (adi_batched): the error that
+    replaces vertex_dist for the symmetric objects (eggbox, glue).  The angle error is arccos of the trace clamped to [-1, 1],
+    so an exact pose gives 0 where the reference's calcAngularDistance can give NaN."""
     dev = output.device
     K = num_keypoints
     boxes, best, _ = region_boxes_batched(output, num_classes, K)
@@ -162,5 +222,43 @@ def evaluate_poses_batched(output, target, vertices, points_3D, internal_calibra
     vertex_dist = (tf_gt - tf_pr).norm(dim=1).mean(dim=1)               # valid.py:176-178
     tr = torch.einsum("bij,bij->b", R_gt, R_pr)                         # trace(R_gt R_pr^T)
     angle = torch.rad2deg(torch.arccos(((tr - 1.0) / 2.0).clamp(-1.0, 1.0)))
-    return dict(boxes=boxes, conf=best, corner_err_px=(pr2d - gt2d).norm(dim=2).mean(dim=1), R_gt=R_gt, t_gt=t_gt, R_pr=R_pr, t_pr=t_pr,
-                pixel_err=pixel_err, vertex_dist=vertex_dist, angle_err_deg=angle, trans_err=(t_gt - t_pr).norm(dim=1))
+    res = dict(boxes=boxes, conf=best, corner_err_px=(pr2d - gt2d).norm(dim=2).mean(dim=1), R_gt=R_gt, t_gt=t_gt, R_pr=R_pr, t_pr=t_pr,
+               pixel_err=pixel_err, vertex_dist=vertex_dist, angle_err_deg=angle, trans_err=(t_gt - t_pr).norm(dim=1))
+    if adds:
+        res["adds_dist"] = adi_batched(vertices, Rt_pr, Rt_gt)
+    return res
+
+
+def _host_array(results, key):
+    v = [r[key] for r in results]
+    v = [x.detach().cpu().numpy() if torch.is_tensor(x) else np.asarray(x) for x in v]
+    return np.concatenate([x.reshape(-1) for x in v]) if v else np.zeros(0)
+
+
+def pose_accuracy(results, diam, px_threshold=5):
+    """The summary of valid.py:202-229 from one result dict of evaluate_poses_batched or a list of them (accumulated in order),
+    with the reference's formulas: a rate is len(where(err <= threshold)) * 100 / (n + 1e-5), a mean error is np.mean over the
+    per-image values, and the translation / angle / pixel errors are the running sums over the images divided by n.
+    -> dict: acc (2-D projection error <= px_threshold px), acc3d10 (vertex_dist, ADD, <= 10 % of diam), acc5cm5deg,
+    corner_acc (mean corner error <= px_threshold px), mean_err_2d, mean_vertex_err, mean_corner_err_2d, mean_trans_err,
+    mean_angle_err, mean_pixel_err, and acc_adds10 (adds_dist <= 10 % of diam) when the results hold adds_dist.
+
+    diam is the object's diameter in the mesh's units: valid.py takes it from calc_pts_diameter of the mesh (mesh_diameter
+    gives the same value on the GPU), train.py:296 from the `diam` entry of the .data file.  The batched tail clamps the
+    angle's cosine to [-1, 1], so an exact pose counts as 0 degrees; the reference's calcAngularDistance can return NaN there,
+    which fails the 5 degree test."""
+    if isinstance(results, dict):
+        results = [results]
+    eps = 1e-5
+    e2d, e3d, ecorner = (_host_array(results, k) for k in ("pixel_err", "vertex_dist", "corner_err_px"))
+    etrans, eangle = _host_array(results, "trans_err"), _host_array(results, "angle_err_deg")
+    n = len(e2d)
+    rate = lambda ok: len(np.where(ok)[0]) * 100. / (n + eps)
+    total = lambda errs: sum(errs, 0.0)                   # valid.py:180-182: += per image, in order, from 0.0
+    out = dict(acc=rate(e2d <= px_threshold), acc3d10=rate(e3d <= diam * 0.1), acc5cm5deg=rate((etrans <= 0.05) & (eangle <= 5)),
+               corner_acc=rate(ecorner <= px_threshold), mean_err_2d=np.mean(e2d), mean_vertex_err=np.mean(e3d),
+               mean_corner_err_2d=np.mean(ecorner), mean_trans_err=total(etrans) / float(n), mean_angle_err=total(eangle) / float(n),
+               mean_pixel_err=total(e2d) / float(n))
+    if all("adds_dist" in r for r in results):
+        out["acc_adds10"] = rate(_host_array(results, "adds_dist") <= diam * 0.1)
+    return out

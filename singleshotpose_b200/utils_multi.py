@@ -8,7 +8,7 @@ import torch
 
 from ._lib import call, ptr, stream_ptr, SspError
 from .utils import (pnp, pnp_batched, compute_projection, compute_transformation, calcAngularDistance, get_3D_corners,  # noqa: F401
-                    get_camera_intrinsic, convert2cpu, convert2cpu_long, project_points_batched)
+                    get_camera_intrinsic, convert2cpu, convert2cpu_long, project_points_batched, adi_batched, mesh_diameter)
 from .utils_host import (makedirs, get_all_files, calc_pts_diameter, adi, get_2d_bb, corner_confidences, corner_confidence,  # noqa: F401
                          sigmoid, softmax, read_truths, read_truths_args, read_pose, load_class_names, image2torch, scale_bboxes,
                          file_lines, get_image_size, logging)
@@ -142,7 +142,7 @@ def projection_accuracy(pixel_err, thresholds=ACCURACY_THRESHOLDS):
 
 
 def evaluate_multi_poses_batched(output, target, conf_thresh, num_classes, num_keypoints, num_anchors, vertices, corners3D,
-                                 internal_calibration, im_width=640, im_height=480):
+                                 internal_calibration, im_width=640, im_height=480, adds=False):
     """GPU version of the multi-object evaluation loop (valid_multi.py:97-149, train_multi.py:196-240) for a whole batch.
 
     output (B, (2K+1+C)*A, H, W) CUDA network output; target (B, 50*(2K+3)) label of dataset_multi.listDataset in test mode, host
@@ -157,7 +157,9 @@ def evaluate_multi_poses_batched(output, target, conf_thresh, num_classes, num_k
 
     Returns a dict of CUDA tensors with leading dimension G (all ground truths of the batch, image-major): image, gt_index, cls,
     box (the chosen box [x0/w, y0/h, ..., det_conf, cls_conf, cls_id]), fallback and carried (bool), R_gt, t_gt, R_pr, t_pr (fp64),
-    pixel_err.  Accumulate pixel_err over batches and pass it to projection_accuracy.
+    pixel_err.  Accumulate pixel_err over batches and pass it to projection_accuracy.  adds=True adds the 3-D errors over the
+    mesh as given, in fp64, from one more launch (utils.adi_batched): vertex_dist (ADD, as valid.py:173-177 computes it) and
+    adds_dist (ADD-S, adi(pts_pr, pts_gt), for the symmetric eggbox and glue), both (G,) fp64.
 
     Deliberate departures: with B > 1 every image is evaluated as the reference's own batch-1 call (the reference takes
     correspondingclass from image 0 and keeps its fallback maxima across the batch); a label with all 50 rows filled is evaluated
@@ -196,7 +198,10 @@ def evaluate_multi_poses_batched(output, target, conf_thresh, num_classes, num_k
     if G == 0:                                                  # nothing to solve: empty poses and errors
         R0 = torch.zeros(0, 3, 3, dtype=torch.float64, device=dev)
         t0 = torch.zeros(0, 3, dtype=torch.float64, device=dev)
-        return dict(res, R_gt=R0, t_gt=t0, R_pr=R0.clone(), t_pr=t0.clone(), pixel_err=torch.zeros(0, dtype=torch.float32, device=dev))
+        res = dict(res, R_gt=R0, t_gt=t0, R_pr=R0.clone(), t_pr=t0.clone(), pixel_err=torch.zeros(0, dtype=torch.float32, device=dev))
+        if adds:
+            res.update(vertex_dist=torch.zeros(0, dtype=torch.float64, device=dev), adds_dist=torch.zeros(0, dtype=torch.float64, device=dev))
+        return res
     c3 = np.asarray(corners3D, dtype=np.float64)[:3]
     P3 = np.array(np.transpose(np.concatenate((np.zeros((3, 1)), c3), axis=1)), dtype="float32")          # valid_multi.py:135
     Kc = torch.as_tensor(np.asarray(internal_calibration, dtype=np.float32)).to(dev)
@@ -210,4 +215,7 @@ def evaluate_multi_poses_batched(output, target, conf_thresh, num_classes, num_k
     # valid_multi.py:143-149.  Elementwise distances, then an fp64 mean: the result of one object does not depend on how many
     # objects the batch holds (a batched fp32 reduction may change its summation order with the shape)
     pixel_err = torch.hypot(d[:, 0], d[:, 1]).double().mean(dim=1).float()
-    return dict(res, R_gt=R[:G], t_gt=t[:G], R_pr=R[G:], t_pr=t[G:], pixel_err=pixel_err)
+    res = dict(res, R_gt=R[:G], t_gt=t[:G], R_pr=R[G:], t_pr=t[G:], pixel_err=pixel_err)
+    if adds:
+        res["adds_dist"], res["vertex_dist"] = adi_batched(vertices, Rt[G:], Rt[:G], with_add=True)
+    return res
