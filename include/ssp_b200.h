@@ -284,6 +284,36 @@ int ssp_augm_plan_finish(const ssp_augm_item* items_host, int n, int out_w, int 
                          long long table_bytes, int* stage_dims_host32);
 int ssp_augm_run(const void* table_dev, int n, const int* stage_dims_host32, void* stream);
 
+/* ---- JPEG decode (dataset.py / image.py open every training and test image with Pillow): baseline Huffman JPEGs decoded for a
+ *      whole batch, byte-identical to PIL's Image.open(f).convert('RGB') on libjpeg-turbo (ISLOW IDCT, fancy upsampling)
+ *      (csrc/jpeg.cu, rules in csrc/jpeg_core.h).
+ *  ssp_jpeg_parse (host only): header of one file.  Returns 0 if the GPU path takes it (1 component, or YCbCr with luma sampling
+ *      in {1,2}x{1,2} and 1x1 chroma, 8-bit, one sequential Huffman scan, ending with EOI), a positive decline code otherwise
+ *      (ssp_jpeg_decline_reason gives the text), SSP_ERR_ARG for a null pointer.  info receives the size either way when known.
+ *  ssp_jpeg_stage_bytes / ssp_jpeg_work_bytes (host only): pinned staging and device workspace sizes of a batch of takeable
+ *      files (SSP_ERR_ARG if one is declined).
+ *  ssp_jpeg_batch_plan (host only, no device access): writes the batch's records, entropy-coded data (without stuffed bytes and
+ *      restart markers) and interval tables into stage_host; dims_host4 receives {largest block count, largest pixel count,
+ *      workspace bytes, staging bytes actually used}.  items[i].out is the DEVICE (height, width, 3) uint8 output.
+ *  ssp_jpeg_batch_run: stage_dev = the device copy of the first dims[3] bytes of the staging buffer (16-B aligned); three
+ *      launches on `stream`, no allocation, no synchronisation.  status[3n] (device int): status[i] | status[n + i] is 0 when
+ *      the output was written, otherwise SSP_JPEG_ST_* bits (the output is left untouched and the image is for Pillow);
+ *      status[2n + i] = the subsequences of image i whose state no speculative candidate linked to, decoded serially.
+ *      n = 0 does nothing. ---- */
+#define SSP_JPEG_ST_ENTROPY 1    /* invalid code, coefficient index past 63, data missing or left over, ... */
+#define SSP_JPEG_ST_RANGE 2      /* a block where libjpeg-turbo's SIMD and C IDCT can differ */
+#define SSP_JPEG_ST_STRUCTURE 4  /* restart markers missing, extra or out of sequence, or another marker inside the scan */
+#define SSP_JPEG_ST_OVERFLOW 8   /* a DC value leaves int32 */
+typedef struct ssp_jpeg_info { int width, height, components, h_samp, v_samp, restart_interval; } ssp_jpeg_info;
+typedef struct ssp_jpeg_item { const void* data; long long size; void* out; } ssp_jpeg_item;
+int ssp_jpeg_parse(const void* data, long long size, ssp_jpeg_info* info);
+const char* ssp_jpeg_decline_reason(int code);
+long long ssp_jpeg_stage_bytes(const ssp_jpeg_item* items_host, int n);
+long long ssp_jpeg_work_bytes(const ssp_jpeg_item* items_host, int n);
+int ssp_jpeg_batch_plan(const ssp_jpeg_item* items_host, int n, void* stage_host, long long stage_bytes, long long* dims_host4);
+int ssp_jpeg_batch_run(const void* stage_dev, int n, const long long* dims_host4, void* work, long long work_bytes, int* status,
+                       void* stream);
+
 #ifdef __cplusplus
 }
 #endif

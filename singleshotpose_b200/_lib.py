@@ -73,8 +73,15 @@ SIGNATURES = {
     "ssp_augm_plan_attempt": [_p, _i, _i, _i, _i, _p, _ll, _p],
     "ssp_augm_plan_finish": [_p, _i, _i, _i, _i, _p, _ll, _p],
     "ssp_augm_run": [_p, _i, _p, _p],
+    "ssp_jpeg_parse": [_p, _ll, _p],
+    "ssp_jpeg_decline_reason": [_i],
+    "ssp_jpeg_stage_bytes": [_p, _i],
+    "ssp_jpeg_work_bytes": [_p, _i],
+    "ssp_jpeg_batch_plan": [_p, _i, _p, _ll, _p],
+    "ssp_jpeg_batch_run": [_p, _i, _p, _p, _ll, _p, _p],
 }
 _RESTYPE = {"ssp_last_error": C.c_char_p, "ssp_flat_alloc_rows": _ll, "ssp_flat_row": _ll,
+            "ssp_jpeg_decline_reason": C.c_char_p, "ssp_jpeg_stage_bytes": _ll, "ssp_jpeg_work_bytes": _ll,
             "ssp_aug_resize_work_bytes": _ll, "ssp_aug_sample_work_bytes": _ll, "ssp_aug_batch_table_bytes": _ll,
             "ssp_augm_work_bytes": _ll, "ssp_augm_table_bytes": _ll, "ssp_adds_work_bytes": _ll}
 

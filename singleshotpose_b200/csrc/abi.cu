@@ -57,6 +57,12 @@ int project_points(const float*, int, int, const double*, const double*, long lo
 long long adds_work_bytes(int, long long);
 int adds_batched(const double*, int, const double*, const double*, long long, double*, double*, void*, long long, cudaStream_t);
 int mesh_diameter(const double*, int, double*, cudaStream_t);
+int jpeg_parse(const void*, long long, ssp_jpeg_info*);
+const char* jpeg_decline_reason(int);
+long long jpeg_stage_bytes(const ssp_jpeg_item*, int);
+long long jpeg_work_bytes(const ssp_jpeg_item*, int);
+int jpeg_batch_plan(const ssp_jpeg_item*, int, void*, long long, long long*);
+int jpeg_batch_run(const void*, int, const long long*, void*, long long, int*, cudaStream_t);
 long long aug_resize_work_bytes(int, int, int, int, int);
 long long aug_sample_work_bytes(int, int, int, int, int, int, int, int, int);
 int aug_resize_u8(const uint8_t*, int, int, int, int, int, int, uint8_t*, int, int, int, uint8_t*, long long, cudaStream_t);
@@ -216,6 +222,16 @@ int ssp_adds_batched(const double* X, int nv, const double* Rt_est, const double
   return adds_batched(X, nv, Rt_est, Rt_gt, n, adds_out, add_out, work, work_bytes, ST(s));
 }
 int ssp_mesh_diameter(const double* X, int nv, double* diam_out, void* s) { return mesh_diameter(X, nv, diam_out, ST(s)); }
+int ssp_jpeg_parse(const void* data, long long size, ssp_jpeg_info* info) { return jpeg_parse(data, size, info); }
+const char* ssp_jpeg_decline_reason(int code) { return jpeg_decline_reason(code); }
+long long ssp_jpeg_stage_bytes(const ssp_jpeg_item* items, int n) { return jpeg_stage_bytes(items, n); }
+long long ssp_jpeg_work_bytes(const ssp_jpeg_item* items, int n) { return jpeg_work_bytes(items, n); }
+int ssp_jpeg_batch_plan(const ssp_jpeg_item* items, int n, void* stage_host, long long stage_bytes, long long* dims) {
+  return jpeg_batch_plan(items, n, stage_host, stage_bytes, dims);
+}
+int ssp_jpeg_batch_run(const void* stage_dev, int n, const long long* dims, void* work, long long work_bytes, int* status, void* s) {
+  return jpeg_batch_run(stage_dev, n, dims, work, work_bytes, status, ST(s));
+}
 long long ssp_aug_resize_work_bytes(int in_w, int in_h, int out_w, int out_h, int resample) { return aug_resize_work_bytes(in_w, in_h, out_w, out_h, resample); }
 int ssp_aug_resize_u8(const void* src, int src_w, int src_h, int x0, int y0, int in_w, int in_h, void* dst, int out_w, int out_h, int resample,
                       void* work, long long work_bytes, void* s) {

@@ -14,6 +14,11 @@ Same constructor, same attributes (`seen`, `shape`, `nbatches`, ...), same multi
 path conventions (image.py:130-131) and -- with the same `random` state -- the same draws as the reference, so the batch equals
 what `listDataset` + `transforms.ToTensor()` + default collate produce there (tests/test_dataset_cpu.py checks this against the
 reference's own output through the committed golden).
+
+`listDataset(..., gpu_decode=True)`: for files that start with a JPEG's SOI marker (by content, not by extension) the workers
+return the file's bytes instead of decoding them, and take the image size from the frame header (`jpeg.read_jpeg_size`), so the
+draws do not change; `GpuCollate` then decodes all of a batch's JPEGs in one `jpeg.GpuJpegDecoder` call, byte-identical to Pillow.
+PNG masks and other formats decode in the workers as before.  The default, False, keeps the workers decoding everything.
 """
 from __future__ import annotations
 
@@ -25,6 +30,7 @@ import torch
 from torch.utils.data import Dataset
 
 from . import image as _image
+from .jpeg import read_jpeg_size
 from .utils_host import read_truths, read_truths_args          # noqa: F401  (dataset.py:12 imports them from utils)
 
 
@@ -43,9 +49,24 @@ def _open_rgb(path):
     return np.asarray(Image.open(path).convert('RGB'))
 
 
+def _load(path, gpu_decode):
+    """decoded RGB array, or -- with gpu_decode, for a JPEG -- the file's bytes (decoded later by GpuCollate on the device)"""
+    if gpu_decode:
+        with open(path, "rb") as f:
+            data = f.read()
+        if data[:2] == b"\xff\xd8" and read_jpeg_size(data) is not None:
+            return data
+    return _open_rgb(path)
+
+
+def _size(img):
+    """(width, height) of a decoded array or of JPEG bytes"""
+    return read_jpeg_size(img) if isinstance(img, bytes) else (img.shape[1], img.shape[0])
+
+
 class listDataset(Dataset):
     def __init__(self, root, shape=None, shuffle=True, transform=None, target_transform=None, train=False, seen=0, batch_size=64,
-                 num_workers=4, cell_size=32, bg_file_names=None, num_keypoints=9, max_num_gt=50):
+                 num_workers=4, cell_size=32, bg_file_names=None, num_keypoints=9, max_num_gt=50, gpu_decode=False):
         with open(root, 'r') as file:
             self.lines = file.readlines()
         if shuffle:
@@ -63,6 +84,7 @@ class listDataset(Dataset):
         self.nbatches = self.nSamples // self.batch_size
         self.num_keypoints = num_keypoints
         self.max_num_gt = max_num_gt
+        self.gpu_decode = gpu_decode
 
     def __len__(self):
         return self.nSamples
@@ -90,15 +112,17 @@ class listDataset(Dataset):
         if self.train:
             jitter, hue, saturation, exposure = 0.2, 0.1, 1.5, 1.5                         # dataset.py:93-97
             bgpath = self.bg_file_names[random.randint(0, len(self.bg_file_names) - 1)]
-            img, mask, bg = _open_rgb(imgpath), _open_rgb(mask_path(imgpath)), _open_rgb(bgpath)
+            g = self.gpu_decode
+            img, mask, bg = _load(imgpath, g), _load(mask_path(imgpath), g), _load(bgpath, g)
             # change_background keeps the image size, so the draws of data_augmentation see (ow, oh) of the image
-            params = _image.draw_augmentation(img.shape[1], img.shape[0], jitter, hue, saturation, exposure, random)
+            ow, oh = _size(img)
+            params = _image.draw_augmentation(ow, oh, jitter, hue, saturation, exposure, random)
             labpath = label_path(imgpath)
             rows = np.loadtxt(labpath) if os.path.getsize(labpath) else np.zeros((0, 2 * self.num_keypoints + 3))
             sample = dict(train=True, img=img, mask=mask, bg=bg, params=params, rows=rows, shape=tuple(self.shape),
                           num_keypoints=self.num_keypoints, max_num_gt=self.max_num_gt)
         else:
-            img = _open_rgb(imgpath)
+            img = _load(imgpath, self.gpu_decode)
             labpath = label_path(imgpath)
             num_labels = 2 * self.num_keypoints + 3
             label = torch.zeros(self.max_num_gt * num_labels)
@@ -132,6 +156,19 @@ class GpuCollate:
         self.device = torch.device(device)
         self.resample = resample
         self._aug = None
+        self._jpeg = None
+
+    def _decoded(self, samples, keys):
+        """the samples' images with every JPEG given as bytes (listDataset(gpu_decode=True)) decoded on the device, in one call"""
+        cols = {k: [s[k] for s in samples] for k in keys}
+        todo = [(k, i) for k in keys for i, a in enumerate(cols[k]) if isinstance(a, bytes)]
+        if todo:
+            if self._jpeg is None:
+                from .jpeg import GpuJpegDecoder
+                self._jpeg = GpuJpegDecoder(self.device)
+            for (k, i), t in zip(todo, self._jpeg([cols[k][i] for k, i in todo])):
+                cols[k][i] = t
+        return cols
 
     def __call__(self, samples):
         if not samples:
@@ -144,10 +181,10 @@ class GpuCollate:
         if train:
             if self._aug is None:
                 self._aug = _image.GpuAugmenter(self.device, self.resample)
-            data, _ = self._aug([s["img"] for s in samples], [s["mask"] for s in samples], [s["bg"] for s in samples], shape,
-                                params=[s["params"] for s in samples])
+            cols = self._decoded(samples, ("img", "mask", "bg"))
+            data, _ = self._aug(cols["img"], cols["mask"], cols["bg"], shape, params=[s["params"] for s in samples])
             return data, host_labels(samples)
         if shape is None:
             raise ValueError("test-mode batches need a network shape (listDataset(shape=...)) to be stackable")
-        data = _image.load_validation_batch([s["img"] for s in samples], shape, self.device, self.resample)
+        data = _image.load_validation_batch(self._decoded(samples, ("img",))["img"], shape, self.device, self.resample)
         return data, torch.stack([s["label"] for s in samples])

@@ -212,6 +212,9 @@ def _stage_plan(imgs, masks, bgs, params, W, H, resample):
             raise ValueError("empty crop window %dx%d" % (p["cw"], p["ch"]))
         o = {}
         for k, a in (("img", im), ("mask", mk), ("bg", bg)):
+            if torch.is_tensor(a) and a.is_cuda:            # already on the device: the kernels read it in place
+                o[k] = None
+                continue
             o[k] = total
             total += _a16(int(np.prod(a.shape)))
         o["luts"] = total
@@ -236,7 +239,9 @@ def _stage_fill(st, imgs, masks, bgs, params, offs):
     def one(args):
         im, mk, bg, p, o = args
         for k, a in (("img", im), ("mask", mk), ("bg", bg)):
-            a = a.cpu().numpy() if torch.is_tensor(a) else a
+            if o[k] is None:
+                continue
+            a = a.numpy() if torch.is_tensor(a) else a
             st[o[k]:o[k] + a.size] = a.reshape(-1)
         lh, ls, lv = distort_luts(p["dhue"], p["dsat"], p["dexp"])
         st[o["luts"]:o["luts"] + 1280] = np.concatenate([pos, neg, lh, ls, lv])
@@ -292,6 +297,10 @@ class GpuAugmenter:
         imgs = [_u8_hwc(a, "img") for a in imgs]
         masks = [_u8_hwc(a, "mask") for a in masks]
         bgs = [_u8_hwc(a, "bg") for a in bgs]
+        here = self.device.index if self.device.index is not None else torch.cuda.current_device()
+        for a in imgs + masks + bgs:
+            if torch.is_tensor(a) and a.is_cuda and a.device.index != here:
+                raise ValueError("input tensor on %s, the augmenter runs on cuda:%d" % (a.device, here))
         if params is None:
             params = [draw_augmentation(im.shape[1], im.shape[0], jitter, hue, saturation, exposure, rng) for im in imgs]
         offs, total, work_bytes = _stage_plan(imgs, masks, bgs, params, W, H, self.resample)
@@ -312,13 +321,16 @@ class GpuAugmenter:
         out = torch.empty(B, 3, H, W, dtype=torch.float32, device=self.device)
         u8 = torch.empty(B, H, W, 3, dtype=torch.uint8, device=self.device) if self.keep_u8 else None
         base = self._dev.data_ptr()
+
+        def at(a, o, k):                    # device address of an input: in place if it is a CUDA tensor, else its staged copy
+            return a.data_ptr() if o[k] is None else base + o[k]
         if self.batched:
             # the op table (device pointers, per-sample geometry) is planned on the host straight into the tail of the pinned
             # staging buffer and travels in the batch's single host->device copy
             items = (_AugItem * B)()
             wbase = self._work.data_ptr()
             for i, (im, bg, p, o) in enumerate(zip(imgs, bgs, params, offs)):
-                items[i] = _AugItem(base + o["img"], base + o["mask"], im.shape[1], im.shape[0], base + o["bg"], bg.shape[1], bg.shape[0],
+                items[i] = _AugItem(at(im, o, "img"), at(masks[i], o, "mask"), im.shape[1], im.shape[0], at(bg, o, "bg"), bg.shape[1], bg.shape[0],
                                     base + o["luts"], p["pleft"], p["ptop"], p["cw"], p["ch"], wbase + i * work_each, work_each,
                                     u8[i].data_ptr() if u8 is not None else None, out[i].data_ptr())
             dims = (C.c_int * 20)()
@@ -333,8 +345,8 @@ class GpuAugmenter:
             self.launches += sum(1 for k in range(10) if dims[2 * k] > 0)
             return (out, params, u8) if self.keep_u8 else (out, params)
         for i, (im, bg, p, o) in enumerate(zip(imgs, bgs, params, offs)):
-            call("ssp_aug_sample", C.c_void_p(base + o["img"]), C.c_void_p(base + o["mask"]), im.shape[1], im.shape[0],
-                 C.c_void_p(base + o["bg"]), bg.shape[1], bg.shape[0], C.c_void_p(base + o["luts"]), p["pleft"], p["ptop"], p["cw"], p["ch"],
+            call("ssp_aug_sample", C.c_void_p(at(im, o, "img")), C.c_void_p(at(masks[i], o, "mask")), im.shape[1], im.shape[0],
+                 C.c_void_p(at(bg, o, "bg")), bg.shape[1], bg.shape[0], C.c_void_p(base + o["luts"]), p["pleft"], p["ptop"], p["cw"], p["ch"],
                  W, H, self.resample, ptr(self._work), self._work.numel(), ptr(u8[i]) if u8 is not None else None, ptr(out[i]), s)
         self.launches += 10 * B             # upper bound: 2 x (2 coefficient + 2 pass) + composite + distort per sample
         return (out, params, u8) if self.keep_u8 else (out, params)
@@ -348,3 +360,6 @@ def load_data_detection_arrays(img, mask, bg, label_rows, shape, jitter, hue, sa
     p = params[0]
     label = fill_truth_detection(label_rows, shape[0], shape[1], p["flip"], p["dx"], p["dy"], 1. / p["sx"], 1. / p["sy"], num_keypoints, max_num_gt)
     return x[0], label
+
+
+from .jpeg import decode_jpeg  # noqa: E402,F401  (JPEG decode on the GPU, byte-identical to Pillow: jpeg.py)

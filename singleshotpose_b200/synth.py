@@ -129,10 +129,14 @@ def label_rows(seed, n=1, num_keypoints=9):
     return rows
 
 
-def write_linemod_like(root, n=4, ow=160, oh=120, num_bg=3):
+def write_linemod_like(root, n=4, ow=160, oh=120, num_bg=3, fmt="png"):
     """A tiny dataset tree with the reference's path conventions (image.py:130-131, train.py:309): JPEGImages/00000i.png, mask/000i.png,
     labels/00000i.txt, a background folder and the list file.  PNG throughout (lossless, so every decoder yields the same bytes).
-    Returns (list file path, background file names)."""
+    fmt="jpg": images and backgrounds are JPEG instead (JPEGImages/00000i.jpg, Pillow quality 95, its default 4:2:0), masks
+    stay PNG -- the layout of the real LINEMOD and VOC trees.  Returns (list file path, background file names)."""
+    if fmt not in ("png", "jpg"):
+        raise ValueError("fmt must be 'png' or 'jpg'")
+    kw = dict(quality=95) if fmt == "jpg" else {}
     from PIL import Image
     base = os.path.join(root, "LINEMOD", "ape")
     for d in ("JPEGImages", "mask", "labels"):
@@ -143,18 +147,18 @@ def write_linemod_like(root, n=4, ow=160, oh=120, num_bg=3):
     for i in range(n):
         img, mask, _bg = photo_sample(50 + i, ow, oh, 8, 8)
         name = "%06d" % i
-        Image.fromarray(img).save(os.path.join(base, "JPEGImages", name + ".png"))
+        Image.fromarray(img).save(os.path.join(base, "JPEGImages", name + "." + fmt), **kw)
         Image.fromarray(mask).save(os.path.join(base, "mask", "%04d.png" % i))
         rows = label_rows(50 + i, n=1 + i % 2)
         with open(os.path.join(base, "labels", name + ".txt"), "w") as f:
             if i != 3:                                   # sample 3 has an empty label file (os.path.getsize == 0 branch)
                 np.savetxt(f, rows)
-        lines.append(os.path.join(base, "JPEGImages", name + ".png"))
+        lines.append(os.path.join(base, "JPEGImages", name + "." + fmt))
     bgs = []
     for j in range(num_bg):
         _i, _m, bg = photo_sample(70 + j, 8, 8, 100 + 13 * j, 75 + 7 * j)
-        pth = os.path.join(bgdir, "bg%d.png" % j)
-        Image.fromarray(bg).save(pth)
+        pth = os.path.join(bgdir, "bg%d.%s" % (j, fmt))
+        Image.fromarray(bg).save(pth, **kw)
         bgs.append(pth)
     listfile = os.path.join(root, "train.txt")
     with open(listfile, "w") as f:
