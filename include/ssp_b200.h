@@ -73,6 +73,25 @@ int ssp_conv_gemm_bnact(int impl, const void* a_hi, const void* a_lo, long long 
                         const void* b_hi, const void* b_lo, int b_rows, int b_ld, int N, int H, int W, int taps, int cout,
                         const float* scale, const float* shift, float slope, void* d_hi, void* d_lo, int d_ld, int d_c0,
                         void* stream);
+/* ---- inference split-K for few output tiles (one camera frame): the per-tap tensor-core kernel with each output tile's K range
+ *      (taps x ceil(cin/64) k-blocks) cut into `splits` slices; slice s walks k-blocks [s*kb/S, (s+1)*kb/S) and stores its fp32
+ *      partial sums unmodified (plain stores, no atomics) into slab s of partial[splits][slab_elems] (rows [row][partial_ld]).
+ *      ssp_bn_apply_splitk then sums the slabs in the order s = 0..S-1 and applies BN(running stats) + leaky + routing exactly as
+ *      ssp_bn_apply does (no arg-max plane: inference only); splits = 1 runs ssp_bn_apply's kernel.
+ *      A result is bit-identical across launches and graph replays; it is NOT bit-identical across batch sizes or shapes whose
+ *      split count differs (the partial sums are added in a different order).
+ *  ssp_conv_gemm_splitk: fp16 hi/lo operands (3 terms) or single-term fp16 (b_lo / a_lo NULL).  SSP_ERR_ARG for splits < 1,
+ *      splits above the k-block count, a NULL or non-16-B-aligned workspace, partial_ld % 4 != 0 or < cout, and slabs
+ *      (slab_elems) smaller than ssp_flat_alloc_rows(N, H, W) * partial_ld, i.e. a workspace under splits * that size.
+ *  ssp_conv_splitk_count: the split rule, S = min(num_sms / tiles, k-blocks / 8), 1 when that is below 2 (tiles = 128-row x
+ *      N-tile output tiles of the per-tap kernel).  Host only. ---- */
+int ssp_conv_gemm_splitk(const void* a_hi, const void* a_lo_or_null, long long a_rows, int a_ld, int cin, const void* b_hi,
+                         const void* b_lo_or_null, int b_rows, int b_ld, int N, int H, int W, int taps, int cout, int splits,
+                         float* partial, long long slab_elems, int partial_ld, void* stream);
+int ssp_conv_splitk_count(int N, int H, int W, int taps, int cin, int cout, int num_sms);
+int ssp_bn_apply_splitk(const float* partial, int splits, long long slab_elems, int partial_ld, const float* scale, const float* shift,
+                        int N, int C, int H, int W, float slope, void* d0_hi, void* d0_lo, int d0_ld, int d0_c0, int d0_route,
+                        void* d1_hi, void* d1_lo, int d1_ld, int d1_c0, int d1_route, void* stream);
 /* ---- first layer nn.Conv2d(3, 32, 3, 1, 1) (darknet.py:156, block 0): direct fp32 convolution of the NCHW image with the
  *      fp32 master weights [32][3][3][3] (k = (kh*3+kw)*3 + ci), output rows [row(n,h,w)][y_ld], optional fp64 BN statistics ---- */
 int ssp_conv0_direct(const float* x_nchw, const float* w, const float* bias_or_null, float* y, int y_ld,

@@ -35,6 +35,9 @@ SIGNATURES = {
     "ssp_l0_bwd": [_p, _p, _i, _i, _i, _p, _f, _i, _i, _i, _p, _p],
     "ssp_l0_bwd_finalize": [_p, _p, _p, _p, _p, _p, _d, _f, _p, _p, _p, _p],
     "ssp_conv_gemm_bnact": [_i, _p, _p, _ll, _i, _i, _p, _p, _i, _i, _i, _i, _i, _i, _i, _p, _p, _f, _p, _p, _i, _i, _p],
+    "ssp_conv_gemm_splitk": [_p, _p, _ll, _i, _i, _p, _p, _i, _i, _i, _i, _i, _i, _i, _i, _p, _ll, _i, _p],
+    "ssp_conv_splitk_count": [_i, _i, _i, _i, _i, _i, _i],
+    "ssp_bn_apply_splitk": [_p, _i, _ll, _i, _p, _p, _i, _i, _i, _i, _f, _p, _p, _i, _i, _i, _p, _p, _i, _i, _i, _p],
     "ssp_wgrad_gemm": [_i, _p, _ll, _i, _i, _i, _p, _ll, _i, _i, _i, _i, _i, _i, _i, _p, _i, _i, _f, _p],
     "ssp_bn_finalize": [_p, _p, _d, _p, _p, _p, _p, _f, _f, _i, _p, _p, _p, _p, _i, _p],
     "ssp_bn_apply": [_p, _i, _p, _p, _i, _i, _i, _i, _f, _p, _p, _i, _i, _i, _p, _p, _i, _i, _i, _p, _i, _p],

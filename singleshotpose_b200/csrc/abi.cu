@@ -14,7 +14,8 @@ int fail_cuda(cudaError_t e, const char* file, int line) {
 int fail_msg(int code, const char* msg) { snprintf(g_err, sizeof(g_err), "%s", msg); return code; }
 
 int conv_gemm_tc(const void*, const void*, long long, int, int, const void*, const void*, int, int, int, int, int, int, int, int, int,
-                 float*, int, long long, int, const float*, double*, double*, cudaStream_t, const FusedAct*);
+                 float*, int, long long, int, const float*, double*, double*, cudaStream_t, const FusedAct*, const SplitK* = nullptr);
+int conv_splitk_count(int, int, int, int, int, int, int);
 int conv_gemm_band(const void*, const void*, long long, int, int, const void*, const void*, int, int, int, int, int, int, int, int, int,
                    float*, int, long long, int, const float*, double*, double*, cudaStream_t);
 int conv_gemm_simt(const void*, const void*, long long, int, int, const void*, const void*, int, int, int, int, int, int, int, int, int,
@@ -36,6 +37,8 @@ int unpack_nchw(const float*, float*, int, int, int, int, int, int, cudaStream_t
 int unpack16_nchw(const void*, const void*, float*, int, int, int, int, int, int, int, cudaStream_t);
 int bn_finalize(double*, double*, double, const float*, const float*, float*, float*, float, float, int, float*, float*, float*, float*, int, cudaStream_t);
 int bn_apply(const float*, int, const float*, const float*, int, int, int, int, float, void*, void*, int, int, int, void*, void*, int, int, int, float*, int, cudaStream_t);
+int bn_apply_splitk(const float*, int, long long, int, const float*, const float*, int, int, int, int, float, void*, void*, int, int, int, void*, void*,
+                    int, int, int, cudaStream_t, float* = nullptr, int = 0);
 int bn_bwd_reduce(const float*, int, const float*, const float*, const float*, const float*, const float*, int, int, int, int, float,
                   const float*, int, int, int, const float*, int, int, int, double*, double*, cudaStream_t);
 int bn_bwd_apply(const float*, int, const float*, const float*, const float*, const float*, const float*, int, int, int, int, float,
@@ -145,6 +148,20 @@ int ssp_conv_gemm_bnact(int impl, const void* a_hi, const void* a_lo, long long 
     return conv_gemm_tc(a_hi, a_lo, a_rows, a_ld, cin, b_hi, b_lo, b_rows, b_ld, SSP_FMT_F16, SSP_FMT_F16, N, H, W, taps, cout, nullptr, 0, 0, EPI_BNACT,
                         nullptr, nullptr, nullptr, ST(s), &fa);
   return fail_msg(SSP_ERR_ARG, "ssp_conv_gemm_bnact: tensor-core implementations only");
+}
+int ssp_conv_gemm_splitk(const void* a_hi, const void* a_lo, long long a_rows, int a_ld, int cin, const void* b_hi, const void* b_lo, int b_rows,
+                         int b_ld, int N, int H, int W, int taps, int cout, int splits, float* partial, long long slab_elems, int partial_ld,
+                         void* s) {
+  const SplitK sk{splits, slab_elems};
+  return conv_gemm_tc(a_hi, a_lo, a_rows, a_ld, cin, b_hi, b_lo, b_rows, b_ld, SSP_FMT_F16, SSP_FMT_F16, N, H, W, taps, cout, partial, partial_ld, 0,
+                      EPI_F32, nullptr, nullptr, nullptr, ST(s), nullptr, &sk);
+}
+int ssp_conv_splitk_count(int N, int H, int W, int taps, int cin, int cout, int num_sms) { return conv_splitk_count(N, H, W, taps, cin, cout, num_sms); }
+int ssp_bn_apply_splitk(const float* partial, int splits, long long slab_elems, int partial_ld, const float* scale, const float* shift, int N, int C,
+                        int H, int W, float slope, void* d0_hi, void* d0_lo, int d0_ld, int d0_c0, int d0_route, void* d1_hi, void* d1_lo, int d1_ld,
+                        int d1_c0, int d1_route, void* s) {
+  return bn_apply_splitk(partial, splits, slab_elems, partial_ld, scale, shift, N, C, H, W, slope, d0_hi, d0_lo, d0_ld, d0_c0, d0_route, d1_hi, d1_lo,
+                         d1_ld, d1_c0, d1_route, ST(s));
 }
 int ssp_wgrad_gemm(int impl, const void* dy, long long dy_rows, int dy_ld, int cout, int dy_fmt, const void* x, long long x_rows, int x_ld,
                    int cin, int x_fmt, int N, int H, int W, int taps, float* dw, int dw_ld, int cin_store, float scale, void* s) {

@@ -41,17 +41,25 @@ struct ConvTcParams {
   double* stat_sq;
   int epi;
   FusedAct fa;            // EPI_BNACT only
+  int splits;             // SPLIT only: K slices per output tile; slice s writes its raw accumulators to out + s * slab_elems
+  long long slab_elems;
 };
 
 static constexpr int kABytes = 128 * 128;     // 128 rows x 64 x 2 B
 static constexpr int kMaxStages = 8;
 static constexpr int kAccCols = 1024;         // per-CTA statistics accumulators (channels)
 static constexpr int kThreads = 256;
+// split-K rule (ssp_conv_splitk_count): S = min(SMs / tiles, k-blocks / kSplitMinKblocks), 1 when that is below 2.  A slice
+// shorter than this spends more of its time filling the TMA pipeline and storing its partial tile than in MMAs.
+static constexpr int kSplitMinKblocks = 8;
 
 // FUSED: the inference epilogue (EPI_BNACT) -- a separate instantiation keeps the training kernel's code unchanged.  BN = N tile (wgmma N),
 // BF = operand format (1 = bf16), NT = products per K step (3: split hi/lo operands, 1: single term).  All compile-time, so that
 // every wgmma of a k-block sits in straight-line code.
-template <bool FUSED, int BN, int BF, int NT>
+// SPLIT: split-K inference instantiation (ssp_conv_gemm_splitk) -- the persistent loop walks (tile, split) work items, split s
+// covers k-blocks [s*kb/S, (s+1)*kb/S) of the taps x kc_per_tap sequence and stores its fp32 accumulator tile unmodified
+// into slab s of the caller's workspace (plain stores, no atomics); ssp_bn_apply_splitk sums the slabs in a fixed order.
+template <bool FUSED, int BN, int BF, int NT, bool SPLIT = false>
 __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_constant__ ConvTcParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // dynamic smem base is only guaranteed 16-B aligned: round up to 1024 (swizzle-128B atoms)
@@ -86,6 +94,31 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
     if (lane == 0) {
       int stage = 0; uint32_t phase = 0;
       const uint32_t tx = (uint32_t)(p.n_terms == 3 ? 2 : 1) * (uint32_t)(kABytes + p.b_bytes);
+      if constexpr (SPLIT) {
+        // (tile, split) work items; the k-block sequence is the one of the loop below, cut at s*kb/S
+        for (int t = blockIdx.x; t < total_tiles * p.splits; t += gridDim.x) {
+          const int tile = t / p.splits, sp = t % p.splits;
+          const int m0 = (tile / p.n_tiles) * 128, n0 = (tile % p.n_tiles) * p.bn;
+          const int kb1 = (int)((long long)(sp + 1) * kblocks / p.splits);
+          for (int kb = (int)((long long)sp * kblocks / p.splits); kb < kb1; kb++) {
+            const int tap = kb / p.kc_per_tap, kc = kb - tap * p.kc_per_tap;
+            const int arow = m0 + p.shifts[tap];
+            mbar_wait(&empty_bar[stage], phase ^ 1);
+            uint8_t* sa = stage_base + (size_t)stage * p.stage_bytes;
+            mbar_expect_tx(&full_bar[stage], tx);
+            const int kcol_b = tap * p.cin + kc * 64;
+            tma_load_2d(sa, &p.tmA[0], &full_bar[stage], kc * 64, arow);
+            if (p.n_terms == 3) {
+              tma_load_2d(sa + kABytes, &p.tmA[1], &full_bar[stage], kc * 64, arow);
+              tma_load_2d(sa + 2 * kABytes, &p.tmB[0], &full_bar[stage], kcol_b, n0);
+              tma_load_2d(sa + 2 * kABytes + p.b_bytes, &p.tmB[1], &full_bar[stage], kcol_b, n0);
+            } else {
+              tma_load_2d(sa + kABytes, &p.tmB[0], &full_bar[stage], kcol_b, n0);
+            }
+            if (++stage == p.stages) { stage = 0; phase ^= 1; }
+          }
+        }
+      } else {
       for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
         const int mt = t / p.n_tiles, nt = t % p.n_tiles;
         const int m0 = mt * 128, n0 = nt * p.bn;
@@ -108,16 +141,23 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
           }
         }
       }
+      }
     }
   } else if (warp >= 4) {
     // ------------------------------------------------------------------ consumer warpgroup: MMA, then epilogue (thread et = tile row et)
     const int et = threadIdx.x - 128;
     int stage = 0; uint32_t phase = 0;
     float acc[2][BN / 2];
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-      const int mt = t / p.n_tiles, nt = t % p.n_tiles;
+    const int items = SPLIT ? total_tiles * p.splits : total_tiles;
+    for (int t = blockIdx.x; t < items; t += gridDim.x) {
+      int tile = t, sp = 0, kb0 = 0, kb1 = kblocks;
+      if constexpr (SPLIT) {
+        tile = t / p.splits; sp = t % p.splits;
+        kb0 = (int)((long long)sp * kblocks / p.splits); kb1 = (int)((long long)(sp + 1) * kblocks / p.splits);
+      }
+      const int mt = tile / p.n_tiles, nt = tile % p.n_tiles;
       int prev = -1;
-      for (int kb = 0; kb < kblocks; kb++) {
+      for (int kb = kb0; kb < kb1; kb++) {
         mbar_wait(&full_bar[stage], phase);
         const uint32_t sa = smem_u32(stage_base + (size_t)stage * p.stage_bytes);
         const uint32_t a_hi = sa, a_lo = sa + kABytes;
@@ -130,7 +170,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
 #pragma unroll
           for (int h = 0; h < 2; h++) {   // rows h * 64 .. h * 64 + 63 of the tile
             const uint64_t dah = gmma_desc_k_sw128(a_hi + h * 8192 + k * 32);
-            const int sd = (kb > 0 || k > 0) ? 1 : 0;
+            const int sd = (kb > kb0 || k > 0) ? 1 : 0;
             if constexpr (NT == 3) {
               wgmma_f32<BN, 0, 0, BF>(acc[h], gmma_desc_k_sw128(a_lo + h * 8192 + k * 32), dbh, sd);   // small cross terms first
               wgmma_f32<BN, 0, 0, BF>(acc[h], dah, gmma_desc_k_sw128(b_lo + k * 32), 1);
@@ -163,6 +203,20 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
         float v[32];
         acc_rows_32<BN>(acc, ch, stg, et, v);
         const int c0 = n0 + ch * 32;
+        if constexpr (SPLIT) {
+          // raw partial sums of this K slice; the reduction reads valid rows only
+          if (can_store) {
+            float* o = p.out + sp * p.slab_elems + m * p.out_ld;
+            if (c0 + 32 <= p.cout) {
+#pragma unroll
+              for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(o + c0 + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
+            } else {
+#pragma unroll
+              for (int j = 0; j < 32; j++) if (c0 + j < p.cout) o[c0 + j] = v[j];
+            }
+          }
+          continue;
+        }
         if constexpr (FUSED) {
           // folded BatchNorm (running statistics) + LeakyReLU in the epilogue; only valid rows are written so that the
           // consumer's pad rows stay zero; the fp32 Y tensor is never materialised in this mode
@@ -238,29 +292,59 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
   }
 }
 
-template <bool FUSED, int BF, int NT>
+template <bool FUSED, int BF, int NT, bool SPLIT = false>
 static int launch_conv_tc(const ConvTcParams& p, int grid, int smem_bytes, cudaStream_t stream) {
   static int configured = 0;
   if (!configured) {
     cudaError_t e = cudaSuccess;
-    for (auto k : {conv_tc_kernel<FUSED, 32, BF, NT>, conv_tc_kernel<FUSED, 64, BF, NT>, conv_tc_kernel<FUSED, 128, BF, NT>})
+    for (auto k : {conv_tc_kernel<FUSED, 32, BF, NT, SPLIT>, conv_tc_kernel<FUSED, 64, BF, NT, SPLIT>, conv_tc_kernel<FUSED, 128, BF, NT, SPLIT>})
       if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) return fail_cuda(e, __FILE__, __LINE__);
     configured = 1;
   }
-  if (p.bn == 32) conv_tc_kernel<FUSED, 32, BF, NT><<<grid, kThreads, smem_bytes, stream>>>(p);
-  else if (p.bn == 64) conv_tc_kernel<FUSED, 64, BF, NT><<<grid, kThreads, smem_bytes, stream>>>(p);
-  else conv_tc_kernel<FUSED, 128, BF, NT><<<grid, kThreads, smem_bytes, stream>>>(p);
+  if (p.bn == 32) conv_tc_kernel<FUSED, 32, BF, NT, SPLIT><<<grid, kThreads, smem_bytes, stream>>>(p);
+  else if (p.bn == 64) conv_tc_kernel<FUSED, 64, BF, NT, SPLIT><<<grid, kThreads, smem_bytes, stream>>>(p);
+  else conv_tc_kernel<FUSED, 128, BF, NT, SPLIT><<<grid, kThreads, smem_bytes, stream>>>(p);
   SSP_CHECK_LAUNCH();
   return SSP_OK;
 }
 
 static int g_num_sms = 0;
 
+// output tiles of the per-tap kernel and the k-blocks each of them walks (the N tile rule of conv_gemm_tc)
+static void tile_geometry(int N, int H, int W, int taps, int cin, int cout, long long* tiles, int* kblocks) {
+  const int bn = cout > 64 ? 128 : ((cout + 31) / 32) * 32;
+  *tiles = ((Geom{N, H, W}.m_rows() + 127) / 128) * (long long)((cout + bn - 1) / bn);
+  *kblocks = taps * ((cin + 63) / 64);
+}
+
+int conv_splitk_count(int N, int H, int W, int taps, int cin, int cout, int num_sms) {
+  if (N <= 0 || H <= 0 || W <= 0 || (taps != 1 && taps != 9) || cin <= 0 || cout <= 0 || num_sms <= 0)
+    return fail_msg(SSP_ERR_ARG, "ssp_conv_splitk_count: bad argument");
+  long long tiles; int kblocks;
+  tile_geometry(N, H, W, taps, cin, cout, &tiles, &kblocks);
+  long long s = num_sms / tiles;
+  if (s > kblocks / kSplitMinKblocks) s = kblocks / kSplitMinKblocks;
+  return s < 2 ? 1 : (int)s;
+}
+
 int conv_gemm_tc(const void* a_hi, const void* a_lo, long long a_rows, int a_ld, int cin,
                  const void* b_hi, const void* b_lo, int b_rows, int b_ld, int a_fmt, int b_fmt,
                  int N, int H, int W, int taps, int cout, float* out, int out_ld, long long out_rows,
-                 int epi, const float* bias, double* stat_sum, double* stat_sq, cudaStream_t stream, const FusedAct* fa) {
+                 int epi, const float* bias, double* stat_sum, double* stat_sq, cudaStream_t stream, const FusedAct* fa,
+                 const SplitK* sk) {
+  if (sk) {
+    long long tiles; int kblocks;
+    tile_geometry(N, H, W, taps, cin, cout, &tiles, &kblocks);
+    if (fa || epi != EPI_F32) return fail_msg(SSP_ERR_ARG, "conv_gemm_tc: split-K stores plain fp32 partial sums");
+    if (sk->splits < 1 || (cin > 0 && (taps == 1 || taps == 9) && sk->splits > kblocks))
+      return fail_msg(SSP_ERR_ARG, "ssp_conv_gemm_splitk: splits must be in [1, k-blocks] (taps * ceil(cin / 64))");
+    if (!out || ((uintptr_t)out % 16) || (out_ld % 4) || out_ld < cout || (sk->slab_elems % 4))
+      return fail_msg(SSP_ERR_ARG, "ssp_conv_gemm_splitk: workspace must be non-null and 16-B aligned, partial_ld % 4 == 0 and >= cout, slab_elems % 4 == 0");
+    if (sk->slab_elems < flat_alloc_rows(N, H, W) * (long long)out_ld)
+      return fail_msg(SSP_ERR_ARG, "ssp_conv_gemm_splitk: a slab must hold ssp_flat_alloc_rows(N, H, W) * partial_ld elements");
+    out_rows = flat_alloc_rows(N, H, W);
+  }
   if (fa) {
     if (!fa->scale || !fa->shift || !fa->d_hi || !fa->d_lo || (cout % 32) || (fa->d_ld % 8) || (fa->d_c0 % 8))
       return fail_msg(SSP_ERR_ARG, "conv_gemm_tc: fused BN+activation epilogue needs cout % 32 == 0 and 16-B aligned destination rows");
@@ -304,6 +388,8 @@ int conv_gemm_tc(const void* a_hi, const void* a_lo, long long a_rows, int a_ld,
   p.stages = stages;
   p.out = out; p.out_ld = out_ld; p.bias = bias; p.stat_sum = stat_sum; p.stat_sq = stat_sq; p.epi = epi;
   if (fa) p.fa = *fa; else p.fa = FusedAct{nullptr, nullptr, 1.f, nullptr, nullptr, 0, 0};
+  p.splits = sk ? sk->splits : 1;
+  p.slab_elems = sk ? sk->slab_elems : 0;
   int rc = 0;
   rc |= tmap_2d_16bit(&p.tmA[0], a_hi, (uint64_t)cin, (uint64_t)a_rows, (uint64_t)a_ld, 64, 128, a_fmt == FMT_BF16);
   rc |= tmap_2d_16bit(&p.tmB[0], b_hi, (uint64_t)taps * cin, (uint64_t)b_rows, (uint64_t)b_ld, 64, bn, b_fmt == FMT_BF16);
@@ -317,6 +403,11 @@ int conv_gemm_tc(const void* a_hi, const void* a_lo, long long a_rows, int a_ld,
   const int grid = total < g_num_sms ? total : g_num_sms;
   // split hi/lo operands are fp16 planes; the fused epilogue (ssp_conv_gemm_bnact) is fp16 only
   if (p.n_terms == 3 && p.fmt == FMT_BF16) return fail_msg(SSP_ERR_ARG, "conv_gemm_tc: split (hi/lo) operands must be fp16");
+  if (sk) {
+    const long long items = (long long)total * sk->splits;
+    const int sgrid = items < g_num_sms ? (int)items : g_num_sms;
+    return p.n_terms == 3 ? launch_conv_tc<false, 0, 3, true>(p, sgrid, smem_bytes, stream) : launch_conv_tc<false, 0, 1, true>(p, sgrid, smem_bytes, stream);
+  }
   if (fa) return p.n_terms == 3 ? launch_conv_tc<true, 0, 3>(p, grid, smem_bytes, stream) : launch_conv_tc<true, 0, 1>(p, grid, smem_bytes, stream);
   if (p.n_terms == 3) return launch_conv_tc<false, 0, 3>(p, grid, smem_bytes, stream);
   return p.fmt == FMT_BF16 ? launch_conv_tc<false, 1, 1>(p, grid, smem_bytes, stream) : launch_conv_tc<false, 0, 1>(p, grid, smem_bytes, stream);

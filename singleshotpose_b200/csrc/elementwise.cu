@@ -154,6 +154,7 @@ struct BnApplyParams {
   float slope;          // 0.1 leaky, 1.0 linear
   ActDst dst[2];
   float* ypool; int ypool_ld;   // POOLED only, optional: conv output y at the arg-max position of every 2x2 window (fp32, pooled geometry)
+  int splits; long long slab;   // SPLIT only: y = sum of the slabs y + s * slab, s = 0 .. splits-1 in this order
 };
 
 __device__ __forceinline__ float leaky(float v, float slope) { return v > 0.f ? v : v * slope; }
@@ -199,7 +200,8 @@ static inline unsigned unit_grid(int C, long long nunits, int per_thread) {
 #endif
 
 // POOLED = true : unit = one 2x2 window (needed when any destination is DST_POOL)
-template <bool POOLED>
+// SPLIT = true  : y is the sum of the split-K partial slabs of ssp_conv_gemm_splitk (inference, no arg-max plane)
+template <bool POOLED, bool SPLIT = false>
 __global__ void SSP_BN_BOUNDS bn_apply_kernel(const BnApplyParams p) {
   const int Hs = POOLED ? p.H / 2 : p.H, Ws = POOLED ? p.W / 2 : p.W;
   UnitWalk wk(p.C, (long long)p.N * Hs * Ws, BN_UNITS_PER_THREAD);
@@ -210,7 +212,9 @@ __global__ void SSP_BN_BOUNDS bn_apply_kernel(const BnApplyParams p) {
   Geom g{p.N, p.H, p.W};
   Geom gh{p.N, p.H / 2, p.W / 2};
   constexpr int NP = POOLED ? 4 : 1;
-  constexpr int UNR = POOLED ? 2 : 4;           // 8 / 4 independent 16-B loads in flight per thread
+  // 8 / 4 independent 16-B loads in flight per thread; the split-K sum keeps one unit's slabs in flight (no spills under the
+  // register cap of SSP_BN_BOUNDS)
+  constexpr int UNR = SPLIT ? 1 : (POOLED ? 2 : 4);
   for (long long u0 = wk.begin + wk.pl; u0 < wk.end; u0 += (long long)UNR * wk.PL) {
     float4 yv[UNR][NP]; long long rows[UNR][NP]; int nn[UNR], hh[UNR], ww[UNR]; bool ok[UNR];
 #pragma unroll
@@ -225,6 +229,12 @@ __global__ void SSP_BN_BOUNDS bn_apply_kernel(const BnApplyParams p) {
         const int h = POOLED ? hh[t] * 2 + (q >> 1) : hh[t], w = POOLED ? ww[t] * 2 + (q & 1) : ww[t];
         rows[t][q] = g.row(nn[t], h, w);
         yv[t][q] = *reinterpret_cast<const float4*>(p.y + rows[t][q] * p.y_ld + c);
+        if constexpr (SPLIT) {
+          for (int s = 1; s < p.splits; s++) {
+            const float4 b = *reinterpret_cast<const float4*>(p.y + s * p.slab + rows[t][q] * p.y_ld + c);
+            yv[t][q].x += b.x; yv[t][q].y += b.y; yv[t][q].z += b.z; yv[t][q].w += b.w;
+          }
+        }
       }
     }
 #pragma unroll
@@ -575,10 +585,22 @@ int bn_finalize(double* ssum, double* ssq, double count, const float* gamma, con
   bn_finalize_kernel<<<nblk(C, 128), 128, 0, s>>>(ssum, ssq, count, gamma, beta, rm, rv, momentum, eps, train, mean, invstd, scale, shift, C);
   SSP_CHECK_LAUNCH(); return SSP_OK;
 }
+int bn_apply_splitk(const float*, int, long long, int, const float*, const float*, int, int, int, int, float, void*, void*, int, int, int, void*,
+                    void*, int, int, int, cudaStream_t, float*, int);
 int bn_apply(const float* y, int y_ld, const float* scale, const float* shift, int N, int C, int H, int W, float slope,
              void* d0_hi, void* d0_lo, int d0_ld, int d0_c0, int d0_kind,
              void* d1_hi, void* d1_lo, int d1_ld, int d1_c0, int d1_kind, float* ypool, int ypool_ld, cudaStream_t s) {
+  return bn_apply_splitk(y, 1, 0, y_ld, scale, shift, N, C, H, W, slope, d0_hi, d0_lo, d0_ld, d0_c0, d0_kind, d1_hi, d1_lo, d1_ld, d1_c0, d1_kind,
+                         s, ypool, ypool_ld);
+}
+// splits == 1 launches the plain kernel (the ssp_bn_apply path); splits > 1 the instantiation that sums the partial slabs first
+int bn_apply_splitk(const float* y, int splits, long long slab, int y_ld, const float* scale, const float* shift, int N, int C, int H, int W,
+                    float slope, void* d0_hi, void* d0_lo, int d0_ld, int d0_c0, int d0_kind, void* d1_hi, void* d1_lo, int d1_ld, int d1_c0,
+                    int d1_kind, cudaStream_t s, float* ypool, int ypool_ld) {
   if (!y || !scale || !shift || (C % 4)) return fail_msg(SSP_ERR_ARG, "bn_apply: bad argument (C must be a multiple of 4)");
+  if (splits < 1 || (splits > 1 && (((uintptr_t)y % 16) || (y_ld % 4) || y_ld < C || (slab % 4) || slab < (long long)y_ld * flat_alloc_rows(N, H, W))))
+    return fail_msg(SSP_ERR_ARG, "bn_apply_splitk: splits >= 1; partial slabs 16-B aligned, partial_ld % 4 == 0 and >= C, slab_elems % 4 == 0 and "
+                                 ">= ssp_flat_alloc_rows(N, H, W) * partial_ld");
   if (ypool && ((ypool_ld % 4) || ypool_ld < C)) return fail_msg(SSP_ERR_ARG, "bn_apply: arg-max plane needs ld % 4 == 0 and ld >= C");
   BnApplyParams p;
   p.y = y; p.y_ld = y_ld; p.scale = scale; p.shift = shift; p.N = N; p.C = C; p.H = H; p.W = W; p.slope = slope;
@@ -587,10 +609,15 @@ int bn_apply(const float* y, int y_ld, const float* scale, const float* shift, i
   const bool pooled = p.dst[0].kind == DST_POOL || p.dst[1].kind == DST_POOL;
   if (ypool && !pooled) return fail_msg(SSP_ERR_ARG, "bn_apply: the arg-max plane belongs to a max-pool destination");
   p.ypool = ypool; p.ypool_ld = ypool_ld;
+  p.splits = splits; p.slab = slab;
   const bool halves = pooled || p.dst[0].kind == DST_REORG || p.dst[1].kind == DST_REORG;
   if (halves && ((H | W) & 1)) return fail_msg(SSP_ERR_ARG, "bn_apply: pool/reorg need even H and W");
-  if (pooled) bn_apply_kernel<true><<<unit_grid(C, (long long)N * (H / 2) * (W / 2), BN_UNITS_PER_THREAD), 256, 0, s>>>(p);
-  else bn_apply_kernel<false><<<unit_grid(C, (long long)N * H * W, BN_UNITS_PER_THREAD), 256, 0, s>>>(p);
+  const unsigned grid = pooled ? unit_grid(C, (long long)N * (H / 2) * (W / 2), BN_UNITS_PER_THREAD) : unit_grid(C, (long long)N * H * W, BN_UNITS_PER_THREAD);
+  if (splits > 1) {
+    if (pooled) bn_apply_kernel<true, true><<<grid, 256, 0, s>>>(p);
+    else bn_apply_kernel<false, true><<<grid, 256, 0, s>>>(p);
+  } else if (pooled) bn_apply_kernel<true><<<grid, 256, 0, s>>>(p);
+  else bn_apply_kernel<false><<<grid, 256, 0, s>>>(p);
   SSP_CHECK_LAUNCH(); return SSP_OK;
 }
 

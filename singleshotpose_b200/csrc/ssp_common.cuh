@@ -47,6 +47,8 @@ struct FusedAct {
   const float* scale; const float* shift; float slope;
   uint16_t* d_hi; uint16_t* d_lo; long long d_ld; int d_c0;
 };
+// inference split-K (ssp_conv_gemm_splitk): `splits` K slices per output tile, slice s stores into out + s * slab_elems
+struct SplitK { int splits; long long slab_elems; };
 struct Geom {
   int N, H, W;
   __host__ __device__ int Wp() const { return W + 1; }

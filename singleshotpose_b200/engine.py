@@ -124,10 +124,18 @@ def _flatten(expr, kind=_lib.ROUTE_DIRECT, c0=0):
 class Buffers:
     """Device buffers for one input shape (N, H, W); zero-initialised so that pad rows stay zero."""
 
-    def __init__(self, eng, N, H, W, train):
+    def __init__(self, eng, N, H, W, train, split_k=False):
         dev = eng.device
         self.N, self.H, self.W = N, H, W
         self.generation = 0
+        # inference split-K (Engine.forward(split_k=True)): per-layer split count (0 = the layer keeps its kernels) and ONE fp32
+        # workspace of max(splits * slab) elements, slab = the layer's rows x ld, shared by the layers (they run one after another)
+        self.split_k = bool(split_k)
+        self.splits = [eng.split_count(L, N, H, W) if split_k else 0 for L in eng.layers]
+        self.split_ld = [_rup(L.cout, 4) for L in eng.layers]
+        self.split_slab = [_lib.flat_alloc_rows(N, *eng.spatial(L, H, W)) * ld for L, ld in zip(eng.layers, self.split_ld)]
+        ws = max([s * slab for s, slab in zip(self.splits, self.split_slab)] or [0])
+        self.split_ws = torch.empty(ws, dtype=torch.float32, device=dev) if ws else None
         f16 = torch.float16
         self.x_hi, self.x_lo, self.y, self.rows = [], [], [], []
         self.dy, self.dx, self.ypool = [], [], []
@@ -200,7 +208,13 @@ class Engine:
         # fp16 epilogue (auto dispatch: per-tap / operand-swapped); forced implementations keep fp32 planes.
         self.dx_f16 = os.environ.get("SSP_DX_F16", "1") != "0" and self.conv_impl < 0 and self.grad_fmt == _lib.FMT_F16
         self.launches = 0
-        self.overlap = os.environ.get("SSP_OVERLAP", "1") != "0"
+        # inference split-K (forward(split_k=True)): launches of ssp_conv_gemm_splitk so far; split_override (internal, for tests and
+        # tools/bench_predict.py): None = ssp_conv_splitk_count's rule, 0 = split-K off, k >= 1 = k splits (at most the k-block
+        # count) for every layer the rule would consider, k = 1 included
+        self.split_launches = 0
+        self.split_override = None
+        self._num_sms = None
+        self.overlap =os.environ.get("SSP_OVERLAP", "1") != "0"
         self.compact_pool_reduce = os.environ.get("SSP_POOL_REDUCE", "compact") != "full"
         self._side = None
         self.grad_ready_hook = None  # fn(first layer index, stream): every gradient of layers >= that index is complete in `stream` order
@@ -372,15 +386,37 @@ class Engine:
             self.launches += 1
         self._weights_version = ver
 
-    def buffers(self, N, H, W, train):
-        key = (N, H, W, bool(train))
+    def buffers(self, N, H, W, train, split_k=False):
+        key = (N, H, W, bool(train), bool(split_k))
         b = self._buffers.get(key)
         if b is None:
             if len(self._buffers) >= 4:
                 self._buffers.clear()
-            b = Buffers(self, N, H, W, train)
+            b = Buffers(self, N, H, W, train, split_k)
             self._buffers[key] = b
         return b
+
+    def _fuse_eval_layer(self, L):
+        """inference layers whose BN + leaky run in the GEMM epilogue (ssp_conv_gemm_bnact)"""
+        return (L.bn and self.fuse_eval and not L.first and self.conv_impl != _lib.IMPL_SIMT and len(L.dests) == 1
+                and L.dests[0][2] == _lib.ROUTE_DIRECT and L.cout % 32 == 0)
+
+    def split_count(self, L, N, H, W):
+        """split-K count of an inference forward of layer L on an N x 3 x H x W input: 0 = the layer keeps its kernels.  Only BN
+        layers whose forward runs on the per-tap tensor-core kernel are split; the rule is ssp_conv_splitk_count's."""
+        if not L.bn or L.first or self.split_override == 0:
+            return 0
+        if not (self._fuse_eval_layer(L) or self._conv_impl(L.cout, L.k_taps, 1 if self.fast else 3) in (_lib.IMPL_TC, _lib.IMPL_TC2)):
+            return 0
+        h, w = self.spatial(L, H, W)
+        if self.split_override is not None:
+            return min(int(self.split_override), L.k_taps * ((L.k_cin + 63) // 64))
+        if self._num_sms is None:
+            self._num_sms = torch.cuda.get_device_properties(self.device).multi_processor_count
+        s = int(_lib.load().ssp_conv_splitk_count(N, h, w, L.k_taps, L.k_cin, L.cout, self._num_sms))
+        if s < 0:
+            raise _lib.SspError("ssp_conv_splitk_count failed: %s" % _lib.load().ssp_last_error().decode())
+        return s if s >= 2 else 0
 
     def _conv_impl(self, n_out, taps=1, terms=3):
         if self.conv_impl >= 0:
@@ -413,15 +449,26 @@ class Engine:
                    ptr(st["ssum"]), ptr(st["ssq"]), s)
 
     # ------------------------------------------------------------------ forward
-    def forward(self, x, train_bn, keep_for_backward):
-        """x: (N,3,H,W) fp32 CUDA -> logits (N,Cout,h,w) fp32.  train_bn: batch statistics + running-stat update."""
+    def forward(self, x, train_bn, keep_for_backward, split_k=False, buffers=None):
+        """x: (N,3,H,W) fp32 CUDA -> logits (N,Cout,h,w) fp32.  train_bn: batch statistics + running-stat update.
+        split_k (inference only): the layers with a split count (split_count, ssp_conv_splitk_count) run ssp_conv_gemm_splitk +
+        ssp_bn_apply_splitk; their result is deterministic but differs in the last bits from the unsplit forward.
+        buffers: a private Buffers of this input shape (built with split_k=True when split_k is set) instead of the engine's cache."""
         if not x.is_cuda:
             raise _lib.SspError("singleshotpose_b200 runs on CUDA tensors only (no CPU fallback); got a CPU tensor")
+        if split_k and (train_bn or keep_for_backward):
+            raise _lib.SspError("split_k is an inference mode: no batch statistics, no backward")
         x = x.contiguous().float()
         N, C, H, W = x.shape
         self.materialize(x.device)
         self.pack_weights()
-        B = self.buffers(N, H, W, keep_for_backward)
+        if buffers is not None:
+            if (buffers.N, buffers.H, buffers.W) != (N, H, W) or buffers.split_k != bool(split_k) or buffers.dy:
+                raise _lib.SspError("buffers were built for input %s (split_k=%s), not %s (split_k=%s) in inference mode"
+                                    % ((buffers.N, 3, buffers.H, buffers.W), buffers.split_k, (N, C, H, W), bool(split_k)))
+            B = buffers
+        else:
+            B = self.buffers(N, H, W, keep_for_backward, split_k)
         B.generation += 1
         s = stream_ptr()
         mods = self.conv_modules()
@@ -445,8 +492,25 @@ class Engine:
                 bias = None
             else:
                 epi, bias = _lib.EPI_BIAS, ptr(conv.bias.data)
-            fuse = (L.bn and not train_bn and not keep_for_backward and self.fuse_eval and not L.first
-                    and self.conv_impl != _lib.IMPL_SIMT and len(L.dests) == 1 and L.dests[0][2] == _lib.ROUTE_DIRECT and L.cout % 32 == 0)
+            S = B.splits[i]
+            if S:
+                # split-K inference: S partial GEMMs over slices of K into the workspace, then BN(running stats) + leaky + routing
+                # from their sum, in a fixed order (csrc/conv_tc.cu SPLIT, csrc/elementwise.cu bn_apply_kernel SPLIT)
+                call("ssp_bn_finalize", None, None, 1.0, ptr(bn.weight.data), ptr(bn.bias.data), ptr(bn.running_mean), ptr(bn.running_var),
+                     0.1, float(bn.eps), 0, ptr(st["mean"]), ptr(st["invstd"]), ptr(st["scale"]), ptr(st["shift"]), L.cout, s)
+                ws, slab, ld = ptr(B.split_ws), B.split_slab[i], B.split_ld[i]
+                self._gemm("fwd", L, N, h, w, "ssp_conv_gemm_splitk", ptr(xin), a_lo, B.rows[i], xin.shape[1], L.k_cin, ptr(self.w_hi[i]), b_lo,
+                           L.cout, self.w_hi[i].shape[1], N, h, w, L.k_taps, L.cout, S, ws, slab, ld, s)
+                d = []
+                for (ci, c0, kind) in L.dests:
+                    d += [ptr(B.x_hi[ci]), ptr(B.x_lo[ci]), B.x_hi[ci].shape[1], c0, kind]
+                if len(L.dests) == 1:
+                    d += [None, None, 0, 0, _lib.ROUTE_NONE]
+                call("ssp_bn_apply_splitk", ws, S, slab, ld, ptr(st["scale"]), ptr(st["shift"]), N, L.cout, h, w, L.slope, *d, s)
+                self.launches += 2
+                self.split_launches += 1
+                continue
+            fuse = not train_bn and not keep_for_backward and self._fuse_eval_layer(L)
             if fuse:
                 # inference: BN(running stats) + LeakyReLU folded into the GEMM epilogue, which writes the consumer's operand
                 # planes directly -- no fp32 Y, no bn_apply pass (reference: conv, bn, leaky as three modules, darknet.py:154-164)

@@ -162,6 +162,48 @@ def image2torch(img):
     return a.permute(2, 0, 1).contiguous().view(1, 3, img.height, img.width).float().div(255.0)
 
 
+def read_ply_vertices(path):
+    """(Nv, 3) float64 x, y, z of the `vertex` element of an ASCII PLY file (the format of the LINEMOD meshes the .data file's
+    `mesh` entry names).  Written from the PLY format: a header of `element <name> <count>` lines, each followed by its
+    `property <type> <name>` / `property list <count type> <item type> <name>` lines, closed by `end_header`; then one text line
+    per element item, the elements in header order.  Binary PLY is refused."""
+    with open(path, "rb") as f:
+        if f.readline().strip() != b"ply":
+            raise ValueError("%s: not a PLY file" % path)
+        elements, fmt = [], None           # [name, count, [property names]]
+        while True:
+            line = f.readline()
+            if not line:
+                raise ValueError("%s: PLY header without end_header" % path)
+            tok = line.decode("ascii", "replace").split()
+            if not tok or tok[0] in ("comment", "obj_info"):
+                continue
+            if tok[0] == "end_header":
+                break
+            if tok[0] == "format":
+                fmt = tok[1] if len(tok) > 1 else None
+            elif tok[0] == "element":
+                elements.append([tok[1], int(tok[2]), []])
+            elif tok[0] == "property" and elements:
+                elements[-1][2].append(tok[-1])
+        if fmt != "ascii":
+            raise ValueError("%s: PLY format %r is not supported (ASCII PLY only)" % (path, fmt))
+        for name, count, props in elements:
+            if name != "vertex":
+                for _ in range(count):     # one text line per item, whatever its properties
+                    f.readline()
+                continue
+            try:
+                cols = [props.index(a) for a in ("x", "y", "z")]
+            except ValueError:
+                raise ValueError("%s: the vertex element has no x, y, z properties" % path)
+            rows = [f.readline().split() for _ in range(count)]
+            if any(len(r) < len(props) for r in rows):
+                raise ValueError("%s: truncated vertex data" % path)
+            return np.array([[float(r[c]) for c in cols] for r in rows], dtype=np.float64).reshape(count, 3)
+    raise ValueError("%s: no vertex element" % path)
+
+
 def read_data_cfg(datacfg):
     """utils.py:343-358: `key = value` lines of a .data file; 'gpus' and 'num_workers' default to '0' and '10'"""
     options = {'gpus': '0', 'num_workers': '10'}

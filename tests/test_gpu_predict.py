@@ -1,0 +1,376 @@
+"""GPU checks of the pose predictor (singleshotpose_b200/predict.py) and the split-K inference convolution behind it."""
+import copy
+import os
+
+import numpy as np
+import pytest
+import torch
+import torch.nn.functional as F
+
+from oracle.darknet_ref import RefDarknet
+from oracle.pnp_ref import pnp_ref
+from singleshotpose_b200 import Darknet, FlatSGD, RegionLoss, _lib, synth, utils
+from singleshotpose_b200._lib import SspError, call, ptr, stream_ptr
+from singleshotpose_b200.engine import Buffers
+from singleshotpose_b200.image import load_validation_batch
+from singleshotpose_b200.predict import PosePredictor, main
+
+pytestmark = pytest.mark.gpu
+DEV = "cuda"
+CORNERS = synth.box_points(with_center=False).T.astype(np.float64)          # (3, 8) in get_3D_corners order
+K = synth.intrinsics()
+
+
+def _rel(a, b):
+    return float((a - b).abs().max() / b.abs().max())
+
+
+def _frames(n, seed, w=640, h=480):
+    return np.random.default_rng(seed).integers(0, 256, size=(n, h, w, 3), dtype=np.uint8)
+
+
+def _populate_eval(model):
+    bns = [m for m in model.modules() if isinstance(m, torch.nn.BatchNorm2d)]
+    for bn in bns:
+        bn.reset_running_stats(); bn.momentum = None
+    model.train()
+    with torch.no_grad():
+        for s in (0, 10, 11):
+            model(synth.images(2, seed=s))
+    for bn in bns:
+        bn.momentum = 0.1
+
+
+@pytest.fixture(scope="module")
+def pair(cfg_path):
+    """oracle network with populated running statistics, and the GPU model with the same state"""
+    torch.manual_seed(0)
+    ref = RefDarknet(cfg_path)
+    _populate_eval(ref)
+    ref.eval()
+    dut = Darknet(cfg_path)
+    dut.load_state_dict(ref.state_dict())
+    return ref, dut.cuda().eval()
+
+
+# ---------------------------------------------------------------------------------------------------- split GEMM + reduction
+def _flat(x, ld=None):
+    N, C, H, W = x.shape
+    ld = ld or C
+    rows = _lib.flat_alloc_rows(N, H, W)
+    hi = torch.zeros(rows, ld, dtype=torch.float16, device=DEV)
+    lo = torch.zeros(rows, ld, dtype=torch.float16, device=DEV)
+    call("ssp_pack_nchw", ptr(x.contiguous()), ptr(hi), ptr(lo), N, C, H, W, ld, 0, _lib.FMT_F16, 1.0, stream_ptr())
+    return hi, lo, rows
+
+
+def _pack_w(w):
+    co, ci, kh, kw = w.shape
+    ldf = (kh * kw * ci + 7) // 8 * 8
+    hi = torch.zeros(co, ldf, dtype=torch.float16, device=DEV)
+    lo = torch.zeros(co, ldf, dtype=torch.float16, device=DEV)
+    call("ssp_pack_weights", ptr(w.permute(0, 2, 3, 1).contiguous()), co, kh * kw, ci, ptr(hi), ptr(lo), ldf, None, 0, 0, stream_ptr())
+    return hi, lo
+
+
+# block: (H, W, cin, cout, k, destinations [(route, channels of the destination plane, channel offset)], rule S at B = 1, 416^2)
+LAYERS = {
+    12: (26, 26, 256, 512, 3, [(_lib.ROUTE_POOL, 512, 0)], 4),
+    16: (26, 26, 256, 512, 3, [(_lib.ROUTE_POOL, 512, 0), (_lib.ROUTE_DIRECT, 512, 0)], 4),
+    18: (13, 13, 512, 1024, 3, [(_lib.ROUTE_DIRECT, 1024, 0)], 8),
+    23: (13, 13, 1024, 1024, 3, [(_lib.ROUTE_DIRECT, 1024, 0)], 8),
+    24: (13, 13, 1024, 1024, 3, [(_lib.ROUTE_DIRECT, 1280, 256)], 8),
+    29: (13, 13, 1280, 1024, 3, [(_lib.ROUTE_DIRECT, 1024, 0)], 8),
+}
+
+
+def _split_run(xh, xl, rows, wh, wl, S, H, W, cin, cout, k, dests, scale, shift):
+    ld = cout
+    slab = rows * ld
+    ws = torch.full((S * slab,), float("nan"), device=DEV)
+    call("ssp_conv_gemm_splitk", ptr(xh), ptr(xl), rows, cin, cin, ptr(wh), ptr(wl), cout, wh.shape[1], 1, H, W, k * k, cout, S,
+         ptr(ws), slab, ld, stream_ptr())
+    planes, d = [], []
+    for (route, C, c0) in dests:
+        ho, wo = (H // 2, W // 2) if route == _lib.ROUTE_POOL else (H, W)
+        r = _lib.flat_alloc_rows(1, ho, wo)
+        hi, lo = torch.zeros(r, C, dtype=torch.float16, device=DEV), torch.zeros(r, C, dtype=torch.float16, device=DEV)
+        planes.append((hi, lo, C, c0, ho, wo))
+        d += [ptr(hi), ptr(lo), C, c0, route]
+    if len(dests) == 1:
+        d += [None, None, 0, 0, _lib.ROUTE_NONE]
+    call("ssp_bn_apply_splitk", ptr(ws), S, slab, ld, ptr(scale), ptr(shift), 1, cout, H, W, 0.1, *d, stream_ptr())
+    torch.cuda.synchronize()
+    return planes
+
+
+@pytest.mark.parametrize("smode", ["two", "rule", "per_kblock"])
+@pytest.mark.parametrize("block", sorted(LAYERS))
+def test_splitk_gemm_and_reduction_match_fp64_and_repeat_bitwise(block, smode):
+    H, W, cin, cout, k, dests, rule = LAYERS[block]
+    kblocks = k * k * ((cin + 63) // 64)
+    S = {"two": 2, "rule": rule, "per_kblock": kblocks}[smode]
+    g = torch.Generator().manual_seed(block * 7 + S)
+    x = torch.randn(1, cin, H, W, generator=g)
+    w = torch.randn(cout, cin, k, k, generator=g) / (cin * k * k) ** 0.5
+    scale = torch.rand(cout, generator=g) + 0.5
+    shift = torch.randn(cout, generator=g) * 0.1
+    y = F.conv2d(x.double(), w.double(), None, padding=(k - 1) // 2) * scale.double().view(1, -1, 1, 1) + shift.double().view(1, -1, 1, 1)
+    z = torch.where(y > 0, y, 0.1 * y)
+    xh, xl, rows = _flat(x.to(DEV))
+    wh, wl = _pack_w(w.to(DEV))
+    sc, sh = scale.to(DEV), shift.to(DEV)
+    assert _lib.load().ssp_conv_splitk_count(1, H, W, k * k, cin, cout, 132) == rule
+    first = _split_run(xh, xl, rows, wh, wl, S, H, W, cin, cout, k, dests, sc, sh)
+    second = _split_run(xh, xl, rows, wh, wl, S, H, W, cin, cout, k, dests, sc, sh)
+    tol = 2e-5 + 5e-9 * cin * k * k
+    for (route, _C, _c0), (hi, lo, C, c0, ho, wo), (hi2, lo2, *_r) in zip(dests, first, second):
+        out = torch.empty(1, cout, ho, wo, device=DEV)
+        call("ssp_unpack16_nchw", ptr(hi), ptr(lo), ptr(out), 1, cout, ho, wo, C, c0, _lib.FMT_F16, stream_ptr())
+        torch.cuda.synchronize()
+        want = F.max_pool2d(z, 2, 2) if route == _lib.ROUTE_POOL else z
+        assert float((out.cpu().double() - want).abs().max() / want.abs().max()) < tol, (block, S, route)
+        assert torch.equal(hi, hi2) and torch.equal(lo, lo2)               # bit-identical across launches
+
+
+def test_one_split_through_the_new_entry_points_is_the_unfused_eval_chain(pair):
+    """S = 1 through ssp_conv_gemm_splitk + ssp_bn_apply_splitk: the same accumulation order and the same epilogue arithmetic and
+    routing as ssp_conv_gemm + ssp_bn_apply, so the logits are bit-identical to the unfused eval forward"""
+    _ref, m = pair
+    eng = m._engine
+    x = synth.images(1, seed=3).cuda()
+    try:
+        eng.fuse_eval = False
+        with torch.no_grad():
+            o_u = m(x)
+        eng.split_override = 1
+        B = Buffers(eng, 1, 416, 416, False, split_k=True)
+        assert sum(1 for s in B.splits if s) >= 10
+        n0 = eng.split_launches
+        o_s, _b, _g = eng.forward(x, False, False, split_k=True, buffers=B)
+        assert eng.split_launches - n0 == sum(1 for s in B.splits if s)
+    finally:
+        eng.fuse_eval, eng.split_override = True, None
+    assert torch.equal(o_s, o_u)
+
+
+# ---------------------------------------------------------------------------------------------------- predictor
+@pytest.mark.parametrize("batch", [1, 3])
+@pytest.mark.parametrize("size", [416, 672])
+def test_predictor_logits_match_oracle_and_model(pair, size, batch):
+    ref, m = pair
+    pred = PosePredictor(m, CORNERS, K, shape=(size, size), batch=batch)
+    pred(_frames(batch, seed=size + batch))
+    x = pred.input.clone()
+    logits = pred.logits.clone()
+    with torch.no_grad():
+        o_ref = ref(x.cpu())
+        o_model = m(x)
+    assert _rel(logits.cpu(), o_ref) < 1e-3
+    # split-K adds each split layer's fp32 partial sums in another order; the stack amplifies that rounding (DESIGN.md numerics) to
+    # 1.4e-4 .. 2.1e-4 relative on an H100 at these shapes (B = 1 and 3, 416^2 and 672^2), 5x below the oracle bound
+    assert _rel(logits, o_model) < 5e-4
+
+
+def test_split_launch_counter(pair):
+    _ref, m = pair
+    eng = m._engine
+    n0 = eng.split_launches
+    PosePredictor(m, CORNERS, K, batch=1, graph=False)(_frames(1, seed=1))
+    assert eng.split_launches > n0
+    n1 = eng.split_launches
+    PosePredictor(m, CORNERS, K, batch=64, graph=False)(_frames(64, seed=2))
+    assert eng.split_launches == n1
+
+
+def test_predictor_input_is_load_validation_batch(pair, tmp_path):
+    _ref, m = pair
+    from PIL import Image
+    from singleshotpose_b200.jpeg import GpuJpegDecoder
+    fr = _frames(2, seed=4, w=320, h=240)
+    pred = PosePredictor(m, CORNERS, K, frame_size=(320, 240), batch=2)
+    assert pred.shape == (m.test_width, m.test_height)
+    want = load_validation_batch(list(fr), pred.shape, DEV)
+    pred(fr)
+    assert torch.equal(pred.input, want)
+    pred(torch.from_numpy(fr).cuda())
+    assert torch.equal(pred.input, want)
+    blobs = []
+    for i, a in enumerate(fr):
+        p = str(tmp_path / ("%d.jpg" % i))
+        Image.fromarray(a).save(p, quality=95)
+        blobs.append(open(p, "rb").read())
+    dec = GpuJpegDecoder(DEV)(blobs)
+    pred(blobs)
+    assert torch.equal(pred.input, load_validation_batch(dec, pred.shape, DEV))
+
+
+def _posed_model(cfg_path, seed=0):
+    """a network whose last layer outputs constant logits encoding, at cell (0, 0), the projection of the box under a known pose:
+    every cell decodes to that projection shifted by whole cells, so the keypoints are close to a perspective projection and
+    the PnP is well posed"""
+    torch.manual_seed(seed)
+    m = Darknet(cfg_path)
+    last = m.models[30][0]
+    ang = np.array([0.3, -0.2, 0.1])
+    th = np.linalg.norm(ang); kx = np.array([[0, -ang[2], ang[1]], [ang[2], 0, -ang[0]], [-ang[1], ang[0], 0]]) / th
+    R = np.eye(3) + np.sin(th) * kx + (1 - np.cos(th)) * kx @ kx
+    t = np.array([-0.315, -0.235, 0.6])
+    P = np.concatenate([np.zeros((3, 1)), CORNERS], 1)
+    cam = K @ (R @ P + t[:, None])
+    uv = cam[:2] / cam[2]                                   # (2, 9) pixels of a 640 x 480 frame
+    gx, gy = uv[0] / 640 * 13, uv[1] / 480 * 13             # in grid units of a 13 x 13 output
+    b = np.zeros(20)
+    assert 0 < gx[0] < 1 and 0 < gy[0] < 1
+    b[0], b[1] = np.log(gx[0] / (1 - gx[0])), np.log(gy[0] / (1 - gy[0]))
+    b[2:18:2], b[3:18:2] = gx[1:], gy[1:]
+    b[18] = 2.0
+    with torch.no_grad():
+        last.weight.zero_()
+        last.bias.copy_(torch.from_numpy(b).float())
+    return m.cuda().eval()
+
+
+def test_predictor_head_matches_batched_calls_and_oracle_pnp(cfg_path):
+    m = _posed_model(cfg_path)
+    pred = PosePredictor(m, CORNERS, K, shape=(416, 416), batch=2)          # a 13 x 13 output, the grid the logits encode
+    r = {k: v.clone() for k, v in pred(_frames(2, seed=5)).items()}
+    boxes, best, _g = utils.region_boxes_batched(pred.logits, 1, 9)
+    assert torch.equal(pred._last.boxes, boxes) and torch.equal(r["conf"], best)
+    kp = boxes[:, :18].reshape(2, 9, 2) * torch.tensor([640.0, 480.0], device=DEV)
+    assert torch.equal(r["keypoints_px"], kp)
+    P3 = np.concatenate([np.zeros((1, 3)), CORNERS.T]).astype(np.float32)
+    R, t = utils.pnp_batched(P3, kp, K.astype(np.float32))
+    assert torch.equal(r["R"], R) and torch.equal(r["t"], t)
+    for i in range(2):
+        Ro, to = pnp_ref(P3, kp[i].cpu().numpy(), K.astype(np.float32))
+        ang = np.degrees(np.arccos(np.clip((np.trace(r["R"][i].cpu().numpy() @ Ro.T) - 1) / 2, -1, 1)))
+        assert ang < 1e-2 and np.abs(r["t"][i].cpu().numpy() - to.reshape(3)).max() * 1e3 < 1e-2
+    Rt = torch.cat([R, t.unsqueeze(2)], 2)
+    X = np.concatenate([np.concatenate([np.zeros((3, 1)), CORNERS], 1), np.ones((1, 9))]).astype(np.float32)
+    proj = utils.project_points_batched(X, Rt, K)
+    assert torch.equal(r["corners_px"], proj.transpose(1, 2))
+    host = pred(_frames(2, seed=5), to_host=True)
+    assert isinstance(host["R"], np.ndarray) and np.array_equal(host["R"], r["R"].cpu().numpy())
+
+
+def _clone(r):
+    return {k: v.clone() for k, v in r.items()}
+
+
+def _equal(a, b):
+    return all(torch.equal(a[k], b[k]) for k in a)
+
+
+def test_graph_replay_equals_eager_and_repeats(pair):
+    _ref, m = pair
+    fr = _frames(1, seed=6)
+    g = PosePredictor(m, CORNERS, K)
+    e = PosePredictor(m, CORNERS, K, graph=False)
+    r_e = _clone(e(fr))
+    r1 = _clone(g(fr))                      # capture + replay
+    r2 = _clone(g(fr))                      # replay
+    assert g._last.graph is not None
+    assert _equal(r1, r_e) and _equal(r1, r2)
+    assert torch.equal(g(torch.from_numpy(fr).cuda())["R"], r_e["R"])      # the device-frame graph too
+
+
+def test_replay_follows_load_weights_and_sgd_step(cfg_path, tmp_path):
+    torch.manual_seed(1)
+    m = Darknet(cfg_path).cuda().eval()
+    fr = _frames(1, seed=7)
+    pred = PosePredictor(m, CORNERS, K)
+    pred(fr)
+    l0 = pred.logits.clone()
+    torch.manual_seed(2)
+    other = Darknet(cfg_path)
+    wf = str(tmp_path / "other.weights")
+    other.save_weights(wf)
+    m.load_weights(wf)
+    r1 = _clone(pred(fr))
+    l1 = pred.logits.clone()
+    assert not torch.equal(l0, l1)                          # the replay read the new weights
+    fresh = PosePredictor(m, CORNERS, K)
+    assert _equal(r1, fresh(fr)) and torch.equal(l1, fresh.logits)
+    m.train()
+    opt = FlatSGD(m, lr=1e-3, momentum=0.9, weight_decay=5e-4)
+    crit = RegionLoss(); crit.verbose = False
+    loss = crit(m(synth.images(2, seed=1).cuda()), synth.targets(2, seed=1), 20)
+    opt.zero_grad(); loss.backward(); opt.step()
+    m.eval()
+    r2 = _clone(pred(fr))
+    l2 = pred.logits.clone()
+    assert not torch.equal(l1, l2)
+    fresh = PosePredictor(m, CORNERS, K)
+    assert _equal(r2, fresh(fr)) and torch.equal(l2, fresh.logits)
+
+
+def test_model_call_and_training_step_between_replays_change_nothing(cfg_path):
+    torch.manual_seed(3)
+    m = Darknet(cfg_path).cuda().eval()
+    fr = _frames(1, seed=8)
+    pred = PosePredictor(m, CORNERS, K)
+    r1 = _clone(pred(fr))
+    l1 = pred.logits.clone()
+    state = copy.deepcopy(m.state_dict())
+    with torch.no_grad():
+        m(synth.images(1, seed=9).cuda())                     # an eval forward of the same shape
+    for bn in (x for x in m.modules() if isinstance(x, torch.nn.BatchNorm2d)):
+        bn.momentum = 0.0                                    # the running statistics stay as they are
+    m.train()
+    opt = FlatSGD(m, lr=0.0, momentum=0.0, weight_decay=0.0)
+    crit = RegionLoss(); crit.verbose = False
+    loss = crit(m(synth.images(1, seed=10).cuda()), synth.targets(1, seed=2), 20)
+    opt.zero_grad(); loss.backward(); opt.step()
+    m.eval()
+    assert all(torch.equal(a, b) for a, b in zip(state.values(), m.state_dict().values()))
+    r2 = pred(fr)
+    assert _equal(r1, r2) and torch.equal(l1, pred.logits)
+
+
+def test_bad_inputs_raise_before_any_launch(pair):
+    _ref, m = pair
+    pred = PosePredictor(m, CORNERS, K, batch=2)
+    eng = m._engine
+    good = _frames(2, seed=11)
+    bad = [good.astype(np.float32), good[0], good[..., :2], good[:1], torch.from_numpy(good), [b"\xff\xd8junk", b"abc"],
+           [b"abc"], "frames", good[:, :0]]
+    n0 = eng.launches
+    for b in bad:
+        with pytest.raises(SspError):
+            pred(b)
+    assert eng.launches == n0 and pred._last is None
+    with pytest.raises(SspError):
+        PosePredictor(m, CORNERS[:, :7], K)
+
+
+def test_cli_writes_what_the_api_returns(cfg_path, tmp_path):
+    from PIL import Image
+    listfile, _bgs = synth.write_linemod_like(str(tmp_path), n=3, fmt="jpg")
+    paths = open(listfile).read().split()
+    V = np.random.default_rng(0).normal(size=(40, 3)) * 0.03
+    ply = str(tmp_path / "obj.ply")
+    with open(ply, "w") as f:
+        f.write("ply\nformat ascii 1.0\nelement vertex %d\nproperty float x\nproperty float y\nproperty float z\nend_header\n" % len(V))
+        for v in V:
+            f.write("%.17g %.17g %.17g\n" % tuple(v))
+    data = tmp_path / "obj.data"
+    data.write_text("mesh = %s\nwidth = 640\nheight = 480\nfx = 572.4114\nfy = 573.5704\nu0 = 325.2611\nv0 = 242.0489\n" % ply)
+    torch.manual_seed(4)
+    wf = str(tmp_path / "m.weights")
+    Darknet(cfg_path).save_weights(wf)
+    out = str(tmp_path / "poses.npz")
+    main(["--datacfg", str(data), "--modelcfg", cfg_path, "--weightfile", wf, "--out", out] + paths)
+    got = np.load(out)
+    m = Darknet(cfg_path)
+    m.load_weights(wf)
+    m.cuda().eval()
+    corners = utils.get_3D_corners(np.c_[V, np.ones((len(V), 1))].T)
+    Km = np.array([[572.4114, 0, 325.2611], [0, 573.5704, 242.0489], [0, 0, 1]])
+    pred = PosePredictor(m, corners, Km)
+    for i, p in enumerate(paths):
+        assert Image.open(p).format == "JPEG"
+        r = pred([open(p, "rb").read()], to_host=True)
+        for k in ("R", "t", "conf", "keypoints_px", "corners_px"):
+            assert np.array_equal(got[k][i], r[k][0]), (p, k)
+    assert list(got["paths"]) == paths
