@@ -198,6 +198,16 @@ int ssp_region_decode_multi(const float* out_nchw, int B, int num_keypoints, int
 int ssp_eval_multi_select(const float* out_nchw, int B, int num_keypoints, int num_classes, int num_anchors, int H, int W,
                           const float* target, int target_stride, const int* gt_offset, float conf_thresh, float im_width,
                           float im_height, float* boxes, int* flags, float* uv, void* stream);
+/* ---- multi-object prediction (no labels): per image b and requested class classes_host[q], the box ssp_eval_multi_select would
+ *      choose for a one-row target of that class -- the listed box of class c with the largest det_conf (first in visiting order),
+ *      else the fallback box of get_multi_region_boxes(..., correspondingclass = c) -- each image as its own batch-1 call.
+ *      classes_host: n_req distinct class ids in [0, num_classes), a HOST array copied into the launch.  Out: boxes
+ *      [B][n_req][2K+3]; flags [B][n_req], bit 0 = fallback box (the class was not listed); uv [B][n_req][K][2] = the box
+ *      keypoints times (frame_w, frame_h) in fp32, the points of ssp_pnp_batched.  SSP_ERR_ARG for a null pointer,
+ *      num_keypoints != 9, H*W*num_anchors > 4096, num_classes > 256, n_req < 1, or a class out of range or listed twice. ---- */
+int ssp_predict_multi_select(const float* out_nchw, int B, int num_keypoints, int num_classes, int num_anchors, int H, int W,
+                             const int* classes_host, int n_req, float conf_thresh, float frame_w, float frame_h, float* boxes,
+                             int* flags, float* uv, void* stream);
 
 /* ---- pnp (utils.py:86-100 -> cv2.solvePnP ITERATIVE + Rodrigues), compute_projection (utils.py:40-45) ---- */
 int ssp_pnp_batched(const float* points3d, int points3d_shared, const float* points2d, const float* K3x3,

@@ -54,6 +54,7 @@ SIGNATURES = {
     "ssp_region_loss_multi_fwd_bwd": [_p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _p, _i, _f, _f, _f, _f, _f, _i, _f, _p],
     "ssp_region_decode_multi": [_p, _i, _i, _i, _i, _i, _i, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p],
     "ssp_eval_multi_select": [_p, _i, _i, _i, _i, _i, _i, _p, _i, _p, _f, _f, _f, _p, _p, _p, _p],
+    "ssp_predict_multi_select": [_p, _i, _i, _i, _i, _i, _i, _p, _i, _f, _f, _f, _p, _p, _p, _p],
     "ssp_pnp_batched": [_p, _i, _p, _p, _i, _ll, _i, _p, _p, _p, _p],
     "ssp_pnp_batched_work": [_p, _i, _p, _p, _i, _ll, _i, _p, _p, _p, _p],
     "ssp_project_points": [_p, _i, _i, _p, _p, _ll, _p, _p],

@@ -55,6 +55,7 @@ int region_loss_multi_fwd_bwd(const float*, const float*, float*, double*, int, 
 int region_decode_multi(const float*, int, int, int, int, int, int, int, int, float*, float*, float*, float*, long long*, float*, float*, cudaStream_t);
 int eval_multi_select(const float*, int, int, int, int, int, int, const float*, int, const int*, float, float, float, float*, int*, float*,
                       cudaStream_t);
+int predict_multi_select(const float*, int, int, int, int, int, int, const int*, int, float, float, float, float*, int*, float*, cudaStream_t);
 int pnp_batched(const float*, int, const float*, const float*, int, long long, int, double*, double*, int*, int*, cudaStream_t);
 int project_points(const float*, int, int, const double*, const double*, long long, float*, cudaStream_t);
 long long adds_work_bytes(int, long long);
@@ -222,6 +223,10 @@ int ssp_eval_multi_select(const float* out, int B, int K, int nC, int nA, int H,
                           const int* gt_offset, float conf_thresh, float im_width, float im_height, float* boxes, int* flags, float* uv,
                           void* s) {
   return eval_multi_select(out, B, K, nC, nA, H, W, target, target_stride, gt_offset, conf_thresh, im_width, im_height, boxes, flags, uv, ST(s));
+}
+int ssp_predict_multi_select(const float* out, int B, int K, int nC, int nA, int H, int W, const int* classes_host, int n_req, float conf_thresh,
+                             float frame_w, float frame_h, float* boxes, int* flags, float* uv, void* s) {
+  return predict_multi_select(out, B, K, nC, nA, H, W, classes_host, n_req, conf_thresh, frame_w, frame_h, boxes, flags, uv, ST(s));
 }
 int ssp_pnp_batched(const float* P3, int shared, const float* uv, const float* K, int np, long long n, int max_iter, double* R, double* t, int* iters, void* s) {
   return pnp_batched(P3, shared, uv, K, np, n, max_iter, R, t, iters, nullptr, ST(s));

@@ -11,6 +11,8 @@
 //     the boxes of class c -- the largest (det bits, ~list index) key, which orders like (det, -index) because det >= 0;
 //     when no box has class c it keeps the box of the previous ground truth of the image;
 //   * the PnP inputs are the box keypoints times (im_width, im_height) in fp32; the ground truth goes through fix_corner_order.
+// The predictor (predict_multi_select_kernel, tests/helpers/predict_multi_host.cpp) applies the same rules without labels: one
+// slot per (image, requested class), chosen as for a first ground truth of that class (predict_slot, fallback_scan).
 #pragma once
 #include <math.h>
 #include <stdint.h>
@@ -40,10 +42,14 @@ struct Decoded {
   float cmax;   // max softmax
   float corr;   // softmax at correspondingclass (0 when it is out of range)
   int id;       // arg-max class (first maximum)
+  float mx, den;  // the softmax's largest class logit and denominator (class_prob)
 };
 
+// softmax[c] of one (cell, anchor) from its decode's mx and den: the arithmetic of Decoded::corr
+SSP_EVM_HD float class_prob(const float* o, int HW, int K, int c, float mx, float den) { return expf(o[(2 * K + 1 + c) * HW] - mx) / den; }
+
 // one (cell, anchor): o points at channel 0 of that anchor at the cell, channels HW apart.  kp (2K floats, or null) receives
-// [x0/W, y0/H, ..., x_{K-1}/W, y_{K-1}/H].  The arithmetic of the reference's decode, in this order, for both kernels.
+// [x0/W, y0/H, ..., x_{K-1}/W, y_{K-1}/H].  The arithmetic of the reference's decode, in this order, for every kernel.
 SSP_EVM_HD Decoded decode_entry(const float* o, int HW, int K, int nC, int cx, int cy, int W, int H, int corr, float* kp) {
   if (kp)
     for (int k = 0; k < K; k++) {
@@ -59,7 +65,8 @@ SSP_EVM_HD Decoded decode_entry(const float* o, int HW, int K, int nC, int cx, i
   for (int c = 0; c < nC; c++) den += expf(o[(2 * K + 1 + c) * HW] - mx);
   d.cmax = 1.f / den;
   d.id = id;
-  d.corr = (corr >= 0 && corr < nC) ? expf(o[(2 * K + 1 + corr) * HW] - mx) / den : 0.f;
+  d.corr = (corr >= 0 && corr < nC) ? class_prob(o, HW, K, corr, mx, den) : 0.f;
+  d.mx = mx; d.den = den;
   return d;
 }
 
@@ -120,12 +127,37 @@ SSP_EVM_HD void write_box(const float* out_img, int src, const Fallback& fb, int
 }
 
 // PnP inputs (valid_multi.py:126-132): label row [cls, x0, y0, ...] -> fix_corner_order'ed pixels; box -> pixels, in fp32
+SSP_EVM_HD void box_uv(const float* box, float im_width, float im_height, int k, float* uv_pr) {
+  uv_pr[2 * k] = box[2 * k] * im_width; uv_pr[2 * k + 1] = box[2 * k + 1] * im_height;
+}
 SSP_EVM_HD void write_uv(const float* label_row, const float* box, float im_width, float im_height, float* uv_gt, float* uv_pr) {
   for (int k = 0; k < kKeypoints; k++) {
     const int s = fix_order(k);
     uv_gt[2 * k] = label_row[1 + 2 * s] * im_width; uv_gt[2 * k + 1] = label_row[2 + 2 * s] * im_height;
-    uv_pr[2 * k] = box[2 * k] * im_width; uv_pr[2 * k + 1] = box[2 * k + 1] * im_height;
+    box_uv(box, im_width, im_height, k, uv_pr);
   }
+}
+
+// ---- prediction (no labels): slot (frame, requested class c) takes the box valid_multi.py would choose for a ground truth of
+// class c that is the image's first, i.e. select_box with correspondingclass = cls = c:
+//   * the listed box best[c] when some listed box has arg-max class c (flags 0);
+//   * otherwise the fallback box for correspondingclass = c (kFlagFallback), from fallback_scan.
+SSP_EVM_HD int predict_slot(const unsigned long long* best, int nC, int c, int* flags) {
+  return select_box(best, nC, c, c >= 0 && c < nC && best[c] != 0ull, c, kSrcFallback, 0, flags);
+}
+
+// the fallback's running maxima for correspondingclass = c over an image's n entries, given each entry's det and its softmax's mx
+// and den (Decoded).  softmax[c] is recomputed by class_prob only where the && of fallback_update reads it (det > max_conf), which
+// gives the maxima of fallback_update over decode_entry(..., corr = c, ...) bit for bit.
+SSP_EVM_HD Fallback fallback_scan(const float* out_img, const float* det, const float* mx, const float* den, int n, int c, int nA, int K,
+                                  int nC, int W, int HW) {
+  Fallback fb = fallback_init();
+  for (int i = 0; i < n; i++)
+    if (det[i] > fb.max_conf) {
+      int cx, cy;
+      fallback_update(fb, det[i], class_prob(entry_ptr(out_img, i, nA, K, nC, W, HW, &cx, &cy), HW, K, c, mx[i], den[i]), i);
+    }
+  return fb;
 }
 
 // valid_multi.py:20-23: label rows up to the first with x0 == 0 (all of them when every row is filled)

@@ -248,6 +248,85 @@ __global__ void __launch_bounds__(256) eval_multi_select_kernel(const float* __r
   }
 }
 
+// ------------------------------------------------------------------------------------------------ prediction selection
+// Slot (image, requested class c) = the box valid_multi.py would choose for a first ground truth of class c (eval_multi_core.h
+// predict_slot): every image as its own batch-1 call.  One CTA per image for all requested classes: every (cell, anchor) is
+// decoded once (det, and the softmax's mx and den kept in dynamic shared memory) and feeds the per-class best listed box (the
+// shared atomicMax over pick_key of eval_multi_select_kernel); then one thread per requested class runs, only when its class
+// has no listed box, the fallback's sequential scan over shared memory (softmax[c] recomputed where the scan reads it) and
+// writes its slot's box, flag and PnP points.
+struct PredictMultiParams {
+  const float* out; float* boxes; int* flags; float* uv;
+  int K, nC, nA, H, W, n_req;
+  float thr, frame_w, frame_h;
+  int classes[ssp_evm::kMaxClasses];
+};
+
+__global__ void __launch_bounds__(256) predict_multi_select_kernel(const PredictMultiParams p) {
+  using namespace ssp_evm;
+  extern __shared__ float s_ent[];                          // [3][n]: det, mx, den
+  __shared__ unsigned long long s_best[kMaxClasses];
+  const int b = blockIdx.x, K = p.K, nC = p.nC, nA = p.nA, W = p.W, H = p.H, HW = H * W, n = HW * nA, nl = 2 * K + 3;
+  float* s_det = s_ent; float* s_mx = s_ent + n; float* s_den = s_ent + 2 * n;
+  const float* o = p.out + (long long)b * nA * (2 * K + 1 + nC) * HW;
+  for (int c = threadIdx.x; c < nC; c += blockDim.x) s_best[c] = 0ull;
+  __syncthreads();
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    int cx, cy;
+    const float* oi = entry_ptr(o, i, nA, K, nC, W, HW, &cx, &cy);
+    const Decoded d = decode_entry(oi, HW, K, nC, cx, cy, W, H, -1, nullptr);
+    s_det[i] = d.det; s_mx[i] = d.mx; s_den[i] = d.den;
+    if (listed(d, p.thr)) atomicMax(&s_best[d.id], pick_key(d.det, i));
+  }
+  __syncthreads();
+  for (int q = threadIdx.x; q < p.n_req; q += blockDim.x) {
+    const int c = p.classes[q];
+    int fl;
+    const int src = predict_slot(s_best, nC, c, &fl);
+    const Fallback fb = src == kSrcFallback ? fallback_scan(o, s_det, s_mx, s_den, n, c, nA, K, nC, W, HW) : fallback_init();
+    const long long slot = (long long)b * p.n_req + q;
+    float box[2 * kKeypoints + 3];
+    write_box(o, src, fb, c, nA, K, nC, W, H, box);
+    for (int j = 0; j < nl; j++) p.boxes[slot * nl + j] = box[j];
+    p.flags[slot] = fl;
+    for (int k = 0; k < kKeypoints; k++) box_uv(box, p.frame_w, p.frame_h, k, p.uv + slot * 2 * kKeypoints);
+  }
+}
+
+int predict_multi_select(const float* out, int B, int K, int nC, int nA, int H, int W, const int* classes_host, int n_req, float conf_thresh,
+                         float frame_w, float frame_h, float* boxes, int* flags, float* uv, cudaStream_t s) {
+  if (!out || !classes_host || !boxes || !flags || !uv) return fail_msg(SSP_ERR_ARG, "predict_multi_select: null pointer");
+  if (K != ssp_evm::kKeypoints)
+    return fail_msg(SSP_ERR_ARG, "predict_multi_select: num_keypoints must be 9 (the PnP points are the 9 keypoints of a box)");
+  if (B < 0 || nC < 1 || nA < 1 || H < 1 || W < 1) return fail_msg(SSP_ERR_ARG, "predict_multi_select: bad argument");
+  if ((long long)H * W * nA > ssp_evm::kMaxEntries)
+    return fail_msg(SSP_ERR_ARG, "predict_multi_select: grid too large (H*W*num_anchors must be at most 4096, e.g. 26x26x5)");
+  if (nC > ssp_evm::kMaxClasses) return fail_msg(SSP_ERR_ARG, "predict_multi_select: at most 256 classes");
+  if (n_req < 1 || n_req > nC) return fail_msg(SSP_ERR_ARG, "predict_multi_select: n_req must be in [1, num_classes]");
+  PredictMultiParams p;
+  bool seen[ssp_evm::kMaxClasses] = {};
+  for (int q = 0; q < n_req; q++) {
+    const int c = classes_host[q];
+    if (c < 0 || c >= nC) return fail_msg(SSP_ERR_ARG, "predict_multi_select: requested class out of [0, num_classes)");
+    if (seen[c]) return fail_msg(SSP_ERR_ARG, "predict_multi_select: requested class listed twice");
+    seen[c] = true; p.classes[q] = c;
+  }
+  if (B == 0) return SSP_OK;
+  static int configured = 0;
+  const int smem = 3 * H * W * nA * (int)sizeof(float);
+  if (!configured) {
+    const cudaError_t e = cudaFuncSetAttribute(predict_multi_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               3 * ssp_evm::kMaxEntries * (int)sizeof(float));
+    if (e != cudaSuccess) return fail_cuda(e, __FILE__, __LINE__);
+    configured = 1;
+  }
+  p.out = out; p.boxes = boxes; p.flags = flags; p.uv = uv;
+  p.K = K; p.nC = nC; p.nA = nA; p.H = H; p.W = W; p.n_req = n_req;
+  p.thr = conf_thresh; p.frame_w = frame_w; p.frame_h = frame_h;
+  predict_multi_select_kernel<<<B, 256, smem, s>>>(p);
+  SSP_CHECK_LAUNCH(); return SSP_OK;
+}
+
 int eval_multi_select(const float* out, int B, int K, int nC, int nA, int H, int W, const float* target, int target_stride,
                       const int* gt_offset, float conf_thresh, float im_width, float im_height, float* boxes, int* flags, float* uv,
                       cudaStream_t s) {

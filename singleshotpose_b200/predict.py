@@ -20,7 +20,8 @@ load_weights / optimiser updates (the planes are re-packed before the replay whe
 re-captured if the parameters were moved to new memory.  The predictor owns its activation buffers, so model(x) or a training
 step between two replays cannot write into memory the graph replays.
 
-Returned device tensors are the predictor's static outputs: the next call overwrites them.
+Returned device tensors are the predictor's static outputs: the next call overwrites them.  Everything but the head lives in
+_FramePredictor, which predict_multi.MultiPosePredictor shares.
 
 Command line: python -m singleshotpose_b200.predict --datacfg cfg/ape.data --modelcfg cfg/yolo-pose.cfg --weightfile w.weights
               --out poses.npz img1.jpg img2.jpg ...
@@ -39,10 +40,10 @@ from .image import BICUBIC
 
 
 class _Chain:
-    """static buffers (and the graph) of one (frame size, frame source)"""
+    """static buffers (and the graph) of one (frame size, frame source); the head's buffers come from pred._head_buffers"""
 
     def __init__(self, pred, Wf, Hf, src):
-        dev, B, K = pred.device, pred.batch, pred.num_keypoints
+        dev, B = pred.device, pred.batch
         W, H = pred.shape
         self.frame, self.src, self.graph = (Wf, Hf), src, None
         self.u8 = torch.zeros(B, Hf, Wf, 3, dtype=torch.uint8, device=dev)
@@ -55,31 +56,25 @@ class _Chain:
             raise SspError("frame size %dx%d cannot be resized to %dx%d" % (Wf, Hf, W, H))
         self.work = torch.empty(nb + 16, dtype=torch.uint8, device=dev)
         self.scale = torch.tensor([Wf, Hf], dtype=torch.float32, device=dev)
-        self.boxes = torch.empty(B, 2 * K + 3, dtype=torch.float32, device=dev)
-        self.conf = torch.empty(B, dtype=torch.float32, device=dev)
-        self.kp = torch.empty(B, K, 2, dtype=torch.float32, device=dev)
-        self.R = torch.empty(B, 3, 3, dtype=torch.float64, device=dev)
-        self.t = torch.empty(B, 3, dtype=torch.float64, device=dev)
-        self.Rt = torch.empty(B, 3, 4, dtype=torch.float64, device=dev)
-        self.proj = torch.empty(B, 2, K, dtype=torch.float32, device=dev)
-        self.corners = torch.empty(B, K, 2, dtype=torch.float32, device=dev)
         self.logits = None
+        pred._head_buffers(self)
 
 
-class PosePredictor:
-    """model: a singleshotpose_b200.Darknet (single-object yolo-pose head, 9 keypoints).  corners3D: (3|4, 8) box corners of the
-    mesh (utils.get_3D_corners); K: (3, 3) camera matrix; frame_size: (width, height) of the camera frames (other sizes are
-    accepted and captured separately); shape: network input (width, height), default the cfg's test size; batch: frames per call.
-    graph=False runs the same launches eagerly (no capture)."""
+class _FramePredictor:
+    """What every pose predictor shares: input checks and the pinned staging buffer; JPEG, host and device frame sources; resize
+    and ToTensor; the split-K eval forward on private Buffers; the per-(frame size, source) LRU of captured graphs; the re-pack
+    and re-capture after the weights change.  A subclass supplies the head: _head_buffers(chain) allocates its static buffers,
+    _head(chain, stream) launches it after the forward and _outputs(chain) names the returned tensors."""
 
-    def __init__(self, model, corners3D, K, frame_size=(640, 480), shape=None, batch=1, graph=True, max_graphs=4):
+    def __init__(self, model, K, frame_size, shape, batch, graph, max_graphs):
+        name = type(self).__name__
         if not torch.cuda.is_available():
-            raise SspError("PosePredictor needs a CUDA device (no CPU fallback)")
+            raise SspError("%s needs a CUDA device (no CPU fallback)" % name)
         self.model, self.eng = model, model._engine
         self.num_keypoints, self.num_classes = int(model.num_keypoints), int(model.num_classes)
         if self.num_keypoints != 9:
-            raise SspError("PosePredictor solves PnP on the centroid + 8 box corners: the model must have 9 keypoints, not %d" % self.num_keypoints)
-        self.shape = (int(shape[0]), int(shape[1])) if shape is not None else (int(model.test_width), int(model.test_height))
+            raise SspError("%s solves PnP on the centroid + 8 box corners: the model must have 9 keypoints, not %d" % (name, self.num_keypoints))
+        self.shape = (int(shape[0]), int(shape[1]))
         self.batch = int(batch)
         if self.batch < 1:
             raise SspError("batch must be >= 1")
@@ -88,26 +83,26 @@ class PosePredictor:
         dev = self.eng.device if self.eng.device is not None else torch.device("cuda", torch.cuda.current_device())
         self.device = dev
         self.eng.materialize(dev)
-        c = np.asarray(corners3D, dtype=np.float64)
-        if c.ndim != 2 or c.shape[0] not in (3, 4) or c.shape[1] != 8:
-            raise SspError("corners3D must be (3|4, 8), got %s" % (c.shape,))
-        P = np.concatenate([np.zeros((3, 1)), c[:3]], axis=1)                     # valid.py:146: [0; corners3D[:3]] as columns
-        self._P3 = torch.from_numpy(np.ascontiguousarray(P.T, dtype=np.float32)).to(dev)           # (9, 3) PnP points
-        # row-major copies: the kernels read raw pointers, and numpy keeps a transposed input's column-major order through
-        # concatenate / astype
-        self._X = torch.from_numpy(np.ascontiguousarray(np.concatenate([P, np.ones((1, 9))], 0), dtype=np.float32)).to(dev)   # (4, 9)
         Km = np.asarray(K, dtype=np.float64)
         if Km.shape != (3, 3):
             raise SspError("K must be (3, 3), got %s" % (Km.shape,))
         self._K32 = torch.from_numpy(np.ascontiguousarray(Km, dtype=np.float32)).to(dev)       # PnP takes float32 K (valid.py:147)
         self._K64 = torch.from_numpy(np.ascontiguousarray(Km)).to(dev)
         W, H = self.shape
-        self.eng.spatial(self.eng.layers[-1], H, W)                               # raises for a shape off the pooling pyramid
+        self.out_hw = self.eng.spatial(self.eng.layers[-1], H, W)               # raises for a shape off the pooling pyramid
         self._bufs = Buffers(self.eng, self.batch, H, W, False, split_k=True)
         self._chains = collections.OrderedDict()
         self._sig = None
         self._jpeg = None
         self._last = None
+
+    @staticmethod
+    def _box_points(corners3D):
+        """(3|4, 8) box corners -> (3, 9) float64 [0; corners3D[:3]] as columns (valid.py:146, valid_multi.py:135)"""
+        c = np.asarray(corners3D, dtype=np.float64)
+        if c.ndim != 2 or c.shape[0] not in (3, 4) or c.shape[1] != 8:
+            raise SspError("corners3D must be (3|4, 8), got %s" % (c.shape,))
+        return np.concatenate([np.zeros((3, 1)), c[:3]], axis=1)
 
     # ------------------------------------------------------------------ inputs
     def _check(self, frames):
@@ -146,7 +141,7 @@ class PosePredictor:
     def _body(self, c, events=None):
         """every launch of one prediction, in stream order; events (4 CUDA events, eager runs only) bracket image / forward / head"""
         s = stream_ptr()
-        B, K = self.batch, self.num_keypoints
+        B = self.batch
         W, H = self.shape
         Wf, Hf = c.frame
         if events:
@@ -161,14 +156,7 @@ class PosePredictor:
         c.logits, _b, _g = self.eng.forward(c.x, False, False, split_k=True, buffers=self._bufs)
         if events:
             events[2].record()
-        h, w = c.logits.shape[2:]
-        call("ssp_region_decode_argmax", ptr(c.logits), B, K, self.num_classes, h, w, 1, ptr(c.boxes), ptr(c.conf), None, s)
-        torch.mul(c.boxes[:, :2 * K].view(B, K, 2), c.scale, out=c.kp)
-        call("ssp_pnp_batched", ptr(self._P3), 1, ptr(c.kp), ptr(self._K32), K, B, 20, ptr(c.R), ptr(c.t), None, s)
-        c.Rt[:, :, :3].copy_(c.R)
-        c.Rt[:, :, 3].copy_(c.t)
-        call("ssp_project_points", ptr(self._X), 4, K, ptr(c.Rt), ptr(self._K64), B, ptr(c.proj), s)
-        c.corners.copy_(c.proj.transpose(1, 2))
+        self._head(c, s)
         if events:
             events[3].record()
 
@@ -235,7 +223,7 @@ class PosePredictor:
             if kind == "host":
                 c.copied.record()
             self._last = c
-        out = dict(R=c.R, t=c.t, conf=c.conf, keypoints_px=c.kp, corners_px=c.corners)
+        out = self._outputs(c)
         if to_host:
             return {k: v.cpu().numpy() for k, v in out.items()}
         return out
@@ -249,6 +237,48 @@ class PosePredictor:
     def input(self):
         """(B, 3, H, W) float32 network input of the last call (resized + ToTensor)"""
         return None if self._last is None else self._last.x
+
+
+class PosePredictor(_FramePredictor):
+    """model: a singleshotpose_b200.Darknet (single-object yolo-pose head, 9 keypoints).  corners3D: (3|4, 8) box corners of the
+    mesh (utils.get_3D_corners); K: (3, 3) camera matrix; frame_size: (width, height) of the camera frames (other sizes are
+    accepted and captured separately); shape: network input (width, height), default the cfg's test size; batch: frames per call.
+    graph=False runs the same launches eagerly (no capture)."""
+
+    def __init__(self, model, corners3D, K, frame_size=(640, 480), shape=None, batch=1, graph=True, max_graphs=4):
+        P = self._box_points(corners3D)
+        super().__init__(model, K, frame_size, shape if shape is not None else (model.test_width, model.test_height), batch, graph,
+                         max_graphs)
+        dev = self.device
+        self._P3 = torch.from_numpy(np.ascontiguousarray(P.T, dtype=np.float32)).to(dev)           # (9, 3) PnP points
+        # row-major copies: the kernels read raw pointers, and numpy keeps a transposed input's column-major order through
+        # concatenate / astype
+        self._X = torch.from_numpy(np.ascontiguousarray(np.concatenate([P, np.ones((1, 9))], 0), dtype=np.float32)).to(dev)   # (4, 9)
+
+    def _head_buffers(self, c):
+        dev, B, K = self.device, self.batch, self.num_keypoints
+        c.boxes = torch.empty(B, 2 * K + 3, dtype=torch.float32, device=dev)
+        c.conf = torch.empty(B, dtype=torch.float32, device=dev)
+        c.kp = torch.empty(B, K, 2, dtype=torch.float32, device=dev)
+        c.R = torch.empty(B, 3, 3, dtype=torch.float64, device=dev)
+        c.t = torch.empty(B, 3, dtype=torch.float64, device=dev)
+        c.Rt = torch.empty(B, 3, 4, dtype=torch.float64, device=dev)
+        c.proj = torch.empty(B, 2, K, dtype=torch.float32, device=dev)
+        c.corners = torch.empty(B, K, 2, dtype=torch.float32, device=dev)
+
+    def _head(self, c, s):
+        B, K = self.batch, self.num_keypoints
+        h, w = c.logits.shape[2:]
+        call("ssp_region_decode_argmax", ptr(c.logits), B, K, self.num_classes, h, w, 1, ptr(c.boxes), ptr(c.conf), None, s)
+        torch.mul(c.boxes[:, :2 * K].view(B, K, 2), c.scale, out=c.kp)
+        call("ssp_pnp_batched", ptr(self._P3), 1, ptr(c.kp), ptr(self._K32), K, B, 20, ptr(c.R), ptr(c.t), None, s)
+        c.Rt[:, :, :3].copy_(c.R)
+        c.Rt[:, :, 3].copy_(c.t)
+        call("ssp_project_points", ptr(self._X), 4, K, ptr(c.Rt), ptr(self._K64), B, ptr(c.proj), s)
+        c.corners.copy_(c.proj.transpose(1, 2))
+
+    def _outputs(self, c):
+        return dict(R=c.R, t=c.t, conf=c.conf, keypoints_px=c.kp, corners_px=c.corners)
 
 
 # ---------------------------------------------------------------------------------------------- command line

@@ -1,0 +1,188 @@
+"""Camera frames -> the 6-D pose of every requested object of a multi-object model (yolo-pose-multi.cfg) in one CUDA graph replay.
+
+    pred = MultiPosePredictor(model, {0: corners_ape, 4: corners_can}, K, frame_size=(640, 480), batch=1)
+    r = pred(frames)            # (B, H, W, 3) uint8 numpy array / CUDA tensor, or a list of B JPEG files' bytes
+    r["R"][b, q], r["t"][b, q], r["detected"][b, q], ...             # slot q is class r["classes"][q] (the sorted class ids)
+
+Frames go through the chain PosePredictor runs (predict.py: resize + ToTensor, the split-K eval forward, the graph LRU, the weight
+re-pack); only the head differs.  Slot (frame b, class c) is the box reference valid_multi.py chooses for a ground truth of class
+c that is the image's first (valid_multi.py:105-123, get_multi_region_boxes(..., correspondingclass=c, only_objectness=0)):
+  * the first box with the largest det_conf among the listed boxes (det_conf * cls_max_conf > conf_thresh) whose arg-max class
+    is c -- detected = True;
+  * otherwise the reference's fallback box for correspondingclass = c (the running maxima of det_conf and softmax[c] in visiting
+    order) -- detected = False.  Every slot therefore has a pose, as valid_multi always has one for the object it evaluates.
+Each frame is its own batch-1 call (utils_multi.evaluate_multi_poses_batched documents the same departure).  Then per slot, as
+valid_multi.py:127-138 computes them: the keypoints times the frame size in fp32, PnP of the 9 points [0; corners3D_c[:3]] of
+class c's own box with the fp32 K, and the projection of the centroid and the 8 corners under that pose.
+
+The head is one ssp_predict_multi_select launch (one CTA per frame, all classes), one ssp_pnp_batched over the B x Q problems
+and one ssp_project_points of every class's 9 points under every slot's pose, of which each slot keeps its own class's columns.
+
+Returned device tensors are the predictor's static outputs: the next call overwrites them.
+
+Command line: python -m singleshotpose_b200.predict_multi --datacfg cfg/occlusion.data --modelcfg cfg/yolo-pose-multi.cfg
+              --weightfile w.weights --object 0=../LINEMOD/ape/ape.ply --object 4=../LINEMOD/can/can.ply --out poses.npz img...
+"""
+from __future__ import annotations
+
+import argparse
+import ctypes as C
+
+import numpy as np
+import torch
+
+from ._lib import SspError, call, ptr
+from .predict import _FramePredictor
+
+MAX_ENTRIES = 4096          # H*W*num_anchors the select kernel keeps in shared memory (eval_multi_core.h kMaxEntries)
+OUTPUT_KEYS = ("R", "t", "conf", "cls_conf", "detected", "keypoints_px", "corners_px")
+
+
+class MultiPosePredictor(_FramePredictor):
+    """model: a singleshotpose_b200.darknet_multi.Darknet (multi-anchor head, 9 keypoints).  objects: {class id: (3|4, 8) box corners
+    of that class's mesh (utils.get_3D_corners)}; the slots follow the sorted class ids.  K: (3, 3) camera matrix; frame_size:
+    (width, height) of the camera frames (other sizes are accepted and captured separately); shape: network input (width,
+    height), default the cfg's training size (valid_multi.py:71); batch: frames per call; conf_thresh: default the cfg net
+    block's conf_thresh (valid_multi.py:40).  graph=False runs the same launches eagerly (no capture).
+
+    Returns dict(classes (Q,), R (B, Q, 3, 3) fp64, t (B, Q, 3) fp64, conf (B, Q) det_conf of the box, cls_conf (B, Q),
+    detected (B, Q) bool, keypoints_px (B, Q, 9, 2), corners_px (B, Q, 9, 2)): device tensors, or numpy with to_host=True."""
+
+    def __init__(self, model, objects, K, frame_size=(640, 480), shape=None, batch=1, conf_thresh=None, graph=True, max_graphs=4):
+        self.num_anchors = int(getattr(model, "num_anchors", 0))
+        if self.num_anchors < 2:
+            raise SspError("MultiPosePredictor needs a multi-anchor region head (yolo-pose-multi.cfg), got %d anchor(s)" % self.num_anchors)
+        nC = int(model.num_classes)
+        if not isinstance(objects, dict) or not objects:
+            raise SspError("objects must be a non-empty {class id: corners3D} dict")
+        ids = sorted(objects)
+        for c in ids:
+            if isinstance(c, bool) or not isinstance(c, (int, np.integer)) or not 0 <= c < nC:
+                raise SspError("class id %r is not in [0, %d)" % (c, nC))
+        pts = [self._box_points(objects[c]) for c in ids]
+        if conf_thresh is None:
+            if "conf_thresh" not in model.blocks[0]:
+                raise SspError("the model's cfg has no conf_thresh in its [net] block: pass conf_thresh")
+            conf_thresh = float(model.blocks[0]["conf_thresh"])
+        self.conf_thresh = float(conf_thresh)
+        super().__init__(model, K, frame_size, shape if shape is not None else (model.width, model.height), batch, graph, max_graphs)
+        h, w = self.out_hw
+        if h * w * self.num_anchors > MAX_ENTRIES:
+            raise SspError("network shape %dx%d gives a %dx%d grid of %d anchors: more than the %d entries the select kernel holds"
+                           % (self.shape[0], self.shape[1], h, w, self.num_anchors, MAX_ENTRIES))
+        dev, B, Q = self.device, self.batch, len(ids)
+        self.classes = np.array(ids, dtype=np.int64)
+        self._cls_host = np.array(ids, dtype=np.int32)                            # copied into the select kernel's launch
+        self._classes = torch.from_numpy(self.classes).to(dev)
+        P3 = np.stack([P.T for P in pts]).astype(np.float32)                      # (Q, 9, 3) PnP points of each class
+        self._P3 = torch.from_numpy(np.repeat(P3[None], B, 0)).to(dev)              # (B, Q, 9, 3): one per slot
+        X = np.concatenate([np.concatenate([P, np.ones((1, 9))], 0) for P in pts], 1)                     # (4, 9Q)
+        self._X = torch.from_numpy(np.ascontiguousarray(X, dtype=np.float32)).to(dev)
+
+    def _head_buffers(self, c):
+        dev, B, K, Q = self.device, self.batch, self.num_keypoints, len(self.classes)
+        c.boxes = torch.empty(B, Q, 2 * K + 3, dtype=torch.float32, device=dev)
+        c.flags = torch.empty(B, Q, dtype=torch.int32, device=dev)
+        c.detected = torch.empty(B, Q, dtype=torch.bool, device=dev)
+        c.kp = torch.empty(B, Q, K, 2, dtype=torch.float32, device=dev)
+        c.R = torch.empty(B, Q, 3, 3, dtype=torch.float64, device=dev)
+        c.t = torch.empty(B, Q, 3, dtype=torch.float64, device=dev)
+        c.Rt = torch.empty(B, Q, 3, 4, dtype=torch.float64, device=dev)
+        c.proj = torch.empty(B * Q, 2, Q * K, dtype=torch.float32, device=dev)
+        c.corners = torch.empty(B, Q, K, 2, dtype=torch.float32, device=dev)
+
+    def _head(self, c, s):
+        B, K, Q = self.batch, self.num_keypoints, len(self.classes)
+        Wf, Hf = c.frame
+        h, w = c.logits.shape[2:]
+        call("ssp_predict_multi_select", ptr(c.logits), B, K, self.num_classes, self.num_anchors, h, w, C.c_void_p(self._cls_host.ctypes.data),
+             Q, self.conf_thresh, float(Wf), float(Hf), ptr(c.boxes), ptr(c.flags), ptr(c.kp), s)
+        torch.eq(c.flags, 0, out=c.detected)
+        call("ssp_pnp_batched", ptr(self._P3), 0, ptr(c.kp), ptr(self._K32), K, B * Q, 20, ptr(c.R), ptr(c.t), None, s)
+        c.Rt[..., :3].copy_(c.R)
+        c.Rt[..., 3].copy_(c.t)
+        # every class's points under every slot's pose (each point is projected on its own, so a slot's own columns are what
+        # ssp_project_points gives for that class's (4, 9) points alone); slot (b, q) keeps the columns of class q
+        call("ssp_project_points", ptr(self._X), 4, Q * K, ptr(c.Rt), ptr(self._K64), B * Q, ptr(c.proj), s)
+        c.corners.copy_(torch.diagonal(c.proj.view(B, Q, 2, Q, K), dim1=1, dim2=3).permute(0, 3, 2, 1))
+
+    def _outputs(self, c):
+        K = self.num_keypoints
+        return dict(classes=self._classes, R=c.R, t=c.t, conf=c.boxes[..., 2 * K], cls_conf=c.boxes[..., 2 * K + 1], detected=c.detected,
+                    keypoints_px=c.kp, corners_px=c.corners)
+
+
+# ---------------------------------------------------------------------------------------------- command line
+def camera_from_multi_data_cfg(datacfg):
+    """-> (K (3, 3) float64, (width, height)) from a multi-object .data file (the keys valid_multi.py:30-35 reads: im_width,
+    im_height, fx, fy, u0, v0)"""
+    from .utils_host import read_data_cfg
+    o = read_data_cfg(datacfg)
+    try:
+        fx, fy, u0, v0 = (float(o[k]) for k in ("fx", "fy", "u0", "v0"))
+        size = (int(o["im_width"]), int(o["im_height"]))
+    except KeyError as e:
+        raise SspError("%s has no %s entry" % (datacfg, e))
+    K = np.array([[fx, 0.0, u0], [0.0, fy, v0], [0.0, 0.0, 1.0]])
+    return K, size
+
+
+def parse_objects(specs):
+    """['0=ape.ply', '4=can.ply'] -> {0: 'ape.ply', 4: 'can.ply'}; raises SspError for a malformed entry or a class given twice"""
+    out = {}
+    for s in specs or ():
+        cls, sep, path = s.partition("=")
+        try:
+            c = int(cls)
+        except ValueError:
+            c = None
+        if not sep or c is None or c < 0 or not path:
+            raise SspError("--object takes CLASS=MESH.ply with a class id >= 0, got %r" % s)
+        if c in out:
+            raise SspError("class %d is given twice (%s and %s)" % (c, out[c], path))
+        out[c] = path
+    if not out:
+        raise SspError("give at least one --object CLASS=MESH.ply")
+    return out
+
+
+def main(argv=None):
+    ap = argparse.ArgumentParser(prog="python -m singleshotpose_b200.predict_multi",
+                                 description="6-D poses of the requested objects of a trained multi-object model in each image")
+    ap.add_argument("--datacfg", required=True, help=".data file: fx fy u0 v0, im_width im_height")
+    ap.add_argument("--modelcfg", required=True)
+    ap.add_argument("--weightfile", required=True)
+    ap.add_argument("--object", action="append", required=True, metavar="CLASS=MESH.ply",
+                    help="a class id of the model and the mesh of its object; repeat for every object to predict")
+    ap.add_argument("--out", default="poses.npz")
+    ap.add_argument("images", nargs="+")
+    a = ap.parse_args(argv)
+    from .darknet_multi import Darknet
+    from .utils import get_3D_corners
+    from .utils_host import read_ply_vertices
+    K, size = camera_from_multi_data_cfg(a.datacfg)
+    objects = {}
+    for c, mesh in parse_objects(a.object).items():
+        V = read_ply_vertices(mesh)
+        objects[c] = get_3D_corners(np.c_[V, np.ones((len(V), 1))].T)
+    model = Darknet(a.modelcfg)
+    model.load_weights(a.weightfile)
+    model.cuda().eval()
+    pred = MultiPosePredictor(model, objects, K, frame_size=size)
+    res = {k: [] for k in OUTPUT_KEYS}
+    for path in a.images:
+        with open(path, "rb") as f:
+            data = f.read()
+        if data[:2] == b"\xff\xd8":
+            r = pred([data], to_host=True)
+        else:
+            from PIL import Image
+            r = pred(np.asarray(Image.open(path).convert("RGB"))[None], to_host=True)
+        for k in res:
+            res[k].append(r[k][0])
+    np.savez(a.out, paths=np.array(a.images), classes=pred.classes, **{k: np.stack(v) for k, v in res.items()})
+    print("%d images x %d objects -> %s" % (len(a.images), len(pred.classes), a.out))
+
+
+if __name__ == "__main__":
+    main()

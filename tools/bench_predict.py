@@ -13,6 +13,12 @@ Reports, all device times from CUDA events after warm-up:
     count and CPU model;
   * the card's name and power limit.
     python tools/bench_predict.py [--reps 50] [--rounds 3]
+
+--multi measures MultiPosePredictor (singleshotpose_b200/predict_multi.py) instead, with the same method: yolo-pose-multi.cfg at
+416^2, B = 1 and 8, all 13 classes requested; the captured predictor against graph=False; the device time per stage (image,
+forward, head) of one eager call; the reference chain on the CPU at B = 1 (oracle Darknet in eval mode, get_multi_region_boxes_ref
+and valid_multi.py's selection for each class, cv2.solvePnP, the projection); the card's name and power limit.
+    python tools/bench_predict.py --multi [--reps 50] [--rounds 3]
 """
 import argparse
 import json
@@ -96,11 +102,104 @@ def _forward_graph_ms(eng, x, split, reps):
     return e0.elapsed_time(e1) / reps, sum(1 for v in B.splits if v)
 
 
+def _stage_split(pred, frames, n=10):
+    """median device time per stage of eager predictor calls"""
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
+    st = {"image": [], "forward": [], "head": []}
+    for _ in range(n):
+        pred(frames, events=ev)
+        ev[3].synchronize()
+        st["image"].append(ev[0].elapsed_time(ev[1])); st["forward"].append(ev[1].elapsed_time(ev[2])); st["head"].append(ev[2].elapsed_time(ev[3]))
+    return {k: float(np.median(v)) for k, v in st.items()}
+
+
+def main_multi(args):
+    import ctypes as C
+    from singleshotpose_b200._lib import call, ptr, stream_ptr
+    from singleshotpose_b200.darknet_multi import Darknet as DarknetMulti
+    from singleshotpose_b200.predict_multi import MultiPosePredictor
+    cfg = write_cfg(multi=True)
+    torch.manual_seed(0)
+    model = DarknetMulti(cfg).cuda().eval()
+    K = synth.intrinsics()
+    objects = {c: synth.box_points((0.03 + 0.002 * c, 0.039, 0.046), with_center=False).T for c in range(13)}
+    res = {"gpu": _gpu_name(), "frame": [640, 480], "classes": 13, "configs": {}}
+    for bsz in (1, 8):
+        frames = np.random.default_rng(bsz).integers(0, 256, size=(bsz, 480, 640, 3), dtype=np.uint8)
+        pred = MultiPosePredictor(model, objects, K, batch=bsz)
+        eager = MultiPosePredictor(model, objects, K, batch=bsz, graph=False)
+        arms = {"pred": lambda: pred(frames, to_host=True), "pred_nograph": lambda: eager(frames, to_host=True)}
+        for f in arms.values():
+            for _ in range(3):
+                f()
+        torch.cuda.synchronize()
+        reps = args.reps if bsz == 1 else max(5, args.reps // 5)
+        lat = {k: [] for k in arms}
+        for _ in range(args.rounds):                         # alternate the arms
+            for k, f in arms.items():
+                lat[k].append(_median_ms(f, reps))
+        c = {k: {"ms": float(np.median(v)), "frames_per_s": bsz / (float(np.median(v)) * 1e-3), "rounds_ms": v} for k, v in lat.items()}
+        c["eager_stage_device_ms"] = _stage_split(pred, frames)
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        ts = []
+        for _ in range(10):
+            e0.record(); pred(frames); e1.record(); e1.synchronize()
+            ts.append(e0.elapsed_time(e1))
+        c["replay_device_ms"] = float(np.median(ts))
+        c["detected"] = int(pred(frames)["detected"].sum())
+        # the select kernel alone (one CTA per frame, 13 classes) on the predictor's logits; the rest of the head is the PnP
+        # launch (one thread per slot), the projection and three small copies
+        lg, ch = pred.logits, pred._last
+        sel = lambda: call("ssp_predict_multi_select", ptr(lg), bsz, 9, 13, 5, lg.shape[2], lg.shape[3], C.c_void_p(pred._cls_host.ctypes.data), 13,
+                           pred.conf_thresh, 640.0, 480.0, ptr(ch.boxes), ptr(ch.flags), ptr(ch.kp), stream_ptr())
+        sel()
+        torch.cuda.synchronize()
+        e0.record()
+        for _ in range(100):
+            sel()
+        e1.record(); e1.synchronize()
+        c["select_kernel_us"] = e0.elapsed_time(e1) * 10.0
+        res["configs"]["B%d_416" % bsz] = c
+        del pred, eager
+        print(json.dumps({"B%d_416" % bsz: c}), flush=True)
+    # reference chain on the CPU, B = 1 at 416^2: every class as valid_multi.py evaluates a first ground truth of that class
+    import cv2
+    from oracle import eval_multi_ref as EM
+    from oracle.darknet_ref import RefDarknet
+    from oracle.decode_multi_ref import get_multi_region_boxes_ref
+    from oracle.eval_ref import compute_projection
+    torch.manual_seed(0)
+    ref = RefDarknet(cfg).eval()
+    xb = synth.images(1, seed=0)
+    K32 = K.astype(np.float32)
+    thr = float(model.blocks[0]["conf_thresh"])
+
+    def ref_chain():
+        with torch.no_grad():
+            o = ref(xb)
+        for c, corners in objects.items():
+            boxes = get_multi_region_boxes_ref(o, thr, 13, 9, synth.MULTI_ANCHORS, 5, c, only_objectness=0)[0]
+            truths = np.zeros((50, 21), np.float32)
+            truths[0, 0], truths[0, 1:] = c, 0.5
+            (j, _carried), = EM.select_ref(boxes, truths, 9)
+            uv = np.array([[float(boxes[j][2 * k]) * 640, float(boxes[j][2 * k + 1]) * 480] for k in range(9)], dtype=np.float32)
+            P = np.concatenate([np.zeros((3, 1)), corners[:3]], 1)
+            _ok, rvec, t = cv2.solvePnP(np.ascontiguousarray(P.T, dtype=np.float32), uv, K32, None, flags=cv2.SOLVEPNP_ITERATIVE)
+            R, _ = cv2.Rodrigues(rvec)
+            compute_projection(np.concatenate([P, np.ones((1, 9))], 0), np.concatenate([R, t], 1), K)
+    ref_chain()
+    res["cpu_reference_B1_416"] = {"ms": _median_ms(ref_chain, 5), "threads": torch.get_num_threads(), "cpu": _cpu_model()}
+    print(json.dumps(res))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=50)
     ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--multi", action="store_true", help="measure the multi-object predictor (13 classes) instead")
     args = ap.parse_args()
+    if args.multi:
+        return main_multi(args)
     dev = torch.device("cuda")
     cfg = write_cfg()
     torch.manual_seed(0)
