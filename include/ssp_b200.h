@@ -51,7 +51,6 @@ long long ssp_flat_alloc_rows(int N, int H, int W);
 long long ssp_flat_row(int n, int h, int w, int H, int W);
 
 /* ---- layout: train.py:83 `data.cuda()` hands NCHW fp32; the conv stack runs on padded-flat rows ---- */
-int ssp_pack_input_im2col(const float* x_nchw, void* hi, void* lo, int N, int H, int W, void* stream);
 int ssp_pack_nchw(const float* x_nchw, void* hi, void* lo_or_null, int N, int C, int H, int W, int ld, int c0,
                   int fmt, float scale, void* stream);
 int ssp_unpack_nchw(const float* y_flat, float* out_nchw, int N, int C, int H, int W, int ld, int c0, void* stream);
@@ -92,10 +91,6 @@ int ssp_conv_splitk_count(int N, int H, int W, int taps, int cin, int cout, int 
 int ssp_bn_apply_splitk(const float* partial, int splits, long long slab_elems, int partial_ld, const float* scale, const float* shift,
                         int N, int C, int H, int W, float slope, void* d0_hi, void* d0_lo, int d0_ld, int d0_c0, int d0_route,
                         void* d1_hi, void* d1_lo, int d1_ld, int d1_c0, int d1_route, void* stream);
-/* ---- first layer nn.Conv2d(3, 32, 3, 1, 1) (darknet.py:156, block 0): direct fp32 convolution of the NCHW image with the
- *      fp32 master weights [32][3][3][3] (k = (kh*3+kw)*3 + ci), output rows [row(n,h,w)][y_ld], optional fp64 BN statistics ---- */
-int ssp_conv0_direct(const float* x_nchw, const float* w, const float* bias_or_null, float* y, int y_ld,
-                     double* stat_sum_or_null, double* stat_sq_or_null, int N, int H, int W, void* stream);
 /* ---- blocks 0-1 of cfg/yolo-pose.cfg as a unit -- nn.Conv2d(3,32,3,1,1) + BatchNorm2d + LeakyReLU + MaxPool2d(2,2) (darknet.py:154-167)
  *      and their autograd (train.py:103) -- without materialising the full-resolution conv output (csrc/l0_fused.cu).
  *      gram: double[SSP_L0_GRAM_DOUBLES]; the first 28*28 hold the matrix (upper triangle: sums of q q^T over all pixels, q = (27 patch

@@ -22,13 +22,11 @@ SIGNATURES = {
     "ssp_last_error": [],
     "ssp_flat_alloc_rows": [_i, _i, _i],
     "ssp_flat_row": [_i, _i, _i, _i, _i],
-    "ssp_pack_input_im2col": [_p, _p, _p, _i, _i, _i, _p],
     "ssp_pack_nchw": [_p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _f, _p],
     "ssp_unpack_nchw": [_p, _p, _i, _i, _i, _i, _i, _i, _p],
     "ssp_unpack16_nchw": [_p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _p],
     "ssp_conv_gemm": [_i, _p, _p, _ll, _i, _i, _p, _p, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p, _i, _ll, _i, _p, _p, _p, _p],
     "ssp_conv_bandt_launches": [],
-    "ssp_conv0_direct": [_p, _p, _p, _p, _i, _p, _p, _i, _i, _i, _p],
     "ssp_l0_gram": [_p, _i, _i, _i, _p, _p],
     "ssp_l0_stats": [_p, _p, _p, _p, _p],
     "ssp_l0_fused_fwd": [_p, _p, _p, _p, _f, _i, _i, _i, _p, _p, _i, _i, _p, _p],

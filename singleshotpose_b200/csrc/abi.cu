@@ -23,7 +23,6 @@ int conv_gemm_simt(const void*, const void*, long long, int, int, const void*, c
 int conv_gemm_bandt(const void*, const void*, long long, int, int, const void*, const void*, int, int, int, int, int, int, int, int, int,
                     float*, int, long long, int, const float*, double*, double*, cudaStream_t);
 int conv_bandt_launch_count();
-int conv0_direct(const float*, const float*, const float*, float*, int, double*, double*, int, int, int, cudaStream_t);
 int l0_gram(const float*, int, int, int, double*, cudaStream_t);
 int l0_stats(const double*, const float*, double*, double*, cudaStream_t);
 int l0_fused_fwd(const float*, const float*, const float*, const float*, float, int, int, int, void*, void*, int, int, uint8_t*, cudaStream_t);
@@ -31,7 +30,6 @@ int l0_bwd(const float*, const void*, int, int, int, const uint8_t*, float, int,
 int l0_bwd_finalize(const double*, const double*, const float*, const float*, const float*, const float*, double, float, float*, float*, float*, cudaStream_t);
 int wgrad_gemm_tc(const void*, long long, int, int, int, const void*, long long, int, int, int, int, int, int, int, float*, int, int, float, cudaStream_t);
 int wgrad_gemm_simt(const void*, long long, int, int, int, const void*, long long, int, int, int, int, int, int, int, float*, int, int, float, cudaStream_t);
-int pack_input_im2col(const float*, void*, void*, int, int, int, cudaStream_t);
 int pack_nchw(const float*, void*, void*, int, int, int, int, int, int, int, float, cudaStream_t);
 int unpack_nchw(const float*, float*, int, int, int, int, int, int, cudaStream_t);
 int unpack16_nchw(const void*, const void*, float*, int, int, int, int, int, int, int, cudaStream_t);
@@ -92,7 +90,6 @@ const char* ssp_last_error(void) { return g_err; }
 long long ssp_flat_alloc_rows(int N, int H, int W) { return flat_alloc_rows(N, H, W); }
 long long ssp_flat_row(int n, int h, int w, int H, int W) { Geom g{1, H, W}; return g.row(n, h, w); }
 
-int ssp_pack_input_im2col(const float* x, void* hi, void* lo, int N, int H, int W, void* s) { return pack_input_im2col(x, hi, lo, N, H, W, ST(s)); }
 int ssp_pack_nchw(const float* x, void* hi, void* lo, int N, int C, int H, int W, int ld, int c0, int fmt, float scale, void* s) {
   return pack_nchw(x, hi, lo, N, C, H, W, ld, c0, fmt, scale, ST(s));
 }
@@ -125,9 +122,6 @@ int ssp_conv_gemm(int impl, const void* a_hi, const void* a_lo, long long a_rows
   return conv_gemm_tc(a_hi, a_lo, a_rows, a_ld, cin, b_hi, b_lo, b_rows, b_ld, a_fmt, b_fmt, N, H, W, taps, cout, out, out_ld, out_rows, epi, bias, ssum, ssq, ST(s), nullptr);
 }
 int ssp_conv_bandt_launches(void) { return conv_bandt_launch_count(); }
-int ssp_conv0_direct(const float* x, const float* w, const float* bias, float* y, int y_ld, double* ssum, double* ssq, int N, int H, int W, void* s) {
-  return conv0_direct(x, w, bias, y, y_ld, ssum, ssq, N, H, W, ST(s));
-}
 int ssp_l0_gram(const float* x, int N, int H, int W, double* gram, void* s) { return l0_gram(x, N, H, W, gram, ST(s)); }
 int ssp_l0_stats(const double* gram, const float* w, double* ssum, double* ssq, void* s) { return l0_stats(gram, w, ssum, ssq, ST(s)); }
 int ssp_l0_fused_fwd(const float* x, const float* w, const float* scale, const float* shift, float slope, int N, int H, int W, void* d_hi,

@@ -241,8 +241,7 @@ int conv_gemm_bandt(const void* a_hi, const void* a_lo, long long a_rows, int a_
   // 32-channel 3x3 layer with a row pitch of exactly 32 channels: overlapping-row tensor map (a legal tensor map: rows may overlap) -- a band row
   // is [pixel | pixel + 1], dense 128 B instead of 64 B + zero fill, and the taps (kh, 0), (kh, 1) share one 64-wide K chunk: six resident
   // weight tiles instead of nine, which is what makes room for a third ring stage (block 2 forward: 477 us at 42 % tensor-active with two)
-  static const int ovl_on = []() { const char* e = getenv("SSP_BANDT_OVL"); return e ? atoi(e) : 1; }();
-  p.ovl = (ovl_on && taps == 9 && cin == 32 && a_ld == 32) ? 1 : 0;
+  p.ovl = (taps == 9 && cin == 32 && a_ld == 32) ? 1 : 0;
   const int mrows = p.stacked ? 128 : ((cout + 7) / 8) * 8;
   p.w_tile_bytes = mrows * 128;
   long long res = (long long)(p.ovl ? 6 : taps * p.kc_per_tap) * p.w_tile_bytes + (128 - mrows) * 128;      // every MMA reads 128 rows from its tile's start

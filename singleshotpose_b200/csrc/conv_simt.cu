@@ -1,6 +1,6 @@
 // fp32 CUDA-core versions of the two GEMM-shaped kernels (same operands, same outputs as conv_tc.cu /
-// wgrad_tc.cu).  They are the on-device cross-check for the tensor-core kernels and the bring-up path
-// (SSP_CONV_IMPL=simt); all arithmetic is fp32 FFMA on hi+lo reconstructed operands.
+// wgrad_tc.cu).  They are the on-device cross-check for the tensor-core kernels (SSP_IMPL_SIMT through the
+// ABI); all arithmetic is fp32 FFMA on hi+lo reconstructed operands.
 #include "ssp_common.cuh"
 
 namespace ssp {

@@ -8,8 +8,7 @@
 //      reference's logits by 3e-2 (DESIGN.md, "numerics").
 // B  = weights [cout][taps*cin] (K contiguous), same hi/lo convention.
 // Every tap is one plain 2-D TMA tile at a shifted row coordinate (negative / past-the-end rows are
-// zero-filled by TMA), so 3x3 convs need no im2col buffer; 1x1 convs and the im2col'ed first layer are
-// the taps==1 case.  Replaces nn.Conv2d in reference darknet.py:156-160 (forward) and, with re-packed
+// zero-filled by TMA), so 3x3 convs need no im2col buffer; 1x1 convs are the taps==1 case.  Replaces nn.Conv2d in reference darknet.py:156-160 (forward) and, with re-packed
 // weights, its data gradient (train.py:103 autograd).
 //
 // CTA = 8 warps, persistent over (m-tile, n-tile) pairs:

@@ -18,44 +18,6 @@
 namespace ssp {
 
 // ------------------------------------------------------------------------------------------------
-// Layer-0 input: NCHW fp32 image -> im2col'ed rows [row(n,h,w)][32] (k = (kh*3+kw)*3 + c, k >= 27 zero), hi/lo fp16.
-__global__ void __launch_bounds__(256) pack_input_im2col_kernel(const float* __restrict__ x, uint16_t* __restrict__ hi,
-                                                                uint16_t* __restrict__ lo, int N, int H, int W) {
-  // one thread per pixel: 27 cached reads (neighbouring threads share them), 2 x 64 B of vector stores
-  const long long pix = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (pix >= (long long)N * H * W) return;
-  const int w = (int)(pix % W);
-  const int h = (int)((pix / W) % H);
-  const int n = (int)(pix / ((long long)W * H));
-  uint32_t ph[16], pl[16];
-  const int HW = H * W;
-  const float* px = x + (long long)n * 3 * HW + (h * W + w);     // one 64-bit address per pixel; taps are 32-bit offsets
-#pragma unroll
-  for (int k2 = 0; k2 < 16; k2++) {
-    uint16_t a[2], b[2];
-#pragma unroll
-    for (int e = 0; e < 2; e++) {
-      const int k = 2 * k2 + e;
-      float v = 0.f;
-      if (k < 27) {
-        const int c = k % 3, tap = k / 3;
-        const int hh = h + tap / 3 - 1, ww = w + tap % 3 - 1;
-        if (hh >= 0 && hh < H && ww >= 0 && ww < W) v = __ldg(px + (c * HW + (tap / 3 - 1) * W + (tap % 3 - 1)));
-      }
-      split_f16(v, a[e], b[e]);
-    }
-    ph[k2] = a[0] | ((uint32_t)a[1] << 16); pl[k2] = b[0] | ((uint32_t)b[1] << 16);
-  }
-  Geom g{N, H, W};
-  const long long o = g.row(n, h, w) * 32;
-  uint4* dh = reinterpret_cast<uint4*>(hi + o); uint4* dl = reinterpret_cast<uint4*>(lo + o);
-#pragma unroll
-  for (int j = 0; j < 4; j++) {
-    dh[j] = make_uint4(ph[4 * j], ph[4 * j + 1], ph[4 * j + 2], ph[4 * j + 3]);
-    if (lo) dl[j] = make_uint4(pl[4 * j], pl[4 * j + 1], pl[4 * j + 2], pl[4 * j + 3]);
-  }
-}
-
 // generic NCHW fp32 -> padded-flat rows (hi/lo fp16, or a single 16-bit plane in `fmt` when lo == nullptr)
 __global__ void pack_nchw_kernel(const float* __restrict__ x, uint16_t* __restrict__ hi, uint16_t* __restrict__ lo,
                                  int N, int C, int H, int W, int ld, int c0, int fmt, float scale) {
@@ -554,12 +516,6 @@ __global__ void sgd_flat_kernel(float* __restrict__ p, const float* __restrict__
 // ================================================================================================ host launchers
 static inline unsigned nblk(long long total, int bs) { return (unsigned)((total + bs - 1) / bs); }
 
-int pack_input_im2col(const float* x, void* hi, void* lo, int N, int H, int W, cudaStream_t s) {
-  if (!x || !hi) return fail_msg(SSP_ERR_ARG, "pack_input_im2col: null pointer");
-  const long long total = (long long)N * H * W;
-  pack_input_im2col_kernel<<<nblk(total, 256), 256, 0, s>>>(x, (uint16_t*)hi, (uint16_t*)lo, N, H, W);
-  SSP_CHECK_LAUNCH(); return SSP_OK;
-}
 int pack_nchw(const float* x, void* hi, void* lo, int N, int C, int H, int W, int ld, int c0, int fmt, float scale, cudaStream_t s) {
   if (!x || !hi) return fail_msg(SSP_ERR_ARG, "pack_nchw: null pointer");
   const long long total = (long long)N * C * H * W;

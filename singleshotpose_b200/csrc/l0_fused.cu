@@ -17,7 +17,6 @@
 // Replaces nn.Conv2d(3,32,3,1,1) + BatchNorm2d + LeakyReLU + MaxPool2d(2,2) of reference darknet.py:154-167 (blocks 0-1 of
 // cfg/yolo-pose.cfg) and their autograd (train.py:103).
 #include "ssp_common.cuh"
-#include <stdlib.h>
 
 namespace ssp {
 
@@ -306,10 +305,10 @@ __global__ void __launch_bounds__(1024) l0_stats_kernel(const double* __restrict
 }
 
 // ------------------------------------------------------------------------------------------------ conv + BN + leaky + 2x2 max-pool
-// thread = one 2x2 pixel window x 16 output channels (64 accumulators); channel ownership 8q + 4*half + j as conv0_direct_kernel,
-// so the two threads of a window fill 16 contiguous bytes of every destination row chunk.
-template <int MINB>      // resident blocks per SM: 2 caps the kernel at 128 registers (a few spills), 1 leaves it the whole file
-__global__ void __launch_bounds__(256, MINB) l0_fused_fwd_kernel(const float* __restrict__ x, const float* __restrict__ wgt /*[32][27]*/,
+// thread = one 2x2 pixel window x 16 output channels (64 accumulators); channel ownership 8q + 4*half + j, so the two threads of a
+// window fill 16 contiguous bytes of every destination row chunk.  One resident block per SM leaves the kernel the whole register
+// file (two cap it at 128 registers, with a few spills).
+__global__ void __launch_bounds__(256, 1) l0_fused_fwd_kernel(const float* __restrict__ x, const float* __restrict__ wgt /*[32][27]*/,
                                                               const float* __restrict__ scale, const float* __restrict__ shift, float slope,
                                                               int N, int H, int W, uint16_t* __restrict__ d_hi, uint16_t* __restrict__ d_lo,
                                                               int d_ld, int d_c0, uint8_t* __restrict__ code /*[pooled rows][32] or null*/) {
@@ -502,8 +501,7 @@ int l0_gram(const float* x, int N, int H, int W, double* gram, cudaStream_t s) {
   if (nt > 0x7fffffffLL) return fail_msg(SSP_ERR_ARG, "l0_gram: bad shape");
   cudaError_t e = cudaMemsetAsync(gram, 0, sizeof(double) * kGramDoubles, s);
   if (e != cudaSuccess) return fail_cuda(e, __FILE__, __LINE__);
-  static const int brute = []() { const char* v = getenv("SSP_L0_GRAM"); return v && v[0] == 'b'; }();      // SSP_L0_GRAM=brute: all 406 products per pixel
-  if (brute || H < 2 || W < 2) {
+  if (H < 2 || W < 2) {
     l0_gram_kernel<<<l0_grid(nt, 2), 256, 0, s>>>(x, gram, N, H, W);
     SSP_CHECK_LAUNCH(); return SSP_OK;
   }
@@ -527,9 +525,7 @@ int l0_fused_fwd(const float* x, const float* w, const float* scale, const float
     return fail_msg(SSP_ERR_ARG, "l0_fused_fwd: bad argument (even H / W, destination rows 8-B aligned)");
   const long long nt = l0_tiles(N, H, W);
   if (nt <= 0 || nt > 0x7fffffffLL) return fail_msg(SSP_ERR_ARG, "l0_fused_fwd: bad shape");
-  static const int occ = []() { const char* e = getenv("SSP_L0_OCC"); return e ? atoi(e) : 1; }();     // SSP_L0_OCC=2: two CTAs per SM (fewer registers)
-  if (occ == 1) l0_fused_fwd_kernel<1><<<l0_grid(nt, 1), 256, 0, s>>>(x, w, scale, shift, slope, N, H, W, (uint16_t*)d_hi, (uint16_t*)d_lo, d_ld, d_c0, code);
-  else l0_fused_fwd_kernel<2><<<l0_grid(nt, 2), 256, 0, s>>>(x, w, scale, shift, slope, N, H, W, (uint16_t*)d_hi, (uint16_t*)d_lo, d_ld, d_c0, code);
+  l0_fused_fwd_kernel<<<l0_grid(nt, 1), 256, 0, s>>>(x, w, scale, shift, slope, N, H, W, (uint16_t*)d_hi, (uint16_t*)d_lo, d_ld, d_c0, code);
   SSP_CHECK_LAUNCH(); return SSP_OK;
 }
 

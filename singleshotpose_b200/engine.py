@@ -38,9 +38,6 @@ class ConvLayer:
         self.leaves = []      # inputs: (producer layer index or -1 for the image, route kind, channel offset, channels)
         self.dests = []       # outputs: (consumer layer index, channel offset, route kind)
         self.first = False
-        # GEMM view of the forward pass
-        self.k_cin = cin      # channels per tap seen by the GEMM (32 for the im2col'ed first layer)
-        self.k_taps = self.taps
 
 
 def build_plan(blocks):
@@ -81,16 +78,17 @@ def build_plan(blocks):
         exprs.append(cur)
     if not layers or layers[-1].bn or layers[-1].slope != 1.0 or cur[0] != "conv":
         raise NotImplementedError("the network must end in a linear, bias-only convolution (region head)")
-    first = layers[0]
-    if first.leaves != [(-1, _lib.ROUTE_DIRECT, 0, first.cin)] or first.size != 3 or first.cin != 3:
-        raise NotImplementedError("first layer must be a 3x3 convolution on the 3-channel image")
-    first.first = True
-    first.k_cin, first.k_taps = 32, 1           # im2col'ed: K = 27 padded to 32, one "tap"
     for L in layers[1:]:
         for (src, kind, c0, c) in L.leaves:
             if src < 0:
                 raise NotImplementedError("only the first layer may read the image")
             layers[src].dests.append((L.index, c0, kind))
+    first = layers[0]
+    if (first.leaves != [(-1, _lib.ROUTE_DIRECT, 0, first.cin)] or first.size != 3 or first.cin != 3 or first.cout != 32 or not first.bn
+            or len(first.dests) != 1 or first.dests[0][2] != _lib.ROUTE_POOL):
+        raise NotImplementedError("blocks 0-1 must be a 3x3 convolution 3 -> 32 of the image with batch_normalize, then a 2x2 / 2 max-pool "
+                                  "(one fused unit, csrc/l0_fused.cu)")
+    first.first = True
     for L in layers[:-1]:
         if not L.bn:
             raise NotImplementedError("hidden convolution without batch_normalize")
@@ -149,10 +147,9 @@ class Buffers:
             # spatial size of this layer for the actual input resolution
             h, w = eng.spatial(L, H, W)
             rows = _lib.flat_alloc_rows(N, h, w)
-            cin_total = L.k_cin if L.first else L.cin
             self.rows.append(rows)
-            if L.first and eng.l0_fused:
-                # blocks 0-1 run as one unit (csrc/l0_fused.cu): no im2col plane, no full-resolution conv output, no dY plane --
+            if L.first:
+                # blocks 0-1 run as one unit (csrc/l0_fused.cu): no operand planes, no full-resolution conv output, no dY plane --
                 # the 28x28 Gram matrix of the image patches, a 1-byte code per pooled cell and 28x32 backward sums instead
                 self.x_hi.append(None); self.x_lo.append(None); self.y.append(None)
                 self.l0_gram = torch.zeros(2816, dtype=torch.float64, device=dev)      # SSP_L0_GRAM_DOUBLES: the 28x28 matrix + ssp_l0_gram's scratch
@@ -161,17 +158,18 @@ class Buffers:
                     self.l0_t1 = torch.zeros(28 * 32, dtype=torch.float64, device=dev)
                     self.ypool.append(None); self.dy.append(None); self.dx.append(None)
                 continue
-            self.x_hi.append(torch.zeros(rows, cin_total, dtype=f16, device=dev))
-            self.x_lo.append(torch.zeros(rows, cin_total, dtype=f16, device=dev))
+            self.x_hi.append(torch.zeros(rows, L.cin, dtype=f16, device=dev))
+            self.x_lo.append(torch.zeros(rows, L.cin, dtype=f16, device=dev))
             self.y.append(torch.zeros(rows, _rup(L.cout, 4), dtype=torch.float32, device=dev))
             if train:
-                pooled = eng.compact_pool_reduce and any(k == _lib.ROUTE_POOL for (_c, _o, k) in L.dests)
+                pooled = any(k == _lib.ROUTE_POOL for (_c, _o, k) in L.dests)
                 # y at the arg-max of every 2x2 window (pooled geometry): the BN-backward reduction of a pooled layer reads this
                 # plane + the pooled gradient (8 B per window) instead of the four full-resolution y values + the gradient (20 B)
                 self.ypool.append(torch.zeros(_lib.flat_alloc_rows(N, h // 2, w // 2), _rup(L.cout, 4), dtype=torch.float32, device=dev) if pooled else None)
-                self.dy.append(torch.zeros(rows, _rup(L.cout, 8), dtype=eng.grad_dtype, device=dev))
-                self.dx.append(None if L.first else torch.zeros(rows, _rup(cin_total, 8) if eng.dx_f16 else cin_total,
-                                                                dtype=torch.float16 if eng.dx_f16 else torch.float32, device=dev))
+                self.dy.append(torch.zeros(rows, _rup(L.cout, 8), dtype=f16, device=dev))
+                # data gradients dX in fp16 (loss-scaled, saturating): the BN backward reads every dX twice, the GEMM epilogue writes it
+                # once -- 6 of the ~22 bytes per activation element of the backward pass
+                self.dx.append(torch.zeros(rows, _rup(L.cin, 8), dtype=f16, device=dev))
 
 
 class Engine:
@@ -184,29 +182,11 @@ class Engine:
         self._views = None
         self._buffers = {}
         self._weights_version = None
-        impl = os.environ.get("SSP_CONV_IMPL", "auto").lower()
-        # "auto": SSP_IMPL_TC2 where the N tile is >= SSP_TC2_MIN_N wide, the band kernels for narrow layers (on sm_90a TC2 and TC
-        # are the same per-tap kernel)
-        self.conv_impl = {"simt": _lib.IMPL_SIMT, "tc2": _lib.IMPL_TC2, "tc": _lib.IMPL_TC, "auto": -1}.get(impl, -1)
-        self.tc2_min_n = int(os.environ.get("SSP_TC2_MIN_N", "128"))
-        self.use_band = os.environ.get("SSP_BAND", "1") != "0"
-        self.use_bandt = os.environ.get("SSP_BANDT", "1") != "0"
-        self.fuse_eval = os.environ.get("SSP_FUSE_EVAL", "1") != "0"
-        self.pack_fn = "ssp_pack_weights"
-        wimpl = os.environ.get("SSP_WGRAD_IMPL", "simt" if impl == "simt" else "tc2").lower()
-        # "tc2" (default) and "tc" select the same tensor-core weight-gradient kernel on sm_90a (csrc/wgrad_tc.cu)
-        self.wgrad_impl = {"simt": _lib.IMPL_SIMT, "tc": _lib.IMPL_TC}.get(wimpl, _lib.IMPL_TC2)
-        # backward operands: one 16-bit format for dY, W and X (wgmma takes both 16-bit operands in one
-        # format).  fp16 + a static loss scale (saturating conversion) is 8x more precise than bf16.
-        # The activation planes are fp16, so dY and the dgrad weights are fp16 too.
-        self.grad_fmt = _lib.FMT_F16
+        self.fuse_eval = True        # inference: BN + leaky in the GEMM epilogue (False: conv, bn_finalize, bn_apply as in training)
+        # backward operands: one 16-bit format for dY, W and X (wgmma takes both 16-bit operands in one format).  fp16 + a static
+        # loss scale (saturating conversion) is 8x more precise than bf16, and the activation planes are fp16 anyway.
         self.grad_scale = float(os.environ.get("SSP_GRAD_SCALE", "256"))
-        self.grad_dtype = torch.float16 if self.grad_fmt == _lib.FMT_F16 else torch.bfloat16
         self.fast = os.environ.get("SSP_PRECISION", "parity").lower() == "fast"   # single-term forward (no hi/lo)
-        # data gradients dX kept in fp16 (loss-scaled, saturating) instead of fp32: the BN backward reads every dX twice, the GEMM
-        # epilogue writes it once -- 6 of the ~22 bytes per activation element of the backward pass.  Needs the kernels that have the
-        # fp16 epilogue (auto dispatch: per-tap / operand-swapped); forced implementations keep fp32 planes.
-        self.dx_f16 = os.environ.get("SSP_DX_F16", "1") != "0" and self.conv_impl < 0 and self.grad_fmt == _lib.FMT_F16
         self.launches = 0
         # inference split-K (forward(split_k=True)): launches of ssp_conv_gemm_splitk so far; split_override (internal, for tests and
         # tools/bench_predict.py): None = ssp_conv_splitk_count's rule, 0 = split-K off, k >= 1 = k splits (at most the k-block
@@ -214,20 +194,11 @@ class Engine:
         self.split_launches = 0
         self.split_override = None
         self._num_sms = None
-        self.overlap =os.environ.get("SSP_OVERLAP", "1") != "0"
-        self.compact_pool_reduce = os.environ.get("SSP_POOL_REDUCE", "compact") != "full"
         self._side = None
         self.grad_ready_hook = None  # fn(first layer index, stream): every gradient of layers >= that index is complete in `stream` order
         self.profile = None          # set to [] to record (kind, layer block, algorithmic flops, start event, end event) per GEMM launch
         net = model.blocks[0]
         self.base_hw = (int(net["height"]), int(net["width"]))
-        # SSP_L0: "fused" (default) = conv + BN + leaky + 2x2 max-pool of blocks 0-1 as one unit from the raw image, statistics from
-        # the patch Gram matrix, backward over the pooled gradient (csrc/l0_fused.cu); "direct" = fp32 direct conv writing the
-        # full-resolution Y (round-1/2 path); "gemm" = im2col + tensor-core GEMM (bring-up path).
-        self.l0_mode = os.environ.get("SSP_L0", "fused").lower()
-        f = self.layers[0]
-        self.l0_fused = (self.l0_mode == "fused" and self.conv_impl != _lib.IMPL_SIMT and not self.fast and f.bn and f.cout == 32
-                         and len(f.dests) == 1 and f.dests[0][2] == _lib.ROUTE_POOL)
 
     # ------------------------------------------------------------------ geometry
     def spatial(self, L, H, W):
@@ -285,13 +256,18 @@ class Engine:
         self._seg_table = None
 
     def _alloc_layer_state(self, dev):
+        """fp16 operand planes of the GEMM layers' weights: W_hi / W_lo [cout][taps*cin] (forward), W_d [cin][taps*cout] (data
+        gradient).  Layer 0 has none: the fused unit of blocks 0-1 reads the fp32 master weights."""
         self.w_hi, self.w_lo, self.w_d = [], [], []
         f16 = torch.float16
         for L in self.layers:
-            kf = _rup(L.k_taps * L.k_cin if not L.first else 32, 8)
+            if L.first:
+                self.w_hi.append(None); self.w_lo.append(None); self.w_d.append(None)
+                continue
+            kf = _rup(L.taps * L.cin, 8)
             self.w_hi.append(torch.zeros(L.cout, kf, dtype=f16, device=dev))
             self.w_lo.append(torch.zeros(L.cout, kf, dtype=f16, device=dev))
-            self.w_d.append(None if L.first else torch.zeros(L.cin, _rup(L.taps * L.cout, 8), dtype=self.grad_dtype, device=dev))
+            self.w_d.append(torch.zeros(L.cin, _rup(L.taps * L.cout, 8), dtype=f16, device=dev))
 
     # ------------------------------------------------------------------ fused SGD + re-pack work list, gradient buckets
     _SEG_DTYPE = [("off", "<i8"), ("n", "<i8"), ("cout", "<i4"), ("taps", "<i4"), ("cin", "<i4"), ("ld_f", "<i4"), ("ld_d", "<i4"),
@@ -304,7 +280,8 @@ class Engine:
             return self._seg_table, self._seg_blocks
         import numpy as np
         lib = _lib.load()
-        conv_of = {id(conv.weight): L for L, (conv, _) in zip(self.layers, self.conv_modules())}
+        # the GEMM layers' weights also rewrite their operand planes; every other tensor (layer 0's weight included) is plain
+        conv_of = {id(conv.weight): L for L, (conv, _) in zip(self.layers, self.conv_modules()) if not L.first}
         params = list(self.model.parameters())
         tab = np.zeros(len(params), dtype=np.dtype(self._SEG_DTYPE))
         assert tab.dtype.itemsize == 72
@@ -316,11 +293,8 @@ class Engine:
             L = conv_of.get(id(p))
             if L is not None:
                 i = L.index
-                if L.first:        # [32][9][3] -> K = 27: a 1-tap GEMM over the im2col'ed input, no data gradient
-                    e["cout"], e["taps"], e["cin"] = L.cout, 1, 27
-                else:
-                    e["cout"], e["taps"], e["cin"] = L.cout, L.taps, L.cin
-                    e["d"], e["ld_d"], e["d_fmt"] = self.w_d[i].data_ptr(), self.w_d[i].shape[1], self.grad_fmt
+                e["cout"], e["taps"], e["cin"] = L.cout, L.taps, L.cin
+                e["d"], e["ld_d"], e["d_fmt"] = self.w_d[i].data_ptr(), self.w_d[i].shape[1], _lib.FMT_F16
                 e["f_hi"], e["f_lo"], e["ld_f"] = self.w_hi[i].data_ptr(), self.w_lo[i].data_ptr(), self.w_hi[i].shape[1]
             nb = int(lib.ssp_sgd_segment_blocks(int(e["cout"]), int(e["taps"]), int(e["cin"]), n))
             blocks.append((b0, nb))
@@ -374,15 +348,12 @@ class Engine:
             return
         s = stream_ptr()
         for L, (conv, _) in zip(self.layers, self.conv_modules()):
+            if L.first:
+                continue
             i = L.index
             off, n, _g = self._slices[id(conv.weight)]
-            w = self.flat_params[off:off + n]
-            if L.first:    # [32][9][3] -> K = 27 (+5 zeros): a 1-tap GEMM over the im2col'ed input
-                call(self.pack_fn, ptr(w), L.cout, 1, 27, ptr(self.w_hi[i]), ptr(self.w_lo[i]), self.w_hi[i].shape[1],
-                     None, 0, 0, s)
-            else:
-                call(self.pack_fn, ptr(w), L.cout, L.taps, L.cin, ptr(self.w_hi[i]), ptr(self.w_lo[i]), self.w_hi[i].shape[1],
-                     ptr(self.w_d[i]), self.w_d[i].shape[1], self.grad_fmt, s)
+            call("ssp_pack_weights", ptr(self.flat_params[off:off + n]), L.cout, L.taps, L.cin, ptr(self.w_hi[i]), ptr(self.w_lo[i]),
+                 self.w_hi[i].shape[1], ptr(self.w_d[i]), self.w_d[i].shape[1], _lib.FMT_F16, s)
             self.launches += 1
         self._weights_version = ver
 
@@ -398,36 +369,36 @@ class Engine:
 
     def _fuse_eval_layer(self, L):
         """inference layers whose BN + leaky run in the GEMM epilogue (ssp_conv_gemm_bnact)"""
-        return (L.bn and self.fuse_eval and not L.first and self.conv_impl != _lib.IMPL_SIMT and len(L.dests) == 1
-                and L.dests[0][2] == _lib.ROUTE_DIRECT and L.cout % 32 == 0)
+        return (L.bn and self.fuse_eval and not L.first and len(L.dests) == 1 and L.dests[0][2] == _lib.ROUTE_DIRECT
+                and L.cout % 32 == 0)
 
     def split_count(self, L, N, H, W):
         """split-K count of an inference forward of layer L on an N x 3 x H x W input: 0 = the layer keeps its kernels.  Only BN
         layers whose forward runs on the per-tap tensor-core kernel are split; the rule is ssp_conv_splitk_count's."""
         if not L.bn or L.first or self.split_override == 0:
             return 0
-        if not (self._fuse_eval_layer(L) or self._conv_impl(L.cout, L.k_taps, 1 if self.fast else 3) in (_lib.IMPL_TC, _lib.IMPL_TC2)):
+        if not (self._fuse_eval_layer(L) or self._conv_impl(L) in (_lib.IMPL_TC, _lib.IMPL_TC2)):
             return 0
         h, w = self.spatial(L, H, W)
         if self.split_override is not None:
-            return min(int(self.split_override), L.k_taps * ((L.k_cin + 63) // 64))
+            return min(int(self.split_override), L.taps * ((L.cin + 63) // 64))
         if self._num_sms is None:
             self._num_sms = torch.cuda.get_device_properties(self.device).multi_processor_count
-        s = int(_lib.load().ssp_conv_splitk_count(N, h, w, L.k_taps, L.k_cin, L.cout, self._num_sms))
+        s = int(_lib.load().ssp_conv_splitk_count(N, h, w, L.taps, L.cin, L.cout, self._num_sms))
         if s < 0:
             raise _lib.SspError("ssp_conv_splitk_count failed: %s" % _lib.load().ssp_last_error().decode())
         return s if s >= 2 else 0
 
-    def _conv_impl(self, n_out, taps=1, terms=3):
-        if self.conv_impl >= 0:
-            return self.conv_impl
-        # few output channels: operands swapped (weights on the M side, 128 / 256 pixels as the MMA's N; csrc/conv_bandt.cu).
-        # The ABI falls back to the kernels below by itself when the layer's weights do not fit next to two activation bands.
-        if self.use_bandt and n_out <= (64 if terms == 3 else 128):
+    def _conv_impl(self, L):
+        """forward kernel of a GEMM layer.  Few output channels: operands swapped (weights on the M side, 128 / 256 pixels as the MMA's
+        N; csrc/conv_bandt.cu); the ABI falls back to the kernels below by itself when the layer's weights do not fit next to two
+        activation bands.  From 128 output channels the per-tap kernel (SSP_IMPL_TC2 = SSP_IMPL_TC on sm_90a), else the
+        activation-band kernel for 3x3 layers."""
+        if L.cout <= (128 if self.fast else 64):
             return _lib.IMPL_BANDT
-        if n_out >= self.tc2_min_n:
+        if L.cout >= 128:
             return _lib.IMPL_TC2
-        return _lib.IMPL_BAND if (taps == 9 and self.use_band) else _lib.IMPL_TC
+        return _lib.IMPL_BAND if L.taps == 9 else _lib.IMPL_TC
 
     def _gemm(self, kind, L, N, h, w, name, *args, stream=None):
         """launch one GEMM-shaped kernel; optionally bracket it with CUDA events on the launching stream (bench roofline)."""
@@ -441,12 +412,24 @@ class Engine:
         e1.record(stream)
         self.profile.append((kind, L.block_ind, 2.0 * N * h * w * L.cout * L.cin * L.taps, e0, e1))
 
-    def _conv_fwd(self, L, B, N, h, w, xin, a_lo, b_lo, epi, bias, st, s):
-        i = L.index
-        self._gemm("fwd", L, N, h, w, "ssp_conv_gemm", self._conv_impl(L.cout, L.k_taps, 1 if self.fast else 3), ptr(xin), a_lo, B.rows[i], xin.shape[1], L.k_cin,
-                   ptr(self.w_hi[i]), b_lo, L.cout, self.w_hi[i].shape[1], _lib.FMT_F16, _lib.FMT_F16,
-                   N, h, w, L.k_taps, L.cout, ptr(B.y[i]), B.y[i].shape[1], B.rows[i], epi, bias,
-                   ptr(st["ssum"]), ptr(st["ssq"]), s)
+    def _bn_finalize(self, bn, st, C, s, count=None, train=False):
+        """mean / invstd and the folded scale / shift of one BatchNorm into `st`: from the running statistics when count is None
+        (inference), else from the batch sums over `count` values when `train` (which also updates the running statistics)"""
+        if count is None:
+            sums, count, momentum = (None, None), 1.0, 0.1
+        else:
+            sums, momentum = (ptr(st["ssum"]), ptr(st["ssq"])), bn.momentum if bn.momentum is not None else 0.1
+        call("ssp_bn_finalize", *sums, float(count), ptr(bn.weight.data), ptr(bn.bias.data), ptr(bn.running_mean), ptr(bn.running_var),
+             float(momentum), float(bn.eps), 1 if train else 0, ptr(st["mean"]), ptr(st["invstd"]), ptr(st["scale"]), ptr(st["shift"]), C, s)
+        self.launches += 1
+
+    @staticmethod
+    def _dests(B, L):
+        """the two destination slots (hi, lo, ld, channel offset, route) of ssp_bn_apply / ssp_bn_apply_splitk for layer L"""
+        d = []
+        for (ci, c0, kind) in L.dests:
+            d += [ptr(B.x_hi[ci]), ptr(B.x_lo[ci]), B.x_hi[ci].shape[1], c0, kind]
+        return d + [None, None, 0, 0, _lib.ROUTE_NONE] * (2 - len(L.dests))
 
     # ------------------------------------------------------------------ forward
     def forward(self, x, train_bn, keep_for_backward, split_k=False, buffers=None):
@@ -472,57 +455,14 @@ class Engine:
         B.generation += 1
         s = stream_ptr()
         mods = self.conv_modules()
-        direct0 = self.conv_impl != _lib.IMPL_SIMT and not self.fast and self.l0_mode in ("direct", "fused")
-        B.x_image = x if self.l0_fused else None   # the layer-0 backward reads the image again (kept alive with the activations)
-        if self.l0_fused:
-            pass
-        elif not direct0 or keep_for_backward:     # the im2col'ed plane feeds the tensor-core GEMMs (forward unless direct, wgrad always)
-            call("ssp_pack_input_im2col", ptr(x), ptr(B.x_hi[0]), None if direct0 else ptr(B.x_lo[0]), N, H, W, s)
-            self.launches += 1
+        B.x_image = x                               # the layer-0 backward reads the image again (kept alive with the activations)
         for L in self.layers:
             i = L.index
             conv, bn = mods[i]
             h, w = self.spatial(L, H, W)
             st = B.stat[i]
-            a_lo = None if self.fast else ptr(B.x_lo[i])
-            b_lo = None if self.fast else ptr(self.w_lo[i])
-            xin = B.x_hi[i]
-            if L.bn:
-                epi = _lib.EPI_STATS if train_bn else _lib.EPI_F32
-                bias = None
-            else:
-                epi, bias = _lib.EPI_BIAS, ptr(conv.bias.data)
-            S = B.splits[i]
-            if S:
-                # split-K inference: S partial GEMMs over slices of K into the workspace, then BN(running stats) + leaky + routing
-                # from their sum, in a fixed order (csrc/conv_tc.cu SPLIT, csrc/elementwise.cu bn_apply_kernel SPLIT)
-                call("ssp_bn_finalize", None, None, 1.0, ptr(bn.weight.data), ptr(bn.bias.data), ptr(bn.running_mean), ptr(bn.running_var),
-                     0.1, float(bn.eps), 0, ptr(st["mean"]), ptr(st["invstd"]), ptr(st["scale"]), ptr(st["shift"]), L.cout, s)
-                ws, slab, ld = ptr(B.split_ws), B.split_slab[i], B.split_ld[i]
-                self._gemm("fwd", L, N, h, w, "ssp_conv_gemm_splitk", ptr(xin), a_lo, B.rows[i], xin.shape[1], L.k_cin, ptr(self.w_hi[i]), b_lo,
-                           L.cout, self.w_hi[i].shape[1], N, h, w, L.k_taps, L.cout, S, ws, slab, ld, s)
-                d = []
-                for (ci, c0, kind) in L.dests:
-                    d += [ptr(B.x_hi[ci]), ptr(B.x_lo[ci]), B.x_hi[ci].shape[1], c0, kind]
-                if len(L.dests) == 1:
-                    d += [None, None, 0, 0, _lib.ROUTE_NONE]
-                call("ssp_bn_apply_splitk", ws, S, slab, ld, ptr(st["scale"]), ptr(st["shift"]), N, L.cout, h, w, L.slope, *d, s)
-                self.launches += 2
-                self.split_launches += 1
-                continue
-            fuse = not train_bn and not keep_for_backward and self._fuse_eval_layer(L)
-            if fuse:
-                # inference: BN(running stats) + LeakyReLU folded into the GEMM epilogue, which writes the consumer's operand
-                # planes directly -- no fp32 Y, no bn_apply pass (reference: conv, bn, leaky as three modules, darknet.py:154-164)
-                call("ssp_bn_finalize", None, None, 1.0, ptr(bn.weight.data), ptr(bn.bias.data), ptr(bn.running_mean), ptr(bn.running_var),
-                     0.1, float(bn.eps), 0, ptr(st["mean"]), ptr(st["invstd"]), ptr(st["scale"]), ptr(st["shift"]), L.cout, s)
-                ci, c0, _k = L.dests[0]
-                self._gemm("fwd", L, N, h, w, "ssp_conv_gemm_bnact", self.conv_impl if self.conv_impl >= 0 else (_lib.IMPL_TC2 if L.cout >= self.tc2_min_n else _lib.IMPL_TC), ptr(xin), a_lo, B.rows[i], xin.shape[1],
-                           L.k_cin, ptr(self.w_hi[i]), b_lo, L.cout, self.w_hi[i].shape[1], N, h, w, L.k_taps, L.cout,
-                           ptr(st["scale"]), ptr(st["shift"]), L.slope, ptr(B.x_hi[ci]), ptr(B.x_lo[ci]), B.x_hi[ci].shape[1], c0, s)
-                self.launches += 1          # bn_finalize (the GEMM is counted by _gemm)
-                continue
-            if L.first and self.l0_fused:
+            if L.first:
+                # blocks 0-1 (conv + BN + leaky + 2x2 max-pool) as one unit from the raw image and the fp32 master weights
                 off, n, _gv = self._slices[id(conv.weight)]
                 w0 = ptr(self.flat_params[off:off + n])
                 if train_bn or keep_for_backward:      # the Gram matrix of the image patches: batch statistics without a pass over y, and
@@ -531,36 +471,51 @@ class Engine:
                 if train_bn:
                     call("ssp_l0_stats", ptr(B.l0_gram), w0, ptr(st["ssum"]), ptr(st["ssq"]), s)
                     self.launches += 1
-                call("ssp_bn_finalize", ptr(st["ssum"]) if train_bn else None, ptr(st["ssq"]) if train_bn else None, float(N * h * w),
-                     ptr(bn.weight.data), ptr(bn.bias.data), ptr(bn.running_mean), ptr(bn.running_var),
-                     float(bn.momentum if bn.momentum is not None else 0.1), float(bn.eps), 1 if train_bn else 0,
-                     ptr(st["mean"]), ptr(st["invstd"]), ptr(st["scale"]), ptr(st["shift"]), L.cout, s)
+                self._bn_finalize(bn, st, L.cout, s, N * h * w, train_bn)
                 ci, c0, _k = L.dests[0]
                 call("ssp_l0_fused_fwd", ptr(x), w0, ptr(st["scale"]), ptr(st["shift"]), L.slope, N, H, W, ptr(B.x_hi[ci]), ptr(B.x_lo[ci]),
                      B.x_hi[ci].shape[1], c0, ptr(B.l0_code) if keep_for_backward else None, s)
-                self.launches += 2
-                continue
-            if L.first and direct0 and L.bn:       # exact fp32 direct convolution of the raw image (HBM-bound layer)
-                off, n, _gv = self._slices[id(conv.weight)]
-                call("ssp_conv0_direct", ptr(x), ptr(self.flat_params[off:off + n]), None, ptr(B.y[i]), B.y[i].shape[1],
-                     ptr(st["ssum"]) if train_bn else None, ptr(st["ssq"]) if train_bn else None, N, H, W, s)
                 self.launches += 1
+                continue
+            xin = B.x_hi[i]
+            a_lo = None if self.fast else ptr(B.x_lo[i])
+            b_lo = None if self.fast else ptr(self.w_lo[i])
+            S = B.splits[i]
+            if S:
+                # split-K inference: S partial GEMMs over slices of K into the workspace, then BN(running stats) + leaky + routing
+                # from their sum, in a fixed order (csrc/conv_tc.cu SPLIT, csrc/elementwise.cu bn_apply_kernel SPLIT)
+                self._bn_finalize(bn, st, L.cout, s)
+                ws, slab, ld = ptr(B.split_ws), B.split_slab[i], B.split_ld[i]
+                self._gemm("fwd", L, N, h, w, "ssp_conv_gemm_splitk", ptr(xin), a_lo, B.rows[i], xin.shape[1], L.cin, ptr(self.w_hi[i]), b_lo,
+                           L.cout, self.w_hi[i].shape[1], N, h, w, L.taps, L.cout, S, ws, slab, ld, s)
+                call("ssp_bn_apply_splitk", ws, S, slab, ld, ptr(st["scale"]), ptr(st["shift"]), N, L.cout, h, w, L.slope, *self._dests(B, L), s)
+                self.launches += 1
+                self.split_launches += 1
+                continue
+            if not train_bn and not keep_for_backward and self._fuse_eval_layer(L):
+                # inference: BN(running stats) + LeakyReLU folded into the GEMM epilogue, which writes the consumer's operand
+                # planes directly -- no fp32 Y, no bn_apply pass (reference: conv, bn, leaky as three modules, darknet.py:154-164)
+                self._bn_finalize(bn, st, L.cout, s)
+                ci, c0, _k = L.dests[0]
+                self._gemm("fwd", L, N, h, w, "ssp_conv_gemm_bnact", _lib.IMPL_TC2 if L.cout >= 128 else _lib.IMPL_TC, ptr(xin), a_lo,
+                           B.rows[i], xin.shape[1], L.cin, ptr(self.w_hi[i]), b_lo, L.cout, self.w_hi[i].shape[1], N, h, w, L.taps, L.cout,
+                           ptr(st["scale"]), ptr(st["shift"]), L.slope, ptr(B.x_hi[ci]), ptr(B.x_lo[ci]), B.x_hi[ci].shape[1], c0, s)
+                continue
+            if L.bn:
+                epi, bias = (_lib.EPI_STATS if train_bn else _lib.EPI_F32), None
             else:
-                self._conv_fwd(L, B, N, h, w, xin, a_lo, b_lo, epi, bias, st, s)
+                epi, bias = _lib.EPI_BIAS, ptr(conv.bias.data)
+            self._gemm("fwd", L, N, h, w, "ssp_conv_gemm", self._conv_impl(L), ptr(xin), a_lo, B.rows[i], xin.shape[1], L.cin,
+                       ptr(self.w_hi[i]), b_lo, L.cout, self.w_hi[i].shape[1], _lib.FMT_F16, _lib.FMT_F16,
+                       N, h, w, L.taps, L.cout, ptr(B.y[i]), B.y[i].shape[1], B.rows[i], epi, bias,
+                       ptr(st["ssum"]), ptr(st["ssq"]), s)
             if not L.bn:
                 continue
-            call("ssp_bn_finalize", ptr(st["ssum"]), ptr(st["ssq"]), float(N * h * w), ptr(bn.weight.data), ptr(bn.bias.data),
-                 ptr(bn.running_mean), ptr(bn.running_var), float(bn.momentum if bn.momentum is not None else 0.1), float(bn.eps),
-                 1 if train_bn else 0, ptr(st["mean"]), ptr(st["invstd"]), ptr(st["scale"]), ptr(st["shift"]), L.cout, s)
-            d = []
-            for (ci, c0, kind) in L.dests:
-                d += [ptr(B.x_hi[ci]), ptr(B.x_lo[ci]), B.x_hi[ci].shape[1], c0, kind]
-            if len(L.dests) == 1:
-                d += [None, None, 0, 0, _lib.ROUTE_NONE]
+            self._bn_finalize(bn, st, L.cout, s, N * h * w, train_bn)
             yp = B.ypool[i] if keep_for_backward else None
-            call("ssp_bn_apply", ptr(B.y[i]), B.y[i].shape[1], ptr(st["scale"]), ptr(st["shift"]), N, L.cout, h, w, L.slope, *d,
+            call("ssp_bn_apply", ptr(B.y[i]), B.y[i].shape[1], ptr(st["scale"]), ptr(st["shift"]), N, L.cout, h, w, L.slope, *self._dests(B, L),
                  ptr(yp), yp.shape[1] if yp is not None else 0, s)
-            self.launches += 2
+            self.launches += 1
         last = self.layers[-1]
         h, w = self.spatial(last, H, W)
         out = torch.empty(N, last.cout, h, w, dtype=torch.float32, device=x.device)
@@ -580,7 +535,7 @@ class Engine:
         g = grad_out.contiguous().float()
         # Weight-gradient GEMMs (tensor/L2 bound) run on a side stream so that they overlap the HBM-bound BN-backward
         # kernels of the next layer on the main stream; joined before returning.  Serial when per-launch profiling is on.
-        overlap = self.overlap and self.profile is None
+        overlap = self.profile is None
         main = torch.cuda.current_stream()
         if overlap:
             if self._side is None or self._side.device != main.device:
@@ -596,8 +551,7 @@ class Engine:
             conv, bn = mods[i]
             h, w = self.spatial(L, H, W)
             st = B.stat[i]
-            dy = B.dy[i]
-            if L.first and self.l0_fused:
+            if L.first:
                 # dW0 / dgamma / dbeta from the pooled gradient, the arg-max codes and the image (csrc/l0_fused.cu); runs where the
                 # weight gradients run, after the data gradient of layer 1 (the last kernel of the main stream)
                 ci, c0, _k = L.dests[0]
@@ -606,7 +560,7 @@ class Engine:
                     ev = torch.cuda.Event()
                     ev.record(main)
                     side.wait_event(ev)
-                self._gemm("l0_bwd", L, N, h, w, "ssp_l0_bwd", ptr(B.x_image), ptr(B.dx[ci]), 1 if self.dx_f16 else 0, B.dx[ci].shape[1], c0, ptr(B.l0_code), L.slope,
+                self._gemm("l0_bwd", L, N, h, w, "ssp_l0_bwd", ptr(B.x_image), ptr(B.dx[ci]), 1, B.dx[ci].shape[1], c0, ptr(B.l0_code), L.slope,
                            N, H, W, ptr(B.l0_t1), ws, stream=wstream)
                 call("ssp_l0_bwd_finalize", ptr(B.l0_t1), ptr(B.l0_gram), ptr(self.flat_params[off:off + n]), ptr(bn.weight.data),
                      ptr(st["mean"]), ptr(st["invstd"]), float(N * h * w), inv, ptr(self.flat_grads[off:off + n]),
@@ -615,9 +569,10 @@ class Engine:
                 if self.grad_ready_hook is not None:
                     self.grad_ready_hook(i, side if overlap else main)
                 continue
+            dy = B.dy[i]
             if L.bn:
                 srcs = []
-                f16 = _lib.ROUTE_F16 if self.dx_f16 else 0
+                f16 = _lib.ROUTE_F16
                 for (ci, c0, kind) in L.dests:
                     srcs += [ptr(B.dx[ci]), B.dx[ci].shape[1], c0, kind | f16]
                 if len(L.dests) == 1:
@@ -638,15 +593,15 @@ class Engine:
                             call("ssp_bn_bwd_reduce", *head, N, L.cout, h, w, L.slope, ptr(B.dx[ci]), B.dx[ci].shape[1], c0, kind | f16,
                                  None, 0, 0, _lib.ROUTE_NONE, ptr(st["s1"]), ptr(st["s2"]), s)
                         self.launches += 1
-                    self.launches -= 1
                 else:
                     call("ssp_bn_bwd_reduce", *common, s)
-                call("ssp_bn_bwd_apply", *common, ptr(dy), dy.shape[1], self.grad_fmt, 1.0, s)
+                    self.launches += 1
+                call("ssp_bn_bwd_apply", *common, ptr(dy), dy.shape[1], _lib.FMT_F16, 1.0, s)
                 call("ssp_bn_bwd_finalize", ptr(st["s1"]), ptr(st["s2"]), ptr(self.grad_view(bn.weight)), ptr(self.grad_view(bn.bias)),
                      L.cout, 0, inv, s)
-                self.launches += 3
+                self.launches += 2
             else:
-                call("ssp_pack_nchw", ptr(g), ptr(dy), None, N, L.cout, h, w, dy.shape[1], 0, self.grad_fmt, self.grad_scale, s)
+                call("ssp_pack_nchw", ptr(g), ptr(dy), None, N, L.cout, h, w, dy.shape[1], 0, _lib.FMT_F16, self.grad_scale, s)
                 call("ssp_bias_grad_nchw", ptr(g), ptr(self.grad_view(conv.bias)), N, L.cout, h * w, 0, 1.0, s)
                 self.launches += 2
             off, n, _gv = self._slices[id(conv.weight)]
@@ -655,22 +610,17 @@ class Engine:
             if overlap:
                 ev = torch.cuda.Event()
                 ev.record(main)                      # dY of this layer is complete
-            if not L.first:                          # data gradient first: it is on the critical path of the next layer
-                wd = self.w_d[i]
-                dimpl = self._conv_impl(L.cin, L.taps, 1)
-                if self.dx_f16 and dimpl not in (_lib.IMPL_BANDT, _lib.IMPL_TC2):
-                    dimpl = _lib.IMPL_TC2          # the kernels that have the fp16 epilogue
-                self._gemm("dgrad", L, N, h, w, "ssp_conv_gemm", dimpl, ptr(dy), None, B.rows[i], dy.shape[1], L.cout,
-                           ptr(wd), None, L.cin, wd.shape[1], self.grad_fmt, self.grad_fmt, N, h, w, L.taps, L.cin, ptr(B.dx[i]),
-                           B.dx[i].shape[1], B.rows[i], _lib.EPI_F16 if self.dx_f16 else _lib.EPI_F32, None, None, None, s)
+            # data gradient first: it is on the critical path of the next layer.  The fp16 dX planes need a kernel with the fp16
+            # epilogue: the operand-swapped one where the layer is narrow enough, else the per-tap kernel.
+            wd = self.w_d[i]
+            dimpl = _lib.IMPL_BANDT if L.cin <= 128 else _lib.IMPL_TC2
+            self._gemm("dgrad", L, N, h, w, "ssp_conv_gemm", dimpl, ptr(dy), None, B.rows[i], dy.shape[1], L.cout,
+                       ptr(wd), None, L.cin, wd.shape[1], _lib.FMT_F16, _lib.FMT_F16, N, h, w, L.taps, L.cin, ptr(B.dx[i]),
+                       B.dx[i].shape[1], B.rows[i], _lib.EPI_F16, None, None, None, s)
             if overlap:
                 side.wait_event(ev)
-            if L.first:
-                self._gemm("wgrad", L, N, h, w, "ssp_wgrad_gemm", self.wgrad_impl, ptr(dy), B.rows[i], dy.shape[1], L.cout, self.grad_fmt,
-                           ptr(xh), B.rows[i], xh.shape[1], 32, self.grad_fmt, N, h, w, 1, ptr(dw), 27, 27, inv, ws, stream=wstream)
-            else:
-                self._gemm("wgrad", L, N, h, w, "ssp_wgrad_gemm", self.wgrad_impl, ptr(dy), B.rows[i], dy.shape[1], L.cout, self.grad_fmt,
-                           ptr(xh), B.rows[i], xh.shape[1], L.cin, self.grad_fmt, N, h, w, L.taps, ptr(dw), L.cin, L.cin, inv, ws, stream=wstream)
+            self._gemm("wgrad", L, N, h, w, "ssp_wgrad_gemm", _lib.IMPL_TC2, ptr(dy), B.rows[i], dy.shape[1], L.cout, _lib.FMT_F16,
+                       ptr(xh), B.rows[i], xh.shape[1], L.cin, _lib.FMT_F16, N, h, w, L.taps, ptr(dw), L.cin, L.cin, inv, ws, stream=wstream)
             if self.grad_ready_hook is not None:
                 # the weight-gradient stream has waited for this layer's dY event, i.e. for every main-stream gradient write
                 # (dgamma / dbeta / dbias) of the layers >= i as well

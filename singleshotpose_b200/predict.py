@@ -176,7 +176,7 @@ class _FramePredictor:
     def _weights_sig(self):
         eng = self.eng
         stats = tuple(t.data_ptr() for _c, bn in eng.conv_modules() if bn is not None for t in (bn.running_mean, bn.running_var))
-        return (eng.flat_params.data_ptr(), tuple(t.data_ptr() for t in eng.w_hi + eng.w_lo)) + stats
+        return (eng.flat_params.data_ptr(), tuple(t.data_ptr() for t in eng.w_hi + eng.w_lo if t is not None)) + stats
 
     def _ensure_current(self):
         eng = self.eng

@@ -402,28 +402,6 @@ def test_library_reports_errors():
         call("ssp_pnp_batched", None, 1, None, None, 9, 1, 20, None, None, None, stream_ptr())
 
 
-@pytest.mark.parametrize("shape", [(2, 32, 40), (1, 13, 7), (3, 64, 64)])
-def test_conv0_direct_matches_torch(shape):
-    N, H, W = shape
-    g = torch.Generator().manual_seed(17)
-    x = torch.rand(N, 3, H, W, generator=g)
-    w = torch.randn(32, 3, 3, 3, generator=g) * 0.2
-    ref = F.conv2d(x.double(), w.double(), padding=1).float()
-    rows = _lib.flat_alloc_rows(N, H, W)
-    y = torch.zeros(rows, 32, device=DEV)
-    ssum = torch.zeros(32, dtype=torch.float64, device=DEV); ssq = torch.zeros_like(ssum)
-    wm = w.permute(0, 2, 3, 1).contiguous().to(DEV)                      # master layout [co][kh][kw][ci]
-    call("ssp_conv0_direct", ptr(x.to(DEV)), ptr(wm), None, ptr(y), 32, ptr(ssum), ptr(ssq), N, H, W, stream_ptr())
-    torch.cuda.synchronize()
-    out = nchw_from_flat(y, N, 32, H, W).cpu()
-    assert (out - ref).abs().max() / ref.abs().max() < 2e-6
-    assert (ssum.cpu() - ref.double().sum(dim=(0, 2, 3))).abs().max() < 1e-3
-    assert ((ssq.cpu() - (ref.double() ** 2).sum(dim=(0, 2, 3))).abs() / (ref.double() ** 2).sum(dim=(0, 2, 3))).max() < 1e-5
-    idx = torch_flat_index(N, H, W)
-    mask = torch.ones(rows, dtype=torch.bool); mask[idx] = False
-    assert float(y.cpu()[mask].abs().max()) == 0.0                       # pad rows untouched
-
-
 @pytest.mark.parametrize("shape", [(2, 32, 64), (1, 48, 80), (3, 16, 32), (2, 34, 70)])
 def test_l0_fused_blocks_match_torch(shape):
     """blocks 0-1 as one unit (csrc/l0_fused.cu: conv 3->32 + BatchNorm(batch statistics) + LeakyReLU + MaxPool 2x2, darknet.py:154-167)

@@ -116,6 +116,40 @@ def test_eval_fused_epilogue_matches_unfused(cfg_path):
         assert torch.isfinite(o_f).all() and _rel(o_f, o_u) < 2e-5
 
 
+def test_fast_precision_trains_and_evaluates(cfg_path, monkeypatch, capsys):
+    """SSP_PRECISION=fast: the forward GEMMs run one fp16 pass instead of three (blocks 0-1 stay the exact fused unit; the next
+    layer reads only its hi plane).  No 1e-3 parity -- DESIGN section 2 emulates a single fp16 pass at 3.3e-2 -- but a training
+    forward + backward + FlatSGD step and an eval forward must stay finite and within 1e-1 of the CPU oracle."""
+    monkeypatch.setenv("SSP_PRECISION", "fast")
+    torch.manual_seed(0)
+    ref = RefDarknet(cfg_path).train()
+    torch.manual_seed(0)
+    dut = Darknet(cfg_path).cuda().train()
+    assert dut._engine.fast
+    x, tgt = synth.images(2, seed=0), synth.targets(2, seed=1)
+    crit = RegionLoss(); crit.verbose = False
+    opt = FlatSGD(dut, lr=1e-4, momentum=0.9, weight_decay=0.0005)
+    with torch.no_grad():
+        o_ref = ref(x)
+    opt.zero_grad()
+    o = dut(x.cuda())
+    crit(o, tgt, 20).backward()
+    assert all(torch.isfinite(p.grad).all() for p in dut.parameters())
+    opt.step()
+    assert all(torch.isfinite(p).all() for p in dut.parameters())
+    e_train = _rel(o.detach().cpu(), o_ref)
+    ref.load_state_dict({k: v.cpu() for k, v in dut.state_dict().items()})     # the stepped weights and the running statistics
+    ref.eval(); dut.eval()
+    with torch.no_grad():
+        o_ref = ref(x)
+        o = dut(x.cuda())
+    assert torch.isfinite(o).all()
+    e_eval = _rel(o.cpu(), o_ref)
+    with capsys.disabled():
+        print("\nSSP_PRECISION=fast logits rel err vs oracle: train %.2e, eval %.2e" % (e_train, e_eval))
+    assert e_train < 1e-1 and e_eval < 1e-1, (e_train, e_eval)
+
+
 @pytest.mark.parametrize("hw", [(352, 480), (224, 224), (672, 672)])
 def test_other_resolutions_match_reference_golden(cfg_path, golden_dir, hw):
     """multi-resolution training shapes (dataset.py:66-90) and the 672^2 test shape: train-mode logits, batch 1, vs the reference"""

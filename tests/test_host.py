@@ -33,7 +33,7 @@ def test_cfg_parse_semantics(cfg_path, cfg_multi_path, capsys):
     assert "   28 route  27 24" in out
 
 
-def test_execution_plan(cfg_path):
+def test_execution_plan_with_fused_first_blocks(cfg_path):
     layers = build_plan(parse_cfg(cfg_path))
     assert len(layers) == 23
     l16 = [L for L in layers if L.block_ind == 16][0]
@@ -41,7 +41,9 @@ def test_execution_plan(cfg_path):
     l29 = [L for L in layers if L.block_ind == 29][0]
     assert l29.cin == 1280
     assert [(layers[s].block_ind, k, c0, c) for (s, k, c0, c) in l29.leaves] == [(26, _lib.ROUTE_REORG, 0, 256), (24, _lib.ROUTE_DIRECT, 256, 1024)]
-    assert layers[0].first and layers[0].k_cin == 32 and layers[0].k_taps == 1
+    assert layers[0].first and not any(L.first for L in layers[1:])                 # blocks 0-1: conv 3 -> 32 + BN + leaky, maxpool 2/2
+    assert (layers[0].cin, layers[0].cout, layers[0].taps, layers[0].bn) == (3, 32, 9, True)
+    assert layers[0].dests == [(1, 0, _lib.ROUTE_POOL)]
     assert not layers[-1].bn and layers[-1].cout == 20
 
 
@@ -50,6 +52,17 @@ def test_unsupported_blocks_raise(tmp_path):
     p = tmp_path / "bad.cfg"
     p.write_text(txt)
     with pytest.raises(NotImplementedError):
+        Darknet(str(p))
+
+
+def test_first_conv_without_maxpool_raises(tmp_path):
+    """blocks 0-1 run as one fused unit (conv 3 -> 32 + BN + leaky + max-pool 2/2): a first conv that feeds another conv is refused"""
+    conv = "[convolutional]\nbatch_normalize=1\nfilters=32\nsize=1\nstride=1\npad=1\nactivation=leaky\n"
+    txt = yolo_pose_cfg_text().replace("[maxpool]\nsize=2\nstride=2\n", conv, 1)
+    assert txt != yolo_pose_cfg_text()
+    p = tmp_path / "bad.cfg"
+    p.write_text(txt)
+    with pytest.raises(NotImplementedError, match="blocks 0-1"):
         Darknet(str(p))
 
 

@@ -76,19 +76,19 @@ def _rule(N, h, w, L):
     """the split rule restated from the tile geometry: 128-row tiles of N(h+1)(w+1) rows x N tiles of 32 / 64 / 128 channels"""
     bn = 128 if L.cout > 64 else (L.cout + 31) // 32 * 32
     tiles = -(-N * (h + 1) * (w + 1) // 128) * -(-L.cout // bn)
-    kb = L.k_taps * -(-L.k_cin // 64)
+    kb = L.taps * -(-L.cin // 64)
     s = min(H100_SMS // tiles, kb // 8)
     return s if s >= 2 else 1
 
 
 @pytest.mark.parametrize("size", [416, 672])
 @pytest.mark.parametrize("N", [1, 8, 64])
-def test_splitk_count_follows_the_tile_table(cfg_path, N, size):
+def test_splitk_count_of_gemm_layers_follows_the_tile_table(cfg_path, N, size):
     lib = _lib.load()
     got = {}
-    for L in _layers(cfg_path):
+    for L in _layers(cfg_path)[1:]:                       # the GEMM layers (layer 0 is the fused unit of blocks 0-1)
         h, w = L.H * size // 416, L.W * size // 416
-        s = lib.ssp_conv_splitk_count(N, h, w, L.k_taps, L.k_cin, L.cout, H100_SMS)
+        s = lib.ssp_conv_splitk_count(N, h, w, L.taps, L.cin, L.cout, H100_SMS)
         assert s == _rule(N, h, w, L), (L.block_ind, N, size)
         got[L.block_ind] = s
     if N == 64:

@@ -255,7 +255,7 @@ def main():
         c["replay_device_ms"] = float(np.median(ts))
         # the forward alone against the floors
         x = pred.input.clone()
-        wbytes = sum(t.numel() * t.element_size() for t in eng.w_hi + eng.w_lo)
+        wbytes = sum(t.numel() * t.element_size() for t in eng.w_hi + eng.w_lo if t is not None)
         flops = 0.0
         for L in eng.layers:
             h, w = eng.spatial(L, size, size)
