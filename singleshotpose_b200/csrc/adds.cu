@@ -107,18 +107,24 @@ __global__ void diameter_finish_kernel(double* out) {
   *out = sqrt(__longlong_as_double((long long)*reinterpret_cast<const unsigned long long*>(out)));
 }
 
-long long adds_work_bytes(int nv, long long n) {
+}  // namespace ssp
+
+using namespace ssp;
+
+extern "C" {
+long long ssp_adds_work_bytes(int nv, long long n) {
   if (nv < 1 || nv > kMaxVertices || n < 0 || n > INT_MAX) return SSP_ERR_ARG;
   return 2LL * n * query_blocks(nv) * (long long)sizeof(double);
 }
 
-int adds_batched(const double* X, int nv, const double* Rt_est, const double* Rt_gt, long long n, double* adds_out, double* add_out,
-                 void* work, long long work_bytes, cudaStream_t s) {
+int ssp_adds_batched(const double* X, int nv, const double* Rt_est, const double* Rt_gt, long long n, double* adds_out, double* add_out,
+                     void* work, long long work_bytes, void* stream) {
+  const cudaStream_t s = (cudaStream_t)stream;
   if (!X || !Rt_est || !Rt_gt || !adds_out || !work || nv < 1 || n < 0)
     return fail_msg(SSP_ERR_ARG, "adds_batched: bad argument (null pointer, Nv < 1 or n < 0)");
   if (nv > kMaxVertices) return fail_msg(SSP_ERR_ARG, "adds_batched: more than SSP_ADDS_MAX_VERTICES vertices");
   if (n > INT_MAX) return fail_msg(SSP_ERR_ARG, "adds_batched: more than 2^31 - 1 pose pairs");
-  if (work_bytes < adds_work_bytes(nv, n)) return fail_msg(SSP_ERR_ARG, "adds_batched: work buffer smaller than ssp_adds_work_bytes()");
+  if (work_bytes < ssp_adds_work_bytes(nv, n)) return fail_msg(SSP_ERR_ARG, "adds_batched: work buffer smaller than ssp_adds_work_bytes()");
   if (n == 0) return SSP_OK;
   const int nblk = query_blocks(nv);
   double* sums_adds = static_cast<double*>(work);
@@ -130,7 +136,8 @@ int adds_batched(const double* X, int nv, const double* Rt_est, const double* Rt
   return SSP_OK;
 }
 
-int mesh_diameter(const double* X, int nv, double* out, cudaStream_t s) {
+int ssp_mesh_diameter(const double* X, int nv, double* out, void* stream) {
+  const cudaStream_t s = (cudaStream_t)stream;
   if (!X || !out || nv < 1) return fail_msg(SSP_ERR_ARG, "mesh_diameter: bad argument (null pointer or Nv < 1)");
   if (nv > kMaxVertices) return fail_msg(SSP_ERR_ARG, "mesh_diameter: more than SSP_ADDS_MAX_VERTICES vertices");
   const cudaError_t e = cudaMemsetAsync(out, 0, sizeof(double), s);          // +0.0: the identity of the max
@@ -142,5 +149,4 @@ int mesh_diameter(const double* X, int nv, double* out, cudaStream_t s) {
   SSP_CHECK_LAUNCH();
   return SSP_OK;
 }
-
-}  // namespace ssp
+}  // extern "C"

@@ -127,27 +127,8 @@ int driver_rc(int rc, const char* who) {
 }
 }  // namespace
 
-long long aug_resize_work_bytes(int in_w, int in_h, int out_w, int out_h, int resample) {
-  if (in_w <= 0 || in_h <= 0 || out_w <= 0 || out_h <= 0) return SSP_ERR_ARG;
-  return resize_work_bytes(in_w, in_h, out_w, out_h, resample);
-}
-long long aug_sample_work_bytes(int ow, int oh, int bw, int bh, int cw, int ch, int out_w, int out_h, int resample) {
-  if (ow <= 0 || oh <= 0 || bw <= 0 || bh <= 0 || cw <= 0 || ch <= 0 || out_w <= 0 || out_h <= 0) return SSP_ERR_ARG;
-  return augment_work_bytes(ow, oh, bw, bh, cw, ch, out_w, out_h, resample);
-}
-
-int aug_resize_u8(const uint8_t* src, int src_w, int src_h, int x0, int y0, int in_w, int in_h, uint8_t* dst, int out_w, int out_h,
-                  int resample, uint8_t* work, long long work_bytes, cudaStream_t s) {
-  if (!src || !dst || !work || src_w <= 0 || src_h <= 0) return fail_msg(SSP_ERR_ARG, "ssp_aug_resize_u8: null pointer or empty source");
-  if ((uintptr_t)work % 16) return fail_msg(SSP_ERR_ARG, "ssp_aug_resize_u8: work buffer must be 16-B aligned");
-  CudaBackend be{s};
-  const int rc = resize_u8_driver(be, src, src_w, src_h, x0, y0, in_w, in_h, dst, out_w, out_h, resample, work, work_bytes);
-  if (rc) return driver_rc(rc, "ssp_aug_resize_u8");
-  SSP_CHECK_LAUNCH();
-  return SSP_OK;
-}
-
-int aug_convert_u8(const uint8_t* src, uint8_t* dst, long long n_px, int mode, cudaStream_t s) {
+// ssp_aug_rgb2hsv_u8 (mode 1) and ssp_aug_hsv2rgb_u8 (mode 2)
+static int aug_convert_u8(const uint8_t* src, uint8_t* dst, long long n_px, int mode, cudaStream_t s) {
   if (!src || !dst || n_px < 0 || (mode != 1 && mode != 2)) return fail_msg(SSP_ERR_ARG, "ssp_aug_rgb2hsv_u8/hsv2rgb_u8: bad argument");
   if (n_px == 0) return SSP_OK;
   aug_distort_kernel<<<blocks_for(n_px, 256), 256, 0, s>>>(src, n_px, nullptr, mode, dst, nullptr);
@@ -155,55 +136,12 @@ int aug_convert_u8(const uint8_t* src, uint8_t* dst, long long n_px, int mode, c
   return SSP_OK;
 }
 
-int aug_to_tensor_u8(const uint8_t* src, long long n_px, float* out_chw, cudaStream_t s) {
-  if (!src || !out_chw || n_px < 0) return fail_msg(SSP_ERR_ARG, "ssp_aug_to_tensor_u8: bad argument");
-  if (n_px == 0) return SSP_OK;
-  aug_to_tensor_kernel<<<blocks_for(n_px, 256), 256, 0, s>>>(src, n_px, out_chw);
-  SSP_CHECK_LAUNCH();
-  return SSP_OK;
-}
-
-long long aug_batch_table_bytes(int n) { return n > 0 ? (long long)kMaxStages * n * (long long)sizeof(AugOp) : SSP_ERR_ARG; }
-
-// host side of the batched path: items (device pointers, host array) -> op table (host memory, to be copied to the device with the
-// batch) + per-stage launch extents
-int aug_batch_plan(const ssp_aug_item* items, int n, int out_w, int out_h, int resample, void* table_host, long long table_bytes, int* stage_dims) {
-  static_assert(sizeof(ssp_aug_item) == sizeof(AugItem), "ssp_aug_item (include/ssp_b200.h) must mirror AugItem (augment_core.h)");
-  if (!items || !table_host || !stage_dims || n <= 0 || table_bytes < aug_batch_table_bytes(n)) return fail_msg(SSP_ERR_ARG, "ssp_aug_batch_plan: bad argument");
-  for (int i = 0; i < n; i++)
-    if (!items[i].img || !items[i].mask || !items[i].bg || !items[i].luts || !items[i].work || (!items[i].out_u8 && !items[i].out_chw) ||
-        ((uintptr_t)items[i].work % 16))
-      return fail_msg(SSP_ERR_ARG, "ssp_aug_batch_plan: null pointer or misaligned work buffer in an item");
-  const int rc = augment_batch_plan(reinterpret_cast<const AugItem*>(items), n, out_w, out_h, resample, (AugOp*)table_host, stage_dims);
-  if (rc) return driver_rc(rc, "ssp_aug_batch_plan");
-  return SSP_OK;
-}
-
-int aug_batch_run(const void* table_dev, int n, const int* stage_dims, cudaStream_t s) {
-  if (!table_dev || !stage_dims || n <= 0 || n > 65535) return fail_msg(SSP_ERR_ARG, "ssp_aug_batch_run: bad argument");
-  const AugOp* ops = (const AugOp*)table_dev;
-  for (int st = 0; st < kMaxStages; st++) {
-    const int nx = stage_dims[2 * st], ny = stage_dims[2 * st + 1];
-    if (nx <= 0 || ny <= 0) continue;
-    dim3 grid((nx + 31) / 32, (ny + 7) / 8, n);
-    aug_stage_kernel<<<grid, 256, 0, s>>>(ops + (long long)st * n);
-  }
-  SSP_CHECK_LAUNCH();
-  return SSP_OK;
-}
-
-// ---- multi-object pipeline: three planned phases over the same stage kernel
-long long augm_work_bytes(int in_w, int in_h, int out_w, int out_h, int resample) {
-  if (in_w <= 0 || in_h <= 0 || out_w <= 0 || out_h <= 0) return SSP_ERR_ARG;
-  return multi_work_bytes(in_w, in_h, out_w, out_h, resample);
-}
-long long augm_table_bytes(int n) { return n > 0 ? (long long)kMaxMultiStages * n * (long long)sizeof(AugOp) : SSP_ERR_ARG; }
-
-int augm_plan(int phase, const ssp_augm_item* items, int n, int out_w, int out_h, int resample, void* table_host, long long table_bytes,
-              int* stage_dims) {
+// ssp_augm_plan_begin / _attempt / _finish (phase MULTI_BEGIN / MULTI_ATTEMPT / MULTI_FINISH)
+static int augm_plan(int phase, const ssp_augm_item* items, int n, int out_w, int out_h, int resample, void* table_host, long long table_bytes,
+                     int* stage_dims) {
   static_assert(sizeof(ssp_augm_item) == sizeof(AugMultiItem), "ssp_augm_item (include/ssp_b200.h) must mirror AugMultiItem (augment_core.h)");
   static const char* who[3] = {"ssp_augm_plan_begin", "ssp_augm_plan_attempt", "ssp_augm_plan_finish"};
-  if (!items || !table_host || !stage_dims || n <= 0 || table_bytes < augm_table_bytes(n)) return fail_msg(SSP_ERR_ARG, "ssp_augm_plan_*: bad argument");
+  if (!items || !table_host || !stage_dims || n <= 0 || table_bytes < ssp_augm_table_bytes(n)) return fail_msg(SSP_ERR_ARG, "ssp_augm_plan_*: bad argument");
   for (int i = 0; i < n; i++) {
     const ssp_augm_item& it = items[i];
     const bool common = it.img && it.luts && it.work && it.main_img && it.main_mask && it.total_img && it.total_mask && (uintptr_t)it.work % 16 == 0;
@@ -217,30 +155,115 @@ int augm_plan(int phase, const ssp_augm_item* items, int n, int out_w, int out_h
   if (rc) return driver_rc(rc, who[phase]);
   return SSP_OK;
 }
+}  // namespace ssp
 
-int augm_run(const void* table_dev, int n, const int* stage_dims, cudaStream_t s) {
+using namespace ssp;
+
+extern "C" {
+long long ssp_aug_resize_work_bytes(int in_w, int in_h, int out_w, int out_h, int resample) {
+  if (in_w <= 0 || in_h <= 0 || out_w <= 0 || out_h <= 0) return SSP_ERR_ARG;
+  return resize_work_bytes(in_w, in_h, out_w, out_h, resample);
+}
+long long ssp_aug_sample_work_bytes(int ow, int oh, int bw, int bh, int cw, int ch, int out_w, int out_h, int resample) {
+  if (ow <= 0 || oh <= 0 || bw <= 0 || bh <= 0 || cw <= 0 || ch <= 0 || out_w <= 0 || out_h <= 0) return SSP_ERR_ARG;
+  return augment_work_bytes(ow, oh, bw, bh, cw, ch, out_w, out_h, resample);
+}
+
+int ssp_aug_resize_u8(const void* src, int src_w, int src_h, int x0, int y0, int in_w, int in_h, void* dst, int out_w, int out_h, int resample,
+                      void* work, long long work_bytes, void* stream) {
+  if (!src || !dst || !work || src_w <= 0 || src_h <= 0) return fail_msg(SSP_ERR_ARG, "ssp_aug_resize_u8: null pointer or empty source");
+  if ((uintptr_t)work % 16) return fail_msg(SSP_ERR_ARG, "ssp_aug_resize_u8: work buffer must be 16-B aligned");
+  CudaBackend be{(cudaStream_t)stream};
+  const int rc = resize_u8_driver(be, (const uint8_t*)src, src_w, src_h, x0, y0, in_w, in_h, (uint8_t*)dst, out_w, out_h, resample, (uint8_t*)work,
+                                  work_bytes);
+  if (rc) return driver_rc(rc, "ssp_aug_resize_u8");
+  SSP_CHECK_LAUNCH();
+  return SSP_OK;
+}
+
+int ssp_aug_rgb2hsv_u8(const void* rgb, void* hsv, long long n_pixels, void* stream) {
+  return aug_convert_u8((const uint8_t*)rgb, (uint8_t*)hsv, n_pixels, 1, (cudaStream_t)stream);
+}
+int ssp_aug_hsv2rgb_u8(const void* hsv, void* rgb, long long n_pixels, void* stream) {
+  return aug_convert_u8((const uint8_t*)hsv, (uint8_t*)rgb, n_pixels, 2, (cudaStream_t)stream);
+}
+
+int ssp_aug_to_tensor_u8(const void* src, long long n_px, float* out_chw, void* stream) {
+  if (!src || !out_chw || n_px < 0) return fail_msg(SSP_ERR_ARG, "ssp_aug_to_tensor_u8: bad argument");
+  if (n_px == 0) return SSP_OK;
+  aug_to_tensor_kernel<<<blocks_for(n_px, 256), 256, 0, (cudaStream_t)stream>>>((const uint8_t*)src, n_px, out_chw);
+  SSP_CHECK_LAUNCH();
+  return SSP_OK;
+}
+
+long long ssp_aug_batch_table_bytes(int n) { return n > 0 ? (long long)kMaxStages * n * (long long)sizeof(AugOp) : SSP_ERR_ARG; }
+
+// host side of the batched path: items (device pointers, host array) -> op table (host memory, to be copied to the device with the
+// batch) + per-stage launch extents
+int ssp_aug_batch_plan(const ssp_aug_item* items, int n, int out_w, int out_h, int resample, void* table_host, long long table_bytes, int* stage_dims) {
+  static_assert(sizeof(ssp_aug_item) == sizeof(AugItem), "ssp_aug_item (include/ssp_b200.h) must mirror AugItem (augment_core.h)");
+  if (!items || !table_host || !stage_dims || n <= 0 || table_bytes < ssp_aug_batch_table_bytes(n)) return fail_msg(SSP_ERR_ARG, "ssp_aug_batch_plan: bad argument");
+  for (int i = 0; i < n; i++)
+    if (!items[i].img || !items[i].mask || !items[i].bg || !items[i].luts || !items[i].work || (!items[i].out_u8 && !items[i].out_chw) ||
+        ((uintptr_t)items[i].work % 16))
+      return fail_msg(SSP_ERR_ARG, "ssp_aug_batch_plan: null pointer or misaligned work buffer in an item");
+  const int rc = augment_batch_plan(reinterpret_cast<const AugItem*>(items), n, out_w, out_h, resample, (AugOp*)table_host, stage_dims);
+  if (rc) return driver_rc(rc, "ssp_aug_batch_plan");
+  return SSP_OK;
+}
+
+int ssp_aug_batch_run(const void* table_dev, int n, const int* stage_dims, void* stream) {
+  if (!table_dev || !stage_dims || n <= 0 || n > 65535) return fail_msg(SSP_ERR_ARG, "ssp_aug_batch_run: bad argument");
+  const AugOp* ops = (const AugOp*)table_dev;
+  for (int st = 0; st < kMaxStages; st++) {
+    const int nx = stage_dims[2 * st], ny = stage_dims[2 * st + 1];
+    if (nx <= 0 || ny <= 0) continue;
+    dim3 grid((nx + 31) / 32, (ny + 7) / 8, n);
+    aug_stage_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(ops + (long long)st * n);
+  }
+  SSP_CHECK_LAUNCH();
+  return SSP_OK;
+}
+
+// ---- multi-object pipeline: three planned phases over the same stage kernel
+long long ssp_augm_work_bytes(int in_w, int in_h, int out_w, int out_h, int resample) {
+  if (in_w <= 0 || in_h <= 0 || out_w <= 0 || out_h <= 0) return SSP_ERR_ARG;
+  return multi_work_bytes(in_w, in_h, out_w, out_h, resample);
+}
+long long ssp_augm_table_bytes(int n) { return n > 0 ? (long long)kMaxMultiStages * n * (long long)sizeof(AugOp) : SSP_ERR_ARG; }
+
+int ssp_augm_plan_begin(const ssp_augm_item* items, int n, int out_w, int out_h, int resample, void* table_host, long long table_bytes, int* dims) {
+  return augm_plan(MULTI_BEGIN, items, n, out_w, out_h, resample, table_host, table_bytes, dims);
+}
+int ssp_augm_plan_attempt(const ssp_augm_item* items, int n, int out_w, int out_h, int resample, void* table_host, long long table_bytes, int* dims) {
+  return augm_plan(MULTI_ATTEMPT, items, n, out_w, out_h, resample, table_host, table_bytes, dims);
+}
+int ssp_augm_plan_finish(const ssp_augm_item* items, int n, int out_w, int out_h, int resample, void* table_host, long long table_bytes, int* dims) {
+  return augm_plan(MULTI_FINISH, items, n, out_w, out_h, resample, table_host, table_bytes, dims);
+}
+
+int ssp_augm_run(const void* table_dev, int n, const int* stage_dims, void* stream) {
   if (!table_dev || !stage_dims || n <= 0 || n > 65535) return fail_msg(SSP_ERR_ARG, "ssp_augm_run: bad argument");
   const AugOp* ops = (const AugOp*)table_dev;
   for (int st = 0; st < kMaxMultiStages; st++) {
     const int nx = stage_dims[2 * st], ny = stage_dims[2 * st + 1];
     if (nx <= 0 || ny <= 0) continue;
     dim3 grid((nx + 31) / 32, (ny + 7) / 8, n);
-    aug_stage_kernel<<<grid, 256, 0, s>>>(ops + (long long)st * n);
+    aug_stage_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(ops + (long long)st * n);
   }
   SSP_CHECK_LAUNCH();
   return SSP_OK;
 }
 
-int aug_sample(const uint8_t* img, const uint8_t* mask, int ow, int oh, const uint8_t* bg, int bw, int bh, const uint8_t* luts, int pleft,
-               int ptop, int cw, int ch, int out_w, int out_h, int resample, uint8_t* work, long long work_bytes, uint8_t* out_u8,
-               float* out_chw, cudaStream_t s) {
+int ssp_aug_sample(const void* img, const void* mask, int ow, int oh, const void* bg, int bw, int bh, const void* luts, int pleft, int ptop, int cw,
+                   int ch, int out_w, int out_h, int resample, void* work, long long work_bytes, void* out_u8, float* out_chw, void* stream) {
   if (!img || !mask || !bg || !luts || !work || (!out_u8 && !out_chw)) return fail_msg(SSP_ERR_ARG, "ssp_aug_sample: null pointer");
   if ((uintptr_t)work % 16) return fail_msg(SSP_ERR_ARG, "ssp_aug_sample: work buffer must be 16-B aligned");
-  CudaBackend be{s};
-  const int rc = augment_sample_driver(be, img, mask, ow, oh, bg, bw, bh, luts, pleft, ptop, cw, ch, out_w, out_h, resample, work, work_bytes,
-                                       out_u8, out_chw);
+  CudaBackend be{(cudaStream_t)stream};
+  const int rc = augment_sample_driver(be, (const uint8_t*)img, (const uint8_t*)mask, ow, oh, (const uint8_t*)bg, bw, bh, (const uint8_t*)luts,
+                                       pleft, ptop, cw, ch, out_w, out_h, resample, (uint8_t*)work, work_bytes, (uint8_t*)out_u8, out_chw);
   if (rc) return driver_rc(rc, "ssp_aug_sample");
   SSP_CHECK_LAUNCH();
   return SSP_OK;
 }
-}  // namespace ssp
+}  // extern "C"

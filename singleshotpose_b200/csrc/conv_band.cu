@@ -9,6 +9,7 @@
 // shared memory (they fit because the layer is narrow).  Row requests per tile drop from 9*(256+2*BN) to 3*272.
 // Same operands / epilogue / outputs as conv_tc.cu; replaces it for block-2-like layers and their data gradients.
 #include "ssp_common.cuh"
+#include "gemm.cuh"
 #include "tmap.cuh"
 
 namespace ssp {

@@ -18,6 +18,7 @@
 // split operands, cout > 128 single-term, bias epilogue, weights that do not fit next to two bands.
 // Replaces nn.Conv2d of reference darknet.py:156-160 for the narrow blocks, and their data gradients (train.py:103).
 #include "ssp_common.cuh"
+#include "gemm.cuh"
 #include "tmap.cuh"
 
 namespace ssp {
@@ -219,7 +220,6 @@ static const BandTKernel bandt_kernels[5][3] = {SSP_BANDT_ROW(0, true, true), SS
 #undef SSP_BANDT_ROW
 
 static int g_bandt_launches = 0;
-int conv_bandt_launch_count() { return g_bandt_launches; }
 
 // returns SSP_OK, or 1 when the layer is not eligible (caller falls back to conv_band / the per-tap kernels)
 int conv_gemm_bandt(const void* a_hi, const void* a_lo, long long a_rows, int a_ld, int cin,
@@ -288,3 +288,7 @@ int conv_gemm_bandt(const void* a_hi, const void* a_lo, long long a_rows, int a_
 }
 
 }  // namespace ssp
+
+extern "C" {
+int ssp_conv_bandt_launches(void) { return ssp::g_bandt_launches; }
+}  // extern "C"

@@ -2,6 +2,7 @@
 // wgrad_tc.cu).  They are the on-device cross-check for the tensor-core kernels (SSP_IMPL_SIMT through the
 // ABI); all arithmetic is fp32 FFMA on hi+lo reconstructed operands.
 #include "ssp_common.cuh"
+#include "gemm.cuh"
 
 namespace ssp {
 

@@ -17,6 +17,7 @@
 //                                          accumulators -> shared memory -> one row per thread -> (bias | BN statistics |
 //                                          fp16 data gradient) -> global
 #include "ssp_common.cuh"
+#include "gemm.cuh"
 #include "tmap.cuh"
 
 namespace ssp {
@@ -317,16 +318,6 @@ static void tile_geometry(int N, int H, int W, int taps, int cin, int cout, long
   *kblocks = taps * ((cin + 63) / 64);
 }
 
-int conv_splitk_count(int N, int H, int W, int taps, int cin, int cout, int num_sms) {
-  if (N <= 0 || H <= 0 || W <= 0 || (taps != 1 && taps != 9) || cin <= 0 || cout <= 0 || num_sms <= 0)
-    return fail_msg(SSP_ERR_ARG, "ssp_conv_splitk_count: bad argument");
-  long long tiles; int kblocks;
-  tile_geometry(N, H, W, taps, cin, cout, &tiles, &kblocks);
-  long long s = num_sms / tiles;
-  if (s > kblocks / kSplitMinKblocks) s = kblocks / kSplitMinKblocks;
-  return s < 2 ? 1 : (int)s;
-}
-
 int conv_gemm_tc(const void* a_hi, const void* a_lo, long long a_rows, int a_ld, int cin,
                  const void* b_hi, const void* b_lo, int b_rows, int b_ld, int a_fmt, int b_fmt,
                  int N, int H, int W, int taps, int cout, float* out, int out_ld, long long out_rows,
@@ -413,3 +404,35 @@ int conv_gemm_tc(const void* a_hi, const void* a_lo, long long a_rows, int a_ld,
 }
 
 }  // namespace ssp
+
+using namespace ssp;
+
+extern "C" {
+int ssp_conv_gemm_bnact(int impl, const void* a_hi, const void* a_lo, long long a_rows, int a_ld, int cin, const void* b_hi, const void* b_lo,
+                        int b_rows, int b_ld, int N, int H, int W, int taps, int cout, const float* scale, const float* shift, float slope,
+                        void* d_hi, void* d_lo, int d_ld, int d_c0, void* stream) {
+  FusedAct fa{scale, shift, slope, (uint16_t*)d_hi, (uint16_t*)d_lo, d_ld, d_c0};
+  if (impl == SSP_IMPL_TC || impl == SSP_IMPL_TC2 || impl == SSP_IMPL_BAND)
+    return conv_gemm_tc(a_hi, a_lo, a_rows, a_ld, cin, b_hi, b_lo, b_rows, b_ld, SSP_FMT_F16, SSP_FMT_F16, N, H, W, taps, cout, nullptr, 0, 0, EPI_BNACT,
+                        nullptr, nullptr, nullptr, (cudaStream_t)stream, &fa, nullptr);
+  return fail_msg(SSP_ERR_ARG, "ssp_conv_gemm_bnact: tensor-core implementations only");
+}
+
+int ssp_conv_gemm_splitk(const void* a_hi, const void* a_lo, long long a_rows, int a_ld, int cin, const void* b_hi, const void* b_lo, int b_rows,
+                         int b_ld, int N, int H, int W, int taps, int cout, int splits, float* partial, long long slab_elems, int partial_ld,
+                         void* stream) {
+  const SplitK sk{splits, slab_elems};
+  return conv_gemm_tc(a_hi, a_lo, a_rows, a_ld, cin, b_hi, b_lo, b_rows, b_ld, SSP_FMT_F16, SSP_FMT_F16, N, H, W, taps, cout, partial, partial_ld, 0,
+                      EPI_F32, nullptr, nullptr, nullptr, (cudaStream_t)stream, nullptr, &sk);
+}
+
+int ssp_conv_splitk_count(int N, int H, int W, int taps, int cin, int cout, int num_sms) {
+  if (N <= 0 || H <= 0 || W <= 0 || (taps != 1 && taps != 9) || cin <= 0 || cout <= 0 || num_sms <= 0)
+    return fail_msg(SSP_ERR_ARG, "ssp_conv_splitk_count: bad argument");
+  long long tiles; int kblocks;
+  tile_geometry(N, H, W, taps, cin, cout, &tiles, &kblocks);
+  long long s = num_sms / tiles;
+  if (s > kblocks / kSplitMinKblocks) s = kblocks / kSplitMinKblocks;
+  return s < 2 ? 1 : (int)s;
+}
+}  // extern "C"

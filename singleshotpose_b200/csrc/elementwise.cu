@@ -516,43 +516,11 @@ __global__ void sgd_flat_kernel(float* __restrict__ p, const float* __restrict__
 // ================================================================================================ host launchers
 static inline unsigned nblk(long long total, int bs) { return (unsigned)((total + bs - 1) / bs); }
 
-int pack_nchw(const float* x, void* hi, void* lo, int N, int C, int H, int W, int ld, int c0, int fmt, float scale, cudaStream_t s) {
-  if (!x || !hi) return fail_msg(SSP_ERR_ARG, "pack_nchw: null pointer");
-  const long long total = (long long)N * C * H * W;
-  pack_nchw_kernel<<<nblk(total, 256), 256, 0, s>>>(x, (uint16_t*)hi, (uint16_t*)lo, N, C, H, W, ld, c0, fmt, scale);
-  SSP_CHECK_LAUNCH(); return SSP_OK;
-}
-int unpack_nchw(const float* y, float* out, int N, int C, int H, int W, int ld, int c0, cudaStream_t s) {
-  if (!y || !out) return fail_msg(SSP_ERR_ARG, "unpack_nchw: null pointer");
-  const long long total = (long long)N * C * H * W;
-  unpack_nchw_kernel<<<nblk(total, 256), 256, 0, s>>>(y, out, N, C, H, W, ld, c0);
-  SSP_CHECK_LAUNCH(); return SSP_OK;
-}
-int unpack16_nchw(const void* hi, const void* lo, float* out, int N, int C, int H, int W, int ld, int c0, int fmt, cudaStream_t s) {
-  if (!hi || !out) return fail_msg(SSP_ERR_ARG, "unpack16_nchw: null pointer");
-  const long long total = (long long)N * C * H * W;
-  unpack16_nchw_kernel<<<nblk(total, 256), 256, 0, s>>>((const uint16_t*)hi, (const uint16_t*)lo, out, N, C, H, W, ld, c0, fmt);
-  SSP_CHECK_LAUNCH(); return SSP_OK;
-}
-int bn_finalize(double* ssum, double* ssq, double count, const float* gamma, const float* beta, float* rm, float* rv,
-                float momentum, float eps, int train, float* mean, float* invstd, float* scale, float* shift, int C, cudaStream_t s) {
-  if (!gamma || !beta || !mean || !invstd || !scale || !shift || (train && (!ssum || !ssq)) || (!train && (!rm || !rv)))
-    return fail_msg(SSP_ERR_ARG, "bn_finalize: null pointer");
-  bn_finalize_kernel<<<nblk(C, 128), 128, 0, s>>>(ssum, ssq, count, gamma, beta, rm, rv, momentum, eps, train, mean, invstd, scale, shift, C);
-  SSP_CHECK_LAUNCH(); return SSP_OK;
-}
-int bn_apply_splitk(const float*, int, long long, int, const float*, const float*, int, int, int, int, float, void*, void*, int, int, int, void*,
-                    void*, int, int, int, cudaStream_t, float*, int);
-int bn_apply(const float* y, int y_ld, const float* scale, const float* shift, int N, int C, int H, int W, float slope,
-             void* d0_hi, void* d0_lo, int d0_ld, int d0_c0, int d0_kind,
-             void* d1_hi, void* d1_lo, int d1_ld, int d1_c0, int d1_kind, float* ypool, int ypool_ld, cudaStream_t s) {
-  return bn_apply_splitk(y, 1, 0, y_ld, scale, shift, N, C, H, W, slope, d0_hi, d0_lo, d0_ld, d0_c0, d0_kind, d1_hi, d1_lo, d1_ld, d1_c0, d1_kind,
-                         s, ypool, ypool_ld);
-}
-// splits == 1 launches the plain kernel (the ssp_bn_apply path); splits > 1 the instantiation that sums the partial slabs first
-int bn_apply_splitk(const float* y, int splits, long long slab, int y_ld, const float* scale, const float* shift, int N, int C, int H, int W,
-                    float slope, void* d0_hi, void* d0_lo, int d0_ld, int d0_c0, int d0_kind, void* d1_hi, void* d1_lo, int d1_ld, int d1_c0,
-                    int d1_kind, cudaStream_t s, float* ypool, int ypool_ld) {
+// ssp_bn_apply and ssp_bn_apply_splitk.  splits == 1 launches the plain kernel (the ssp_bn_apply path); splits > 1 the instantiation
+// that sums the partial slabs first
+static int bn_apply_splitk(const float* y, int splits, long long slab, int y_ld, const float* scale, const float* shift, int N, int C, int H, int W,
+                           float slope, void* d0_hi, void* d0_lo, int d0_ld, int d0_c0, int d0_kind, void* d1_hi, void* d1_lo, int d1_ld, int d1_c0,
+                           int d1_kind, cudaStream_t s, float* ypool, int ypool_ld) {
   if (!y || !scale || !shift || (C % 4)) return fail_msg(SSP_ERR_ARG, "bn_apply: bad argument (C must be a multiple of 4)");
   if (splits < 1 || (splits > 1 && (((uintptr_t)y % 16) || (y_ld % 4) || y_ld < C || (slab % 4) || slab < (long long)y_ld * flat_alloc_rows(N, H, W))))
     return fail_msg(SSP_ERR_ARG, "bn_apply_splitk: splits >= 1; partial slabs 16-B aligned, partial_ld % 4 == 0 and >= C, slab_elems % 4 == 0 and "
@@ -591,10 +559,54 @@ static int fill_bwd(BnBwdParams& p, const float* y, int y_ld, const float* scale
   p.dy = nullptr; p.dy_ld = 0; p.dy_fmt = 0; p.dy_scale = 1.f;
   return SSP_OK;
 }
-int bn_bwd_reduce(const float* y, int y_ld, const float* scale, const float* shift, const float* mean, const float* invstd,
-                  const float* gamma, int N, int C, int H, int W, float slope,
-                  const float* g0, int g0_ld, int g0_c0, int g0_kind, const float* g1, int g1_ld, int g1_c0, int g1_kind,
-                  double* s1, double* s2, cudaStream_t s) {
+
+}  // namespace ssp
+
+using namespace ssp;
+
+extern "C" {
+int ssp_pack_nchw(const float* x, void* hi, void* lo, int N, int C, int H, int W, int ld, int c0, int fmt, float scale, void* stream) {
+  if (!x || !hi) return fail_msg(SSP_ERR_ARG, "pack_nchw: null pointer");
+  const long long total = (long long)N * C * H * W;
+  pack_nchw_kernel<<<nblk(total, 256), 256, 0, (cudaStream_t)stream>>>(x, (uint16_t*)hi, (uint16_t*)lo, N, C, H, W, ld, c0, fmt, scale);
+  SSP_CHECK_LAUNCH(); return SSP_OK;
+}
+int ssp_unpack_nchw(const float* y, float* out, int N, int C, int H, int W, int ld, int c0, void* stream) {
+  if (!y || !out) return fail_msg(SSP_ERR_ARG, "unpack_nchw: null pointer");
+  const long long total = (long long)N * C * H * W;
+  unpack_nchw_kernel<<<nblk(total, 256), 256, 0, (cudaStream_t)stream>>>(y, out, N, C, H, W, ld, c0);
+  SSP_CHECK_LAUNCH(); return SSP_OK;
+}
+int ssp_unpack16_nchw(const void* hi, const void* lo, float* out, int N, int C, int H, int W, int ld, int c0, int fmt, void* stream) {
+  if (!hi || !out) return fail_msg(SSP_ERR_ARG, "unpack16_nchw: null pointer");
+  const long long total = (long long)N * C * H * W;
+  unpack16_nchw_kernel<<<nblk(total, 256), 256, 0, (cudaStream_t)stream>>>((const uint16_t*)hi, (const uint16_t*)lo, out, N, C, H, W, ld, c0, fmt);
+  SSP_CHECK_LAUNCH(); return SSP_OK;
+}
+int ssp_bn_finalize(double* ssum, double* ssq, double count, const float* gamma, const float* beta, float* rm, float* rv,
+                    float momentum, float eps, int train, float* mean, float* invstd, float* scale, float* shift, int C, void* stream) {
+  if (!gamma || !beta || !mean || !invstd || !scale || !shift || (train && (!ssum || !ssq)) || (!train && (!rm || !rv)))
+    return fail_msg(SSP_ERR_ARG, "bn_finalize: null pointer");
+  bn_finalize_kernel<<<nblk(C, 128), 128, 0, (cudaStream_t)stream>>>(ssum, ssq, count, gamma, beta, rm, rv, momentum, eps, train, mean, invstd,
+                                                                     scale, shift, C);
+  SSP_CHECK_LAUNCH(); return SSP_OK;
+}
+int ssp_bn_apply(const float* y, int y_ld, const float* scale, const float* shift, int N, int C, int H, int W, float slope,
+                 void* d0_hi, void* d0_lo, int d0_ld, int d0_c0, int d0_kind,
+                 void* d1_hi, void* d1_lo, int d1_ld, int d1_c0, int d1_kind, float* ypool, int ypool_ld, void* stream) {
+  return bn_apply_splitk(y, 1, 0, y_ld, scale, shift, N, C, H, W, slope, d0_hi, d0_lo, d0_ld, d0_c0, d0_kind, d1_hi, d1_lo, d1_ld, d1_c0, d1_kind,
+                         (cudaStream_t)stream, ypool, ypool_ld);
+}
+int ssp_bn_apply_splitk(const float* partial, int splits, long long slab_elems, int partial_ld, const float* scale, const float* shift, int N, int C,
+                        int H, int W, float slope, void* d0_hi, void* d0_lo, int d0_ld, int d0_c0, int d0_kind, void* d1_hi, void* d1_lo, int d1_ld,
+                        int d1_c0, int d1_kind, void* stream) {
+  return bn_apply_splitk(partial, splits, slab_elems, partial_ld, scale, shift, N, C, H, W, slope, d0_hi, d0_lo, d0_ld, d0_c0, d0_kind, d1_hi, d1_lo,
+                         d1_ld, d1_c0, d1_kind, (cudaStream_t)stream, nullptr, 0);
+}
+int ssp_bn_bwd_reduce(const float* y, int y_ld, const float* scale, const float* shift, const float* mean, const float* invstd,
+                      const float* gamma, int N, int C, int H, int W, float slope,
+                      const float* g0, int g0_ld, int g0_c0, int g0_kind, const float* g1, int g1_ld, int g1_c0, int g1_kind,
+                      double* s1, double* s2, void* stream) {
   BnBwdParams p;
   if (fill_bwd(p, y, y_ld, scale, shift, mean, invstd, gamma, N, C, H, W, slope, g0, g0_ld, g0_c0, g0_kind, g1, g1_ld, g1_c0, g1_kind, s1, s2) || !s1 || !s2 || !p.has_bn)
     return fail_msg(SSP_ERR_ARG, "bn_bwd_reduce: bad argument");
@@ -616,13 +628,13 @@ int bn_bwd_reduce(const float* y, int y_ld, const float* scale, const float* shi
     else if (k0 == SRC_REORG && k1 == SRC_DIRECT) KERN<SRC_REORG, SRC_DIRECT><<<__VA_ARGS__>>>(p);                  \
     else return fail_msg(SSP_ERR_ARG, "bn_bwd: unsupported combination of gradient routes");                         \
   } while (0)
-  SSP_BWD_DISPATCH(bn_bwd_reduce_kernel, grid, 256, sm, s);
+  SSP_BWD_DISPATCH(bn_bwd_reduce_kernel, grid, 256, sm, (cudaStream_t)stream);
   SSP_CHECK_LAUNCH(); return SSP_OK;
 }
-int bn_bwd_apply(const float* y, int y_ld, const float* scale, const float* shift, const float* mean, const float* invstd,
-                 const float* gamma, int N, int C, int H, int W, float slope,
-                 const float* g0, int g0_ld, int g0_c0, int g0_kind, const float* g1, int g1_ld, int g1_c0, int g1_kind,
-                 double* s1, double* s2, void* dy, int dy_ld, int dy_fmt, float dy_scale, cudaStream_t s) {
+int ssp_bn_bwd_apply(const float* y, int y_ld, const float* scale, const float* shift, const float* mean, const float* invstd,
+                     const float* gamma, int N, int C, int H, int W, float slope,
+                     const float* g0, int g0_ld, int g0_c0, int g0_kind, const float* g1, int g1_ld, int g1_c0, int g1_kind,
+                     double* s1, double* s2, void* dy, int dy_ld, int dy_fmt, float dy_scale, void* stream) {
   BnBwdParams p;
   if (fill_bwd(p, y, y_ld, scale, shift, mean, invstd, gamma, N, C, H, W, slope, g0, g0_ld, g0_c0, g0_kind, g1, g1_ld, g1_c0, g1_kind, s1, s2) || !dy)
     return fail_msg(SSP_ERR_ARG, "bn_bwd_apply: bad argument");
@@ -631,30 +643,29 @@ int bn_bwd_apply(const float* y, int y_ld, const float* scale, const float* shif
   const bool pooled = p.src[0].kind == SRC_POOL || p.src[1].kind == SRC_POOL;
   const long long nunits = (long long)N * (pooled ? H / 2 : H) * (pooled ? W / 2 : W);
   const unsigned grid = unit_grid(C, nunits, BN_UNITS_PER_THREAD);
-  SSP_BWD_DISPATCH(bn_bwd_apply_kernel, grid, 256, 0, s);
+  SSP_BWD_DISPATCH(bn_bwd_apply_kernel, grid, 256, 0, (cudaStream_t)stream);
   SSP_CHECK_LAUNCH(); return SSP_OK;
 }
-int bn_bwd_finalize(double* s1, double* s2, float* dgamma, float* dbeta, int C, int accumulate, float scale, cudaStream_t s) {
+int ssp_bn_bwd_finalize(double* s1, double* s2, float* dgamma, float* dbeta, int C, int accumulate, float scale, void* stream) {
   if (!s1 || !s2 || !dgamma || !dbeta) return fail_msg(SSP_ERR_ARG, "bn_bwd_finalize: null pointer");
-  bn_bwd_finalize_kernel<<<nblk(C, 128), 128, 0, s>>>(s1, s2, dgamma, dbeta, C, accumulate, scale);
+  bn_bwd_finalize_kernel<<<nblk(C, 128), 128, 0, (cudaStream_t)stream>>>(s1, s2, dgamma, dbeta, C, accumulate, scale);
   SSP_CHECK_LAUNCH(); return SSP_OK;
 }
-int bias_grad_nchw(const float* g, float* db, int N, int C, int HW, int accumulate, float scale, cudaStream_t s) {
+int ssp_bias_grad_nchw(const float* g, float* db, int N, int C, int HW, int accumulate, float scale, void* stream) {
   if (!g || !db) return fail_msg(SSP_ERR_ARG, "bias_grad_nchw: null pointer");
-  bias_grad_nchw_kernel<<<C, 256, 0, s>>>(g, db, N, C, HW, accumulate, scale);
+  bias_grad_nchw_kernel<<<C, 256, 0, (cudaStream_t)stream>>>(g, db, N, C, HW, accumulate, scale);
   SSP_CHECK_LAUNCH(); return SSP_OK;
 }
-int pack_weights(const float* w, int cout, int taps, int cin, void* f_hi, void* f_lo, int ld_f, void* d, int ld_d, int d_fmt, cudaStream_t s) {
+int ssp_pack_weights(const float* w, int cout, int taps, int cin, void* f_hi, void* f_lo, int ld_f, void* d, int ld_d, int d_fmt, void* stream) {
   if (!w || cout <= 0 || taps <= 0 || cin <= 0 || taps > 65535) return fail_msg(SSP_ERR_ARG, "pack_weights: bad argument");
   dim3 grid((cin + 63) / 64, (cout + 63) / 64, taps);
   if (grid.y > 65535) return fail_msg(SSP_ERR_ARG, "pack_weights: cout too large");
-  pack_weights_tiled_kernel<<<grid, 256, 0, s>>>(w, cout, taps, cin, (uint16_t*)f_hi, (uint16_t*)f_lo, ld_f, (uint16_t*)d, ld_d, d_fmt);
+  pack_weights_tiled_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(w, cout, taps, cin, (uint16_t*)f_hi, (uint16_t*)f_lo, ld_f, (uint16_t*)d, ld_d, d_fmt);
   SSP_CHECK_LAUNCH(); return SSP_OK;
 }
-int sgd_step_flat(float* p, const float* g, float* v, long long n, float lr, float mu, float wd, float gscale, cudaStream_t s) {
+int ssp_sgd_step_flat(float* p, const float* g, float* v, long long n, float lr, float mu, float wd, float gscale, void* stream) {
   if (!p || !g || !v) return fail_msg(SSP_ERR_ARG, "sgd_step_flat: null pointer");
-  sgd_flat_kernel<<<nblk((n + 3) / 4, 256), 256, 0, s>>>(p, g, v, n, lr, mu, wd, gscale);
+  sgd_flat_kernel<<<nblk((n + 3) / 4, 256), 256, 0, (cudaStream_t)stream>>>(p, g, v, n, lr, mu, wd, gscale);
   SSP_CHECK_LAUNCH(); return SSP_OK;
 }
-
-}  // namespace ssp
+}  // extern "C"

@@ -291,18 +291,6 @@ __global__ void __launch_bounds__(256) color_kernel(const uint8_t* __restrict__ 
 }  // namespace
 
 // -------------------------------------------------------------------------------------------------------------- host
-int jpeg_parse(const void* data, long long size, ssp_jpeg_info* info) {
-  if (!data || size < 0 || !info) return fail_msg(SSP_ERR_ARG, "jpeg_parse: bad argument (null pointer or size < 0)");
-  static thread_local Desc d;
-  const int rc = parse(static_cast<const uint8_t*>(data), size, d);
-  memset(info, 0, sizeof(*info));
-  info->width = d.w; info->height = d.h; info->components = d.ncomp;
-  info->h_samp = d.comp[0].h; info->v_samp = d.comp[0].v; info->restart_interval = d.ri;
-  return rc;
-}
-
-const char* jpeg_decline_reason(int code) { return code >= 0 && code < kNumDecline ? kDeclineText[code] : "unknown code"; }
-
 // sizes: stage = records + payloads + interval tables, work = per image workspace (all 16-B aligned)
 static int jpeg_sizes(const ssp_jpeg_item* items, int n, long long* stage, long long* work, std::vector<Desc>* descs) {
   if (!items || n < 0) return fail_msg(SSP_ERR_ARG, "jpeg: bad argument (null items or n < 0)");
@@ -321,18 +309,35 @@ static int jpeg_sizes(const ssp_jpeg_item* items, int n, long long* stage, long 
   return SSP_OK;
 }
 
-long long jpeg_stage_bytes(const ssp_jpeg_item* items, int n) {
+}  // namespace ssp
+
+using namespace ssp;
+
+extern "C" {
+int ssp_jpeg_parse(const void* data, long long size, ssp_jpeg_info* info) {
+  if (!data || size < 0 || !info) return fail_msg(SSP_ERR_ARG, "jpeg_parse: bad argument (null pointer or size < 0)");
+  static thread_local Desc d;
+  const int rc = parse(static_cast<const uint8_t*>(data), size, d);
+  memset(info, 0, sizeof(*info));
+  info->width = d.w; info->height = d.h; info->components = d.ncomp;
+  info->h_samp = d.comp[0].h; info->v_samp = d.comp[0].v; info->restart_interval = d.ri;
+  return rc;
+}
+
+const char* ssp_jpeg_decline_reason(int code) { return code >= 0 && code < kNumDecline ? kDeclineText[code] : "unknown code"; }
+
+long long ssp_jpeg_stage_bytes(const ssp_jpeg_item* items, int n) {
   long long s, w;
   const int rc = jpeg_sizes(items, n, &s, &w, nullptr);
   return rc ? rc : s;
 }
-long long jpeg_work_bytes(const ssp_jpeg_item* items, int n) {
+long long ssp_jpeg_work_bytes(const ssp_jpeg_item* items, int n) {
   long long s, w;
   const int rc = jpeg_sizes(items, n, &s, &w, nullptr);
   return rc ? rc : w;
 }
 
-int jpeg_batch_plan(const ssp_jpeg_item* items, int n, void* stage_host, long long stage_bytes, long long* dims) {
+int ssp_jpeg_batch_plan(const ssp_jpeg_item* items, int n, void* stage_host, long long stage_bytes, long long* dims) {
   if (!stage_host || !dims) return fail_msg(SSP_ERR_ARG, "jpeg_batch_plan: bad argument (null pointer)");
   std::vector<Desc> descs;
   long long need_s, need_w;
@@ -378,7 +383,8 @@ int jpeg_batch_plan(const ssp_jpeg_item* items, int n, void* stage_host, long lo
   return SSP_OK;
 }
 
-int jpeg_batch_run(const void* stage_dev, int n, const long long* dims, void* work, long long work_bytes, int* status, cudaStream_t s) {
+int ssp_jpeg_batch_run(const void* stage_dev, int n, const long long* dims, void* work, long long work_bytes, int* status, void* stream) {
+  const cudaStream_t s = (cudaStream_t)stream;
   if (n < 0 || !dims) return fail_msg(SSP_ERR_ARG, "jpeg_batch_run: bad argument (n < 0 or null dims)");
   if (n == 0) return SSP_OK;
   if (!stage_dev || !work || !status) return fail_msg(SSP_ERR_ARG, "jpeg_batch_run: bad argument (null pointer)");
@@ -396,5 +402,4 @@ int jpeg_batch_run(const void* stage_dev, int n, const long long* dims, void* wo
   SSP_CHECK_LAUNCH();
   return SSP_OK;
 }
-
-}  // namespace ssp
+}  // extern "C"

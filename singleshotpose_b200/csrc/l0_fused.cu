@@ -495,7 +495,13 @@ static int l0_grid(long long ntiles, int per_sm) {
 }
 static long long l0_tiles(int N, int H, int W) { return (long long)N * ((H + kTH - 1) / kTH) * ((W + kTW - 1) / kTW); }
 
-int l0_gram(const float* x, int N, int H, int W, double* gram, cudaStream_t s) {
+}  // namespace ssp
+
+using namespace ssp;
+
+extern "C" {
+int ssp_l0_gram(const float* x, int N, int H, int W, double* gram, void* stream) {
+  const cudaStream_t s = (cudaStream_t)stream;
   if (!x || !gram || N <= 0 || H <= 0 || W <= 0) return fail_msg(SSP_ERR_ARG, "l0_gram: bad argument");
   const long long nt = l0_tiles(N, H, W);
   if (nt > 0x7fffffffLL) return fail_msg(SSP_ERR_ARG, "l0_gram: bad shape");
@@ -513,24 +519,25 @@ int l0_gram(const float* x, int N, int H, int W, double* gram, cudaStream_t s) {
   SSP_CHECK_LAUNCH(); return SSP_OK;
 }
 
-int l0_stats(const double* gram, const float* w, double* ssum, double* ssq, cudaStream_t s) {
+int ssp_l0_stats(const double* gram, const float* w, double* ssum, double* ssq, void* stream) {
   if (!gram || !w || !ssum || !ssq) return fail_msg(SSP_ERR_ARG, "l0_stats: bad argument");
-  l0_stats_kernel<<<1, 1024, 0, s>>>(gram, w, ssum, ssq);
+  l0_stats_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(gram, w, ssum, ssq);
   SSP_CHECK_LAUNCH(); return SSP_OK;
 }
 
-int l0_fused_fwd(const float* x, const float* w, const float* scale, const float* shift, float slope, int N, int H, int W,
-                 void* d_hi, void* d_lo, int d_ld, int d_c0, uint8_t* code, cudaStream_t s) {
+int ssp_l0_fused_fwd(const float* x, const float* w, const float* scale, const float* shift, float slope, int N, int H, int W,
+                     void* d_hi, void* d_lo, int d_ld, int d_c0, uint8_t* code, void* stream) {
   if (!x || !w || !scale || !shift || !d_hi || !d_lo || (H & 1) || (W & 1) || (d_ld % 4) || (d_c0 % 4) || d_ld < d_c0 + kC0)
     return fail_msg(SSP_ERR_ARG, "l0_fused_fwd: bad argument (even H / W, destination rows 8-B aligned)");
   const long long nt = l0_tiles(N, H, W);
   if (nt <= 0 || nt > 0x7fffffffLL) return fail_msg(SSP_ERR_ARG, "l0_fused_fwd: bad shape");
-  l0_fused_fwd_kernel<<<l0_grid(nt, 1), 256, 0, s>>>(x, w, scale, shift, slope, N, H, W, (uint16_t*)d_hi, (uint16_t*)d_lo, d_ld, d_c0, code);
+  l0_fused_fwd_kernel<<<l0_grid(nt, 1), 256, 0, (cudaStream_t)stream>>>(x, w, scale, shift, slope, N, H, W, (uint16_t*)d_hi, (uint16_t*)d_lo, d_ld, d_c0, code);
   SSP_CHECK_LAUNCH(); return SSP_OK;
 }
 
-int l0_bwd(const float* x, const void* g, int g_f16, int g_ld, int g_c0, const uint8_t* code, float slope, int N, int H, int W, double* t1,
-           cudaStream_t s) {
+int ssp_l0_bwd(const float* x, const void* g, int g_f16, int g_ld, int g_c0, const uint8_t* code, float slope, int N, int H, int W, double* t1,
+               void* stream) {
+  const cudaStream_t s = (cudaStream_t)stream;
   if (!x || !g || !code || !t1 || (H & 1) || (W & 1)) return fail_msg(SSP_ERR_ARG, "l0_bwd: bad argument");
   const long long nt = l0_tiles(N, H, W);
   if (nt <= 0 || nt > 0x7fffffffLL) return fail_msg(SSP_ERR_ARG, "l0_bwd: bad shape");
@@ -541,12 +548,11 @@ int l0_bwd(const float* x, const void* g, int g_f16, int g_ld, int g_c0, const u
   SSP_CHECK_LAUNCH(); return SSP_OK;
 }
 
-int l0_bwd_finalize(const double* t1, const double* gram, const float* w, const float* gamma, const float* mean, const float* invstd,
-                    double count, float gscale, float* dW, float* dgamma, float* dbeta, cudaStream_t s) {
+int ssp_l0_bwd_finalize(const double* t1, const double* gram, const float* w, const float* gamma, const float* mean, const float* invstd,
+                        double count, float gscale, float* dW, float* dgamma, float* dbeta, void* stream) {
   if (!t1 || !gram || !w || !gamma || !mean || !invstd || !dW || !dgamma || !dbeta || !(count > 0))
     return fail_msg(SSP_ERR_ARG, "l0_bwd_finalize: bad argument");
-  l0_bwd_finalize_kernel<<<1, 1024, 0, s>>>(t1, gram, w, gamma, mean, invstd, count, gscale, dW, dgamma, dbeta);
+  l0_bwd_finalize_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(t1, gram, w, gamma, mean, invstd, count, gscale, dW, dgamma, dbeta);
   SSP_CHECK_LAUNCH(); return SSP_OK;
 }
-
-}  // namespace ssp
+}  // extern "C"

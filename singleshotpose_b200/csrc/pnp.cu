@@ -48,20 +48,35 @@ __global__ void project_points_kernel(const float* __restrict__ X4 /*[4][nv] or 
   out[(b * 2 + 1) * nv + v] = (float)(py / pz);
 }
 
-int pnp_batched(const float* P3, int p3_shared, const float* uv, const float* K, int np, long long n, int max_iter,
-                double* R_out, double* t_out, int* iters_out, int* work_out, cudaStream_t s) {
+// ssp_pnp_batched and ssp_pnp_batched_work
+static int pnp_batched(const float* P3, int p3_shared, const float* uv, const float* K, int np, long long n, int max_iter,
+                       double* R_out, double* t_out, int* iters_out, int* work_out, cudaStream_t s) {
   if (!P3 || !uv || !K || !R_out || !t_out || np < 6 || np > PNP_MAXP || n < 0) return fail_msg(SSP_ERR_ARG, "pnp_batched: bad argument (6 <= points <= 16)");
   if (n == 0) return SSP_OK;
   pnp_kernel<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(P3, p3_shared ? 0 : 3LL * np, uv, K, np, n, max_iter, R_out, t_out, iters_out, work_out);
   SSP_CHECK_LAUNCH(); return SSP_OK;
 }
 
-int project_points(const float* X, int rows, int nv, const double* Rt, const double* K, long long n, float* out, cudaStream_t s) {
+}  // namespace ssp
+
+using namespace ssp;
+
+extern "C" {
+int ssp_pnp_batched(const float* P3, int shared, const float* uv, const float* K, int np, long long n, int max_iter, double* R, double* t, int* iters,
+                    void* stream) {
+  return pnp_batched(P3, shared, uv, K, np, n, max_iter, R, t, iters, nullptr, (cudaStream_t)stream);
+}
+
+int ssp_pnp_batched_work(const float* P3, int shared, const float* uv, const float* K, int np, long long n, int max_iter, double* R, double* t,
+                         int* work, void* stream) {
+  return pnp_batched(P3, shared, uv, K, np, n, max_iter, R, t, nullptr, work, (cudaStream_t)stream);
+}
+
+int ssp_project_points(const float* X, int rows, int nv, const double* Rt, const double* K, long long n, float* out, void* stream) {
   if (!X || !Rt || !K || !out || (rows != 3 && rows != 4)) return fail_msg(SSP_ERR_ARG, "project_points: bad argument");
   const long long total = n * nv;
   if (total == 0) return SSP_OK;
-  project_points_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(X, rows, nv, Rt, K, n, out);
+  project_points_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(X, rows, nv, Rt, K, n, out);
   SSP_CHECK_LAUNCH(); return SSP_OK;
 }
-
-}  // namespace ssp
+}  // extern "C"

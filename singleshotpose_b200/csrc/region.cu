@@ -165,9 +165,15 @@ __global__ void region_pick_global_kernel(const float* __restrict__ boxes, const
   }
 }
 
-int region_loss_fwd_bwd(const float* out, const float* target, float* grad, double* acc, int B, int K, int nC, int H, int W,
-                        float coord_scale, float noobject_scale, float object_scale, float thresh, int use_conf,
-                        float grad_scale, cudaStream_t s) {
+}  // namespace ssp
+
+using namespace ssp;
+
+extern "C" {
+int ssp_region_loss_fwd_bwd(const float* out, const float* target, float* grad, double* acc, int B, int K, int nC, int H, int W,
+                            float coord_scale, float noobject_scale, float object_scale, float thresh, int use_conf,
+                            float grad_scale, void* stream) {
+  const cudaStream_t s = (cudaStream_t)stream;
   if (!out || !target || !acc || K < 1 || K > SSP_MAX_KP) return fail_msg(SSP_ERR_ARG, "region_loss_fwd_bwd: bad argument");
   cudaError_t e = cudaMemsetAsync(acc, 0, 8 * sizeof(double), s);
   if (e != cudaSuccess) return fail_cuda(e, __FILE__, __LINE__);
@@ -176,13 +182,13 @@ int region_loss_fwd_bwd(const float* out, const float* target, float* grad, doub
   SSP_CHECK_LAUNCH(); return SSP_OK;
 }
 
-int region_decode_argmax(const float* out, int B, int K, int nC, int H, int W, int only_objectness,
-                         float* boxes, float* best_conf, float* box_global, cudaStream_t s) {
+int ssp_region_decode_argmax(const float* out, int B, int K, int nC, int H, int W, int only_objectness,
+                             float* boxes, float* best_conf, float* box_global, void* stream) {
+  const cudaStream_t s = (cudaStream_t)stream;
   if (!out || !boxes || !best_conf || K < 1 || K > SSP_MAX_KP) return fail_msg(SSP_ERR_ARG, "region_decode_argmax: bad argument");
   region_decode_kernel<<<B, 256, 0, s>>>(out, B, K, nC, H, W, only_objectness, boxes, best_conf);
   SSP_CHECK_LAUNCH();
   if (box_global) { region_pick_global_kernel<<<1, 32, 0, s>>>(boxes, best_conf, B, 2 * K + 3, box_global); SSP_CHECK_LAUNCH(); }
   return SSP_OK;
 }
-
-}  // namespace ssp
+}  // extern "C"

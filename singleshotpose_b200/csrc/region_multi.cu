@@ -293,8 +293,13 @@ __global__ void __launch_bounds__(256) predict_multi_select_kernel(const Predict
   }
 }
 
-int predict_multi_select(const float* out, int B, int K, int nC, int nA, int H, int W, const int* classes_host, int n_req, float conf_thresh,
-                         float frame_w, float frame_h, float* boxes, int* flags, float* uv, cudaStream_t s) {
+}  // namespace ssp
+
+using namespace ssp;
+
+extern "C" {
+int ssp_predict_multi_select(const float* out, int B, int K, int nC, int nA, int H, int W, const int* classes_host, int n_req, float conf_thresh,
+                             float frame_w, float frame_h, float* boxes, int* flags, float* uv, void* stream) {
   if (!out || !classes_host || !boxes || !flags || !uv) return fail_msg(SSP_ERR_ARG, "predict_multi_select: null pointer");
   if (K != ssp_evm::kKeypoints)
     return fail_msg(SSP_ERR_ARG, "predict_multi_select: num_keypoints must be 9 (the PnP points are the 9 keypoints of a box)");
@@ -323,13 +328,13 @@ int predict_multi_select(const float* out, int B, int K, int nC, int nA, int H, 
   p.out = out; p.boxes = boxes; p.flags = flags; p.uv = uv;
   p.K = K; p.nC = nC; p.nA = nA; p.H = H; p.W = W; p.n_req = n_req;
   p.thr = conf_thresh; p.frame_w = frame_w; p.frame_h = frame_h;
-  predict_multi_select_kernel<<<B, 256, smem, s>>>(p);
+  predict_multi_select_kernel<<<B, 256, smem, (cudaStream_t)stream>>>(p);
   SSP_CHECK_LAUNCH(); return SSP_OK;
 }
 
-int eval_multi_select(const float* out, int B, int K, int nC, int nA, int H, int W, const float* target, int target_stride,
-                      const int* gt_offset, float conf_thresh, float im_width, float im_height, float* boxes, int* flags, float* uv,
-                      cudaStream_t s) {
+int ssp_eval_multi_select(const float* out, int B, int K, int nC, int nA, int H, int W, const float* target, int target_stride,
+                          const int* gt_offset, float conf_thresh, float im_width, float im_height, float* boxes, int* flags, float* uv,
+                          void* stream) {
   if (K != ssp_evm::kKeypoints)
     return fail_msg(SSP_ERR_ARG, "eval_multi_select: num_keypoints must be 9 (fix_corner_order is defined for the 9 keypoints of a box)");
   if (!out || !target || !gt_offset || !boxes || !flags || !uv || B < 0 || nC < 1 || nA < 1 || H < 1 || W < 1 || target_stride < 2 * K + 3)
@@ -338,14 +343,15 @@ int eval_multi_select(const float* out, int B, int K, int nC, int nA, int H, int
     return fail_msg(SSP_ERR_ARG, "eval_multi_select: grid too large (H*W*num_anchors must be at most 4096, e.g. 26x26x5)");
   if (nC > ssp_evm::kMaxClasses) return fail_msg(SSP_ERR_ARG, "eval_multi_select: at most 256 classes");
   if (B == 0) return SSP_OK;
-  eval_multi_select_kernel<<<B, 256, 0, s>>>(out, B, K, nC, nA, H, W, target, target_stride, gt_offset, conf_thresh, im_width, im_height,
-                                             boxes, flags, uv);
+  eval_multi_select_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(out, B, K, nC, nA, H, W, target, target_stride, gt_offset, conf_thresh, im_width,
+                                                              im_height, boxes, flags, uv);
   SSP_CHECK_LAUNCH(); return SSP_OK;
 }
 
-int region_loss_multi_fwd_bwd(const float* out, const float* target, float* grad, double* acc, int B, int K, int nC, int nA, int H, int W,
-                              const float* anchors_host, int anchor_step, float coord_scale, float noobject_scale, float object_scale,
-                              float class_scale, float thresh, int use_conf, float grad_scale, cudaStream_t s) {
+int ssp_region_loss_multi_fwd_bwd(const float* out, const float* target, float* grad, double* acc, int B, int K, int nC, int nA, int H, int W,
+                                  const float* anchors_host, int anchor_step, float coord_scale, float noobject_scale, float object_scale,
+                                  float class_scale, float thresh, int use_conf, float grad_scale, void* stream) {
+  const cudaStream_t s = (cudaStream_t)stream;
   if (!out || !target || !acc || !anchors_host || K < 1 || K > SSPM_MAX_KP || nA < 1 || nA > SSPM_MAX_ANCHORS || anchor_step < 2)
     return fail_msg(SSP_ERR_ARG, "region_loss_multi_fwd_bwd: bad argument");
   cudaError_t e = cudaMemsetAsync(acc, 0, 8 * sizeof(double), s);
@@ -359,8 +365,9 @@ int region_loss_multi_fwd_bwd(const float* out, const float* target, float* grad
   SSP_CHECK_LAUNCH(); return SSP_OK;
 }
 
-int region_decode_multi(const float* out, int B, int K, int nC, int nA, int H, int W, int only_objectness, int corr, float* boxes,
-                        float* conf_sel, float* det, float* cls_corr, long long* max_ind, float* max_conf, float* max_cls, cudaStream_t s) {
+int ssp_region_decode_multi(const float* out, int B, int K, int nC, int nA, int H, int W, int only_objectness, int corr, float* boxes,
+                            float* conf_sel, float* det, float* cls_corr, long long* max_ind, float* max_conf, float* max_cls, void* stream) {
+  const cudaStream_t s = (cudaStream_t)stream;
   if (!out || !boxes || !conf_sel || !det || !cls_corr || !max_ind || !max_conf || !max_cls || K < 1 || K > SSPM_MAX_KP)
     return fail_msg(SSP_ERR_ARG, "region_decode_multi: bad argument");
   const long long total = (long long)B * H * W * nA;
@@ -369,5 +376,4 @@ int region_decode_multi(const float* out, int B, int K, int nC, int nA, int H, i
   region_decode_multi_fallback_kernel<<<1, 32, 0, s>>>(det, cls_corr, B, H * W * nA, max_ind, max_conf, max_cls);
   SSP_CHECK_LAUNCH(); return SSP_OK;
 }
-
-}  // namespace ssp
+}  // extern "C"

@@ -138,14 +138,26 @@ __global__ void __launch_bounds__(256) sgd_pack_kernel(const ssp_sgd_segment* __
   }
 }
 
-int sgd_pack_step(const ssp_sgd_segment* segs_dev, int n_seg, int block_begin, int block_end, float* p, const float* g, float* v,
-                  float lr, float mu, float wd, float gscale, cudaStream_t s) {
+}  // namespace ssp
+
+using namespace ssp;
+
+extern "C" {
+// blocks of one segment, in the decomposition sgd_pack_kernel undoes: 1024 elements per block for a plain tensor, one
+// 64(ci) x 64(co) tile of one tap per block for a conv weight
+int ssp_sgd_segment_blocks(int cout, int taps, int cin, long long n) {
+  if (taps == 0) return (int)((n + 1023) / 1024);
+  return ((cin + 63) / 64) * ((cout + 63) / 64) * taps;
+}
+
+int ssp_sgd_pack_step(const ssp_sgd_segment* segs_dev, int n_seg, int block_begin, int block_end, float* p, const float* g, float* v,
+                      float lr, float mu, float wd, float gscale, void* stream) {
   if (!segs_dev || !p || !g || !v || n_seg <= 0 || block_begin < 0 || block_end < block_begin)
     return fail_msg(SSP_ERR_ARG, "sgd_pack_step: bad argument");
   if (block_end == block_begin) return SSP_OK;
-  sgd_pack_kernel<<<(unsigned)(block_end - block_begin), 256, 0, s>>>(segs_dev, n_seg, block_begin, p, g, v, SgdScalars{lr, mu, wd, gscale});
+  sgd_pack_kernel<<<(unsigned)(block_end - block_begin), 256, 0, (cudaStream_t)stream>>>(segs_dev, n_seg, block_begin, p, g, v,
+                                                                                       SgdScalars{lr, mu, wd, gscale});
   SSP_CHECK_LAUNCH();
   return SSP_OK;
 }
-
-}  // namespace ssp
+}  // extern "C"

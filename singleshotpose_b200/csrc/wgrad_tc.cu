@@ -12,6 +12,7 @@
 // [co][tap][ci] is the layout the master weights are kept in (engine.py), i.e. the gradient of nn.Conv2d.weight seen through a
 // permuted view.  Replaces the conv weight-gradient autograd computes for reference train.py:103.
 #include "ssp_common.cuh"
+#include "gemm.cuh"
 #include "tmap.cuh"
 
 namespace ssp {
