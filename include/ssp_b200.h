@@ -231,6 +231,23 @@ int ssp_adds_batched(const double* X, int nv, const double* Rt_est, const double
                      double* add_out_or_null, void* work, long long work_bytes, void* stream);
 int ssp_mesh_diameter(const double* X, int nv, double* diam_out, void* stream);
 
+/* ---- silhouette masks of a mesh under n poses: the mask/<n>.png files a training set needs (image.py:131,135), which the
+ *      reference leaves to the user (label_file_creation.md).  csrc/render.cu; the rules are in csrc/render_core.h.
+ *      X [rows][nv] fp32 vertices, rows 3 or 4 (as ssp_project_points); faces [nf][3] int32; Rt [n][3][4] fp64; K3x3 fp64.
+ *  ssp_render_masks: masks [n][H][W] uint8, 255 where the pixel centre (x, y) -- compute_projection's coordinates -- lies inside
+ *      a non-degenerate triangle of either winding, else 0.  The vertices are the fp32 coordinates ssp_project_points returns,
+ *      snapped to 1/256 px (round half to even); edge functions are exact int64, and a centre on an edge counts for top and left
+ *      edges only (Direct3D's rule).  status [n] int32: bit 0 a vertex at camera depth <= 0, bit 1 a projected coordinate that
+ *      is not finite or outside +-2^20 px, bit 2 a face index outside [0, nv); a pose with any bit set gets an all-zero mask.
+ *      work: device scratch of at least ssp_render_work_bytes(nv, nf, n, W, H) bytes (256-B aligned).  Each pose's mask depends
+ *      on nothing but its own inputs.  SSP_ERR_ARG for a null pointer, rows not 3 or 4, nv < 3, nf < 1, W or H outside
+ *      [1, 16384], n < 0 or a work buffer that is too small (ssp_render_work_bytes returns SSP_ERR_ARG for bad sizes).
+ *      n = 0 does nothing. ---- */
+long long ssp_render_work_bytes(int nv, int nf, long long n, int W, int H);
+int ssp_render_masks(const float* X, int rows, int nv, const int* faces, int nf, const double* Rt, const double* K3x3,
+                     long long n, int W, int H, unsigned char* masks, int* status, void* work, long long work_bytes,
+                     void* stream);
+
 /* ---- training-image pipeline (SURVEY 8f.3): byte-exact with the Pillow routines image.py calls.  Images are device
  *      uint8 HWC RGB, dense.  resample = PIL.Image.Resampling value (0 NEAREST, 2 BILINEAR, 3 BICUBIC = resize()'s default
  *      in Pillow >= 7).  `work` is caller-provided device scratch (16-B aligned) of at least *_work_bytes() bytes.

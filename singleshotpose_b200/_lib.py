@@ -59,6 +59,8 @@ SIGNATURES = {
     "ssp_adds_work_bytes": [_i, _ll],
     "ssp_adds_batched": [_p, _i, _p, _p, _ll, _p, _p, _p, _ll, _p],
     "ssp_mesh_diameter": [_p, _i, _p, _p],
+    "ssp_render_work_bytes": [_i, _i, _ll, _i, _i],
+    "ssp_render_masks": [_p, _i, _i, _p, _i, _p, _p, _ll, _i, _i, _p, _p, _p, _ll, _p],
     "ssp_aug_resize_work_bytes": [_i, _i, _i, _i, _i],
     "ssp_aug_resize_u8": [_p, _i, _i, _i, _i, _i, _i, _p, _i, _i, _i, _p, _ll, _p],
     "ssp_aug_rgb2hsv_u8": [_p, _p, _ll, _p],
@@ -85,7 +87,7 @@ SIGNATURES = {
 _RESTYPE = {"ssp_last_error": C.c_char_p, "ssp_flat_alloc_rows": _ll, "ssp_flat_row": _ll,
             "ssp_jpeg_decline_reason": C.c_char_p, "ssp_jpeg_stage_bytes": _ll, "ssp_jpeg_work_bytes": _ll,
             "ssp_aug_resize_work_bytes": _ll, "ssp_aug_sample_work_bytes": _ll, "ssp_aug_batch_table_bytes": _ll,
-            "ssp_augm_work_bytes": _ll, "ssp_augm_table_bytes": _ll, "ssp_adds_work_bytes": _ll}
+            "ssp_augm_work_bytes": _ll, "ssp_augm_table_bytes": _ll, "ssp_adds_work_bytes": _ll, "ssp_render_work_bytes": _ll}
 
 _lib = None
 

@@ -166,6 +166,51 @@ def write_linemod_like(root, n=4, ow=160, oh=120, num_bg=3, fmt="png"):
     return listfile, bgs
 
 
+def closed_mesh(rings=60, segments=100, half_extents=(0.038, 0.039, 0.046), bumps=0.15, seed=0):
+    """A closed, LINEMOD-sized triangle mesh: a latitude-longitude ellipsoid (two poles, `rings` rings of `segments` vertices)
+    whose radius is modulated by a few seeded bumps (bumps=0: the plain ellipsoid, which is convex).  The defaults give 6002
+    vertices and 12000 faces, about the size of a LINEMOD mesh.  Returns (vertices (Nv, 3) float64, rounded to 6 decimals as an
+    ASCII PLY stores them, faces (Nf, 3) int32), every face wound the same way."""
+    rng = np.random.default_rng(seed)
+    th = np.pi * (np.arange(rings) + 1) / (rings + 1)                       # polar angle of each ring
+    ph = 2 * np.pi * np.arange(segments) / segments
+    T, P = np.meshgrid(th, ph, indexing="ij")
+    d = np.stack([np.sin(T) * np.cos(P), np.sin(T) * np.sin(P), np.cos(T)], -1).reshape(-1, 3)
+    d = np.concatenate([[[0.0, 0.0, 1.0]], d, [[0.0, 0.0, -1.0]]])
+    k = rng.normal(size=(4, 3))
+    k /= np.linalg.norm(k, axis=1, keepdims=True)
+    r = 1.0 + bumps * np.tanh(np.cos(3 * d @ k.T + rng.uniform(0, 2 * np.pi, 4)).sum(1))
+    V = np.round(d * r[:, None] * np.asarray(half_extents), 6)
+    ring = lambda i, j: 1 + i * segments + j % segments
+    F = [[0, ring(0, j + 1), ring(0, j)] for j in range(segments)]
+    for i in range(rings - 1):
+        for j in range(segments):
+            a, b, c, e = ring(i, j), ring(i, j + 1), ring(i + 1, j), ring(i + 1, j + 1)
+            F += [[a, b, e], [a, e, c]]
+    last = len(d) - 1
+    F += [[last, ring(rings - 1, j), ring(rings - 1, j + 1)] for j in range(segments)]
+    return V, np.array(F, dtype=np.int32)
+
+
+def write_ply(path, vertices, faces):
+    """ASCII PLY with a vertex element (x, y, z) and a face element (vertex_indices), the layout of the LINEMOD meshes"""
+    with open(path, "w") as f:
+        f.write("ply\nformat ascii 1.0\nelement vertex %d\nproperty float x\nproperty float y\nproperty float z\n"
+                "element face %d\nproperty list uchar int vertex_indices\nend_header\n" % (len(vertices), len(faces)))
+        f.writelines("%.6f %.6f %.6f\n" % tuple(v) for v in vertices)
+        f.writelines("3 %d %d %d\n" % tuple(t) for t in faces)
+
+
+def object_poses(n, seed=0, depth=(0.6, 1.1)):
+    """n poses (R (n, 3, 3), t (n, 3)) of an object-sized mesh in front of the LINEMOD camera, fully inside a 640 x 480 view"""
+    rng = np.random.default_rng(seed)
+    ax = rng.normal(size=(n, 3))
+    ax /= np.linalg.norm(ax, axis=1, keepdims=True)
+    R = _rodrigues(ax * rng.uniform(0, np.pi, size=(n, 1)))
+    t = np.stack([rng.uniform(-.08, .08, n), rng.uniform(-.06, .06, n), rng.uniform(*depth, n)], 1)
+    return R, t
+
+
 LINEMOD_OBJECTS = ("ape", "benchvise", "cam", "can", "cat", "driller", "duck", "eggbox", "glue", "holepuncher", "iron", "lamp", "phone")
 
 

@@ -13,7 +13,8 @@ import torch
 from ._lib import call, load, ptr, stream_ptr, SspError
 from .utils_host import (makedirs, get_all_files, calc_pts_diameter, adi, get_2d_bb, compute_2d_bb, compute_2d_bb_from_orig_pix,  # noqa: F401
                          corner_confidences, corner_confidence, sigmoid, softmax, fix_corner_order, read_truths, read_truths_args,
-                         read_pose, load_class_names, image2torch, read_data_cfg, scale_bboxes, file_lines, get_image_size, logging)
+                         read_pose, load_class_names, image2torch, read_data_cfg, scale_bboxes, file_lines, get_image_size, logging,
+                         label_rows_from_projection)
 
 
 def _dev():
@@ -184,6 +185,57 @@ def mesh_diameter(pts):
     out = torch.empty(1, dtype=torch.float64, device=dev)
     call("ssp_mesh_diameter", ptr(P), P.shape[0], ptr(out), stream_ptr())
     return float(out.item())
+
+
+# ------------------------------------------------------------------------------------------ training-set creation
+RENDER_CHUNK_BYTES = 1 << 30           # device scratch of one ssp_render_masks launch; larger batches go in chunks
+
+
+def render_masks(vertices, faces, Rt, K, width, height):
+    """Silhouette masks of a mesh under n poses, as LINEMOD's mask/*.png: (n, H, W) uint8 CUDA tensor, 255 where the pixel
+    centre (x, y) lies inside the projected mesh, and (n,) int32 status (bit 0 a vertex behind the camera, bit 1 a projected
+    coordinate outside +-2^20 px, bit 2 a bad face index; such a pose's mask is all zeros).  The vertices are projected by
+    ssp_project_points, the kernel of project_points_batched, so masks and label rows agree.  The exact rule is in
+    csrc/render_core.h.  vertices (Nv, 3) or (3|4, Nv); faces (Nf, 3) int; Rt (n, 3, 4); K (3, 3)."""
+    dev = _dev()
+    V = torch.as_tensor(np.asarray(vertices) if not torch.is_tensor(vertices) else vertices)
+    if V.dim() != 2 or not (V.shape[0] in (3, 4) or V.shape[1] == 3):
+        raise SspError("vertices must be (3|4, Nv) or (Nv, 3), got %s" % (tuple(V.shape),))
+    X = (V if V.shape[0] in (3, 4) else V.t()).to(dev, torch.float32).contiguous()
+    F = torch.as_tensor(np.asarray(faces) if not torch.is_tensor(faces) else faces).to(dev, torch.int32).contiguous()
+    if F.dim() != 2 or F.shape[1] != 3:
+        raise SspError("faces must be (Nf, 3), got %s" % (tuple(F.shape),))
+    T = _pose_stack(Rt, dev)
+    Kd = torch.as_tensor(np.asarray(K) if not torch.is_tensor(K) else K).to(dev, torch.float64).contiguous()
+    n, nv, nf, W, H = T.shape[0], X.shape[1], F.shape[0], int(width), int(height)
+    masks = torch.empty(n, H, W, dtype=torch.uint8, device=dev)
+    status = torch.empty(n, dtype=torch.int32, device=dev)
+    lib = load()
+    per_pose = int(lib.ssp_render_work_bytes(nv, nf, 1, W, H))
+    if per_pose < 0:
+        raise SspError("ssp_render_work_bytes: bad size (Nv = %d, Nf = %d, %d x %d)" % (nv, nf, W, H))
+    chunk = max(1, RENDER_CHUNK_BYTES // per_pose)
+    work = None
+    for p0 in range(0, n, chunk):
+        m = min(chunk, n - p0)
+        wb = int(lib.ssp_render_work_bytes(nv, nf, m, W, H))
+        if work is None:
+            work = torch.empty(wb, dtype=torch.uint8, device=dev)
+        call("ssp_render_masks", ptr(X), X.shape[0], nv, ptr(F), nf, ptr(T[p0:p0 + m]), ptr(Kd), m, W, H, ptr(masks[p0:p0 + m]),
+             ptr(status[p0:p0 + m]), ptr(work), work.numel(), stream_ptr())
+    return masks, status
+
+
+def pose_label_rows(corners3D, Rt, K, width, height, class_id=0):
+    """(n, 21) float64 label rows of label_file_creation.md for n poses: the class, the projected model origin [0, 0, 0] and
+    the 8 corners (corners3D (3|4, 8), get_3D_corners' order) over the image size, then the x and y ranges of the 8 projected
+    corners over the image size.  The projection is project_points_batched's; the row rule is label_rows_from_projection."""
+    C3 = np.asarray(corners3D, dtype=np.float64)[:3]
+    if C3.shape != (3, 8):
+        raise SspError("corners3D must be (3|4, 8), got %s" % (C3.shape,))
+    P9 = np.concatenate([np.zeros((3, 1)), C3], 1)
+    px = project_points_batched(P9, Rt, K).cpu().numpy()
+    return label_rows_from_projection(px, width, height, class_id)
 
 
 # ------------------------------------------------------------------------------------------ batched evaluation tail

@@ -143,6 +143,24 @@ def read_truths_args(lab_path, num_keypoints=9):
     return np.ascontiguousarray(truths[:, :num_labels]).reshape(-1)
 
 
+def label_rows_from_projection(px, width, height, class_id=0):
+    """Label rows of label_file_creation.md from the projected keypoints px (n, 2, 9) -- column 0 the model origin [0, 0, 0],
+    columns 1-8 the get_3D_corners corners, in pixels as compute_projection returns them -> (n, 21) float64:
+    [class, x0/w, y0/h, ..., x8/w, y8/h, x range, y range], the ranges being the width and height of the tight box around the 8
+    projected corners only (step 4), over the image size.  The pixel values are taken as float64, then divided."""
+    P = np.asarray(px, dtype=np.float64)
+    if P.ndim != 3 or P.shape[1:] != (2, 9):
+        raise ValueError("projected keypoints must be (n, 2, 9), got %s" % (P.shape,))
+    n = P.shape[0]
+    rows = np.empty((n, 21))
+    rows[:, 0] = class_id
+    rows[:, 1:19:2] = P[:, 0] / float(width)
+    rows[:, 2:19:2] = P[:, 1] / float(height)
+    rows[:, 19] = (P[:, 0, 1:].max(1) - P[:, 0, 1:].min(1)) / float(width)
+    rows[:, 20] = (P[:, 1, 1:].max(1) - P[:, 1, 1:].min(1)) / float(height)
+    return rows
+
+
 def read_pose(lab_path):
     """utils.py:419-424"""
     if os.path.getsize(lab_path):
@@ -164,9 +182,22 @@ def image2torch(img):
 
 def read_ply_vertices(path):
     """(Nv, 3) float64 x, y, z of the `vertex` element of an ASCII PLY file (the format of the LINEMOD meshes the .data file's
-    `mesh` entry names).  Written from the PLY format: a header of `element <name> <count>` lines, each followed by its
-    `property <type> <name>` / `property list <count type> <item type> <name>` lines, closed by `end_header`; then one text line
-    per element item, the elements in header order.  Binary PLY is refused."""
+    `mesh` entry names).  Binary PLY is refused."""
+    return _read_ply(path, faces=False)[0]
+
+
+def read_ply_mesh(path):
+    """(vertices (Nv, 3) float64, faces (Nf, 3) int32) of an ASCII PLY file: the `vertex` element's x, y, z and the `face`
+    element's vertex index lists.  Every face must be a triangle ("triangulate the mesh first") whose indices lie in [0, Nv).
+    Binary PLY is refused."""
+    return _read_ply(path, faces=True)
+
+
+def _read_ply(path, faces):
+    """Written from the PLY format: a header of `element <name> <count>` lines, each followed by its `property <type> <name>` /
+    `property list <count type> <item type> <name>` lines, closed by `end_header`; then one text line per element item, the
+    elements in header order.  faces=False stops after the vertex element and returns (V, None)."""
+    V = F = None
     with open(path, "rb") as f:
         if f.readline().strip() != b"ply":
             raise ValueError("%s: not a PLY file" % path)
@@ -189,19 +220,41 @@ def read_ply_vertices(path):
         if fmt != "ascii":
             raise ValueError("%s: PLY format %r is not supported (ASCII PLY only)" % (path, fmt))
         for name, count, props in elements:
-            if name != "vertex":
+            if name == "vertex" and V is None:
+                try:
+                    cols = [props.index(a) for a in ("x", "y", "z")]
+                except ValueError:
+                    raise ValueError("%s: the vertex element has no x, y, z properties" % path)
+                rows = [f.readline().split() for _ in range(count)]
+                if any(len(r) < len(props) for r in rows):
+                    raise ValueError("%s: truncated vertex data" % path)
+                V = np.array([[float(r[c]) for c in cols] for r in rows], dtype=np.float64).reshape(count, 3)
+                if not faces:
+                    return V, None
+            elif name == "face" and faces and F is None:
+                if not props or props[0] not in ("vertex_indices", "vertex_index"):
+                    raise ValueError("%s: the face element does not start with a vertex_indices list" % path)
+                rows = [f.readline().split() for _ in range(count)]
+                if any(not r for r in rows):
+                    raise ValueError("%s: truncated face data" % path)
+                for i, r in enumerate(rows):
+                    if int(r[0]) != 3:
+                        raise ValueError("%s: face %d has %s vertices: triangulate the mesh first" % (path, i, r[0]))
+                    if len(r) < 4:
+                        raise ValueError("%s: truncated face data" % path)
+                F = np.array([[int(v) for v in r[1:4]] for r in rows], dtype=np.int64).reshape(count, 3)
+            else:
                 for _ in range(count):     # one text line per item, whatever its properties
                     f.readline()
-                continue
-            try:
-                cols = [props.index(a) for a in ("x", "y", "z")]
-            except ValueError:
-                raise ValueError("%s: the vertex element has no x, y, z properties" % path)
-            rows = [f.readline().split() for _ in range(count)]
-            if any(len(r) < len(props) for r in rows):
-                raise ValueError("%s: truncated vertex data" % path)
-            return np.array([[float(r[c]) for c in cols] for r in rows], dtype=np.float64).reshape(count, 3)
-    raise ValueError("%s: no vertex element" % path)
+    if V is None:
+        raise ValueError("%s: no vertex element" % path)
+    if F is None:
+        raise ValueError("%s: no face element" % path)
+    bad = (F < 0) | (F >= len(V))
+    if bad.any():
+        i = int(np.flatnonzero(bad.any(axis=1))[0])
+        raise ValueError("%s: face %d has a vertex index outside [0, %d)" % (path, i, len(V)))
+    return V, F.astype(np.int32)
 
 
 def read_data_cfg(datacfg):
