@@ -255,29 +255,26 @@ int ssp_render_masks(const float* X, int rows, int nv, const int* faces, int nf,
  *      the crop window may stick out of the source (zero fill), pass (0, 0, src_w, src_h) for a plain resize.
  *  ssp_aug_rgb2hsv_u8 / hsv2rgb_u8: Image.convert('HSV') / ('RGB') (image.py:15,30).
  *  ssp_aug_to_tensor_u8: torchvision ToTensor (the `transform` of dataset.py:103-118) of a dense uint8 HWC image: float32 CHW,
- *      byte / 255 as an IEEE division (what the CPU reference computes; a reciprocal multiply differs by 1 ulp).
- *  ssp_aug_sample: change_background (image.py:110-127) -> crop -> resize -> distort_image (image.py:14-32) -> ToTensor
- *      (dataset.py transform) for one sample.  luts = 5 x 256 bytes: posmask, negmask (image.py:121-122), hue, saturation,
- *      value (image.py:17-27) point() tables, built by the host exactly as Image.point() builds them.  Crop window
- *      (pleft, ptop, cw, ch) with cw = swidth - 1, ch = sheight - 1 (image.py:64).  out_u8 (HWC) and out_chw (float32
- *      CHW in [0,1]) are both optional, at least one required. ---- */
+ *      byte / 255 as an IEEE division (what the CPU reference computes; a reciprocal multiply differs by 1 ulp). ---- */
 long long ssp_aug_resize_work_bytes(int in_w, int in_h, int out_w, int out_h, int resample);
 int ssp_aug_resize_u8(const void* src, int src_w, int src_h, int x0, int y0, int in_w, int in_h, void* dst, int out_w,
                       int out_h, int resample, void* work, long long work_bytes, void* stream);
 int ssp_aug_rgb2hsv_u8(const void* rgb, void* hsv, long long n_pixels, void* stream);
 int ssp_aug_hsv2rgb_u8(const void* hsv, void* rgb, long long n_pixels, void* stream);
 int ssp_aug_to_tensor_u8(const void* hwc_u8, long long n_pixels, float* out_chw, void* stream);
-long long ssp_aug_sample_work_bytes(int ow, int oh, int bw, int bh, int cw, int ch, int out_w, int out_h, int resample);
-int ssp_aug_sample(const void* img, const void* mask, int ow, int oh, const void* bg, int bw, int bh, const void* luts,
-                   int pleft, int ptop, int cw, int ch, int out_w, int out_h, int resample, void* work,
-                   long long work_bytes, void* out_u8_or_null, float* out_chw_or_null, void* stream);
 
-/* Batched form of ssp_aug_sample: ONE launch per pipeline stage for the whole batch (<= 10 launches instead of ~10 per sample).
- *   ssp_aug_batch_plan (host only, no device access): items[n] hold the per-sample arguments of ssp_aug_sample with DEVICE
- *     pointers (each sample its own work buffer of ssp_aug_sample_work_bytes()); writes the op table (table_bytes >=
- *     ssp_aug_batch_table_bytes(n)) into HOST memory -- typically the tail of the pinned staging buffer, so that it travels in the
- *     batch's single host->device copy -- and stage_dims[20].
+/* Training-image batch: change_background (image.py:110-127) -> crop -> resize -> distort_image (image.py:14-32) -> ToTensor
+ * (dataset.py transform) for every sample, with ONE launch per pipeline stage for the whole batch (<= 10 launches).
+ *   ssp_aug_item, one per sample, with DEVICE pointers: img and mask (ow x oh), bg (bw x bh); luts = 5 x 256 bytes: posmask,
+ *     negmask (image.py:121-122), hue, saturation, value (image.py:17-27) point() tables, built by the host exactly as
+ *     Image.point() builds them; crop window (pleft, ptop, cw, ch) with cw = swidth - 1, ch = sheight - 1 (image.py:64); its own
+ *     work buffer of ssp_aug_sample_work_bytes() bytes; out_u8 (HWC) and out_chw (float32 CHW in [0,1]) are both optional, at
+ *     least one required.
+ *   ssp_aug_batch_plan (host only, no device access): writes the op table (table_bytes >= ssp_aug_batch_table_bytes(n)) into
+ *     HOST memory -- typically the tail of the pinned staging buffer, so that it travels in the batch's single host->device
+ *     copy -- and stage_dims[20].
  *   ssp_aug_batch_run: table_dev = the device copy of that table; launches the stages on `stream`. */
+long long ssp_aug_sample_work_bytes(int ow, int oh, int bw, int bh, int cw, int ch, int out_w, int out_h, int resample);
 typedef struct ssp_aug_item {
   const void* img; const void* mask; int ow, oh; const void* bg; int bw, bh; const void* luts; int pleft, ptop, cw, ch;
   void* work; long long work_bytes; void* out_u8; float* out_chw;
@@ -290,7 +287,7 @@ int ssp_aug_batch_run(const void* table_dev, int n, const int* stage_dims_host20
 /* ---- multi-object training-image pipeline (multi_obj_pose_estimation/image_multi.py load_data_detection), byte-exact with the
  *      Pillow routines it calls.  Per sample the caller owns four network-size (out_w x out_h x 3 bytes) device images --
  *      main_img, main_mask, total_img, total_mask -- and counts[4] (unsigned): [S, I, accepted, unused].  luts = posmask | negmask
- *      (2 x 256 bytes, as in ssp_aug_sample).  Every item needs its own 16-B aligned work buffer of
+ *      (2 x 256 bytes, as in ssp_aug_item).  Every item needs its own 16-B aligned work buffer of
  *      ssp_augm_work_bytes(in_w, in_h, out_w, out_h) bytes, with (in_w, in_h) = the crop window (cw, ch) for begin / attempt
  *      and the background size for finish.  The plan calls only write HOST memory (no allocation, no device access, no
  *      synchronisation); ssp_augm_run launches the planned stages of one phase (<= 16 launches for the whole batch) on

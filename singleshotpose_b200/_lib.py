@@ -70,7 +70,6 @@ SIGNATURES = {
     "ssp_aug_batch_plan": [_p, _i, _i, _i, _i, _p, _ll, _p],
     "ssp_aug_batch_run": [_p, _i, _p, _p],
     "ssp_aug_sample_work_bytes": [_i, _i, _i, _i, _i, _i, _i, _i, _i],
-    "ssp_aug_sample": [_p, _p, _i, _i, _p, _i, _i, _p, _i, _i, _i, _i, _i, _i, _i, _p, _ll, _p, _p, _p],
     "ssp_augm_work_bytes": [_i, _i, _i, _i, _i],
     "ssp_augm_table_bytes": [_i],
     "ssp_augm_plan_begin": [_p, _i, _i, _i, _i, _p, _ll, _p],

@@ -28,36 +28,14 @@ __global__ void aug_nearest_kernel(const PassArgs a) {
   if (x < a.dst_w && y < a.dst_h) nearest_px(a, x, y);
 }
 
-__global__ void aug_composite_kernel(const uint8_t* __restrict__ img, const uint8_t* __restrict__ bg, const uint8_t* __restrict__ mask,
-                                     const uint8_t* __restrict__ lut_pos, const uint8_t* __restrict__ lut_neg, long long n,
-                                     uint8_t* __restrict__ out) {
-  __shared__ uint8_t lp[256], ln[256];
-  for (int i = threadIdx.x; i < 256; i += blockDim.x) { lp[i] = lut_pos[i]; ln[i] = lut_neg[i]; }
-  __syncthreads();
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-    out[i] = composite_px(img[i], bg[i], mask[i], lp, ln);
-}
-
-// mode 0: distort_image (three tables) ; 1: rgb -> hsv only ; 2: hsv -> rgb only (the last two for exhaustive parity tests)
-__global__ void aug_distort_kernel(const uint8_t* __restrict__ src, long long n_px, const uint8_t* __restrict__ luts, int mode,
-                                   uint8_t* __restrict__ out_u8, float* __restrict__ out_chw) {
-  __shared__ uint8_t lut[768];
-  if (mode == 0) {
-    for (int i = threadIdx.x; i < 768; i += blockDim.x) lut[i] = luts[i];
-    __syncthreads();
-  }
+// mode 1: rgb -> hsv only ; 2: hsv -> rgb only (the halves of distort_px, for exhaustive parity tests)
+__global__ void aug_distort_kernel(const uint8_t* __restrict__ src, long long n_px, int mode, uint8_t* __restrict__ out_u8) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n_px; i += (long long)gridDim.x * blockDim.x) {
     const uint8_t* s = src + 3 * i;
     uint8_t o[3];
-    if (mode == 0) distort_px(s, lut, lut + 256, lut + 512, o);
-    else if (mode == 1) rgb2hsv_px(s[0], s[1], s[2], o);
+    if (mode == 1) rgb2hsv_px(s[0], s[1], s[2], o);
     else hsv2rgb_px(s[0], s[1], s[2], o);
-    if (out_u8) { out_u8[3 * i] = o[0]; out_u8[3 * i + 1] = o[1]; out_u8[3 * i + 2] = o[2]; }
-    if (out_chw) {                      // torchvision ToTensor: byte -> float32, divided by 255 (IEEE division), CHW planes
-      out_chw[i] = (float)o[0] / 255.0f;
-      out_chw[n_px + i] = (float)o[1] / 255.0f;
-      out_chw[2 * n_px + i] = (float)o[2] / 255.0f;
-    }
+    out_u8[3 * i] = o[0]; out_u8[3 * i + 1] = o[1]; out_u8[3 * i + 2] = o[2];
   }
 }
 
@@ -111,13 +89,6 @@ struct CudaBackend {
     dim3 b(32, 8), g((a.dst_w + 31) / 32, (a.dst_h + 7) / 8);
     aug_nearest_kernel<<<g, b, 0, s>>>(a);
   }
-  void composite(const uint8_t* img, const uint8_t* bg, const uint8_t* mask, const uint8_t* lp, const uint8_t* ln, long long n, uint8_t* out) {
-    aug_composite_kernel<<<blocks_for(n, 256), 256, 0, s>>>(img, bg, mask, lp, ln, n, out);
-  }
-  void distort(const uint8_t* src, int w, int h, const uint8_t* luts, uint8_t* out_u8, float* out_chw) {
-    const long long n = (long long)w * h;
-    aug_distort_kernel<<<blocks_for(n, 256), 256, 0, s>>>(src, n, luts, 0, out_u8, out_chw);
-  }
 };
 int driver_rc(int rc, const char* who) {
   if (rc == 0) return SSP_OK;
@@ -131,7 +102,7 @@ int driver_rc(int rc, const char* who) {
 static int aug_convert_u8(const uint8_t* src, uint8_t* dst, long long n_px, int mode, cudaStream_t s) {
   if (!src || !dst || n_px < 0 || (mode != 1 && mode != 2)) return fail_msg(SSP_ERR_ARG, "ssp_aug_rgb2hsv_u8/hsv2rgb_u8: bad argument");
   if (n_px == 0) return SSP_OK;
-  aug_distort_kernel<<<blocks_for(n_px, 256), 256, 0, s>>>(src, n_px, nullptr, mode, dst, nullptr);
+  aug_distort_kernel<<<blocks_for(n_px, 256), 256, 0, s>>>(src, n_px, mode, dst);
   SSP_CHECK_LAUNCH();
   return SSP_OK;
 }
@@ -251,18 +222,6 @@ int ssp_augm_run(const void* table_dev, int n, const int* stage_dims, void* stre
     dim3 grid((nx + 31) / 32, (ny + 7) / 8, n);
     aug_stage_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(ops + (long long)st * n);
   }
-  SSP_CHECK_LAUNCH();
-  return SSP_OK;
-}
-
-int ssp_aug_sample(const void* img, const void* mask, int ow, int oh, const void* bg, int bw, int bh, const void* luts, int pleft, int ptop, int cw,
-                   int ch, int out_w, int out_h, int resample, void* work, long long work_bytes, void* out_u8, float* out_chw, void* stream) {
-  if (!img || !mask || !bg || !luts || !work || (!out_u8 && !out_chw)) return fail_msg(SSP_ERR_ARG, "ssp_aug_sample: null pointer");
-  if ((uintptr_t)work % 16) return fail_msg(SSP_ERR_ARG, "ssp_aug_sample: work buffer must be 16-B aligned");
-  CudaBackend be{(cudaStream_t)stream};
-  const int rc = augment_sample_driver(be, (const uint8_t*)img, (const uint8_t*)mask, ow, oh, (const uint8_t*)bg, bw, bh, (const uint8_t*)luts,
-                                       pleft, ptop, cw, ch, out_w, out_h, resample, (uint8_t*)work, work_bytes, (uint8_t*)out_u8, out_chw);
-  if (rc) return driver_rc(rc, "ssp_aug_sample");
   SSP_CHECK_LAUNCH();
   return SSP_OK;
 }

@@ -9,10 +9,6 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 SOURCES = ["abi.cu", "conv_tc.cu", "conv_band.cu", "conv_bandt.cu", "wgrad_tc.cu", "conv_simt.cu", "l0_fused.cu", "elementwise.cu", "sgd_pack.cu", "region.cu", "region_multi.cu", "pnp.cu", "augment.cu", "adds.cu", "jpeg.cu", "render.cu"]
 # augment.cu restates Pillow's float/double pixel arithmetic bit for bit: no multiply-add contraction there
 EXTRA = {"augment.cu": ["-fmad=false"]}
-for _env, _macro in (("SSP_BN_MINBLOCKS", "SSP_BN_MINBLOCKS"), ("SSP_BN_UNITS", "BN_UNITS_PER_THREAD"),
-                     ("SSP_BN_REDUCE_UNITS", "BWD_REDUCE_UNITS_PER_THREAD")):      # experiment knobs, see elementwise.cu
-    if os.environ.get(_env):
-        EXTRA.setdefault("elementwise.cu", []).append("-D%s=%d" % (_macro, int(os.environ[_env])))
 LIB = os.path.join(HERE, "libssp_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",

@@ -9,11 +9,8 @@
 // Occupancy of the HBM-bound BN kernels: uncapped they use 97-118 registers -> 2 blocks/SM, 23 % warps active, 47-63 % of DRAM
 // peak under ncu (round 1).  Capped at 85 registers for a third resident block (a few spilled bytes per thread): same-box A/B
 // of the batch-64 step in round 2: 18.35 -> 17.92 ms (a fourth block, 64 registers, spills too much: 18.86 ms).
-// SSP_BN_MINBLOCKS=n python csrc/build.py rebuilds with another cap.
-#ifndef SSP_BN_MINBLOCKS
-#define SSP_BN_MINBLOCKS 3
-#endif
-#define SSP_BN_BOUNDS __launch_bounds__(256, SSP_BN_MINBLOCKS)
+constexpr int kBnMinBlocks = 3;
+#define SSP_BN_BOUNDS __launch_bounds__(256, kBnMinBlocks)
 
 namespace ssp {
 
@@ -157,16 +154,14 @@ static inline unsigned unit_grid(int C, long long nunits, int per_thread) {
   const long long per = (long long)PL * per_thread;
   return (unsigned)(((nunits + per - 1) / per) * cblocks);
 }
-#ifndef BN_UNITS_PER_THREAD      // build-time sweep knob (SSP_BN_UNITS=n python csrc/build.py); 8 is the measured default
-#define BN_UNITS_PER_THREAD 8
-#endif
+constexpr int kBnUnitsPerThread = 8;          // BN units (channel quad x pixel or 2x2 window) per thread, chosen by a measured sweep
 
 // POOLED = true : unit = one 2x2 window (needed when any destination is DST_POOL)
 // SPLIT = true  : y is the sum of the split-K partial slabs of ssp_conv_gemm_splitk (inference, no arg-max plane)
 template <bool POOLED, bool SPLIT = false>
 __global__ void SSP_BN_BOUNDS bn_apply_kernel(const BnApplyParams p) {
   const int Hs = POOLED ? p.H / 2 : p.H, Ws = POOLED ? p.W / 2 : p.W;
-  UnitWalk wk(p.C, (long long)p.N * Hs * Ws, BN_UNITS_PER_THREAD);
+  UnitWalk wk(p.C, (long long)p.N * Hs * Ws, kBnUnitsPerThread);
   if (!wk.active) return;
   const int c = wk.c;
   const float4 sc = *reinterpret_cast<const float4*>(p.scale + c);
@@ -339,16 +334,14 @@ struct BwdUnit {
   }
 };
 
-#ifndef BWD_REDUCE_UNITS_PER_THREAD   // build-time sweep knob (SSP_BN_REDUCE_UNITS=n); 32 is the measured default
-#define BWD_REDUCE_UNITS_PER_THREAD 32
-#endif
+constexpr int kBwdReduceUnitsPerThread = 32;  // the same for the BN-backward reduction, chosen by a measured sweep
 
 template <int K0, int K1>
 __global__ void SSP_BN_BOUNDS bn_bwd_reduce_kernel(const BnBwdParams p) {
   extern __shared__ float red[];           // [2][PL][CG*4]
   constexpr bool POOLED = BwdUnit<K0, K1>::POOLED;
   const int Hs = POOLED ? p.H / 2 : p.H, Ws = POOLED ? p.W / 2 : p.W;
-  UnitWalk wk(p.C, (long long)p.N * Hs * Ws, BWD_REDUCE_UNITS_PER_THREAD);
+  UnitWalk wk(p.C, (long long)p.N * Hs * Ws, kBwdReduceUnitsPerThread);
   constexpr int NP = POOLED ? 4 : 1;
   constexpr int UNR = POOLED ? 1 : 4;
   const int c = wk.c;
@@ -392,7 +385,7 @@ template <int K0, int K1>
 __global__ void SSP_BN_BOUNDS bn_bwd_apply_kernel(const BnBwdParams p) {
   constexpr bool POOLED = BwdUnit<K0, K1>::POOLED;
   const int Hs = POOLED ? p.H / 2 : p.H, Ws = POOLED ? p.W / 2 : p.W;
-  UnitWalk wk(p.C, (long long)p.N * Hs * Ws, BN_UNITS_PER_THREAD);
+  UnitWalk wk(p.C, (long long)p.N * Hs * Ws, kBnUnitsPerThread);
   if (!wk.active) return;
   constexpr int NP = POOLED ? 4 : 1;
   constexpr int UNR = POOLED ? 1 : 4;
@@ -536,7 +529,7 @@ static int bn_apply_splitk(const float* y, int splits, long long slab, int y_ld,
   p.splits = splits; p.slab = slab;
   const bool halves = pooled || p.dst[0].kind == DST_REORG || p.dst[1].kind == DST_REORG;
   if (halves && ((H | W) & 1)) return fail_msg(SSP_ERR_ARG, "bn_apply: pool/reorg need even H and W");
-  const unsigned grid = pooled ? unit_grid(C, (long long)N * (H / 2) * (W / 2), BN_UNITS_PER_THREAD) : unit_grid(C, (long long)N * H * W, BN_UNITS_PER_THREAD);
+  const unsigned grid = pooled ? unit_grid(C, (long long)N * (H / 2) * (W / 2), kBnUnitsPerThread) : unit_grid(C, (long long)N * H * W, kBnUnitsPerThread);
   if (splits > 1) {
     if (pooled) bn_apply_kernel<true, true><<<grid, 256, 0, s>>>(p);
     else bn_apply_kernel<false, true><<<grid, 256, 0, s>>>(p);
@@ -614,7 +607,7 @@ int ssp_bn_bwd_reduce(const float* y, int y_ld, const float* scale, const float*
   const int cgs = C / 4, CG = cgs < 256 ? cgs : 256, PL = 256 / CG;
   const long long nunits = (long long)N * (pooled ? H / 2 : H) * (pooled ? W / 2 : W);
   const size_t sm = (size_t)2 * PL * CG * 4 * sizeof(float);
-  const unsigned grid = unit_grid(C, nunits, BWD_REDUCE_UNITS_PER_THREAD);
+  const unsigned grid = unit_grid(C, nunits, kBwdReduceUnitsPerThread);
 #define SSP_BWD_DISPATCH(KERN, ...)                                                                                  \
   do {                                                                                                              \
     const int k0 = p.src[0].kind, k1 = p.src[1].kind;                                                               \
@@ -642,7 +635,7 @@ int ssp_bn_bwd_apply(const float* y, int y_ld, const float* scale, const float* 
   p.dy = (uint16_t*)dy; p.dy_ld = dy_ld; p.dy_fmt = dy_fmt; p.dy_scale = dy_scale;
   const bool pooled = p.src[0].kind == SRC_POOL || p.src[1].kind == SRC_POOL;
   const long long nunits = (long long)N * (pooled ? H / 2 : H) * (pooled ? W / 2 : W);
-  const unsigned grid = unit_grid(C, nunits, BN_UNITS_PER_THREAD);
+  const unsigned grid = unit_grid(C, nunits, kBnUnitsPerThread);
   SSP_BWD_DISPATCH(bn_bwd_apply_kernel, grid, 256, 0, (cudaStream_t)stream);
   SSP_CHECK_LAUNCH(); return SSP_OK;
 }

@@ -7,10 +7,14 @@ from __future__ import annotations
 
 import torch
 
+from .optim import FlatSGD
+
 
 class GraphedTrainStep:
     def __init__(self, model, criterion, optimizer, batch_shape, target_shape, epoch, device, all_reduce=False, warmup=3):
         self.model, self.criterion, self.optimizer, self.epoch = model, criterion, optimizer, epoch
+        # any other optimizer (torch.optim.SGD on the parameter views) leaves the conv operand planes stale after its step
+        self._sgd_repacks = isinstance(optimizer, FlatSGD)
         self.x = torch.zeros(batch_shape, dtype=torch.float32, device=device)
         self.t = torch.zeros(target_shape, dtype=torch.float32, device=device)
         self.all_reduce = all_reduce
@@ -20,7 +24,7 @@ class GraphedTrainStep:
         self._captured = None
 
     def _hyper(self):
-        """everything the captured launches carry BY VALUE: lr / momentum / weight decay (kernel scalars of ssp_sgd_step_flat) and
+        """everything the captured launches carry BY VALUE: lr / momentum / weight decay (kernel scalars of ssp_sgd_pack_step) and
         the confidence-loss gate epoch > pretrain_num_epochs (region_loss.py:156).  adjust_learning_rate (train.py:34-46) rewrites
         param_groups every batch and the gate flips once per run: a replay with stale values would silently train wrong."""
         g = self.optimizer.param_groups[0]
@@ -34,12 +38,12 @@ class GraphedTrainStep:
         if self.graph is None or self._captured != self._hyper():
             self.capture(warmup=0 if self.graph is not None else None)
         eng = self.model._engine
-        if getattr(self.optimizer, "fused", False):
+        if self._sgd_repacks:
             eng.pack_weights()      # no-op unless the weights changed outside the graph (load_weights, load_state_dict): the
                                     # captured step has no re-pack of its own, FlatSGD rewrites the operand planes as it updates
 
     def _after_replay(self):
-        if not getattr(self.optimizer, "fused", False):
+        if not self._sgd_repacks:
             self.model._engine.invalidate_packed_weights()     # the replayed SGD moved the master weights past the packed copies
 
     def _step(self):
@@ -65,7 +69,7 @@ class GraphedTrainStep:
         torch.cuda.synchronize()
         g = torch.cuda.CUDAGraph()
         self.optimizer.zero_grad()
-        if getattr(self.optimizer, "fused", False):
+        if self._sgd_repacks:
             eng.pack_weights()                     # FlatSGD rewrites the operand planes itself: start the graph from current ones
         else:
             eng.invalidate_packed_weights()        # the weight re-pack must be part of the captured step

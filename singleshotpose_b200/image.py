@@ -7,7 +7,8 @@ Split of work, per sample:
            121-122), built the way Pillow's Image.point() builds them (round, then clip to 8 bits); the label transform
            (fill_truth_detection, image.py:77-108).  JPEG/PNG decoding stays with PIL in the loader workers.
   device - background resize, mask compositing, jitter crop (zero fill), resize to the network shape, RGB->HSV->RGB
-           distortion, ToTensor: libssp_b200.so `ssp_aug_sample` (csrc/augment.cu), byte-exact with Pillow's
+           distortion, ToTensor: libssp_b200.so `ssp_aug_batch_plan` + `ssp_aug_batch_run` for the whole batch
+           (csrc/augment.cu), byte-exact with Pillow's
            ImagingResample / rgb2hsv / hsv2rgb, which the reference calls through PIL.
 
 There is no CPU fallback: the tensors come back on the CUDA device, and a missing library raises.
@@ -17,7 +18,6 @@ BICUBIC on every Pillow since 7.0 (the default here) and NEAREST on the Pillow 5
 """
 from __future__ import annotations
 
-import os
 import random as _random
 
 import numpy as np
@@ -265,7 +265,7 @@ class _AugItem(C.Structure):
 
 class GpuAugmenter:
     """change_background + data_augmentation + ToTensor for a whole batch: one pinned staging buffer, ONE host->device copy,
-    then the per-sample kernels on the current stream, writing straight into the (B,3,H,W) float32 network input.
+    then one launch per pipeline stage for the whole batch on the current stream, writing straight into the (B,3,H,W) float32 network input.
 
         aug = GpuAugmenter(device)
         x, params = aug(imgs, masks, bgs, shape=(416, 416), jitter=0.2, hue=0.1, saturation=1.5, exposure=1.5)
@@ -274,10 +274,8 @@ class GpuAugmenter:
     imgs / masks / bgs: sequences of uint8 HxWx3 RGB arrays (or PIL images), what `Image.open(path).convert('RGB')` gives in
     load_data_detection (image.py:134-136).  `params` (optional argument) replays earlier draws instead of drawing."""
 
-    def __init__(self, device, resample=BICUBIC, keep_u8=False, batched=None):
+    def __init__(self, device, resample=BICUBIC, keep_u8=False):
         self.device = torch.device(device)
-        # one launch per pipeline stage for the whole batch (ssp_aug_batch_plan/run) instead of ~10 launches per sample
-        self.batched = (os.environ.get("SSP_AUG_BATCHED", "1") != "0") if batched is None else bool(batched)
         if self.device.type != "cuda":
             raise SspError("GpuAugmenter needs a CUDA device (no CPU fallback); got %s" % self.device)
         self.resample = resample
@@ -306,9 +304,9 @@ class GpuAugmenter:
         offs, total, work_bytes = _stage_plan(imgs, masks, bgs, params, W, H, self.resample)
         lib = load()
         table_off = _a16(total)
-        table_bytes = int(lib.ssp_aug_batch_table_bytes(B)) if self.batched else 0
+        table_bytes = int(lib.ssp_aug_batch_table_bytes(B))
         work_each = _a16(work_bytes)
-        work_total = work_each * (B if self.batched else 1)      # concurrent samples need their own scratch
+        work_total = work_each * B          # concurrent samples need their own scratch
         total = table_off + table_bytes
         if self._stage is None or self._stage.numel() < total:
             self._stage = torch.empty(total, dtype=torch.uint8).pin_memory()
@@ -324,31 +322,22 @@ class GpuAugmenter:
 
         def at(a, o, k):                    # device address of an input: in place if it is a CUDA tensor, else its staged copy
             return a.data_ptr() if o[k] is None else base + o[k]
-        if self.batched:
-            # the op table (device pointers, per-sample geometry) is planned on the host straight into the tail of the pinned
-            # staging buffer and travels in the batch's single host->device copy
-            items = (_AugItem * B)()
-            wbase = self._work.data_ptr()
-            for i, (im, bg, p, o) in enumerate(zip(imgs, bgs, params, offs)):
-                items[i] = _AugItem(at(im, o, "img"), at(masks[i], o, "mask"), im.shape[1], im.shape[0], at(bg, o, "bg"), bg.shape[1], bg.shape[0],
-                                    base + o["luts"], p["pleft"], p["ptop"], p["cw"], p["ch"], wbase + i * work_each, work_each,
-                                    u8[i].data_ptr() if u8 is not None else None, out[i].data_ptr())
-            dims = (C.c_int * 20)()
-            call("ssp_aug_batch_plan", items, B, W, H, self.resample, C.c_void_p(self._stage.data_ptr() + table_off), table_bytes, dims)
+        # the op table (device pointers, per-sample geometry) is planned on the host straight into the tail of the pinned
+        # staging buffer and travels in the batch's single host->device copy
+        items = (_AugItem * B)()
+        wbase = self._work.data_ptr()
+        for i, (im, bg, p, o) in enumerate(zip(imgs, bgs, params, offs)):
+            items[i] = _AugItem(at(im, o, "img"), at(masks[i], o, "mask"), im.shape[1], im.shape[0], at(bg, o, "bg"), bg.shape[1], bg.shape[0],
+                                base + o["luts"], p["pleft"], p["ptop"], p["cw"], p["ch"], wbase + i * work_each, work_each,
+                                u8[i].data_ptr() if u8 is not None else None, out[i].data_ptr())
+        dims = (C.c_int * 20)()
+        call("ssp_aug_batch_plan", items, B, W, H, self.resample, C.c_void_p(self._stage.data_ptr() + table_off), table_bytes, dims)
         self._dev[:total].copy_(self._stage[:total], non_blocking=True)
         self._copied = torch.cuda.Event()
         self._copied.record()
         self.h2d_bytes = total
-        s = stream_ptr()
-        if self.batched:
-            call("ssp_aug_batch_run", C.c_void_p(base + table_off), B, dims, s)
-            self.launches += sum(1 for k in range(10) if dims[2 * k] > 0)
-            return (out, params, u8) if self.keep_u8 else (out, params)
-        for i, (im, bg, p, o) in enumerate(zip(imgs, bgs, params, offs)):
-            call("ssp_aug_sample", C.c_void_p(at(im, o, "img")), C.c_void_p(at(masks[i], o, "mask")), im.shape[1], im.shape[0],
-                 C.c_void_p(at(bg, o, "bg")), bg.shape[1], bg.shape[0], C.c_void_p(base + o["luts"]), p["pleft"], p["ptop"], p["cw"], p["ch"],
-                 W, H, self.resample, ptr(self._work), self._work.numel(), ptr(u8[i]) if u8 is not None else None, ptr(out[i]), s)
-        self.launches += 10 * B             # upper bound: 2 x (2 coefficient + 2 pass) + composite + distort per sample
+        call("ssp_aug_batch_run", C.c_void_p(base + table_off), B, dims, stream_ptr())
+        self.launches += sum(1 for k in range(10) if dims[2 * k] > 0)
         return (out, params, u8) if self.keep_u8 else (out, params)
 
 

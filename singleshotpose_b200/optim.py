@@ -5,8 +5,6 @@ from __future__ import annotations
 
 import torch
 
-import os
-
 from ._lib import call, ptr, stream_ptr
 
 
@@ -29,8 +27,7 @@ def dp_hyperparams(learning_rate, decay, per_gpu_batch):
 
 class FlatSGD:
     """optim.SGD(model.parameters(), lr, momentum, dampening=0, weight_decay) of train.py:388 as one kernel over the engine's flat
-    buffers, which also rewrites the conv operand planes from the updated weights (csrc/sgd_pack.cu; SSP_SGD_FUSED=0 falls back to
-    ssp_sgd_step_flat + a re-pack at the next forward).
+    buffers, which also rewrites the conv operand planes from the updated weights (csrc/sgd_pack.cu).
 
     Data parallelism (SURVEY 8e): `overlap_all_reduce(n_buckets)` splits the flat gradient buffer into contiguous buckets in
     REVERSE layer order; backward hands each bucket to NCCL on a communication stream as soon as its last weight gradient has
@@ -41,7 +38,6 @@ class FlatSGD:
         self.model = model
         self.param_groups = [dict(lr=lr, momentum=momentum, weight_decay=weight_decay)]   # adjust_learning_rate() writes lr here
         self._v = None
-        self.fused = os.environ.get("SSP_SGD_FUSED", "1") != "0"
         self._buckets = None          # [(first layer, (elem lo, hi), (block lo, hi))] when overlap_all_reduce() is on
         self._comm = None
         self._done = {}               # bucket -> event recorded on the communication stream after its all-reduce
@@ -95,12 +91,6 @@ class FlatSGD:
             self._v = torch.zeros_like(eng.flat_params)
         g = self.param_groups[0]
         hyper = (float(g["lr"]), float(g["momentum"]), float(g["weight_decay"]), float(grad_scale))
-        if not self.fused:
-            self._wait_buckets()
-            call("ssp_sgd_step_flat", ptr(eng.flat_params), ptr(eng.flat_grads), ptr(self._v), eng.flat_params.numel(), *hyper, stream_ptr())
-            eng.launches += 1
-            eng.invalidate_packed_weights()        # the next forward re-packs the fp16 operand copies of the weights
-            return
         table, blocks = eng.sgd_segments()
         n_seg = len(blocks)
         if self._buckets is not None and self._done:
@@ -117,12 +107,6 @@ class FlatSGD:
                  ptr(self._v), *hyper, stream_ptr())
             eng.launches += 1
         eng._weights_version = eng._params_version()       # the operand planes were rewritten from the updated weights
-
-    def _wait_buckets(self):
-        cur = torch.cuda.current_stream()
-        for ev in self._done.values():
-            cur.wait_event(ev)
-        self._done = {}
 
     # ------------------------------------------------------------------ checkpointing (SURVEY 8f.4; absent in the reference,
     # which only saves model weights -- train.py:409).  The layout is torch.optim.SGD's own state_dict, so a checkpoint moves

@@ -176,7 +176,7 @@ def test_image_pipeline_has_no_cpu_path():
 
 
 def test_staging_layout_feeds_the_kernel_core(host):
-    """GpuAugmenter's host half (batch plan, pinned-buffer fill with the thread pool, argument order of ssp_aug_sample) driven
+    """GpuAugmenter's host half (batch plan, pinned-buffer fill with the thread pool, argument order of augment_sample_driver) driven
     into the host build of the kernel core: a mixed-size batch equals the oracle sample by sample."""
     sizes = [((160, 120), (100, 75)), ((96, 128), (64, 64)), ((200, 150), (333, 41)), ((160, 120), (160, 120)), ((64, 48), (20, 30))]
     samples = [synth.photo_sample(10 + i, ow, oh, bw, bh) for i, ((ow, oh), (bw, bh)) in enumerate(sizes)]

@@ -107,19 +107,18 @@ def test_decode_jpeg_one_file():
     assert np.array_equal(decode_jpeg(b).cpu().numpy(), JC.pillow_rgb(b))
 
 
-def test_augmenter_with_device_resident_inputs_matches_host_arrays():
+def test_batched_augmenter_device_resident_inputs_match_host_arrays():
     import random
     from singleshotpose_b200 import image, synth
     ims, mks, bgs = zip(*[synth.photo_sample(i, 160 + 8 * i, 120, 100 + 5 * i, 75) for i in range(5)])
     params = [image.draw_augmentation(im.shape[1], im.shape[0], 0.2, 0.1, 1.5, 1.5, random.Random(i)) for i, im in enumerate(ims)]
-    for batched in (True, False):
-        aug = image.GpuAugmenter("cuda", keep_u8=True, batched=batched)
-        x_host, _, u8_host = aug(list(ims), list(mks), list(bgs), (96, 64), params=params)
-        dev = lambda arrs: [torch.from_numpy(a).cuda() for a in arrs]
-        mixed_masks = [torch.from_numpy(m).cuda() if i % 2 else m for i, m in enumerate(mks)]   # device and host in one batch
-        x_dev, _, u8_dev = aug(dev(ims), mixed_masks, dev(bgs), (96, 64), params=params)
-        assert torch.equal(u8_dev, u8_host) and torch.equal(x_dev, x_host)
-        assert aug.h2d_bytes < sum(a.nbytes for a in ims + bgs)            # device inputs are not staged
+    aug = image.GpuAugmenter("cuda", keep_u8=True)
+    x_host, _, u8_host = aug(list(ims), list(mks), list(bgs), (96, 64), params=params)
+    dev = lambda arrs: [torch.from_numpy(a).cuda() for a in arrs]
+    mixed_masks = [torch.from_numpy(m).cuda() if i % 2 else m for i, m in enumerate(mks)]   # device and host in one batch
+    x_dev, _, u8_dev = aug(dev(ims), mixed_masks, dev(bgs), (96, 64), params=params)
+    assert torch.equal(u8_dev, u8_host) and torch.equal(x_dev, x_host)
+    assert aug.h2d_bytes < sum(a.nbytes for a in ims + bgs)            # device inputs are not staged
 
 
 @pytest.mark.parametrize("shape", [(96, 96), (128, 96)])

@@ -13,6 +13,7 @@ import torch
 from oracle.darknet_ref import RefDarknet
 from oracle import region_loss_ref as RL
 from singleshotpose_b200 import Darknet, RegionLoss, FlatSGD, synth
+from singleshotpose_b200._lib import call, ptr, stream_ptr
 
 pytestmark = pytest.mark.gpu
 
@@ -273,6 +274,18 @@ def test_load_weights_after_forward_refreshes_operand_planes(cfg_path, tmp_path)
     assert not torch.equal(before, after)
 
 
+def _plain_sgd_step(opt):
+    """the unfused update FlatSGD.step() is checked against: ssp_sgd_step_flat over the engine's flat buffers and the optimizer's
+    momentum buffer, then a re-pack of the operand planes at the next forward"""
+    eng = opt.model._engine
+    if opt._v is None:
+        opt._v = torch.zeros_like(eng.flat_params)
+    g = opt.param_groups[0]
+    call("ssp_sgd_step_flat", ptr(eng.flat_params), ptr(eng.flat_grads), ptr(opt._v), eng.flat_params.numel(),
+         float(g["lr"]), float(g["momentum"]), float(g["weight_decay"]), 1.0, stream_ptr())
+    eng.invalidate_packed_weights()
+
+
 def test_fused_sgd_repack_and_bucketed_step_match_plain(cfg_path, monkeypatch):
     """FlatSGD's fused update + operand-plane rewrite (csrc/sgd_pack.cu), also issued bucket by bucket in reverse layer order
     (the data-parallel overlap path, world size 1 here), gives the weights AND the next forward of the unfused path
@@ -285,7 +298,6 @@ def test_fused_sgd_repack_and_bucketed_step_match_plain(cfg_path, monkeypatch):
     for mode in ("plain", "plain", "fused", "bucketed"):      # the second plain run measures the run-to-run noise of step 2
         m = copy.deepcopy(base)
         opt = FlatSGD(m, lr=1e-4, momentum=0.9, weight_decay=0.032)
-        opt.fused = mode != "plain"
         logits = []
         for it in range(2):
             opt.zero_grad()
@@ -297,7 +309,10 @@ def test_fused_sgd_repack_and_bucketed_step_match_plain(cfg_path, monkeypatch):
                 assert len(opt._buckets) == 4 and opt._buckets[-1][1][0] == 0 and opt._buckets[0][1][1] == m._engine.flat_params.numel()
                 assert all(a[1][0] == b[1][1] for a, b in zip(opt._buckets[:-1], opt._buckets[1:]))     # contiguous, last layers first
             opt.all_reduce_grads()
-            opt.step()
+            if mode == "plain":
+                _plain_sgd_step(opt)
+            else:
+                opt.step()
             if it == 0:
                 first = [p.detach().clone() for p in m.parameters()]
         outs.append((logits, first, [p.detach().clone() for p in m.parameters()]))
