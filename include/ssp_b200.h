@@ -1,9 +1,9 @@
 /* ssp_b200.h -- C ABI of libssp_b200.so: the sm_90a (H100) kernels behind the singleshotpose hot path.
  *
- * The reference (microsoft/singleshotpose) has no FFI: its hot path is the Python surface
- * Darknet.forward / RegionLoss.forward / get_region_boxes / pnp.  Each entry point below names the
- * reference code it replaces (file:line under /root/reference); singleshotpose_b200/*.py are the
- * thin Python mirrors of that surface that bind these symbols with ctypes (INTEGRATION.md).
+ * The reference (microsoft/singleshotpose) has no FFI: its hot path is the Python surface Darknet.forward / RegionLoss.forward /
+ * get_region_boxes / pnp.  Each entry point below names the reference code it replaces (file:line under /root/reference);
+ * singleshotpose_b200/*.py are the thin Python mirrors of that surface (INTEGRATION.md).  Their ctypes binding is read from this
+ * file at import (signatures, SSP_* integer macros, structs): a new entry point is declared here and defined in its kernel file.
  *
  * Conventions: plain pointers and sizes only; every pointer is a DEVICE pointer unless stated; all
  * functions are asynchronous on `stream` (a cudaStream_t passed as void*), never allocate, never
@@ -225,7 +225,7 @@ int ssp_project_points(const float* X, int rows, int nv, const double* Rt, const
  *  ssp_mesh_diameter: *diam_out = the largest distance between two vertices, bit-identical to calc_pts_diameter on float64.
  *  SSP_ERR_ARG for a null pointer, nv < 1, nv > SSP_ADDS_MAX_VERTICES, n < 0 or n > 2^31 - 1 (ssp_adds_work_bytes returns
  *  SSP_ERR_ARG for these sizes too). ---- */
-#define SSP_ADDS_MAX_VERTICES (1 << 20)
+#define SSP_ADDS_MAX_VERTICES 1048576 /* 1 << 20 */
 long long ssp_adds_work_bytes(int nv, long long n);
 int ssp_adds_batched(const double* X, int nv, const double* Rt_est, const double* Rt_gt, long long n, double* adds_out,
                      double* add_out_or_null, void* work, long long work_bytes, void* stream);

@@ -1,98 +1,81 @@
-"""ctypes binding of libssp_b200.so (include/ssp_b200.h).  There is NO fallback: if the library is missing
-or a call fails, an exception is raised -- the product path never routes through the CPU oracle."""
+"""ctypes binding of libssp_b200.so, read from include/ssp_b200.h itself: the argument and return types of every entry point,
+the SSP_* integer macros and the structs that cross the boundary are parsed from the header, so there is no second copy of them
+to keep in step.  There is NO fallback: if the library is missing or a call fails, an exception is raised -- the product path
+never routes through the CPU oracle."""
 from __future__ import annotations
 
 import ctypes as C
 import os
+import re
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("SSP_LIB") or os.path.join(_HERE, "csrc", "libssp_b200.so")   # SSP_LIB: A/B experiments only
 
-FMT_F16, FMT_BF16 = 0, 1
-IMPL_TC, IMPL_SIMT, IMPL_TC2, IMPL_BAND, IMPL_BANDT = 0, 1, 2, 3, 4
-EPI_F32, EPI_STATS, EPI_BIAS, EPI_F16 = 0, 1, 2, 8
-ROUTE_NONE, ROUTE_DIRECT, ROUTE_POOL, ROUTE_REORG = 0, 1, 2, 3
-ROUTE_F16 = 16          # OR-ed into a gradient route of ssp_bn_bwd_*: that plane holds fp16
-
-_p, _i, _ll, _f, _d = C.c_void_p, C.c_int, C.c_longlong, C.c_float, C.c_double
-
-# name -> argtypes (restype int unless stated); must list every symbol of include/ssp_b200.h
-SIGNATURES = {
-    "ssp_version": [],
-    "ssp_last_error": [],
-    "ssp_flat_alloc_rows": [_i, _i, _i],
-    "ssp_flat_row": [_i, _i, _i, _i, _i],
-    "ssp_pack_nchw": [_p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _f, _p],
-    "ssp_unpack_nchw": [_p, _p, _i, _i, _i, _i, _i, _i, _p],
-    "ssp_unpack16_nchw": [_p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _p],
-    "ssp_conv_gemm": [_i, _p, _p, _ll, _i, _i, _p, _p, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p, _i, _ll, _i, _p, _p, _p, _p],
-    "ssp_conv_bandt_launches": [],
-    "ssp_l0_gram": [_p, _i, _i, _i, _p, _p],
-    "ssp_l0_stats": [_p, _p, _p, _p, _p],
-    "ssp_l0_fused_fwd": [_p, _p, _p, _p, _f, _i, _i, _i, _p, _p, _i, _i, _p, _p],
-    "ssp_l0_bwd": [_p, _p, _i, _i, _i, _p, _f, _i, _i, _i, _p, _p],
-    "ssp_l0_bwd_finalize": [_p, _p, _p, _p, _p, _p, _d, _f, _p, _p, _p, _p],
-    "ssp_conv_gemm_bnact": [_i, _p, _p, _ll, _i, _i, _p, _p, _i, _i, _i, _i, _i, _i, _i, _p, _p, _f, _p, _p, _i, _i, _p],
-    "ssp_conv_gemm_splitk": [_p, _p, _ll, _i, _i, _p, _p, _i, _i, _i, _i, _i, _i, _i, _i, _p, _ll, _i, _p],
-    "ssp_conv_splitk_count": [_i, _i, _i, _i, _i, _i, _i],
-    "ssp_bn_apply_splitk": [_p, _i, _ll, _i, _p, _p, _i, _i, _i, _i, _f, _p, _p, _i, _i, _i, _p, _p, _i, _i, _i, _p],
-    "ssp_wgrad_gemm": [_i, _p, _ll, _i, _i, _i, _p, _ll, _i, _i, _i, _i, _i, _i, _i, _p, _i, _i, _f, _p],
-    "ssp_bn_finalize": [_p, _p, _d, _p, _p, _p, _p, _f, _f, _i, _p, _p, _p, _p, _i, _p],
-    "ssp_bn_apply": [_p, _i, _p, _p, _i, _i, _i, _i, _f, _p, _p, _i, _i, _i, _p, _p, _i, _i, _i, _p, _i, _p],
-    "ssp_bn_bwd_reduce": [_p, _i, _p, _p, _p, _p, _p, _i, _i, _i, _i, _f, _p, _i, _i, _i, _p, _i, _i, _i, _p, _p, _p],
-    "ssp_bn_bwd_apply": [_p, _i, _p, _p, _p, _p, _p, _i, _i, _i, _i, _f, _p, _i, _i, _i, _p, _i, _i, _i, _p, _p, _p, _i, _i, _f, _p],
-    "ssp_bn_bwd_finalize": [_p, _p, _p, _p, _i, _i, _f, _p],
-    "ssp_bias_grad_nchw": [_p, _p, _i, _i, _i, _i, _f, _p],
-    "ssp_pack_weights": [_p, _i, _i, _i, _p, _p, _i, _p, _i, _i, _p],
-    "ssp_sgd_step_flat": [_p, _p, _p, _ll, _f, _f, _f, _f, _p],
-    "ssp_sgd_segment_blocks": [_i, _i, _i, _ll],
-    "ssp_sgd_pack_step": [_p, _i, _i, _i, _p, _p, _p, _f, _f, _f, _f, _p],
-    "ssp_region_loss_fwd_bwd": [_p, _p, _p, _p, _i, _i, _i, _i, _i, _f, _f, _f, _f, _i, _f, _p],
-    "ssp_region_decode_argmax": [_p, _i, _i, _i, _i, _i, _i, _p, _p, _p, _p],
-    "ssp_region_loss_multi_fwd_bwd": [_p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _p, _i, _f, _f, _f, _f, _f, _i, _f, _p],
-    "ssp_region_decode_multi": [_p, _i, _i, _i, _i, _i, _i, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p],
-    "ssp_eval_multi_select": [_p, _i, _i, _i, _i, _i, _i, _p, _i, _p, _f, _f, _f, _p, _p, _p, _p],
-    "ssp_predict_multi_select": [_p, _i, _i, _i, _i, _i, _i, _p, _i, _f, _f, _f, _p, _p, _p, _p],
-    "ssp_pnp_batched": [_p, _i, _p, _p, _i, _ll, _i, _p, _p, _p, _p],
-    "ssp_pnp_batched_work": [_p, _i, _p, _p, _i, _ll, _i, _p, _p, _p, _p],
-    "ssp_project_points": [_p, _i, _i, _p, _p, _ll, _p, _p],
-    "ssp_adds_work_bytes": [_i, _ll],
-    "ssp_adds_batched": [_p, _i, _p, _p, _ll, _p, _p, _p, _ll, _p],
-    "ssp_mesh_diameter": [_p, _i, _p, _p],
-    "ssp_render_work_bytes": [_i, _i, _ll, _i, _i],
-    "ssp_render_masks": [_p, _i, _i, _p, _i, _p, _p, _ll, _i, _i, _p, _p, _p, _ll, _p],
-    "ssp_aug_resize_work_bytes": [_i, _i, _i, _i, _i],
-    "ssp_aug_resize_u8": [_p, _i, _i, _i, _i, _i, _i, _p, _i, _i, _i, _p, _ll, _p],
-    "ssp_aug_rgb2hsv_u8": [_p, _p, _ll, _p],
-    "ssp_aug_hsv2rgb_u8": [_p, _p, _ll, _p],
-    "ssp_aug_to_tensor_u8": [_p, _ll, _p, _p],
-    "ssp_aug_batch_table_bytes": [_i],
-    "ssp_aug_batch_plan": [_p, _i, _i, _i, _i, _p, _ll, _p],
-    "ssp_aug_batch_run": [_p, _i, _p, _p],
-    "ssp_aug_sample_work_bytes": [_i, _i, _i, _i, _i, _i, _i, _i, _i],
-    "ssp_augm_work_bytes": [_i, _i, _i, _i, _i],
-    "ssp_augm_table_bytes": [_i],
-    "ssp_augm_plan_begin": [_p, _i, _i, _i, _i, _p, _ll, _p],
-    "ssp_augm_plan_attempt": [_p, _i, _i, _i, _i, _p, _ll, _p],
-    "ssp_augm_plan_finish": [_p, _i, _i, _i, _i, _p, _ll, _p],
-    "ssp_augm_run": [_p, _i, _p, _p],
-    "ssp_jpeg_parse": [_p, _ll, _p],
-    "ssp_jpeg_decline_reason": [_i],
-    "ssp_jpeg_stage_bytes": [_p, _i],
-    "ssp_jpeg_work_bytes": [_p, _i],
-    "ssp_jpeg_batch_plan": [_p, _i, _p, _ll, _p],
-    "ssp_jpeg_batch_run": [_p, _i, _p, _p, _ll, _p, _p],
-}
-_RESTYPE = {"ssp_last_error": C.c_char_p, "ssp_flat_alloc_rows": _ll, "ssp_flat_row": _ll,
-            "ssp_jpeg_decline_reason": C.c_char_p, "ssp_jpeg_stage_bytes": _ll, "ssp_jpeg_work_bytes": _ll,
-            "ssp_aug_resize_work_bytes": _ll, "ssp_aug_sample_work_bytes": _ll, "ssp_aug_batch_table_bytes": _ll,
-            "ssp_augm_work_bytes": _ll, "ssp_augm_table_bytes": _ll, "ssp_adds_work_bytes": _ll, "ssp_render_work_bytes": _ll}
-
-_lib = None
-
 
 class SspError(RuntimeError):
     pass
+
+
+_CTYPES = {"int": C.c_int, "unsigned": C.c_uint, "long long": C.c_longlong, "float": C.c_float, "double": C.c_double}
+
+
+def _ctype(decl, where):
+    """the ctypes type of a C type as the header spells it; every pointer is a c_void_p (callers pass ptr(t), None or byref)"""
+    decl = " ".join(decl.split()).removeprefix("const ")
+    if decl.endswith("*"):
+        return C.c_void_p
+    if decl not in _CTYPES:
+        raise SspError("ssp_b200.h: unknown type '%s' in: %s" % (decl, " ".join(where.split())))
+    return _CTYPES[decl]
+
+
+def _decls(text, sep, where):
+    """[(name, ctype)] of a parameter list (sep ',') or a struct body (sep ';', where 'int ow, oh' declares two fields)"""
+    out = []
+    for decl in filter(None, map(str.strip, text.split(sep))):
+        first, *names = decl.split(",")
+        m = re.fullmatch(r"(.*[\s*])(\w+)", first.strip(), re.S)
+        if not m:
+            raise SspError("ssp_b200.h: no 'type name' in '%s' of: %s" % (decl, " ".join(where.split())))
+        out += [(n.strip(), _ctype(m.group(1), where)) for n in [m.group(2)] + names]
+    return out
+
+
+def parse_header(text):
+    """The binding the header text declares: ({symbol: argtypes}, {symbol: restype}, {macro: int}, {struct name: Structure class}).
+    Reads the constructs include/ssp_b200.h uses and nothing else of C; anything it cannot read is an SspError, never a guess."""
+    text = re.sub(r"/\*.*?\*/", " ", text, flags=re.S)
+    text = re.sub(r"#ifdef __cplusplus.*?#endif", "", text, flags=re.S)            # the extern "C" braces
+    constants = {}
+    for name, value in re.findall(r"^#define[ \t]+(\w+)[ \t]+(\S.*?)[ \t]*$", text, re.M):
+        if not re.fullmatch(r"-?\d+|\(-?\d+\)", value):
+            raise SspError("ssp_b200.h: #define %s %s is not an integer literal" % (name, value))
+        constants[name] = int(value.strip("()"))
+    text = re.sub(r"^#.*$", "", text, flags=re.M)
+    structs = {}
+
+    def struct(m):
+        structs[m.group(1)] = type(m.group(1), (C.Structure,), {"_fields_": _decls(m.group(2), ";", m.group(0))})
+        return ""
+    text = re.sub(r"typedef struct (\w+) \{(.*?)\} \1;", struct, text, flags=re.S)
+    signatures, returns = {}, {}
+    for stmt in filter(None, map(str.strip, text.split(";"))):
+        m = re.fullmatch(r"(.*?[\s*])(ssp_\w+)\s*\((.*)\)", stmt, re.S)
+        if not m:
+            raise SspError("ssp_b200.h: neither a prototype nor a struct: %s" % " ".join(stmt.split()))
+        ret, name, args = m.groups()
+        returns[name] = C.c_char_p if ret.split() == ["const", "char*"] else _ctype(ret, stmt)
+        signatures[name] = [] if args.strip() == "void" else [t for _, t in _decls(args, ",", stmt)]
+    return signatures, returns, constants, structs
+
+
+# Parsed once at import (the constants are read by importers at their import); the library itself is opened lazily by load().
+with open(os.path.join(_HERE, "..", "include", "ssp_b200.h")) as _f:
+    SIGNATURES, RETURNS, CONSTANTS, STRUCTS = parse_header(_f.read())
+# FMT_F16, IMPL_BANDT, EPI_STATS, ROUTE_POOL, ...: the header's SSP_FMT_* / SSP_IMPL_* / SSP_EPI_* / SSP_ROUTE_* without the prefix
+globals().update((k[4:], v) for k, v in CONSTANTS.items() if k.startswith(("SSP_FMT_", "SSP_IMPL_", "SSP_EPI_", "SSP_ROUTE_")))
+
+_lib = None
 
 
 def load():
@@ -106,7 +89,7 @@ def load():
         for name, args in SIGNATURES.items():
             fn = getattr(lib, name)            # AttributeError if the .so lacks a declared symbol
             fn.argtypes = args
-            fn.restype = _RESTYPE.get(name, _i)
+            fn.restype = RETURNS[name]
         _lib = lib
     return _lib
 

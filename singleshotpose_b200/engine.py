@@ -152,7 +152,7 @@ class Buffers:
                 # blocks 0-1 run as one unit (csrc/l0_fused.cu): no operand planes, no full-resolution conv output, no dY plane --
                 # the 28x28 Gram matrix of the image patches, a 1-byte code per pooled cell and 28x32 backward sums instead
                 self.x_hi.append(None); self.x_lo.append(None); self.y.append(None)
-                self.l0_gram = torch.zeros(2816, dtype=torch.float64, device=dev)      # SSP_L0_GRAM_DOUBLES: the 28x28 matrix + ssp_l0_gram's scratch
+                self.l0_gram = torch.zeros(_lib.CONSTANTS["SSP_L0_GRAM_DOUBLES"], dtype=torch.float64, device=dev)      # the 28x28 matrix + ssp_l0_gram's scratch
                 if train:
                     self.l0_code = torch.zeros(_lib.flat_alloc_rows(N, h // 2, w // 2), 32, dtype=torch.uint8, device=dev)
                     self.l0_t1 = torch.zeros(28 * 32, dtype=torch.float64, device=dev)
@@ -270,9 +270,6 @@ class Engine:
             self.w_d.append(torch.zeros(L.cin, _rup(L.taps * L.cout, 8), dtype=f16, device=dev))
 
     # ------------------------------------------------------------------ fused SGD + re-pack work list, gradient buckets
-    _SEG_DTYPE = [("off", "<i8"), ("n", "<i8"), ("cout", "<i4"), ("taps", "<i4"), ("cin", "<i4"), ("ld_f", "<i4"), ("ld_d", "<i4"),
-                  ("d_fmt", "<i4"), ("f_hi", "<u8"), ("f_lo", "<u8"), ("d", "<u8"), ("block0", "<i4"), ("reserved", "<i4")]
-
     def sgd_segments(self):
         """device table (ssp_sgd_segment, include/ssp_b200.h) for ssp_sgd_pack_step: one entry per parameter tensor in flat order.
         Returns (table tensor, [(block0, nblocks)] per parameter)."""
@@ -283,8 +280,7 @@ class Engine:
         # the GEMM layers' weights also rewrite their operand planes; every other tensor (layer 0's weight included) is plain
         conv_of = {id(conv.weight): L for L, (conv, _) in zip(self.layers, self.conv_modules()) if not L.first}
         params = list(self.model.parameters())
-        tab = np.zeros(len(params), dtype=np.dtype(self._SEG_DTYPE))
-        assert tab.dtype.itemsize == 72
+        tab = np.zeros(len(params), dtype=np.dtype(_lib.STRUCTS["ssp_sgd_segment"]))
         blocks, b0 = [], 0
         for k, p in enumerate(params):
             off, n, _g = self._slices[id(p)]

@@ -23,7 +23,7 @@ import random as _random
 import numpy as np
 import torch
 
-from ._lib import C, SspError, call, load, ptr, stream_ptr
+from ._lib import C, STRUCTS, SspError, call, load, ptr, stream_ptr
 
 NEAREST, BILINEAR, BICUBIC = 0, 2, 3          # PIL.Image.Resampling values
 
@@ -256,11 +256,7 @@ def _stage_fill(st, imgs, masks, bgs, params, offs):
     list(_POOL.map(one, jobs))
 
 
-class _AugItem(C.Structure):
-    """ssp_aug_item (include/ssp_b200.h)"""
-    _fields_ = [("img", C.c_void_p), ("mask", C.c_void_p), ("ow", C.c_int), ("oh", C.c_int), ("bg", C.c_void_p), ("bw", C.c_int), ("bh", C.c_int),
-                ("luts", C.c_void_p), ("pleft", C.c_int), ("ptop", C.c_int), ("cw", C.c_int), ("ch", C.c_int), ("work", C.c_void_p),
-                ("work_bytes", C.c_longlong), ("out_u8", C.c_void_p), ("out_chw", C.c_void_p)]
+_AugItem = STRUCTS["ssp_aug_item"]
 
 
 class GpuAugmenter:

@@ -29,7 +29,7 @@ import random as _random
 import numpy as np
 import torch
 
-from ._lib import C, SspError, call, load, stream_ptr
+from ._lib import C, STRUCTS, SspError, call, load, stream_ptr
 from .image import BICUBIC, mask_luts
 
 PIXEL_THRESHOLD = 200                 # image_multi.py:301
@@ -137,15 +137,7 @@ def _a16(n):
     return (int(n) + 15) & ~15
 
 
-class _MultiItem(C.Structure):
-    """ssp_augm_item (include/ssp_b200.h)"""
-    _fields_ = [("img", C.c_void_p), ("mask", C.c_void_p), ("src_w", C.c_int), ("src_h", C.c_int),
-                ("pleft", C.c_int), ("ptop", C.c_int), ("cw", C.c_int), ("ch", C.c_int),
-                ("flip", C.c_int), ("shift_x", C.c_int), ("shift_y", C.c_int), ("mask_bg", C.c_int),
-                ("main_img", C.c_void_p), ("main_mask", C.c_void_p), ("total_img", C.c_void_p), ("total_mask", C.c_void_p),
-                ("counts", C.c_void_p), ("luts", C.c_void_p), ("work", C.c_void_p), ("work_bytes", C.c_longlong),
-                ("out_u8", C.c_void_p), ("out_chw", C.c_void_p)]
-
+_MultiItem = STRUCTS["ssp_augm_item"]
 
 _POOL = None
 

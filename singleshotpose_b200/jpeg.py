@@ -21,19 +21,14 @@ import numpy as np
 import torch
 from PIL import Image
 
-from ._lib import SspError, call, load, stream_ptr
+from ._lib import STRUCTS, SspError, call, load, stream_ptr
 
 _SOF = {0xC0, 0xC1, 0xC2, 0xC3, 0xC5, 0xC6, 0xC7, 0xC9, 0xCA, 0xCB, 0xCD, 0xCE, 0xCF}
 STATUS_BITS = {1: "corrupt entropy-coded data", 2: "IDCT outside the SIMD/C agreement range", 4: "restart marker structure",
                8: "DC value outside int32"}
 
 
-class _Info(C.Structure):
-    _fields_ = [(k, C.c_int) for k in ("width", "height", "components", "h_samp", "v_samp", "restart_interval")]
-
-
-class _Item(C.Structure):
-    _fields_ = [("data", C.c_void_p), ("size", C.c_longlong), ("out", C.c_void_p)]
+_Info, _Item = STRUCTS["ssp_jpeg_info"], STRUCTS["ssp_jpeg_item"]
 
 
 def read_jpeg_size(data):

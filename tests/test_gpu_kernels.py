@@ -336,8 +336,7 @@ def test_sgd_flat_matches_torch_sgd():
 def _seg_table(entries):
     """entries: dicts of ssp_sgd_segment fields -> (device table, total blocks)"""
     import numpy as np
-    from singleshotpose_b200.engine import Engine
-    tab = np.zeros(len(entries), dtype=np.dtype(Engine._SEG_DTYPE))
+    tab = np.zeros(len(entries), dtype=np.dtype(_lib.STRUCTS["ssp_sgd_segment"]))
     b0 = 0
     for e, d in zip(tab, entries):
         for k, v in d.items():
@@ -426,7 +425,7 @@ def test_l0_fused_blocks_match_torch(shape):
     # ---- device
     xd = x.to(DEV)
     wm = w.permute(0, 2, 3, 1).contiguous().to(DEV)                      # master layout [co][kh][kw][ci]
-    gram = torch.zeros(2816, dtype=torch.float64, device=DEV)             # SSP_L0_GRAM_DOUBLES: matrix + scratch
+    gram = torch.zeros(_lib.CONSTANTS["SSP_L0_GRAM_DOUBLES"], dtype=torch.float64, device=DEV)             # matrix + scratch
     ssum = torch.zeros(32, dtype=torch.float64, device=DEV); ssq = torch.zeros_like(ssum)
     s = stream_ptr()
     call("ssp_l0_gram", ptr(xd), N, H, W, ptr(gram), s)

@@ -1,5 +1,6 @@
-"""CPU-only tests: host logic (cfg parsing, execution plan, .weights format), the C-ABI surface, and the N>1
+"""CPU-only tests: host logic (cfg parsing, execution plan, .weights format), the C-ABI surface and its binding, and the N>1
 gradient all-reduce path with the gloo backend (world size 2).  No GPU, no compute calls into the library."""
+import ctypes as C
 import os
 import re
 import subprocess
@@ -116,6 +117,89 @@ def test_abi_exports_every_declared_symbol():
         assert hasattr(lib, name), name
     assert lib.ssp_version() >= 100
     assert _lib.flat_alloc_rows(64, 416, 416) >= 64 * 417 * 417 + 417 + 2
+
+
+# (restype, argtypes) of the entry points with the most mixed argument lists, written out by hand: what _lib must read from the header
+_p, _i, _ll, _f, _d = C.c_void_p, C.c_int, C.c_longlong, C.c_float, C.c_double
+_PINNED = {
+    "ssp_last_error": (C.c_char_p, []),
+    "ssp_flat_alloc_rows": (_ll, [_i, _i, _i]),
+    "ssp_jpeg_decline_reason": (C.c_char_p, [_i]),
+    "ssp_conv_gemm": (_i, [_i, _p, _p, _ll, _i, _i, _p, _p, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p, _i, _ll, _i, _p, _p, _p, _p]),
+    "ssp_wgrad_gemm": (_i, [_i, _p, _ll, _i, _i, _i, _p, _ll, _i, _i, _i, _i, _i, _i, _i, _p, _i, _i, _f, _p]),
+    "ssp_bn_finalize": (_i, [_p, _p, _d, _p, _p, _p, _p, _f, _f, _i, _p, _p, _p, _p, _i, _p]),
+    "ssp_l0_bwd_finalize": (_i, [_p, _p, _p, _p, _p, _p, _d, _f, _p, _p, _p, _p]),
+    "ssp_pnp_batched": (_i, [_p, _i, _p, _p, _i, _ll, _i, _p, _p, _p, _p]),
+    "ssp_jpeg_batch_run": (_i, [_p, _i, _p, _p, _ll, _p, _p]),
+    "ssp_render_masks": (_i, [_p, _i, _i, _p, _i, _p, _p, _ll, _i, _i, _p, _p, _p, _ll, _p]),
+}
+
+
+def test_abi_signatures_read_from_the_header():
+    for name, (restype, argtypes) in _PINNED.items():
+        assert (_lib.RETURNS[name], _lib.SIGNATURES[name]) == (restype, argtypes), name
+    lib = _lib.load()
+    assert all(getattr(lib, n).argtypes == a and getattr(lib, n).restype == _lib.RETURNS[n] for n, a in _lib.SIGNATURES.items())
+    wide = {n for n, r in _lib.RETURNS.items() if r is not _i}          # every return that is not an int status
+    assert wide == {"ssp_last_error", "ssp_jpeg_decline_reason", "ssp_flat_alloc_rows", "ssp_flat_row", "ssp_jpeg_stage_bytes",
+                    "ssp_jpeg_work_bytes", "ssp_aug_resize_work_bytes", "ssp_aug_sample_work_bytes", "ssp_aug_batch_table_bytes",
+                    "ssp_augm_work_bytes", "ssp_augm_table_bytes", "ssp_adds_work_bytes", "ssp_render_work_bytes"}
+
+
+_STRUCT_NAMES = ["ssp_sgd_segment", "ssp_aug_item", "ssp_augm_item", "ssp_jpeg_info", "ssp_jpeg_item"]
+
+
+@pytest.fixture(scope="module")
+def compiled_header(tmp_path_factory):
+    """what the C compiler makes of include/ssp_b200.h: sizeof and every offsetof of the structs, the value of every macro"""
+    d = tmp_path_factory.mktemp("abi")
+    layout = ["sizeof(%s)" % s + "".join(", offsetof(%s, %s)" % (s, f) for f, _ in _lib.STRUCTS[s]._fields_) for s in _STRUCT_NAMES]
+    (d / "abi.c").write_text('#include <stddef.h>\n#include "ssp_b200.h"\nconst long long layout[] = {%s};\nconst long long constants[] = {%s};\n'
+                             % (", ".join(layout), ", ".join(_lib.CONSTANTS)))
+    subprocess.check_call(["gcc", "-shared", "-fPIC", "-I", os.path.join(REPO, "include"), "-o", str(d / "libabi.so"), str(d / "abi.c")])
+    return C.CDLL(str(d / "libabi.so"))
+
+
+def test_abi_struct_layouts_match_the_compiler(compiled_header):
+    assert sorted(_lib.STRUCTS) == sorted(_STRUCT_NAMES)
+    want = []
+    for s in _STRUCT_NAMES:
+        cls = _lib.STRUCTS[s]
+        want += [C.sizeof(cls)] + [getattr(cls, f).offset for f, _ in cls._fields_]
+    assert list((C.c_longlong * len(want)).in_dll(compiled_header, "layout")) == want
+    assert C.sizeof(_lib.STRUCTS["ssp_sgd_segment"]) == np.dtype(_lib.STRUCTS["ssp_sgd_segment"]).itemsize == 72
+    hdr = open(os.path.join(REPO, "include", "ssp_b200.h")).read()
+    for s in _STRUCT_NAMES:                      # no declarator lost: as many fields as names before a ';' or ',' in the struct's body
+        body = re.search(r"typedef struct %s \{(.*?)\}" % s, re.sub(r"/\*.*?\*/", "", hdr, flags=re.S), re.S).group(1)
+        assert [f for f, _ in _lib.STRUCTS[s]._fields_] == re.findall(r"(\w+)\s*[;,]", body), s
+
+
+def test_abi_constants_match_the_compiler(compiled_header):
+    hdr = open(os.path.join(REPO, "include", "ssp_b200.h")).read()
+    assert set(_lib.CONSTANTS) == set(re.findall(r"^#define (SSP_\w+)[ \t]+\S", hdr, re.M))       # all but the include guard
+    got = list((C.c_longlong * len(_lib.CONSTANTS)).in_dll(compiled_header, "constants"))
+    assert got == list(_lib.CONSTANTS.values())
+    assert (_lib.CONSTANTS["SSP_ERR_ARG"], _lib.CONSTANTS["SSP_L0_GRAM_DOUBLES"], _lib.CONSTANTS["SSP_JPEG_ST_OVERFLOW"]) == (-1, 2816, 8)
+    assert (_lib.FMT_BF16, _lib.IMPL_BANDT, _lib.EPI_F16, _lib.ROUTE_REORG, _lib.ROUTE_F16) == (1, 4, 8, 3, 16)
+
+
+@pytest.mark.parametrize("text, complaint", [
+    ("int ssp_a(int n, size_t bytes);", "unknown type 'size_t'"),
+    ("short ssp_a(void);", "unknown type 'short'"),
+    ("int ssp_a(int, float x);", "no 'type name'"),
+    ("typedef struct ssp_s { int a; long long b;\nint ssp_a(const ssp_s* s);", "neither a prototype nor a struct"),
+    ("#define SSP_N (1 << 4)", "not an integer literal"),
+])
+def test_abi_parser_refuses_what_it_cannot_read(text, complaint):
+    with pytest.raises(_lib.SspError, match=re.escape(complaint)):
+        _lib.parse_header(text)
+
+
+def test_abi_parser_reads_each_construct():
+    sig, ret, const, structs = _lib.parse_header("#define SSP_N (-3)\ntypedef struct ssp_s { unsigned* p; int a, b; } ssp_s;\n"
+                                                 "const char* ssp_a(const ssp_s* s, /* note */ double x);")
+    assert (sig, ret, const) == ({"ssp_a": [_p, _d]}, {"ssp_a": C.c_char_p}, {"SSP_N": -3})
+    assert structs["ssp_s"]._fields_ == [("p", _p), ("a", _i), ("b", _i)]
 
 
 def test_no_cpu_fallback(cfg_path):

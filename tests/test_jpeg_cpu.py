@@ -179,8 +179,7 @@ def test_jpeg_abi_rejects_bad_arguments(cases):
     assert lib.ssp_jpeg_parse(b"\xff\xd8", -1, info.ctypes.data) < 0
     assert lib.ssp_jpeg_parse(b"GIF89a", 6, info.ctypes.data) > 0
 
-    class Item(C.Structure):
-        _fields_ = [("data", C.c_void_p), ("size", C.c_longlong), ("out", C.c_void_p)]
+    Item = _lib.STRUCTS["ssp_jpeg_item"]
     good = cases[0][1]
     prog = JC.declined()[0][1]
     items = (Item * 2)(Item(C.cast(C.c_char_p(good), C.c_void_p), len(good), 1), Item(C.cast(C.c_char_p(good), C.c_void_p), len(good), 1))
