@@ -203,6 +203,19 @@ int ssp_eval_multi_select(const float* out_nchw, int B, int num_keypoints, int n
 int ssp_predict_multi_select(const float* out_nchw, int B, int num_keypoints, int num_classes, int num_anchors, int H, int W,
                              const int* classes_host, int n_req, float conf_thresh, float frame_w, float frame_h, float* boxes,
                              int* flags, float* uv, void* stream);
+/* ---- every instance in a frame (rules: csrc/detect_core.h): per image b, each as its own call, the candidates are the boxes
+ *      get_multi_region_boxes(..., only_objectness=0) lists (det_conf * cls_max_conf > conf_thresh, no fallback box) whose arg-max
+ *      class is requested, in descending (det_conf, then lower entry) order; greedy suppression within each class drops a
+ *      candidate whose rectangle of the 8 corner keypoints (frame pixels) has fp32 IoU > nms_thresh with a kept box of its class.
+ *      The reference's nms (YOLO boxes) is not reproduced.  classes_host: n_req distinct class ids, a HOST array copied into the
+ *      launch.  Out: boxes [B][max_instances][2K+3], cls [B][max_instances], uv [B][max_instances][K][2] (the box keypoints times
+ *      (frame_w, frame_h) in fp32) of the first max_instances kept boxes in that order; slots >= count[b] are zero with cls -1;
+ *      count [B] = min(kept, max_instances), kept [B] = boxes kept before the truncation.  SSP_ERR_ARG for a null pointer,
+ *      num_keypoints != 9, H*W*num_anchors > 4096, num_classes > 256, n_req < 1, a class out of range or listed twice,
+ *      nms_thresh outside [0, 1] or max_instances outside [1, 256]. ---- */
+int ssp_detect_instances(const float* out_nchw, int B, int num_keypoints, int num_classes, int num_anchors, int H, int W,
+                         const int* classes_host, int n_req, float conf_thresh, float nms_thresh, int max_instances, float frame_w,
+                         float frame_h, float* boxes, int* cls, float* uv, int* count, int* kept, void* stream);
 
 /* ---- pnp (utils.py:86-100 -> cv2.solvePnP ITERATIVE + Rodrigues), compute_projection (utils.py:40-45) ---- */
 int ssp_pnp_batched(const float* points3d, int points3d_shared, const float* points2d, const float* K3x3,
@@ -213,6 +226,11 @@ int ssp_pnp_batched(const float* points3d, int points3d_shared, const float* poi
 int ssp_pnp_batched_work(const float* points3d, int points3d_shared, const float* points2d, const float* K3x3,
                          int num_points, long long n, int max_iter, double* R_out, double* t_out, int* work_out,
                          void* stream);
+/* same solve over groups x per_group problems with per-problem points3d [groups*per_group][num_points][3]: problem (g, m) is
+ * solved only when m < count[g] (count: DEVICE int [groups], so a graph replay needs no host read-back); the others get zero
+ * R and t.  The slots of ssp_detect_instances are such groups. */
+int ssp_pnp_batched_counted(const float* points3d, const float* points2d, const float* K3x3, int num_points, int groups,
+                            int per_group, const int* count, int max_iter, double* R_out, double* t_out, void* stream);
 int ssp_project_points(const float* X, int rows, int nv, const double* Rt, const double* K3x3, long long n,
                        float* out, void* stream);
 

@@ -19,12 +19,20 @@
 
 namespace ssp {
 
+// kCounted: problem id = g * per_group + m is solved only when m < count[g] (count in device memory); the others get zero R, t
+template <bool kCounted>
 __global__ void __launch_bounds__(128) pnp_kernel(const float* __restrict__ P3, long long p3_stride, const float* __restrict__ uv,
                                                   const float* __restrict__ Kmat, int np, long long n, int max_iter,
                                                   double* __restrict__ R_out, double* __restrict__ t_out, int* __restrict__ iters_out,
-                                                  int* __restrict__ work_out /*[n][3]: Jacobi sweeps, LM iterations, LM solves; or null*/) {
+                                                  int* __restrict__ work_out /*[n][3]: Jacobi sweeps, LM iterations, LM solves; or null*/,
+                                                  const int* __restrict__ count, int per_group) {
   const long long id = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (id >= n) return;
+  if (kCounted && id % per_group >= count[id / per_group]) {
+    for (int k = 0; k < 9; k++) R_out[id * 9 + k] = 0.0;
+    for (int k = 0; k < 3; k++) t_out[id * 3 + k] = 0.0;
+    return;
+  }
   int work[3];
   ssp_pnp::pnp_solve_one(P3 + id * p3_stride, uv + id * 2 * np, Kmat, np, max_iter, R_out + id * 9, t_out + id * 3, work);
   if (iters_out) iters_out[id] = work[1];
@@ -48,12 +56,13 @@ __global__ void project_points_kernel(const float* __restrict__ X4 /*[4][nv] or 
   out[(b * 2 + 1) * nv + v] = (float)(py / pz);
 }
 
-// ssp_pnp_batched and ssp_pnp_batched_work
+// ssp_pnp_batched and ssp_pnp_batched_work (ssp_pnp_batched_counted launches pnp_kernel<true> itself)
 static int pnp_batched(const float* P3, int p3_shared, const float* uv, const float* K, int np, long long n, int max_iter,
                        double* R_out, double* t_out, int* iters_out, int* work_out, cudaStream_t s) {
   if (!P3 || !uv || !K || !R_out || !t_out || np < 6 || np > PNP_MAXP || n < 0) return fail_msg(SSP_ERR_ARG, "pnp_batched: bad argument (6 <= points <= 16)");
   if (n == 0) return SSP_OK;
-  pnp_kernel<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(P3, p3_shared ? 0 : 3LL * np, uv, K, np, n, max_iter, R_out, t_out, iters_out, work_out);
+  pnp_kernel<false><<<(unsigned)((n + 127) / 128), 128, 0, s>>>(P3, p3_shared ? 0 : 3LL * np, uv, K, np, n, max_iter, R_out, t_out, iters_out,
+                                                                work_out, nullptr, 1);
   SSP_CHECK_LAUNCH(); return SSP_OK;
 }
 
@@ -70,6 +79,17 @@ int ssp_pnp_batched(const float* P3, int shared, const float* uv, const float* K
 int ssp_pnp_batched_work(const float* P3, int shared, const float* uv, const float* K, int np, long long n, int max_iter, double* R, double* t,
                          int* work, void* stream) {
   return pnp_batched(P3, shared, uv, K, np, n, max_iter, R, t, nullptr, work, (cudaStream_t)stream);
+}
+
+int ssp_pnp_batched_counted(const float* P3, const float* uv, const float* K, int np, int groups, int per_group, const int* count, int max_iter,
+                            double* R, double* t, void* stream) {
+  if (!P3 || !uv || !K || !count || !R || !t || np < 6 || np > PNP_MAXP || groups < 0 || per_group < 1)
+    return fail_msg(SSP_ERR_ARG, "pnp_batched_counted: bad argument (6 <= points <= 16, groups >= 0, per_group >= 1)");
+  const long long n = (long long)groups * per_group;
+  if (n == 0) return SSP_OK;
+  pnp_kernel<true><<<(unsigned)((n + 127) / 128), 128, 0, (cudaStream_t)stream>>>(P3, 3LL * np, uv, K, np, n, max_iter, R, t, nullptr, nullptr,
+                                                                                 count, per_group);
+  SSP_CHECK_LAUNCH(); return SSP_OK;
 }
 
 int ssp_project_points(const float* X, int rows, int nv, const double* Rt, const double* K, long long n, float* out, void* stream) {

@@ -5,6 +5,7 @@
 // PREVIOUS image at the ground-truth cell, wrapping to the last image for b = 0) is reproduced on purpose.
 #include "ssp_common.cuh"
 #include "eval_multi_core.h"
+#include "detect_core.h"
 
 namespace ssp {
 
@@ -293,11 +294,177 @@ __global__ void __launch_bounds__(256) predict_multi_select_kernel(const Predict
   }
 }
 
+// ------------------------------------------------------------------------------------------------ every instance
+// ssp_detect_instances: the candidates, order and class-wise greedy suppression of detect_core.h, every image as its own call.
+// One CTA per image.  Every (cell, anchor) is decoded once; a candidate leaves its rectangle and class in shared memory (indexed by
+// entry) and its pick_key in a list whose bitonic sort (descending, zero-padded to a power of two) gives the key order whatever
+// order the atomics appended in.  The greedy pass runs one warp per requested class: the warp walks the sorted list, and each
+// of its class's candidates is tested against the class's kept boxes 32 at a time (a ballot decides).  A block-wide scan of
+// the keep flags in key order then gives each kept box its output slot; the first max_instances are written (the box
+// re-decoded by write_box, as the multi-object predictor writes its slots) and the rest of the slots are zeroed.
+constexpr int kDetectThreads = 512;
+
+struct DetectParams {
+  const float* out; float* boxes; int* cls; float* uv; int* count; int* kept;
+  int K, nC, nA, H, W, n_req, max_inst;
+  float thr, nms, frame_w, frame_h;
+  int classes[ssp_evm::kMaxClasses];
+};
+
+__host__ __device__ inline int pow2_at_least(int n) { int p = 1; while (p < n) p <<= 1; return p; }
+
+// dynamic shared memory of an image of n entries: keys [pow2(n)] u64, rectangles [n], kept entries [n] int, keep flags and
+// classes [n] bytes each
+__host__ __device__ inline int detect_smem_bytes(int n) {
+  return pow2_at_least(n) * 8 + n * (int)sizeof(ssp_det::Rect) + n * 4 + 2 * n;
+}
+
+__global__ void __launch_bounds__(kDetectThreads) detect_instances_kernel(const DetectParams p) {
+  using namespace ssp_evm;
+  using ssp_det::Rect;
+  extern __shared__ __align__(16) unsigned char s_raw[];
+  __shared__ unsigned char s_req[kMaxClasses];
+  __shared__ int s_off[kMaxClasses];                      // candidates per class, then the class's offset into s_kidx
+  __shared__ int s_ncand;
+  __shared__ int s_wsum[kDetectThreads / 32];
+  const int b = blockIdx.x, tid = threadIdx.x, K = p.K, nC = p.nC, nA = p.nA, W = p.W, H = p.H, HW = H * W, n = HW * nA;
+  const int nl = 2 * K + 3, M = p.max_inst;
+  unsigned long long* s_key = reinterpret_cast<unsigned long long*>(s_raw);
+  Rect* s_rect = reinterpret_cast<Rect*>(s_key + pow2_at_least(n));
+  int* s_kidx = reinterpret_cast<int*>(s_rect + n);
+  unsigned char* s_keep = reinterpret_cast<unsigned char*>(s_kidx + n);
+  unsigned char* s_ecls = s_keep + n;
+  const float* o = p.out + (long long)b * nA * (2 * K + 1 + nC) * HW;
+  for (int c = tid; c < nC; c += blockDim.x) { s_req[c] = 0; s_off[c] = 0; }
+  if (tid == 0) s_ncand = 0;
+  __syncthreads();
+  for (int q = tid; q < p.n_req; q += blockDim.x) s_req[p.classes[q]] = 1;
+  __syncthreads();
+  for (int t = tid; t < n; t += blockDim.x) {
+    const int a = t / HW, cell = t - a * HW, i = cell * nA + a;   // cells fastest across threads; i is the visiting order
+    float kp[2 * kKeypoints];
+    const Decoded d = decode_entry(o + (long long)a * (2 * K + 1 + nC) * HW + cell, HW, K, nC, cell % W, cell / W, W, H, -1, kp);
+    if (ssp_det::candidate(d, p.thr, s_req)) {
+      float uv[2 * kKeypoints];
+      s_rect[i] = ssp_det::entry_rect(kp, p.frame_w, p.frame_h, uv);
+      s_ecls[i] = (unsigned char)d.id;
+      atomicAdd(&s_off[d.id], 1);
+      s_key[atomicAdd(&s_ncand, 1)] = pick_key(d.det, i);
+    }
+  }
+  __syncthreads();
+  const int m = s_ncand, P = pow2_at_least(m);
+  for (int j = m + tid; j < P; j += blockDim.x) s_key[j] = 0ull;   // keys are never 0: the padding sorts last
+  if (tid == 0)
+    for (int c = 0, s = 0; c < nC; c++) { const int h = s_off[c]; s_off[c] = s; s += h; }
+  __syncthreads();
+  for (int k = 2; k <= P; k <<= 1)
+    for (int j = k >> 1; j > 0; j >>= 1) {
+      for (int t = tid; t < P; t += blockDim.x) {
+        const int u = t ^ j;
+        if (u > t) {
+          const unsigned long long x = s_key[t], y = s_key[u];
+          if ((t & k) == 0 ? x < y : x > y) { s_key[t] = y; s_key[u] = x; }
+        }
+      }
+      __syncthreads();
+    }
+  const int lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5;
+  for (int q = warp; q < p.n_req; q += nw) {
+    const int c = p.classes[q];
+    int* kl = s_kidx + s_off[c];                            // kept entries of class c, in key order
+    int nk = 0;
+    for (int j0 = 0; j0 < m; j0 += 32) {
+      const int j = j0 + lane;
+      const int e = j < m ? key_index(s_key[j]) : 0;
+      unsigned mine = __ballot_sync(0xffffffffu, j < m && s_ecls[e] == c);
+      while (mine) {
+        const int src = __ffs(mine) - 1;
+        mine &= mine - 1;
+        const int ej = __shfl_sync(0xffffffffu, e, src);
+        const Rect r = s_rect[ej];
+        bool sup = false;
+        for (int k = lane; k < nk && !sup; k += 32) sup = ssp_det::suppresses(s_rect[kl[k]], r, p.nms);
+        const bool keep = !__any_sync(0xffffffffu, sup);
+        if (lane == 0) { s_keep[j0 + src] = keep; if (keep) kl[nk] = ej; }
+        nk += keep;
+        __syncwarp();
+      }
+    }
+  }
+  __syncthreads();
+  int base = 0;                                             // kept boxes before the current chunk (the same in every thread)
+  for (int j0 = 0; j0 < m; j0 += blockDim.x) {
+    const int j = j0 + tid;
+    const bool f = j < m && s_keep[j];
+    const unsigned bal = __ballot_sync(0xffffffffu, f);
+    if (lane == 0) s_wsum[warp] = __popc(bal);
+    __syncthreads();
+    int rank = base + __popc(bal & ((1u << lane) - 1u)), total = 0;
+    for (int w = 0; w < nw; w++) { if (w < warp) rank += s_wsum[w]; total += s_wsum[w]; }
+    if (f && rank < M) {
+      const long long slot = (long long)b * M + rank;
+      float box[2 * kKeypoints + 3];
+      write_box(o, key_index(s_key[j]), fallback_init(), -1, nA, K, nC, W, H, box);
+      for (int v = 0; v < nl; v++) p.boxes[slot * nl + v] = box[v];
+      p.cls[slot] = (int)box[2 * K + 2];
+      for (int k = 0; k < kKeypoints; k++) box_uv(box, p.frame_w, p.frame_h, k, p.uv + slot * 2 * kKeypoints);
+    }
+    base += total;
+    __syncthreads();
+  }
+  const int cnt = min(base, M);
+  for (int r = cnt + tid; r < M; r += blockDim.x) {
+    const long long slot = (long long)b * M + r;
+    for (int v = 0; v < nl; v++) p.boxes[slot * nl + v] = 0.f;
+    for (int v = 0; v < 2 * kKeypoints; v++) p.uv[slot * 2 * kKeypoints + v] = 0.f;
+    p.cls[slot] = -1;
+  }
+  if (tid == 0) { p.count[b] = cnt; p.kept[b] = base; }
+}
+
 }  // namespace ssp
 
 using namespace ssp;
 
 extern "C" {
+int ssp_detect_instances(const float* out, int B, int K, int nC, int nA, int H, int W, const int* classes_host, int n_req, float conf_thresh,
+                         float nms_thresh, int max_instances, float frame_w, float frame_h, float* boxes, int* cls, float* uv, int* count,
+                         int* kept, void* stream) {
+  if (!out || !classes_host || !boxes || !cls || !uv || !count || !kept) return fail_msg(SSP_ERR_ARG, "detect_instances: null pointer");
+  if (K != ssp_evm::kKeypoints)
+    return fail_msg(SSP_ERR_ARG, "detect_instances: num_keypoints must be 9 (the overlap box is the 8 corners of a pose box)");
+  if (B < 0 || nC < 1 || nA < 1 || H < 1 || W < 1) return fail_msg(SSP_ERR_ARG, "detect_instances: bad argument");
+  if ((long long)H * W * nA > ssp_evm::kMaxEntries)
+    return fail_msg(SSP_ERR_ARG, "detect_instances: grid too large (H*W*num_anchors must be at most 4096, e.g. 26x26x5)");
+  if (nC > ssp_evm::kMaxClasses) return fail_msg(SSP_ERR_ARG, "detect_instances: at most 256 classes");
+  if (n_req < 1 || n_req > nC) return fail_msg(SSP_ERR_ARG, "detect_instances: n_req must be in [1, num_classes]");
+  if (!(nms_thresh >= 0.f && nms_thresh <= 1.f)) return fail_msg(SSP_ERR_ARG, "detect_instances: nms_thresh must be in [0, 1]");
+  if (max_instances < 1 || max_instances > ssp_det::kMaxInstances)
+    return fail_msg(SSP_ERR_ARG, "detect_instances: max_instances must be in [1, 256]");
+  DetectParams p;
+  bool seen[ssp_evm::kMaxClasses] = {};
+  for (int q = 0; q < n_req; q++) {
+    const int c = classes_host[q];
+    if (c < 0 || c >= nC) return fail_msg(SSP_ERR_ARG, "detect_instances: requested class out of [0, num_classes)");
+    if (seen[c]) return fail_msg(SSP_ERR_ARG, "detect_instances: requested class listed twice");
+    seen[c] = true; p.classes[q] = c;
+  }
+  if (B == 0) return SSP_OK;
+  static int configured = 0;
+  if (!configured) {
+    const cudaError_t e = cudaFuncSetAttribute(detect_instances_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               detect_smem_bytes(ssp_evm::kMaxEntries));
+    if (e != cudaSuccess) return fail_cuda(e, __FILE__, __LINE__);
+    configured = 1;
+  }
+  p.out = out; p.boxes = boxes; p.cls = cls; p.uv = uv; p.count = count; p.kept = kept;
+  p.K = K; p.nC = nC; p.nA = nA; p.H = H; p.W = W; p.n_req = n_req; p.max_inst = max_instances;
+  p.thr = conf_thresh; p.nms = nms_thresh; p.frame_w = frame_w; p.frame_h = frame_h;
+  detect_instances_kernel<<<B, kDetectThreads, detect_smem_bytes(H * W * nA), (cudaStream_t)stream>>>(p);
+  SSP_CHECK_LAUNCH(); return SSP_OK;
+}
+
 int ssp_predict_multi_select(const float* out, int B, int K, int nC, int nA, int H, int W, const int* classes_host, int n_req, float conf_thresh,
                              float frame_w, float frame_h, float* boxes, int* flags, float* uv, void* stream) {
   if (!out || !classes_host || !boxes || !flags || !uv) return fail_msg(SSP_ERR_ARG, "predict_multi_select: null pointer");

@@ -3,6 +3,8 @@ The dense per-(cell, anchor) arithmetic and the reference's sequential fallback 
 applies the confidence mask (one device->host copy).  The pose helpers are shared with utils.py."""
 from __future__ import annotations
 
+import ctypes as _ctypes
+
 import numpy as np
 import torch
 
@@ -116,6 +118,39 @@ def get_multi_region_boxes(output, conf_thresh, num_classes, num_keypoints, anch
             cur.append([float(v) for v in src[:2 * K]] + [float(max_conf[b]), float(max_cls[b]), int(correspondingclass)])
         all_boxes.append(cur)
     return all_boxes
+
+
+def detect_instances(output, conf_thresh, nms_thresh, num_classes, num_keypoints, num_anchors, frame_size, classes=None,
+                     max_instances=32):
+    """Every instance of the requested classes in each image of a CUDA network output (B, (2K+1+C)*A, H, W): one
+    ssp_detect_instances launch (rules: csrc/detect_core.h).  Candidates are the boxes get_multi_region_boxes(...,
+    only_objectness=0) lists (det_conf * cls_max_conf > conf_thresh, never its fallback box) whose arg-max class is in `classes`
+    (default: all); they are ranked by det_conf (the earlier box on ties) and a candidate is dropped when the rectangle of its 8
+    corner keypoints in frame pixels has IoU > nms_thresh with a kept box of its own class.  The reference's nms, written for YOLO
+    boxes, is not reproduced.  frame_size = (width, height) the keypoints are scaled to.
+
+    Returns padded device tensors: count (B,) int32 = min(kept, max_instances), kept (B,) = boxes kept before the truncation,
+    cls (B, M) int32 (-1 in empty slots), conf (B, M) det_conf, cls_conf (B, M), keypoints_px (B, M, K, 2); empty slots are zero."""
+    if output.dim() == 3:
+        output = output.unsqueeze(0)
+    if not output.is_cuda:
+        raise SspError("detect_instances runs on CUDA tensors only")
+    out = output.detach().contiguous().float()
+    B, C, H, W = out.shape
+    K, nC, nA, M = int(num_keypoints), int(num_classes), int(num_anchors), int(max_instances)
+    if C != (2 * K + 1 + nC) * nA:
+        raise SspError("output has %d channels, expected (2K+1+C)*A = %d" % (C, (2 * K + 1 + nC) * nA))
+    cls_host = np.ascontiguousarray(range(nC) if classes is None else [int(c) for c in classes], dtype=np.int32)
+    dev = out.device
+    boxes = torch.empty(B, M, 2 * K + 3, dtype=torch.float32, device=dev)
+    cls = torch.empty(B, M, dtype=torch.int32, device=dev)
+    uv = torch.empty(B, M, K, 2, dtype=torch.float32, device=dev)
+    count = torch.empty(B, dtype=torch.int32, device=dev)
+    kept = torch.empty(B, dtype=torch.int32, device=dev)
+    call("ssp_detect_instances", ptr(out), B, K, nC, nA, H, W, _ctypes.c_void_p(cls_host.ctypes.data), len(cls_host), float(conf_thresh),
+         float(nms_thresh), M, float(frame_size[0]), float(frame_size[1]), ptr(boxes), ptr(cls), ptr(uv), ptr(count), ptr(kept),
+         stream_ptr())
+    return dict(count=count, kept=kept, cls=cls, conf=boxes[..., 2 * K], cls_conf=boxes[..., 2 * K + 1], keypoints_px=uv)
 
 
 # ------------------------------------------------------------------------------------------ batched evaluation tail
