@@ -231,6 +231,33 @@ int ssp_pnp_batched_work(const float* points3d, int points3d_shared, const float
  * R and t.  The slots of ssp_detect_instances are such groups. */
 int ssp_pnp_batched_counted(const float* points3d, const float* points2d, const float* K3x3, int num_points, int groups,
                             int per_group, const int* count, int max_iter, double* R_out, double* t_out, void* stream);
+/* the counted solve where problem i with use_guess[i] != 0 starts Levenberg-Marquardt from guess [i][6] = (rvec, t) and skips the
+ * DLT, as cv2.solvePnP(..., useExtrinsicGuess=True) does; the others are solved as by ssp_pnp_batched_counted (bit-identical R, t).
+ * guess, use_guess: DEVICE [groups*per_group][6] fp64 and [groups*per_group] int.  Out: params_out [n][6] fp64 = the final LM vector
+ * (cv2's rvec, tvec); work_out_or_null [n][3] as ssp_pnp_batched_work (0 DLT sweeps for a warm start).  Empty slots get zeros. */
+int ssp_pnp_batched_guess(const float* points3d, const float* points2d, const float* K3x3, int num_points, int groups,
+                          int per_group, const int* count, const double* guess, const int* use_guess, int max_iter, double* R_out,
+                          double* t_out, double* params_out, int* work_out_or_null, void* stream);
+
+/* ---- tracking instances across frames (rules: csrc/track_core.h): each row b is its own camera stream with T = max_tracks slots
+ *      (1 <= T <= 256).  The state is four DEVICE arrays, zeroed for a fresh start (alive 0, ids from 0):
+ *        tracks  int    [B][T][5]  alive, id, cls, misses (consecutive frames unmatched), hits;  fields of a slot with alive 0 are stale
+ *        rects   float  [B][T][4]  x0, y0, x1, y1: the corner rectangle of the track's last detection in frame pixels
+ *        poses   double [B][T][6]  rvec, t: the final Levenberg-Marquardt vector of the track's last solve
+ *        next_id int    [B]        the id the next new track of the stream gets
+ *      The detections are ssp_detect_instances' outputs for the frame: count [B], cls [B][max_det], uv [B][max_det][9][2].
+ *      ssp_track_associate matches the detections to the alive tracks of their class (highest corner-rectangle IoU > match_iou, in
+ *      detector order), ages the unmatched tracks (a track dies at misses > max_misses) and gives each unmatched detection the lowest
+ *      free slot and the next id.  Out per detection slot: slot [B][max_det] (the track slot, -1 for an empty or untracked slot),
+ *      track_id [B][max_det] (-1 likewise), guess [B][max_det][6] fp64 (the matched track's pose, else 0) and use_guess [B][max_det]
+ *      (1 when matched): the inputs of ssp_pnp_batched_guess.  ssp_track_commit then stores each matched or born track's rectangle,
+ *      the solve's params [B][max_det][6] (ssp_pnp_batched_guess' params_out), misses = 0 and hits + 1.  SSP_ERR_ARG for a null
+ *      pointer, B < 0, max_tracks or max_det outside [1, 256], match_iou outside [0, 1] or max_misses < 0. ---- */
+int ssp_track_associate(int B, int max_tracks, int max_det, const int* count, const int* cls, const float* uv, float match_iou,
+                        int max_misses, int* tracks, const float* rects, const double* poses, int* next_id, int* slot, int* track_id,
+                        double* guess, int* use_guess, void* stream);
+int ssp_track_commit(int B, int max_tracks, int max_det, const int* count, const float* uv, const int* slot, const double* params,
+                     int* tracks, float* rects, double* poses, void* stream);
 int ssp_project_points(const float* X, int rows, int nv, const double* Rt, const double* K3x3, long long n,
                        float* out, void* stream);
 

@@ -6,7 +6,7 @@ import subprocess
 import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-SOURCES = ["abi.cu", "conv_tc.cu", "conv_band.cu", "conv_bandt.cu", "wgrad_tc.cu", "conv_simt.cu", "l0_fused.cu", "elementwise.cu", "sgd_pack.cu", "region.cu", "region_multi.cu", "pnp.cu", "augment.cu", "adds.cu", "jpeg.cu", "render.cu"]
+SOURCES = ["abi.cu", "conv_tc.cu", "conv_band.cu", "conv_bandt.cu", "wgrad_tc.cu", "conv_simt.cu", "l0_fused.cu", "elementwise.cu", "sgd_pack.cu", "region.cu", "region_multi.cu", "pnp.cu", "track.cu", "augment.cu", "adds.cu", "jpeg.cu", "render.cu"]
 # augment.cu restates Pillow's float/double pixel arithmetic bit for bit: no multiply-add contraction there
 EXTRA = {"augment.cu": ["-fmad=false"]}
 LIB = os.path.join(HERE, "libssp_b200.so")

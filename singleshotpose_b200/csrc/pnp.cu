@@ -39,6 +39,29 @@ __global__ void __launch_bounds__(128) pnp_kernel(const float* __restrict__ P3, 
   if (work_out) { work_out[3 * id] = work[0]; work_out[3 * id + 1] = work[1]; work_out[3 * id + 2] = work[2]; }
 }
 
+// the counted solve of pnp_kernel<true>, where problem id starts LM from guess[id] (no DLT) when use_guess[id] != 0, and the final
+// LM vector goes to params_out[id].  A kernel of its own, so that the two pnp_kernel instantiations keep their code.
+__global__ void __launch_bounds__(128) pnp_guess_kernel(const float* __restrict__ P3, const float* __restrict__ uv,
+                                                        const float* __restrict__ Kmat, int np, long long n, int max_iter,
+                                                        const int* __restrict__ count, int per_group, const double* __restrict__ guess,
+                                                        const int* __restrict__ use_guess, double* __restrict__ R_out,
+                                                        double* __restrict__ t_out, double* __restrict__ params_out,
+                                                        int* __restrict__ work_out) {
+  const long long id = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (id >= n) return;
+  if (id % per_group >= count[id / per_group]) {
+    for (int k = 0; k < 9; k++) R_out[id * 9 + k] = 0.0;
+    for (int k = 0; k < 3; k++) t_out[id * 3 + k] = 0.0;
+    for (int k = 0; k < 6; k++) params_out[id * 6 + k] = 0.0;
+    if (work_out) { work_out[3 * id] = 0; work_out[3 * id + 1] = 0; work_out[3 * id + 2] = 0; }
+    return;
+  }
+  int work[3];
+  ssp_pnp::pnp_solve_one(P3 + id * 3 * np, uv + id * 2 * np, Kmat, np, max_iter, R_out + id * 9, t_out + id * 3, work, nullptr,
+                         use_guess[id] ? guess + id * 6 : nullptr, params_out + id * 6);
+  if (work_out) { work_out[3 * id] = work[0]; work_out[3 * id + 1] = work[1]; work_out[3 * id + 2] = work[2]; }
+}
+
 // compute_projection (utils.py:40-45): uv = K [R|t] X / z for every vertex; fp64 math, fp32 result [n][2][nv]
 __global__ void project_points_kernel(const float* __restrict__ X4 /*[4][nv] or [3][nv]*/, int rows, int nv,
                                       const double* __restrict__ Rt /*[n][3][4]*/, const double* __restrict__ Kd /*[9]*/, long long n,
@@ -89,6 +112,18 @@ int ssp_pnp_batched_counted(const float* P3, const float* uv, const float* K, in
   if (n == 0) return SSP_OK;
   pnp_kernel<true><<<(unsigned)((n + 127) / 128), 128, 0, (cudaStream_t)stream>>>(P3, 3LL * np, uv, K, np, n, max_iter, R, t, nullptr, nullptr,
                                                                                  count, per_group);
+  SSP_CHECK_LAUNCH(); return SSP_OK;
+}
+
+int ssp_pnp_batched_guess(const float* P3, const float* uv, const float* K, int np, int groups, int per_group, const int* count,
+                          const double* guess, const int* use_guess, int max_iter, double* R, double* t, double* params, int* work,
+                          void* stream) {
+  if (!P3 || !uv || !K || !count || !guess || !use_guess || !R || !t || !params || np < 6 || np > PNP_MAXP || groups < 0 || per_group < 1)
+    return fail_msg(SSP_ERR_ARG, "pnp_batched_guess: bad argument (6 <= points <= 16, groups >= 0, per_group >= 1)");
+  const long long n = (long long)groups * per_group;
+  if (n == 0) return SSP_OK;
+  pnp_guess_kernel<<<(unsigned)((n + 127) / 128), 128, 0, (cudaStream_t)stream>>>(P3, uv, K, np, n, max_iter, count, per_group, guess, use_guess,
+                                                                                R, t, params, work);
   SSP_CHECK_LAUNCH(); return SSP_OK;
 }
 

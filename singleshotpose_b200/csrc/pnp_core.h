@@ -325,91 +325,101 @@ SSP_HD double reproj_err(const double* M, const double* m, int np, const double 
 }
 
 // p3: np x 3 object points, q: np x 2 image points (pixels), Kmat: 3x3 row-major intrinsics (float32 like the reference passes them);
-// R_out[9], t_out[3] in fp64; work[3] = {Jacobi sweeps of the DLT, accepted LM iterations, LM linear solves}
+// R_out[9], t_out[3] in fp64; work[3] = {Jacobi sweeps of the DLT (0 when started from a guess), accepted LM iterations, LM linear solves}.
+// The solve has two stages: the DLT gives the initial LM vector p = (rvec, t), LM refines it.  guess (6, or null): LM starts from this
+// (rvec, t) and the DLT is skipped, as cvFindExtrinsicCameraParams2 does with useExtrinsicGuess (same LM, same max_iter, same
+// FLT_EPSILON stop).  params_out (6, or null): the final LM vector, what cv2.solvePnP returns as rvec, tvec.  Both stay in this one
+// function (not two called ones) because that keeps the code nvcc generates for guess == params_out == null unchanged.
 SSP_HD void pnp_solve_one(const float* p3, const float* q, const float* Kmat, int np, int max_iter, double* R_out, double* t_out, int* work,
-                          double* dbg = nullptr /*[20]: smallest eigenvalue, its eigenvector, det, initial (rvec, t) -- probes only*/) {
+                          double* dbg = nullptr /*[20]: smallest eigenvalue, its eigenvector, det, initial (rvec, t) -- probes only*/,
+                          const double* guess = nullptr, double* params_out = nullptr) {
   const double fx = Kmat[0], fy = Kmat[4], cx = Kmat[2], cy = Kmat[5];
   double M[3 * PNP_MAXP], m[2 * PNP_MAXP];
   for (int i = 0; i < 3 * np; i++) M[i] = (double)p3[i];
   for (int i = 0; i < 2 * np; i++) m[i] = (double)q[i];
 
-  // ---- DLT (cvFindExtrinsicCameraParams2, non-planar branch): smallest eigenvector of L^T L on the raw coordinates ----
-  // the four 4 x 4 blocks of L^T L; the smallest eigenvector through the block solve (dlt_smallest_eigvec), the cyclic Jacobi on the
-  // assembled 12 x 12 matrix only if that declines (PNP_DLT_JACOBI=1 forces it: the two must agree, tests/test_pnp_host.py)
-  DltBlocks Bk;
-  for (int a = 0; a < 4; a++) for (int b = 0; b < 4; b++) { Bk.S[a][b] = 0.0; Bk.Sx[a][b] = 0.0; Bk.Sy[a][b] = 0.0; Bk.Sq[a][b] = 0.0; }
-  for (int i = 0; i < np; i++) {
-    const double X[4] = {M[3 * i], M[3 * i + 1], M[3 * i + 2], 1.0};
-    const double x = (m[2 * i] - cx) / fx, y = (m[2 * i + 1] - cy) / fy, qq = x * x + y * y;
-    for (int a = 0; a < 4; a++)
-      for (int b = 0; b < 4; b++) {
-        const double xx = X[a] * X[b];
-        Bk.S[a][b] += xx; Bk.Sx[a][b] += x * xx; Bk.Sy[a][b] += y * xx; Bk.Sq[a][b] += qq * xx;
-      }
-  }
-  double ev[12], lam_min = 0.0; int sweeps = 0;
+  double p[6];
+  int sweeps = 0;
+  if (guess) {
+    for (int i = 0; i < 6; i++) p[i] = guess[i];
+  } else {
+    // ---- DLT (cvFindExtrinsicCameraParams2, non-planar branch): smallest eigenvector of L^T L on the raw coordinates ----
+    // the four 4 x 4 blocks of L^T L; the smallest eigenvector through the block solve (dlt_smallest_eigvec), the cyclic Jacobi on the
+    // assembled 12 x 12 matrix only if that declines (PNP_DLT_JACOBI=1 forces it: the two must agree, tests/test_pnp_host.py)
+    DltBlocks Bk;
+    for (int a = 0; a < 4; a++) for (int b = 0; b < 4; b++) { Bk.S[a][b] = 0.0; Bk.Sx[a][b] = 0.0; Bk.Sy[a][b] = 0.0; Bk.Sq[a][b] = 0.0; }
+    for (int i = 0; i < np; i++) {
+      const double X[4] = {M[3 * i], M[3 * i + 1], M[3 * i + 2], 1.0};
+      const double x = (m[2 * i] - cx) / fx, y = (m[2 * i + 1] - cy) / fy, qq = x * x + y * y;
+      for (int a = 0; a < 4; a++)
+        for (int b = 0; b < 4; b++) {
+          const double xx = X[a] * X[b];
+          Bk.S[a][b] += xx; Bk.Sx[a][b] += x * xx; Bk.Sy[a][b] += y * xx; Bk.Sq[a][b] += qq * xx;
+        }
+    }
+    double ev[12], lam_min = 0.0;
 #ifndef PNP_DLT_JACOBI
 #define PNP_DLT_JACOBI 0
 #endif
-  bool have = false;
-  if (!PNP_DLT_JACOBI) { int st = 0; have = dlt_smallest_eigvec(Bk, ev, &lam_min, &st); sweeps = -st; }      // work[0] < 0: block-solve steps
-  if (!have) {
-    double LL[12][12], LV[12][12];
-    for (int a = 0; a < 12; a++) for (int b = 0; b < 12; b++) LL[a][b] = 0.0;
-    for (int a = 0; a < 4; a++)
-      for (int b = 0; b < 4; b++) {
-        LL[a][b] = Bk.S[a][b]; LL[4 + a][4 + b] = Bk.S[a][b];
-        LL[a][8 + b] = -Bk.Sx[a][b]; LL[4 + a][8 + b] = -Bk.Sy[a][b];
-        LL[8 + a][8 + b] = Bk.Sq[a][b];
-      }
-    for (int a = 0; a < 8; a++) for (int b = 8; b < 12; b++) LL[b][a] = LL[a][b];
-    sweeps = jacobi_eig<12>(LL, LV);
-    int kmin = 0;
-    for (int k = 1; k < 12; k++) if (LL[k][k] < LL[kmin][kmin]) kmin = k;
-    for (int i = 0; i < 12; i++) ev[i] = LV[i][kmin];
-    lam_min = LL[kmin][kmin];
-  }
-  double RR[9], tt[3];
-  for (int r = 0; r < 3; r++) {
-    RR[3 * r] = ev[4 * r]; RR[3 * r + 1] = ev[4 * r + 1]; RR[3 * r + 2] = ev[4 * r + 2];
-    tt[r] = ev[4 * r + 3];
-  }
-  const double det = RR[0] * (RR[4] * RR[8] - RR[5] * RR[7]) - RR[1] * (RR[3] * RR[8] - RR[5] * RR[6]) + RR[2] * (RR[3] * RR[7] - RR[4] * RR[6]);
-  if (det < 0) { for (int i = 0; i < 9; i++) RR[i] = -RR[i]; for (int i = 0; i < 3; i++) tt[i] = -tt[i]; }
-  double sc = 0; for (int i = 0; i < 9; i++) sc += RR[i] * RR[i];
-  sc = sqrt(sc);
-  // polar decomposition: R = RR (RR^T RR)^(-1/2)
-  double G[3][3], Vg[3][3];
-  for (int a = 0; a < 3; a++) for (int b = 0; b < 3; b++) { double v = 0; for (int k = 0; k < 3; k++) v += RR[3 * k + a] * RR[3 * k + b]; G[a][b] = v; }
-  jacobi_eig<3>(G, Vg);
-  double Gi[3][3];
-  for (int a = 0; a < 3; a++) for (int b = 0; b < 3; b++) { double v = 0; for (int k = 0; k < 3; k++) v += Vg[a][k] * Vg[b][k] / sqrt(fmax(G[k][k], 1e-300)); Gi[a][b] = v; }
-  double R0[9];
-  for (int a = 0; a < 3; a++) for (int b = 0; b < 3; b++) { double v = 0; for (int k = 0; k < 3; k++) v += RR[3 * a + k] * Gi[k][b]; R0[3 * a + b] = v; }
-  double p[6];
-  { const double f = sqrt(3.0) / sc; p[3] = tt[0] * f; p[4] = tt[1] * f; p[5] = tt[2] * f; }
-  {  // rotation matrix -> axis-angle (cv2.Rodrigues inverse branch structure)
-    const double rv[3] = {R0[7] - R0[5], R0[2] - R0[6], R0[3] - R0[1]};
-    const double s = sqrt((rv[0] * rv[0] + rv[1] * rv[1] + rv[2] * rv[2]) * 0.25);
-    double c = (R0[0] + R0[4] + R0[8] - 1.0) * 0.5; c = c > 1.0 ? 1.0 : (c < -1.0 ? -1.0 : c);
-    const double th = acos(c);
-    if (s < 1e-5) {
-      if (c > 0) { p[0] = p[1] = p[2] = 0.0; }
-      else {
-        double tx = sqrt(fmax((R0[0] + 1) * 0.5, 0.0));
-        double ty = sqrt(fmax((R0[4] + 1) * 0.5, 0.0)) * (R0[1] < 0 ? -1.0 : 1.0);
-        double tz = sqrt(fmax((R0[8] + 1) * 0.5, 0.0)) * (R0[2] < 0 ? -1.0 : 1.0);
-        if (fabs(tx) < fabs(ty) && fabs(tx) < fabs(tz) && ((R0[5] > 0) != (ty * tz > 0))) tz = -tz;
-        const double nn = th / sqrt(tx * tx + ty * ty + tz * tz);
-        p[0] = tx * nn; p[1] = ty * nn; p[2] = tz * nn;
-      }
-    } else {
-      const double f = 0.5 / s * th;
-      p[0] = rv[0] * f; p[1] = rv[1] * f; p[2] = rv[2] * f;
+    bool have = false;
+    if (!PNP_DLT_JACOBI) { int st = 0; have = dlt_smallest_eigvec(Bk, ev, &lam_min, &st); sweeps = -st; }      // work[0] < 0: block-solve steps
+    if (!have) {
+      double LL[12][12], LV[12][12];
+      for (int a = 0; a < 12; a++) for (int b = 0; b < 12; b++) LL[a][b] = 0.0;
+      for (int a = 0; a < 4; a++)
+        for (int b = 0; b < 4; b++) {
+          LL[a][b] = Bk.S[a][b]; LL[4 + a][4 + b] = Bk.S[a][b];
+          LL[a][8 + b] = -Bk.Sx[a][b]; LL[4 + a][8 + b] = -Bk.Sy[a][b];
+          LL[8 + a][8 + b] = Bk.Sq[a][b];
+        }
+      for (int a = 0; a < 8; a++) for (int b = 8; b < 12; b++) LL[b][a] = LL[a][b];
+      sweeps = jacobi_eig<12>(LL, LV);
+      int kmin = 0;
+      for (int k = 1; k < 12; k++) if (LL[k][k] < LL[kmin][kmin]) kmin = k;
+      for (int i = 0; i < 12; i++) ev[i] = LV[i][kmin];
+      lam_min = LL[kmin][kmin];
     }
-  }
+    double RR[9], tt[3];
+    for (int r = 0; r < 3; r++) {
+      RR[3 * r] = ev[4 * r]; RR[3 * r + 1] = ev[4 * r + 1]; RR[3 * r + 2] = ev[4 * r + 2];
+      tt[r] = ev[4 * r + 3];
+    }
+    const double det = RR[0] * (RR[4] * RR[8] - RR[5] * RR[7]) - RR[1] * (RR[3] * RR[8] - RR[5] * RR[6]) + RR[2] * (RR[3] * RR[7] - RR[4] * RR[6]);
+    if (det < 0) { for (int i = 0; i < 9; i++) RR[i] = -RR[i]; for (int i = 0; i < 3; i++) tt[i] = -tt[i]; }
+    double sc = 0; for (int i = 0; i < 9; i++) sc += RR[i] * RR[i];
+    sc = sqrt(sc);
+    // polar decomposition: R = RR (RR^T RR)^(-1/2)
+    double G[3][3], Vg[3][3];
+    for (int a = 0; a < 3; a++) for (int b = 0; b < 3; b++) { double v = 0; for (int k = 0; k < 3; k++) v += RR[3 * k + a] * RR[3 * k + b]; G[a][b] = v; }
+    jacobi_eig<3>(G, Vg);
+    double Gi[3][3];
+    for (int a = 0; a < 3; a++) for (int b = 0; b < 3; b++) { double v = 0; for (int k = 0; k < 3; k++) v += Vg[a][k] * Vg[b][k] / sqrt(fmax(G[k][k], 1e-300)); Gi[a][b] = v; }
+    double R0[9];
+    for (int a = 0; a < 3; a++) for (int b = 0; b < 3; b++) { double v = 0; for (int k = 0; k < 3; k++) v += RR[3 * a + k] * Gi[k][b]; R0[3 * a + b] = v; }
+    { const double f = sqrt(3.0) / sc; p[3] = tt[0] * f; p[4] = tt[1] * f; p[5] = tt[2] * f; }
+    {  // rotation matrix -> axis-angle (cv2.Rodrigues inverse branch structure)
+      const double rv[3] = {R0[7] - R0[5], R0[2] - R0[6], R0[3] - R0[1]};
+      const double s = sqrt((rv[0] * rv[0] + rv[1] * rv[1] + rv[2] * rv[2]) * 0.25);
+      double c = (R0[0] + R0[4] + R0[8] - 1.0) * 0.5; c = c > 1.0 ? 1.0 : (c < -1.0 ? -1.0 : c);
+      const double th = acos(c);
+      if (s < 1e-5) {
+        if (c > 0) { p[0] = p[1] = p[2] = 0.0; }
+        else {
+          double tx = sqrt(fmax((R0[0] + 1) * 0.5, 0.0));
+          double ty = sqrt(fmax((R0[4] + 1) * 0.5, 0.0)) * (R0[1] < 0 ? -1.0 : 1.0);
+          double tz = sqrt(fmax((R0[8] + 1) * 0.5, 0.0)) * (R0[2] < 0 ? -1.0 : 1.0);
+          if (fabs(tx) < fabs(ty) && fabs(tx) < fabs(tz) && ((R0[5] > 0) != (ty * tz > 0))) tz = -tz;
+          const double nn = th / sqrt(tx * tx + ty * ty + tz * tz);
+          p[0] = tx * nn; p[1] = ty * nn; p[2] = tz * nn;
+        }
+      } else {
+        const double f = 0.5 / s * th;
+        p[0] = rv[0] * f; p[1] = rv[1] * f; p[2] = rv[2] * f;
+      }
+    }
 
-  if (dbg) { dbg[0] = lam_min; for (int i = 0; i < 12; i++) dbg[1 + i] = ev[i]; dbg[13] = det; for (int i = 0; i < 6; i++) dbg[14 + i] = p[i]; }
+    if (dbg) { dbg[0] = lam_min; for (int i = 0; i < 12; i++) dbg[1 + i] = ev[i]; dbg[13] = det; for (int i = 0; i < 6; i++) dbg[14 + i] = p[i]; }
+  }
 
   // ---- Levenberg-Marquardt (CvLevMarq schedule) ----
   int lam_lg10 = -3, iters = 0, solves = 0;
@@ -466,6 +476,7 @@ SSP_HD void pnp_solve_one(const float* p3, const float* q, const float* Kmat, in
   rodrigues(p, R, nullptr);
   for (int i = 0; i < 9; i++) R_out[i] = R[i];
   for (int i = 0; i < 3; i++) t_out[i] = p[3 + i];
+  if (params_out) for (int i = 0; i < 6; i++) params_out[i] = p[i];
   work[0] = sweeps; work[1] = iters; work[2] = solves;
 }
 

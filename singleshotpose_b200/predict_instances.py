@@ -24,8 +24,13 @@ class's columns, masked to zero in the empty slots.
 
 Returned device tensors are the predictor's static outputs: the next call overwrites them.
 
+TrackingPosePredictor adds stable track ids across calls (each batch row is a camera stream) and PnP warm-started from each
+track's last pose (utils_multi.InstanceTracker, rules: csrc/track_core.h).
+
 Command line: python -m singleshotpose_b200.predict_instances --datacfg cfg/occlusion.data --modelcfg cfg/yolo-pose-multi.cfg
               --weightfile w.weights --object 0=../LINEMOD/ape/ape.ply --object 4=../LINEMOD/can/can.ply --out det.npz img...
+              [--track [--match-iou 0.3 --max-misses 5 --max-tracks 64]]: the images, in the order given, as one stream, with a
+              track_id column
 """
 from __future__ import annotations
 
@@ -38,6 +43,7 @@ import torch
 from ._lib import SspError, call, ptr
 from .predict import _FramePredictor
 from .predict_multi import MAX_ENTRIES, parse_objects
+from .utils_multi import MAX_TRACKS, InstanceTracker, check_track_args
 
 MAX_INSTANCES = 256         # largest max_instances (detect_core.h kMaxInstances)
 OUTPUT_KEYS = ("count", "kept", "cls", "R", "t", "conf", "cls_conf", "keypoints_px", "corners_px")
@@ -121,6 +127,11 @@ class InstancePosePredictor(_FramePredictor):
         c.corners = torch.empty(B, M, K, 2, dtype=torch.float32, device=dev)
 
     def _head(self, c, s):
+        self._detect(c, s)
+        self._solve(c, s)
+        self._project(c, s)
+
+    def _detect(self, c, s):
         B, K, M, Q = self.batch, self.num_keypoints, self.max_instances, self._Q
         Wf, Hf = c.frame
         h, w = c.logits.shape[2:]
@@ -128,7 +139,13 @@ class InstancePosePredictor(_FramePredictor):
              Q, self.conf_thresh, self.nms_thresh, M, float(Wf), float(Hf), ptr(c.boxes), ptr(c.cls), ptr(c.kp), ptr(c.count), ptr(c.kept), s)
         torch.clamp(c.cls, min=0, out=c.cls0)                  # empty slots hold -1: any in-range index will do, PnP skips them
         torch.index_select(self._P3_table, 0, c.cls0.view(-1), out=c.P3)
-        call("ssp_pnp_batched_counted", ptr(c.P3), ptr(c.kp), ptr(self._K32), K, B, M, ptr(c.count), 20, ptr(c.R), ptr(c.t), s)
+
+    def _solve(self, c, s):
+        call("ssp_pnp_batched_counted", ptr(c.P3), ptr(c.kp), ptr(self._K32), self.num_keypoints, self.batch, self.max_instances,
+             ptr(c.count), 20, ptr(c.R), ptr(c.t), s)
+
+    def _project(self, c, s):
+        B, K, M, Q = self.batch, self.num_keypoints, self.max_instances, self._Q
         c.Rt[..., :3].copy_(c.R)
         c.Rt[..., 3].copy_(c.t)
         # every requested class's points under every slot's pose (each point is projected on its own, so a slot's own columns are
@@ -142,6 +159,55 @@ class InstancePosePredictor(_FramePredictor):
         K = self.num_keypoints
         return dict(count=c.count, kept=c.kept, cls=c.cls, R=c.R, t=c.t, conf=c.boxes[..., 2 * K], cls_conf=c.boxes[..., 2 * K + 1],
                     keypoints_px=c.kp, corners_px=c.corners)
+
+
+class TrackingPosePredictor(InstancePosePredictor):
+    """InstancePosePredictor whose instances keep their identity across calls: each row b of a batch is its own camera stream, and
+    each instance is matched to a track of its class (utils_multi.InstanceTracker, rules: csrc/track_core.h).  A matched instance's
+    PnP starts Levenberg-Marquardt from its track's last pose (cv2.solvePnP's useExtrinsicGuess), the others are solved cold.
+    No motion model: a track is matched against its last corner rectangle, and the guess is its last pose.
+
+    max_tracks in [1, 256] track slots per stream, match_iou in [0, 1] (a match needs IoU > match_iou), max_misses >= 0 (a track
+    dies after max_misses + 1 frames in a row without a match); the other arguments are InstancePosePredictor's.
+
+    Returns InstancePosePredictor's dict plus track_id (B, M) int32 (-1 in empty and untracked slots) and warm (B, M) bool (the
+    slot's solve started from its track's pose).  The track state is shared by every frame size and source (one set of device
+    arrays, zeroed in place by reset); the warm-up runs before a graph capture do not advance it."""
+
+    def __init__(self, model, objects, K, frame_size=(640, 480), shape=None, batch=1, conf_thresh=None, nms_thresh=0.4, max_instances=32,
+                 max_tracks=64, match_iou=0.3, max_misses=5, graph=True, max_graphs=4):
+        check_track_args(max_tracks, match_iou, max_misses)
+        super().__init__(model, objects, K, frame_size, shape, batch, conf_thresh, nms_thresh, max_instances, graph, max_graphs)
+        if not isinstance(objects, dict):
+            objects = {0: objects}
+        self._tracker = InstanceTracker(objects, K, self.num_classes, self.num_anchors, self.frame_size, self.batch, self.conf_thresh,
+                                        self.nms_thresh, self.max_instances, max_tracks, match_iou, max_misses, device=self.device)
+        self.max_tracks, self.match_iou, self.max_misses = self._tracker.max_tracks, self._tracker.match_iou, self._tracker.max_misses
+
+    def reset(self, streams=None):
+        """forget the tracks of the given streams (default: all); their ids start again from 0"""
+        with torch.cuda.device(self.device):
+            self._tracker.reset(streams)
+
+    def tracks(self, to_host=False):
+        """the alive tracks (utils_multi.InstanceTracker.tracks): stream, slot, id, cls, misses, hits, rvec, R, t, rect"""
+        with torch.cuda.device(self.device):
+            return self._tracker.tracks(to_host)
+
+    def _head_buffers(self, c):
+        super()._head_buffers(c)
+        self._tracker.buffers(c)
+
+    def _solve(self, c, s):
+        self._tracker.solve(c, s, c.P3, self._K32)
+
+    def _capture(self, c, warmup=2):
+        saved = self._tracker.snapshot()          # the warm-up runs advance the tracks: put them back before the first replay
+        super()._capture(c, warmup)
+        self._tracker.restore(saved)
+
+    def _outputs(self, c):
+        return dict(super()._outputs(c), track_id=c.track_id, warm=c.warm)
 
 
 # ---------------------------------------------------------------------------------------------- command line
@@ -163,7 +229,8 @@ def camera_from_any_data_cfg(datacfg):
 
 
 def parse_args(argv=None):
-    """the command line, checked before any model is built: raises SspError for a bad --object, --nms-thresh or --max-instances"""
+    """the command line, checked before any model is built: raises SspError for a bad --object, --nms-thresh, --max-instances,
+    --match-iou, --max-misses or --max-tracks"""
     ap = argparse.ArgumentParser(prog="python -m singleshotpose_b200.predict_instances",
                                  description="6-D pose of every detected instance of the requested objects in each image")
     ap.add_argument("--datacfg", required=True, help=".data file: fx fy u0 v0 and width height (or im_width im_height); mesh")
@@ -174,12 +241,23 @@ def parse_args(argv=None):
     ap.add_argument("--nms-thresh", type=float, default=0.4)
     ap.add_argument("--max-instances", type=int, default=32)
     ap.add_argument("--out", default="instances.npz")
+    ap.add_argument("--track", action="store_true",
+                    help="treat the images, in the order given, as one camera stream: add a track_id column (TrackingPosePredictor)")
+    ap.add_argument("--match-iou", type=float, default=0.3)
+    ap.add_argument("--max-misses", type=int, default=5)
+    ap.add_argument("--max-tracks", type=int, default=64)
     ap.add_argument("images", nargs="+")
     a = ap.parse_args(argv)
     if not 0.0 <= a.nms_thresh <= 1.0:
         raise SspError("--nms-thresh must be in [0, 1], got %r" % a.nms_thresh)
     if not 1 <= a.max_instances <= MAX_INSTANCES:
         raise SspError("--max-instances must be in [1, %d], got %d" % (MAX_INSTANCES, a.max_instances))
+    if not 0.0 <= a.match_iou <= 1.0:
+        raise SspError("--match-iou must be in [0, 1], got %r" % a.match_iou)
+    if a.max_misses < 0:
+        raise SspError("--max-misses must be >= 0, got %d" % a.max_misses)
+    if not 1 <= a.max_tracks <= MAX_TRACKS:
+        raise SspError("--max-tracks must be in [1, %d], got %d" % (MAX_TRACKS, a.max_tracks))
     a.objects = parse_objects(a.object) if a.object else None
     return a
 
@@ -213,8 +291,12 @@ def main(argv=None):
     model = Darknet(a.modelcfg)
     model.load_weights(a.weightfile)
     model.cuda().eval()
-    pred = InstancePosePredictor(model, objects, K, frame_size=size, nms_thresh=a.nms_thresh, max_instances=a.max_instances)
-    rows = {k: [] for k in ROW_KEYS}
+    if a.track:
+        pred = TrackingPosePredictor(model, objects, K, frame_size=size, nms_thresh=a.nms_thresh, max_instances=a.max_instances,
+                                     max_tracks=a.max_tracks, match_iou=a.match_iou, max_misses=a.max_misses)
+    else:
+        pred = InstancePosePredictor(model, objects, K, frame_size=size, nms_thresh=a.nms_thresh, max_instances=a.max_instances)
+    rows = {k: [] for k in ROW_KEYS + (("track_id",) if a.track else ())}
     image = []
     for i, path in enumerate(a.images):
         with open(path, "rb") as f:

@@ -153,6 +153,180 @@ def detect_instances(output, conf_thresh, nms_thresh, num_classes, num_keypoints
     return dict(count=count, kept=kept, cls=cls, conf=boxes[..., 2 * K], cls_conf=boxes[..., 2 * K + 1], keypoints_px=uv)
 
 
+# ------------------------------------------------------------------------------------------ tracking across frames
+MAX_TRACKS = 256            # largest max_tracks (track_core.h kMaxTracks)
+
+
+def check_track_args(max_tracks, match_iou, max_misses):
+    """-> (max_tracks, match_iou, max_misses) as int, float, int; SspError for max_tracks outside [1, 256], match_iou outside [0, 1]
+    or max_misses < 0"""
+    if isinstance(max_tracks, bool) or not isinstance(max_tracks, (int, np.integer)) or not 1 <= max_tracks <= MAX_TRACKS:
+        raise SspError("max_tracks must be an integer in [1, %d], got %r" % (MAX_TRACKS, max_tracks))
+    match_iou = float(match_iou)
+    if not 0.0 <= match_iou <= 1.0:
+        raise SspError("match_iou must be in [0, 1], got %r" % match_iou)
+    if isinstance(max_misses, bool) or not isinstance(max_misses, (int, np.integer)) or max_misses < 0:
+        raise SspError("max_misses must be an integer >= 0, got %r" % (max_misses,))
+    return int(max_tracks), match_iou, int(max_misses)
+
+
+def rodrigues_batched(r):
+    """(n, 3) fp64 rotation vectors -> (n, 3, 3) rotation matrices (cv2.Rodrigues' formula; the identity below machine epsilon)"""
+    th = torch.linalg.vector_norm(r, dim=1)
+    small = th < np.finfo(np.float64).eps
+    u = r / torch.where(small, torch.ones_like(th), th).unsqueeze(1)
+    c, s = torch.cos(th)[:, None, None], torch.sin(th)[:, None, None]
+    z = torch.zeros_like(th)
+    ux = torch.stack([z, -u[:, 2], u[:, 1], u[:, 2], z, -u[:, 0], -u[:, 1], u[:, 0], z], 1).view(-1, 3, 3)
+    eye = torch.eye(3, dtype=r.dtype, device=r.device).expand(len(r), 3, 3)
+    R = c * eye + (1 - c) * u.unsqueeze(2) * u.unsqueeze(1) + s * ux
+    return torch.where(small[:, None, None], eye, R)
+
+
+class InstanceTracker:
+    """Stable track ids across the frames of B camera streams, and PnP warm-started from each track's last pose (rules:
+    csrc/track_core.h).  Per frame: the instances of detect_instances; ssp_track_associate matches each to an alive track of its
+    class (highest IoU of the corner rectangles > match_iou, in det_conf order), ages the unmatched tracks (a track dies after
+    max_misses + 1 missed frames in a row) and gives the other detections the lowest free slot and the stream's next id;
+    ssp_pnp_batched_guess starts Levenberg-Marquardt from the matched track's pose (no DLT) and solves the others cold;
+    ssp_track_commit stores each track's rectangle and final LM vector.  No motion model: a track is matched against its last
+    rectangle and the guess is its last pose.  update(logits) is the eager, logits-level surface; predict_instances.
+    TrackingPosePredictor issues the same launches inside its graph replay.
+
+    objects: {class id: (3|4, 8) box corners}; K (3, 3); frame_size (width, height); batch = streams; max_tracks in [1, 256] slots
+    per stream, match_iou in [0, 1], max_misses >= 0.  The state lives in four device arrays allocated once (graphs bake their
+    addresses in): tracks (B, T, 5) int32 = alive, id, cls, misses, hits; rects (B, T, 4) fp32; poses (B, T, 6) fp64 = (rvec, t);
+    next_id (B,) int32.  reset() zeroes them in place."""
+
+    def __init__(self, objects, K, num_classes, num_anchors, frame_size, batch=1, conf_thresh=0.05, nms_thresh=0.4, max_instances=32,
+                 max_tracks=64, match_iou=0.3, max_misses=5, num_keypoints=9, device=None):
+        self.max_tracks, self.match_iou, self.max_misses = check_track_args(max_tracks, match_iou, max_misses)
+        if not isinstance(objects, dict):
+            objects = {0: objects}
+        nC = int(num_classes)
+        if not objects or any(isinstance(c, bool) or not isinstance(c, (int, np.integer)) or not 0 <= c < nC for c in objects):
+            raise SspError("objects must be a non-empty {class id in [0, %d): corners3D} dict" % nC)
+        Km = np.asarray(K, dtype=np.float64)
+        if Km.shape != (3, 3):
+            raise SspError("K must be (3, 3), got %s" % (Km.shape,))
+        if int(num_keypoints) != 9:
+            raise SspError("tracking solves PnP on the centroid + 8 box corners: 9 keypoints, not %d" % int(num_keypoints))
+        self.batch, self.max_instances = int(batch), int(max_instances)
+        if self.batch < 1:
+            raise SspError("batch must be >= 1")
+        self.num_classes, self.num_anchors, self.num_keypoints = nC, int(num_anchors), 9
+        self.frame_size = (float(frame_size[0]), float(frame_size[1]))
+        self.conf_thresh, self.nms_thresh = float(conf_thresh), float(nms_thresh)
+        self.classes = np.array(sorted(objects), np.int32)
+        dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        self.device = dev
+        table = np.zeros((nC, 9, 3), np.float32)
+        for c in self.classes:
+            cc = np.asarray(objects[int(c)], dtype=np.float64)
+            if cc.ndim != 2 or cc.shape[0] not in (3, 4) or cc.shape[1] != 8:
+                raise SspError("corners3D must be (3|4, 8), got %s" % (cc.shape,))
+            table[c, 1:] = cc[:3].T
+        self._P3_table = torch.from_numpy(table).to(dev)
+        self._K32 = torch.from_numpy(np.ascontiguousarray(Km, dtype=np.float32)).to(dev)
+        B, T = self.batch, self.max_tracks
+        self.state_tracks = torch.zeros(B, T, 5, dtype=torch.int32, device=dev)
+        self.state_rects = torch.zeros(B, T, 4, dtype=torch.float32, device=dev)
+        self.state_poses = torch.zeros(B, T, 6, dtype=torch.float64, device=dev)
+        self.state_next_id = torch.zeros(B, dtype=torch.int32, device=dev)
+        self._bufs = None
+
+    # ------------------------------------------------------------------ state
+    def _state(self):
+        return (self.state_tracks, self.state_rects, self.state_poses, self.state_next_id)
+
+    def reset(self, streams=None):
+        """forget every track of the given streams (default: all), in place: ids start again from 0"""
+        idx = slice(None) if streams is None else torch.as_tensor(np.asarray(streams, np.int64).reshape(-1), device=self.device)
+        for t in self._state():
+            t[idx] = 0
+
+    def snapshot(self):
+        return tuple(t.clone() for t in self._state())
+
+    def restore(self, saved):
+        for t, s in zip(self._state(), saved):
+            t.copy_(s)
+
+    def tracks(self, to_host=False):
+        """the alive tracks of every stream, ordered by (stream, slot): stream, slot, id, cls, misses, hits (n,) int32; rvec (n, 3),
+        R (n, 3, 3) (Rodrigues of rvec), t (n, 3) fp64 = the track's last pose; rect (n, 4) fp32 = its last corner rectangle"""
+        st = self.state_tracks
+        b, s = torch.nonzero(st[..., 0] != 0, as_tuple=True)
+        f, pose = st[b, s], self.state_poses[b, s]
+        out = dict(stream=b.int(), slot=s.int(), id=f[:, 1], cls=f[:, 2], misses=f[:, 3], hits=f[:, 4], rvec=pose[:, :3],
+                   R=rodrigues_batched(pose[:, :3]), t=pose[:, 3:], rect=self.state_rects[b, s])
+        if to_host:
+            return {k: v.cpu().numpy() for k, v in out.items()}
+        return out
+
+    # ------------------------------------------------------------------ launches
+    def buffers(self, c):
+        """the per-frame device buffers of the tracking launches, as attributes of c (B streams x M detection slots)"""
+        dev, B, M = self.device, self.batch, self.max_instances
+        c.slot = torch.empty(B, M, dtype=torch.int32, device=dev)
+        c.track_id = torch.empty(B, M, dtype=torch.int32, device=dev)
+        c.guess = torch.empty(B, M, 6, dtype=torch.float64, device=dev)
+        c.use_guess = torch.empty(B, M, dtype=torch.int32, device=dev)
+        c.params = torch.empty(B, M, 6, dtype=torch.float64, device=dev)
+        c.warm = torch.empty(B, M, dtype=torch.bool, device=dev)
+
+    def solve(self, c, s, P3, K32):
+        """associate, warm-started PnP, commit: reads c.count, c.cls, c.kp (ssp_detect_instances' outputs) and P3 (B*M, 9, 3) the
+        slots' PnP points; writes c.R, c.t, c.params, c.slot, c.track_id, c.guess, c.use_guess, c.warm"""
+        B, T, M = self.batch, self.max_tracks, self.max_instances
+        call("ssp_track_associate", B, T, M, ptr(c.count), ptr(c.cls), ptr(c.kp), self.match_iou, self.max_misses, ptr(self.state_tracks),
+             ptr(self.state_rects), ptr(self.state_poses), ptr(self.state_next_id), ptr(c.slot), ptr(c.track_id), ptr(c.guess),
+             ptr(c.use_guess), s)
+        call("ssp_pnp_batched_guess", ptr(P3), ptr(c.kp), ptr(K32), 9, B, M, ptr(c.count), ptr(c.guess), ptr(c.use_guess), 20, ptr(c.R),
+             ptr(c.t), ptr(c.params), None, s)
+        call("ssp_track_commit", B, T, M, ptr(c.count), ptr(c.kp), ptr(c.slot), ptr(c.params), ptr(self.state_tracks), ptr(self.state_rects),
+             ptr(self.state_poses), s)
+        torch.ne(c.use_guess, 0, out=c.warm)
+
+    def update(self, logits):
+        """one frame of every stream from the network output (B, (2K+1+C)*A, H, W) -> dict of device tensors: count, kept (B,);
+        cls, track_id (B, M) int32 (-1 in empty and untracked slots); warm (B, M) bool; conf, cls_conf (B, M); keypoints_px
+        (B, M, 9, 2); R (B, M, 3, 3), t (B, M, 3), params (B, M, 6) fp64 (zero in empty slots).  Returned tensors are reused."""
+        if not logits.is_cuda:
+            raise SspError("InstanceTracker.update runs on CUDA tensors only")
+        out = logits.detach().contiguous().float()
+        B, Cn, H, W = out.shape
+        K, nC, nA, M = 9, self.num_classes, self.num_anchors, self.max_instances
+        if B != self.batch:
+            raise SspError("this tracker follows %d streams, got a batch of %d" % (self.batch, B))
+        if Cn != (2 * K + 1 + nC) * nA:
+            raise SspError("output has %d channels, expected (2K+1+C)*A = %d" % (Cn, (2 * K + 1 + nC) * nA))
+        c = self._bufs
+        if c is None:
+            import types
+            dev = self.device
+            c = self._bufs = types.SimpleNamespace()
+            c.boxes = torch.empty(B, M, 2 * K + 3, dtype=torch.float32, device=dev)
+            c.cls = torch.empty(B, M, dtype=torch.int32, device=dev)
+            c.cls0 = torch.empty(B, M, dtype=torch.int32, device=dev)
+            c.kp = torch.empty(B, M, K, 2, dtype=torch.float32, device=dev)
+            c.count = torch.empty(B, dtype=torch.int32, device=dev)
+            c.kept = torch.empty(B, dtype=torch.int32, device=dev)
+            c.P3 = torch.empty(B * M, K, 3, dtype=torch.float32, device=dev)
+            c.R = torch.empty(B, M, 3, 3, dtype=torch.float64, device=dev)
+            c.t = torch.empty(B, M, 3, dtype=torch.float64, device=dev)
+            self.buffers(c)
+        s = stream_ptr()
+        call("ssp_detect_instances", ptr(out), B, K, nC, nA, H, W, _ctypes.c_void_p(self.classes.ctypes.data), len(self.classes),
+             self.conf_thresh, self.nms_thresh, M, self.frame_size[0], self.frame_size[1], ptr(c.boxes), ptr(c.cls), ptr(c.kp),
+             ptr(c.count), ptr(c.kept), s)
+        torch.clamp(c.cls, min=0, out=c.cls0)
+        torch.index_select(self._P3_table, 0, c.cls0.view(-1), out=c.P3)
+        self.solve(c, s, c.P3, self._K32)
+        return dict(count=c.count, kept=c.kept, cls=c.cls, track_id=c.track_id, warm=c.warm, conf=c.boxes[..., 2 * K],
+                    cls_conf=c.boxes[..., 2 * K + 1], keypoints_px=c.kp, R=c.R, t=c.t, params=c.params)
+
+
 # ------------------------------------------------------------------------------------------ batched evaluation tail
 ACCURACY_THRESHOLDS = (5, 10, 15, 20, 25, 30, 35, 40, 45, 50)
 
