@@ -238,6 +238,26 @@ int ssp_pnp_batched_counted(const float* points3d, const float* points2d, const 
 int ssp_pnp_batched_guess(const float* points3d, const float* points2d, const float* K3x3, int num_points, int groups,
                           int per_group, const int* count, const double* guess, const int* use_guess, int max_iter, double* R_out,
                           double* t_out, double* params_out, int* work_out_or_null, void* stream);
+/* ---- consensus PnP over keypoint subsets (rule: csrc/pnp_consensus_core.h): a pose that survives wrong keypoints.  Per problem,
+ *      hypothesis 0 is the plain cold solve on all num_points points and hypothesis h >= 1 the cold solve on the 6 points of
+ *      subsets_host[h-1]; each is scored on all points (no inliers if any point lies at camera depth <= 0, else point i is an inlier
+ *      when its squared reprojection error <= reproj_thresh^2 px^2); the one with the most inliers wins, the lower index on a tie.
+ *      If its inliers differ from its own points and number >= 6, LM refines it on them from its pose (useExtrinsicGuess).  When
+ *      hypothesis 0 has every point as an inlier the result is bit-identical to ssp_pnp_batched.
+ *      points3d [n][num_points][3], or one shared [num_points][3] when points3d_shared != 0; n = groups * per_group problems.
+ *      count_or_null: DEVICE int [groups] as ssp_pnp_batched_counted (problem (g, m) is solved only when m < count[g], the others
+ *      get zeros), or NULL to solve all n.  subsets_host: n_subsets (1..210) HOST uint16 masks of exactly 6 bits below num_points,
+ *      copied into the launch; their order is the tie-break order.  work: DEVICE scratch (8-B aligned) of at least the
+ *      *bytes_out (a HOST long long) that ssp_pnp_consensus_work_bytes(num_points, n_subsets, n, bytes_out) writes.  Out: R_out [n][9], t_out [n][3], params_out [n][6] (the
+ *      final LM vector: rvec, t), inliers_out [n] int bitmask of the chosen hypothesis's inliers (bit i = point i), hyp_out [n]
+ *      (the chosen hypothesis, -1 when none has an inlier: hypothesis 0's pose with an empty mask).  SSP_ERR_ARG for a null pointer,
+ *      num_points outside 7..10, a bad table, reproj_thresh <= 0 or not finite, max_iter < 1, groups < 0, per_group < 1 or a
+ *      workspace that is too small (ssp_pnp_consensus_work_bytes returns SSP_ERR_ARG for bad sizes or a null bytes_out). ---- */
+int ssp_pnp_consensus_work_bytes(int num_points, int n_subsets, long long n, long long* bytes_out);
+int ssp_pnp_consensus(const float* points3d, int points3d_shared, const float* points2d, const float* K3x3, int num_points, int groups,
+                      int per_group, const int* count_or_null, const unsigned short* subsets_host, int n_subsets, double reproj_thresh,
+                      int max_iter, double* R_out, double* t_out, double* params_out, int* inliers_out, int* hyp_out, void* work,
+                      long long work_bytes, void* stream);
 
 /* ---- tracking instances across frames (rules: csrc/track_core.h): each row b is its own camera stream with T = max_tracks slots
  *      (1 <= T <= 256).  The state is four DEVICE arrays, zeroed for a fresh start (alive 0, ids from 0):

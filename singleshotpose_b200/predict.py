@@ -37,6 +37,7 @@ import torch
 from ._lib import SspError, call, load, ptr, stream_ptr
 from .engine import Buffers
 from .image import BICUBIC
+from .utils import check_pnp_args, consensus_subsets, consensus_work_bytes
 
 
 class _Chain:
@@ -95,6 +96,35 @@ class _FramePredictor:
         self._sig = None
         self._jpeg = None
         self._last = None
+
+    # ------------------------------------------------------------------ PnP: plain (ssp_pnp_batched*) or consensus (ssp_pnp_consensus)
+    def _init_pnp(self, pnp, reproj_thresh, point_sets):
+        """point_sets: the (9, 3) PnP points of every class; all give the subset table (box points share their structure)"""
+        self.pnp, self.reproj_thresh = check_pnp_args(pnp, reproj_thresh)
+        self._subsets = consensus_subsets(np.stack(point_sets)) if self.pnp == "consensus" else None
+        self._bits = torch.tensor([1 << i for i in range(self.num_keypoints)], dtype=torch.int32, device=self.device)
+
+    def _consensus_buffers(self, c, lead):
+        """the consensus solve's outputs and workspace for the problems of shape `lead` (nothing for the plain solve)"""
+        if self.pnp != "consensus":
+            return
+        dev, K, n = self.device, self.num_keypoints, int(np.prod(lead))
+        c.params = torch.empty(*lead, 6, dtype=torch.float64, device=dev)
+        c.inl_mask = torch.empty(*lead, dtype=torch.int32, device=dev)
+        c.hyp = torch.empty(*lead, dtype=torch.int32, device=dev)
+        c.inliers = torch.empty(*lead, K, dtype=torch.bool, device=dev)
+        wb = consensus_work_bytes(K, len(self._subsets), n)
+        c.pnp_work = torch.empty(max(wb, 8) // 8, dtype=torch.float64, device=dev)
+
+    def _consensus(self, c, s, P3, shared, groups, per_group, count):
+        """the consensus solve of groups x per_group problems into c.R, c.t, c.params, c.inliers, c.hyp (count: device int [groups] or None)"""
+        call("ssp_pnp_consensus", ptr(P3), shared, ptr(c.kp), ptr(self._K32), self.num_keypoints, groups, per_group, ptr(count),
+             self._subsets.ctypes.data, len(self._subsets), self.reproj_thresh, 20, ptr(c.R), ptr(c.t), ptr(c.params), ptr(c.inl_mask),
+             ptr(c.hyp), ptr(c.pnp_work), c.pnp_work.numel() * 8, s)
+        torch.ne(torch.bitwise_and(c.inl_mask.unsqueeze(-1), self._bits), 0, out=c.inliers)
+
+    def _consensus_outputs(self, c):
+        return dict(inliers=c.inliers, hyp=c.hyp) if self.pnp == "consensus" else {}
 
     @staticmethod
     def _box_points(corners3D):
@@ -243,12 +273,17 @@ class PosePredictor(_FramePredictor):
     """model: a singleshotpose_b200.Darknet (single-object yolo-pose head, 9 keypoints).  corners3D: (3|4, 8) box corners of the
     mesh (utils.get_3D_corners); K: (3, 3) camera matrix; frame_size: (width, height) of the camera frames (other sizes are
     accepted and captured separately); shape: network input (width, height), default the cfg's test size; batch: frames per call.
-    graph=False runs the same launches eagerly (no capture)."""
+    graph=False runs the same launches eagerly (no capture).
+    pnp="consensus" solves each pose with the consensus PnP (utils.pnp_consensus_batched): a pose that survives one or two wrong
+    keypoints, with inlier keypoints within reproj_thresh frame pixels; the outputs then add inliers (B, 9) bool and hyp (B,) int32.
+    pnp="plain" (default) is the all-point solve."""
 
-    def __init__(self, model, corners3D, K, frame_size=(640, 480), shape=None, batch=1, graph=True, max_graphs=4):
+    def __init__(self, model, corners3D, K, frame_size=(640, 480), shape=None, batch=1, graph=True, max_graphs=4, pnp="plain",
+                 reproj_thresh=8.0):
         P = self._box_points(corners3D)
         super().__init__(model, K, frame_size, shape if shape is not None else (model.test_width, model.test_height), batch, graph,
                          max_graphs)
+        self._init_pnp(pnp, reproj_thresh, [P.T])
         dev = self.device
         self._P3 = torch.from_numpy(np.ascontiguousarray(P.T, dtype=np.float32)).to(dev)           # (9, 3) PnP points
         # row-major copies: the kernels read raw pointers, and numpy keeps a transposed input's column-major order through
@@ -265,23 +300,36 @@ class PosePredictor(_FramePredictor):
         c.Rt = torch.empty(B, 3, 4, dtype=torch.float64, device=dev)
         c.proj = torch.empty(B, 2, K, dtype=torch.float32, device=dev)
         c.corners = torch.empty(B, K, 2, dtype=torch.float32, device=dev)
+        self._consensus_buffers(c, (B,))
 
     def _head(self, c, s):
         B, K = self.batch, self.num_keypoints
         h, w = c.logits.shape[2:]
         call("ssp_region_decode_argmax", ptr(c.logits), B, K, self.num_classes, h, w, 1, ptr(c.boxes), ptr(c.conf), None, s)
         torch.mul(c.boxes[:, :2 * K].view(B, K, 2), c.scale, out=c.kp)
-        call("ssp_pnp_batched", ptr(self._P3), 1, ptr(c.kp), ptr(self._K32), K, B, 20, ptr(c.R), ptr(c.t), None, s)
+        if self.pnp == "consensus":
+            self._consensus(c, s, self._P3, 1, B, 1, None)
+        else:
+            call("ssp_pnp_batched", ptr(self._P3), 1, ptr(c.kp), ptr(self._K32), K, B, 20, ptr(c.R), ptr(c.t), None, s)
         c.Rt[:, :, :3].copy_(c.R)
         c.Rt[:, :, 3].copy_(c.t)
         call("ssp_project_points", ptr(self._X), 4, K, ptr(c.Rt), ptr(self._K64), B, ptr(c.proj), s)
         c.corners.copy_(c.proj.transpose(1, 2))
 
     def _outputs(self, c):
-        return dict(R=c.R, t=c.t, conf=c.conf, keypoints_px=c.kp, corners_px=c.corners)
+        return dict(R=c.R, t=c.t, conf=c.conf, keypoints_px=c.kp, corners_px=c.corners, **self._consensus_outputs(c))
 
 
 # ---------------------------------------------------------------------------------------------- command line
+CONSENSUS_KEYS = {"plain": (), "consensus": ("inliers", "hyp")}          # the .npz columns each --pnp adds
+
+
+def add_pnp_args(ap):
+    ap.add_argument("--pnp", choices=("plain", "consensus"), default="plain",
+                    help="consensus: a pose that survives wrong keypoints (PnP over keypoint subsets); adds inliers and hyp columns")
+    ap.add_argument("--reproj-thresh", type=float, default=8.0, help="inlier threshold of --pnp consensus, frame pixels")
+
+
 def camera_from_data_cfg(datacfg):
     """-> (mesh path, K (3, 3) float64, (width, height)) from a .data file (utils.py read_data_cfg keys mesh, fx, fy, u0, v0, width,
     height; valid.py:26-35)"""
@@ -304,8 +352,10 @@ def main(argv=None):
     ap.add_argument("--modelcfg", required=True)
     ap.add_argument("--weightfile", required=True)
     ap.add_argument("--out", default="poses.npz")
+    add_pnp_args(ap)
     ap.add_argument("images", nargs="+")
     a = ap.parse_args(argv)
+    check_pnp_args(a.pnp, a.reproj_thresh)
     from .darknet import Darknet
     from .utils_host import read_ply_vertices
     from .utils import get_3D_corners
@@ -315,8 +365,8 @@ def main(argv=None):
     model = Darknet(a.modelcfg)
     model.load_weights(a.weightfile)
     model.cuda().eval()
-    pred = PosePredictor(model, corners3D, K, frame_size=size)
-    res = {k: [] for k in ("R", "t", "conf", "keypoints_px", "corners_px")}
+    pred = PosePredictor(model, corners3D, K, frame_size=size, pnp=a.pnp, reproj_thresh=a.reproj_thresh)
+    res = {k: [] for k in ("R", "t", "conf", "keypoints_px", "corners_px") + CONSENSUS_KEYS[a.pnp]}
     for path in a.images:
         with open(path, "rb") as f:
             data = f.read()

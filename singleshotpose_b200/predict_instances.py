@@ -31,6 +31,7 @@ Command line: python -m singleshotpose_b200.predict_instances --datacfg cfg/occl
               --weightfile w.weights --object 0=../LINEMOD/ape/ape.ply --object 4=../LINEMOD/can/can.ply --out det.npz img...
               [--track [--match-iou 0.3 --max-misses 5 --max-tracks 64]]: the images, in the order given, as one stream, with a
               track_id column
+              [--pnp consensus [--reproj-thresh 8]]: the consensus PnP, with inliers and hyp columns (not with --track)
 """
 from __future__ import annotations
 
@@ -41,8 +42,9 @@ import numpy as np
 import torch
 
 from ._lib import SspError, call, ptr
-from .predict import _FramePredictor
+from .predict import CONSENSUS_KEYS, _FramePredictor, add_pnp_args
 from .predict_multi import MAX_ENTRIES, parse_objects
+from .utils import check_pnp_args
 from .utils_multi import MAX_TRACKS, InstanceTracker, check_track_args
 
 MAX_INSTANCES = 256         # largest max_instances (detect_core.h kMaxInstances)
@@ -59,10 +61,13 @@ class InstancePosePredictor(_FramePredictor):
     [0, 1]; max_instances in [1, 256] slots per frame.  graph=False runs the same launches eagerly (no capture).
 
     Returns dict(count (B,) int32, kept (B,) int32, cls (B, M) int32, R (B, M, 3, 3) fp64, t (B, M, 3) fp64, conf (B, M) det_conf,
-    cls_conf (B, M), keypoints_px (B, M, 9, 2), corners_px (B, M, 9, 2)): device tensors, or numpy with to_host=True."""
+    cls_conf (B, M), keypoints_px (B, M, 9, 2), corners_px (B, M, 9, 2)): device tensors, or numpy with to_host=True.
+    pnp="consensus" solves each slot with the consensus PnP (utils.pnp_consensus_batched, inliers within reproj_thresh frame
+    pixels) and adds inliers (B, M, 9) bool and hyp (B, M) int32 (empty slots: False and 0); pnp="plain" (default) is the all-point
+    solve."""
 
     def __init__(self, model, objects, K, frame_size=(640, 480), shape=None, batch=1, conf_thresh=None, nms_thresh=0.4, max_instances=32,
-                 graph=True, max_graphs=4):
+                 graph=True, max_graphs=4, pnp="plain", reproj_thresh=8.0):
         self.num_anchors = int(getattr(model, "num_anchors", 0))
         if self.num_anchors < 1:
             raise SspError("InstancePosePredictor needs a model with a region head")
@@ -89,6 +94,7 @@ class InstancePosePredictor(_FramePredictor):
         if shape is None:
             shape = (model.test_width, model.test_height) if self.num_anchors == 1 else (model.width, model.height)
         super().__init__(model, K, frame_size, shape, batch, graph, max_graphs)
+        self._init_pnp(pnp, reproj_thresh, [P.T for P in pts])
         h, w = self.out_hw
         if h * w * self.num_anchors > MAX_ENTRIES:
             raise SspError("network shape %dx%d gives a %dx%d grid of %d anchors: more than the %d entries the detect kernel holds"
@@ -125,6 +131,7 @@ class InstancePosePredictor(_FramePredictor):
         c.Rt = torch.empty(B, M, 3, 4, dtype=torch.float64, device=dev)
         c.proj = torch.empty(B * M, 2, Q * K, dtype=torch.float32, device=dev)
         c.corners = torch.empty(B, M, K, 2, dtype=torch.float32, device=dev)
+        self._consensus_buffers(c, (B, M))
 
     def _head(self, c, s):
         self._detect(c, s)
@@ -141,6 +148,9 @@ class InstancePosePredictor(_FramePredictor):
         torch.index_select(self._P3_table, 0, c.cls0.view(-1), out=c.P3)
 
     def _solve(self, c, s):
+        if self.pnp == "consensus":
+            self._consensus(c, s, c.P3, 0, self.batch, self.max_instances, c.count)
+            return
         call("ssp_pnp_batched_counted", ptr(c.P3), ptr(c.kp), ptr(self._K32), self.num_keypoints, self.batch, self.max_instances,
              ptr(c.count), 20, ptr(c.R), ptr(c.t), s)
 
@@ -158,7 +168,7 @@ class InstancePosePredictor(_FramePredictor):
     def _outputs(self, c):
         K = self.num_keypoints
         return dict(count=c.count, kept=c.kept, cls=c.cls, R=c.R, t=c.t, conf=c.boxes[..., 2 * K], cls_conf=c.boxes[..., 2 * K + 1],
-                    keypoints_px=c.kp, corners_px=c.corners)
+                    keypoints_px=c.kp, corners_px=c.corners, **self._consensus_outputs(c))
 
 
 class TrackingPosePredictor(InstancePosePredictor):
@@ -172,10 +182,12 @@ class TrackingPosePredictor(InstancePosePredictor):
 
     Returns InstancePosePredictor's dict plus track_id (B, M) int32 (-1 in empty and untracked slots) and warm (B, M) bool (the
     slot's solve started from its track's pose).  The track state is shared by every frame size and source (one set of device
-    arrays, zeroed in place by reset); the warm-up runs before a graph capture do not advance it."""
+    arrays, zeroed in place by reset); the warm-up runs before a graph capture do not advance it.
+    Only pnp="plain": the consensus solve has no rule yet for how a track's warm guess competes with its subset hypotheses."""
 
     def __init__(self, model, objects, K, frame_size=(640, 480), shape=None, batch=1, conf_thresh=None, nms_thresh=0.4, max_instances=32,
-                 max_tracks=64, match_iou=0.3, max_misses=5, graph=True, max_graphs=4):
+                 max_tracks=64, match_iou=0.3, max_misses=5, graph=True, max_graphs=4, pnp="plain"):
+        check_tracking_pnp(pnp)
         check_track_args(max_tracks, match_iou, max_misses)
         super().__init__(model, objects, K, frame_size, shape, batch, conf_thresh, nms_thresh, max_instances, graph, max_graphs)
         if not isinstance(objects, dict):
@@ -210,6 +222,12 @@ class TrackingPosePredictor(InstancePosePredictor):
         return dict(super()._outputs(c), track_id=c.track_id, warm=c.warm)
 
 
+def check_tracking_pnp(pnp):
+    if pnp != "plain":
+        raise SspError("tracking solves with pnp='plain' only, got %r: the consensus solve has no rule for how a track's warm guess "
+                       "competes with its subset hypotheses" % (pnp,))
+
+
 # ---------------------------------------------------------------------------------------------- command line
 def camera_from_any_data_cfg(datacfg):
     """-> (mesh path or None, K (3, 3) float64, (width, height)) from a single-object .data file (mesh, width, height) or a
@@ -230,7 +248,7 @@ def camera_from_any_data_cfg(datacfg):
 
 def parse_args(argv=None):
     """the command line, checked before any model is built: raises SspError for a bad --object, --nms-thresh, --max-instances,
-    --match-iou, --max-misses or --max-tracks"""
+    --match-iou, --max-misses, --max-tracks or --reproj-thresh, and for --track with --pnp consensus"""
     ap = argparse.ArgumentParser(prog="python -m singleshotpose_b200.predict_instances",
                                  description="6-D pose of every detected instance of the requested objects in each image")
     ap.add_argument("--datacfg", required=True, help=".data file: fx fy u0 v0 and width height (or im_width im_height); mesh")
@@ -246,8 +264,12 @@ def parse_args(argv=None):
     ap.add_argument("--match-iou", type=float, default=0.3)
     ap.add_argument("--max-misses", type=int, default=5)
     ap.add_argument("--max-tracks", type=int, default=64)
+    add_pnp_args(ap)
     ap.add_argument("images", nargs="+")
     a = ap.parse_args(argv)
+    check_pnp_args(a.pnp, a.reproj_thresh)
+    if a.track:
+        check_tracking_pnp(a.pnp)
     if not 0.0 <= a.nms_thresh <= 1.0:
         raise SspError("--nms-thresh must be in [0, 1], got %r" % a.nms_thresh)
     if not 1 <= a.max_instances <= MAX_INSTANCES:
@@ -295,8 +317,9 @@ def main(argv=None):
         pred = TrackingPosePredictor(model, objects, K, frame_size=size, nms_thresh=a.nms_thresh, max_instances=a.max_instances,
                                      max_tracks=a.max_tracks, match_iou=a.match_iou, max_misses=a.max_misses)
     else:
-        pred = InstancePosePredictor(model, objects, K, frame_size=size, nms_thresh=a.nms_thresh, max_instances=a.max_instances)
-    rows = {k: [] for k in ROW_KEYS + (("track_id",) if a.track else ())}
+        pred = InstancePosePredictor(model, objects, K, frame_size=size, nms_thresh=a.nms_thresh, max_instances=a.max_instances,
+                                     pnp=a.pnp, reproj_thresh=a.reproj_thresh)
+    rows = {k: [] for k in ROW_KEYS + (("track_id",) if a.track else ()) + CONSENSUS_KEYS[a.pnp]}
     image = []
     for i, path in enumerate(a.images):
         with open(path, "rb") as f:

@@ -32,7 +32,8 @@ import numpy as np
 import torch
 
 from ._lib import SspError, call, ptr
-from .predict import _FramePredictor
+from .predict import CONSENSUS_KEYS, _FramePredictor, add_pnp_args
+from .utils import check_pnp_args
 
 MAX_ENTRIES = 4096          # H*W*num_anchors the select kernel keeps in shared memory (eval_multi_core.h kMaxEntries)
 OUTPUT_KEYS = ("R", "t", "conf", "cls_conf", "detected", "keypoints_px", "corners_px")
@@ -46,9 +47,12 @@ class MultiPosePredictor(_FramePredictor):
     block's conf_thresh (valid_multi.py:40).  graph=False runs the same launches eagerly (no capture).
 
     Returns dict(classes (Q,), R (B, Q, 3, 3) fp64, t (B, Q, 3) fp64, conf (B, Q) det_conf of the box, cls_conf (B, Q),
-    detected (B, Q) bool, keypoints_px (B, Q, 9, 2), corners_px (B, Q, 9, 2)): device tensors, or numpy with to_host=True."""
+    detected (B, Q) bool, keypoints_px (B, Q, 9, 2), corners_px (B, Q, 9, 2)): device tensors, or numpy with to_host=True.
+    pnp="consensus" solves each slot with the consensus PnP (utils.pnp_consensus_batched, inliers within reproj_thresh frame
+    pixels) and adds inliers (B, Q, 9) bool and hyp (B, Q) int32; pnp="plain" (default) is the all-point solve."""
 
-    def __init__(self, model, objects, K, frame_size=(640, 480), shape=None, batch=1, conf_thresh=None, graph=True, max_graphs=4):
+    def __init__(self, model, objects, K, frame_size=(640, 480), shape=None, batch=1, conf_thresh=None, graph=True, max_graphs=4,
+                 pnp="plain", reproj_thresh=8.0):
         self.num_anchors = int(getattr(model, "num_anchors", 0))
         if self.num_anchors < 2:
             raise SspError("MultiPosePredictor needs a multi-anchor region head (yolo-pose-multi.cfg), got %d anchor(s)" % self.num_anchors)
@@ -66,6 +70,7 @@ class MultiPosePredictor(_FramePredictor):
             conf_thresh = float(model.blocks[0]["conf_thresh"])
         self.conf_thresh = float(conf_thresh)
         super().__init__(model, K, frame_size, shape if shape is not None else (model.width, model.height), batch, graph, max_graphs)
+        self._init_pnp(pnp, reproj_thresh, [P.T for P in pts])
         h, w = self.out_hw
         if h * w * self.num_anchors > MAX_ENTRIES:
             raise SspError("network shape %dx%d gives a %dx%d grid of %d anchors: more than the %d entries the select kernel holds"
@@ -90,6 +95,7 @@ class MultiPosePredictor(_FramePredictor):
         c.Rt = torch.empty(B, Q, 3, 4, dtype=torch.float64, device=dev)
         c.proj = torch.empty(B * Q, 2, Q * K, dtype=torch.float32, device=dev)
         c.corners = torch.empty(B, Q, K, 2, dtype=torch.float32, device=dev)
+        self._consensus_buffers(c, (B, Q))
 
     def _head(self, c, s):
         B, K, Q = self.batch, self.num_keypoints, len(self.classes)
@@ -98,7 +104,10 @@ class MultiPosePredictor(_FramePredictor):
         call("ssp_predict_multi_select", ptr(c.logits), B, K, self.num_classes, self.num_anchors, h, w, C.c_void_p(self._cls_host.ctypes.data),
              Q, self.conf_thresh, float(Wf), float(Hf), ptr(c.boxes), ptr(c.flags), ptr(c.kp), s)
         torch.eq(c.flags, 0, out=c.detected)
-        call("ssp_pnp_batched", ptr(self._P3), 0, ptr(c.kp), ptr(self._K32), K, B * Q, 20, ptr(c.R), ptr(c.t), None, s)
+        if self.pnp == "consensus":
+            self._consensus(c, s, self._P3, 0, B * Q, 1, None)
+        else:
+            call("ssp_pnp_batched", ptr(self._P3), 0, ptr(c.kp), ptr(self._K32), K, B * Q, 20, ptr(c.R), ptr(c.t), None, s)
         c.Rt[..., :3].copy_(c.R)
         c.Rt[..., 3].copy_(c.t)
         # every class's points under every slot's pose (each point is projected on its own, so a slot's own columns are what
@@ -109,7 +118,7 @@ class MultiPosePredictor(_FramePredictor):
     def _outputs(self, c):
         K = self.num_keypoints
         return dict(classes=self._classes, R=c.R, t=c.t, conf=c.boxes[..., 2 * K], cls_conf=c.boxes[..., 2 * K + 1], detected=c.detected,
-                    keypoints_px=c.kp, corners_px=c.corners)
+                    keypoints_px=c.kp, corners_px=c.corners, **self._consensus_outputs(c))
 
 
 # ---------------------------------------------------------------------------------------------- command line
@@ -155,8 +164,10 @@ def main(argv=None):
     ap.add_argument("--object", action="append", required=True, metavar="CLASS=MESH.ply",
                     help="a class id of the model and the mesh of its object; repeat for every object to predict")
     ap.add_argument("--out", default="poses.npz")
+    add_pnp_args(ap)
     ap.add_argument("images", nargs="+")
     a = ap.parse_args(argv)
+    check_pnp_args(a.pnp, a.reproj_thresh)
     from .darknet_multi import Darknet
     from .utils import get_3D_corners
     from .utils_host import read_ply_vertices
@@ -168,8 +179,8 @@ def main(argv=None):
     model = Darknet(a.modelcfg)
     model.load_weights(a.weightfile)
     model.cuda().eval()
-    pred = MultiPosePredictor(model, objects, K, frame_size=size)
-    res = {k: [] for k in OUTPUT_KEYS}
+    pred = MultiPosePredictor(model, objects, K, frame_size=size, pnp=a.pnp, reproj_thresh=a.reproj_thresh)
+    res = {k: [] for k in OUTPUT_KEYS + CONSENSUS_KEYS[a.pnp]}
     for path in a.images:
         with open(path, "rb") as f:
             data = f.read()

@@ -116,6 +116,104 @@ def pnp(points_3D, points_2D, cameraMatrix):
     return R[0].cpu().numpy(), t[0].cpu().numpy().reshape(3, 1)
 
 
+# ------------------------------------------------------------------------------------------ consensus pose (csrc/pnp_consensus_core.h)
+PNP_MODES = ("plain", "consensus")
+
+
+def check_pnp_args(pnp, reproj_thresh):
+    """-> (pnp, reproj_thresh as float); SspError for an unknown mode or a threshold that is not > 0 and finite"""
+    if pnp not in PNP_MODES:
+        raise SspError("pnp must be one of %s, got %r" % (", ".join(PNP_MODES), pnp))
+    thr = float(reproj_thresh)
+    if not (np.isfinite(thr) and thr > 0):
+        raise SspError("reproj_thresh must be > 0 and finite (pixels), got %r" % (reproj_thresh,))
+    return pnp, thr
+
+
+def consensus_subsets(point_sets, size=6):
+    """(H,) uint16 bitmasks of the `size`-subsets of the P points, in lexicographic order, without those in which 5 points are
+    coplanar for any of the given point sets: the DLT of cv2.solvePnP's ITERATIVE solve is degenerate there.  Coplanar means the
+    smallest singular value of the centred 5 x 3 matrix is below 1e-6 times the set's largest extent (largest coordinate range).
+    point_sets: one (P, 3) array or a sequence of them, all with the same P.  For the 9 box points (centroid + 8 corners) 60 of 84
+    subsets are kept: each of the six diagonal planes through two opposite edges holds 4 corners and the centroid."""
+    import itertools
+    sets = np.asarray(point_sets, np.float64)
+    sets = sets[None] if sets.ndim == 2 else sets
+    if sets.ndim != 3 or sets.shape[2] != 3:
+        raise SspError("point_sets must be (P, 3) or (S, P, 3), got %s" % (sets.shape,))
+    P = sets.shape[1]
+    if size != 6 or not 7 <= P <= 10:
+        raise SspError("consensus subsets are 6 of 7..10 points, got %d of %d" % (size, P))
+    extent = np.ptp(sets, axis=1).max(axis=1)                       # (S,)
+    coplanar = set()
+    for five in itertools.combinations(range(P), 5):
+        X = sets[:, list(five)]
+        X = X - X.mean(axis=1, keepdims=True)
+        smin = np.linalg.svd(X, compute_uv=False)[:, -1]
+        if (smin < 1e-6 * extent).any():
+            coplanar.add(five)
+    out = [sum(1 << i for i in S) for S in itertools.combinations(range(P), size)
+           if not any(f in coplanar for f in itertools.combinations(S, 5))]
+    return np.array(out, np.uint16)
+
+
+def pnp_consensus_batched(points_3D, points_2D, cameraMatrix, reproj_thresh=8.0, max_iter=20, subsets=None):
+    """Consensus PnP of n problems on the GPU (ssp_pnp_consensus, rule: csrc/pnp_consensus_core.h): the plain all-point solve and
+    one cold solve per 6-point subset, each scored by its inliers (squared reprojection error <= reproj_thresh^2 px^2, none if a
+    point lies behind the camera); the best is refined on its inliers.  A pose that survives one or two wrong keypoints; where
+    the all-point solve already has every point as an inlier the result is bit-identical to pnp_batched.
+    points_3D (P,3) shared or (n,P,3), 7 <= P <= 10; points_2D (n,P,2); K (3,3); reproj_thresh in pixels (8, cv2.solvePnPRansac's
+    default); subsets: (H,) uint16 masks, default consensus_subsets(points_3D).
+    -> R (n,3,3) f64, t (n,3) f64, params (n,6) f64 (rvec, t), inliers (n,P) bool, hyp (n,) int32 (the chosen hypothesis: 0 the
+    all-point solve, h the subset subsets[h-1], -1 none had an inlier), CUDA tensors."""
+    dev = _dev()
+    _, thr = check_pnp_args("consensus", reproj_thresh)
+    P3 = torch.as_tensor(np.asarray(points_3D, dtype=np.float32) if not torch.is_tensor(points_3D) else points_3D)
+    uv = torch.as_tensor(np.asarray(points_2D, dtype=np.float32) if not torch.is_tensor(points_2D) else points_2D)
+    K = torch.as_tensor(np.asarray(cameraMatrix, dtype=np.float32) if not torch.is_tensor(cameraMatrix) else cameraMatrix)
+    P3 = P3.to(dev, torch.float32).contiguous(); uv = uv.to(dev, torch.float32).contiguous(); K = K.to(dev, torch.float32).contiguous()
+    if uv.dim() == 2:
+        uv = uv.unsqueeze(0)
+    n, npts = uv.shape[0], uv.shape[1]
+    shared = P3.dim() == 2
+    if P3.shape[-2] != npts or P3.shape[-1] != 3 or uv.shape[-1] != 2 or (not shared and P3.shape[0] != n):
+        raise SspError("points_3D %s does not match points_2D %s" % (tuple(P3.shape), tuple(uv.shape)))
+    if subsets is None:
+        subsets = consensus_subsets(P3.cpu().numpy())
+    tab = np.ascontiguousarray(subsets, np.uint16).reshape(-1)
+    R = torch.empty(n, 3, 3, dtype=torch.float64, device=dev)
+    t = torch.empty(n, 3, dtype=torch.float64, device=dev)
+    params = torch.empty(n, 6, dtype=torch.float64, device=dev)
+    inl = torch.empty(n, dtype=torch.int32, device=dev)
+    hyp = torch.empty(n, dtype=torch.int32, device=dev)
+    wb = consensus_work_bytes(npts, len(tab), n)
+    work = torch.empty(max(wb, 8) // 8, dtype=torch.float64, device=dev)
+    call("ssp_pnp_consensus", ptr(P3), 1 if shared else 0, ptr(uv), ptr(K), npts, n, 1, None, tab.ctypes.data, len(tab), thr, max_iter,
+         ptr(R), ptr(t), ptr(params), ptr(inl), ptr(hyp), ptr(work), work.numel() * 8, stream_ptr())
+    return R, t, params, inlier_bits(inl, npts), hyp
+
+
+def consensus_work_bytes(npts, n_subsets, n):
+    """bytes of device workspace ssp_pnp_consensus needs for n problems of npts points and n_subsets subsets"""
+    import ctypes
+    out = ctypes.c_longlong(0)
+    call("ssp_pnp_consensus_work_bytes", int(npts), int(n_subsets), int(n), ctypes.byref(out))
+    return out.value
+
+
+def inlier_bits(mask, npts):
+    """(...,) int32 bitmasks -> (..., npts) bool"""
+    return ((mask.unsqueeze(-1) >> torch.arange(npts, dtype=torch.int32, device=mask.device)) & 1) != 0
+
+
+def pnp_consensus(points_3D, points_2D, cameraMatrix, reproj_thresh=8.0):
+    """pnp's contract (numpy in, R (3,3) and t (3,1) float64 out) with the consensus solve of pnp_consensus_batched, plus the
+    indices of the inlier keypoints (int64, ascending)."""
+    assert points_3D.shape[0] == points_2D.shape[0], "points 3D and points 2D must have same number of vertices"
+    R, t, _p, inl, _h = pnp_consensus_batched(points_3D, np.ascontiguousarray(points_2D[:, :2]), cameraMatrix, reproj_thresh)
+    return R[0].cpu().numpy(), t[0].cpu().numpy().reshape(3, 1), np.nonzero(inl[0].cpu().numpy())[0]
+
+
 def project_points_batched(points_3D, Rt, internal_calibration):
     """points_3D (3|4, Nv); Rt (n,3,4) -> (n, 2, Nv) float32 CUDA tensor (compute_projection for n poses)."""
     dev = _dev()
@@ -240,7 +338,7 @@ def pose_label_rows(corners3D, Rt, K, width, height, class_id=0):
 
 # ------------------------------------------------------------------------------------------ batched evaluation tail
 def evaluate_poses_batched(output, target, vertices, points_3D, internal_calibration, num_classes=1, num_keypoints=9,
-                           im_width=640, im_height=480, adds=False):
+                           im_width=640, im_height=480, adds=False, pnp="plain", reproj_thresh=8.0):
     """GPU-resident version of the per-image evaluation loop of reference valid.py:123-183 (SURVEY 8f.1): per-image decode
     (arg-max cell of EACH image, not the whole batch), PnP of the ground-truth and the predicted keypoints, reprojection of
     all mesh vertices, pixel / 3-D / angular / translation errors -- no Python loop over images.
@@ -249,7 +347,11 @@ def evaluate_poses_batched(output, target, vertices, points_3D, internal_calibra
     vertices (3|4, Nv); points_3D (K, 3); internal_calibration (3, 3).  Returns a dict of CUDA tensors with leading dim B.
     adds=True adds `adds_dist` (B,) fp64, adi(pts_pr, pts_gt) over the mesh as given in fp64 (adi_batched): the error that
     replaces vertex_dist for the symmetric objects (eggbox, glue).  The angle error is arccos of the trace clamped to [-1, 1],
-    so an exact pose gives 0 where the reference's calcAngularDistance can give NaN."""
+    so an exact pose gives 0 where the reference's calcAngularDistance can give NaN.
+    pnp="consensus" solves the predicted pose with the consensus PnP (pnp_consensus_batched, inliers within reproj_thresh pixels of
+    the im_width x im_height image) and adds `inliers` (B, K) bool and `hyp` (B,) int32; the ground-truth pose stays the plain
+    solve.  Passing the results of both modes of one network output to pose_accuracy compares the two solves."""
+    pnp, reproj_thresh = check_pnp_args(pnp, reproj_thresh)
     dev = output.device
     K = num_keypoints
     boxes, best, _ = region_boxes_batched(output, num_classes, K)
@@ -259,8 +361,14 @@ def evaluate_poses_batched(output, target, vertices, points_3D, internal_calibra
     gt2d = torch.as_tensor(target)[:, 1:1 + 2 * K].to(dev, torch.float32).reshape(B, K, 2) * scale
     Kc = torch.as_tensor(np.asarray(internal_calibration, dtype=np.float32)).to(dev)
     P3 = torch.as_tensor(np.asarray(points_3D, dtype=np.float32)).to(dev)
-    R, t = pnp_batched(P3, torch.cat([gt2d, pr2d], 0), Kc)             # 2B problems in one launch
-    R_gt, R_pr, t_gt, t_pr = R[:B], R[B:], t[:B], t[B:]
+    extra = {}
+    if pnp == "consensus":
+        R_gt, t_gt = pnp_batched(P3, gt2d, Kc)
+        R_pr, t_pr, _p, inl, hyp = pnp_consensus_batched(P3, pr2d, Kc, reproj_thresh)
+        extra = dict(inliers=inl, hyp=hyp)
+    else:
+        R, t = pnp_batched(P3, torch.cat([gt2d, pr2d], 0), Kc)         # 2B problems in one launch
+        R_gt, R_pr, t_gt, t_pr = R[:B], R[B:], t[:B], t[B:]
     Rt_gt = torch.cat([R_gt, t_gt.unsqueeze(2)], 2)
     Rt_pr = torch.cat([R_pr, t_pr.unsqueeze(2)], 2)
     V = torch.as_tensor(np.asarray(vertices, dtype=np.float32)).to(dev)
@@ -275,7 +383,7 @@ def evaluate_poses_batched(output, target, vertices, points_3D, internal_calibra
     tr = torch.einsum("bij,bij->b", R_gt, R_pr)                         # trace(R_gt R_pr^T)
     angle = torch.rad2deg(torch.arccos(((tr - 1.0) / 2.0).clamp(-1.0, 1.0)))
     res = dict(boxes=boxes, conf=best, corner_err_px=(pr2d - gt2d).norm(dim=2).mean(dim=1), R_gt=R_gt, t_gt=t_gt, R_pr=R_pr, t_pr=t_pr,
-               pixel_err=pixel_err, vertex_dist=vertex_dist, angle_err_deg=angle, trans_err=(t_gt - t_pr).norm(dim=1))
+               pixel_err=pixel_err, vertex_dist=vertex_dist, angle_err_deg=angle, trans_err=(t_gt - t_pr).norm(dim=1), **extra)
     if adds:
         res["adds_dist"] = adi_batched(vertices, Rt_pr, Rt_gt)
     return res

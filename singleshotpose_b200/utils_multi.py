@@ -10,7 +10,8 @@ import torch
 
 from ._lib import call, ptr, stream_ptr, SspError
 from .utils import (pnp, pnp_batched, compute_projection, compute_transformation, calcAngularDistance, get_3D_corners,  # noqa: F401
-                    get_camera_intrinsic, convert2cpu, convert2cpu_long, project_points_batched, adi_batched, mesh_diameter)
+                    get_camera_intrinsic, convert2cpu, convert2cpu_long, project_points_batched, adi_batched, mesh_diameter,
+                    check_pnp_args, pnp_consensus_batched)
 from .utils_host import (makedirs, get_all_files, calc_pts_diameter, adi, get_2d_bb, corner_confidences, corner_confidence,  # noqa: F401
                          sigmoid, softmax, read_truths, read_truths_args, read_pose, load_class_names, image2torch, scale_bboxes,
                          file_lines, get_image_size, logging)
@@ -351,7 +352,7 @@ def projection_accuracy(pixel_err, thresholds=ACCURACY_THRESHOLDS):
 
 
 def evaluate_multi_poses_batched(output, target, conf_thresh, num_classes, num_keypoints, num_anchors, vertices, corners3D,
-                                 internal_calibration, im_width=640, im_height=480, adds=False):
+                                 internal_calibration, im_width=640, im_height=480, adds=False, pnp="plain", reproj_thresh=8.0):
     """GPU version of the multi-object evaluation loop (valid_multi.py:97-149, train_multi.py:196-240) for a whole batch.
 
     output (B, (2K+1+C)*A, H, W) CUDA network output; target (B, 50*(2K+3)) label of dataset_multi.listDataset in test mode, host
@@ -373,7 +374,12 @@ def evaluate_multi_poses_batched(output, target, conf_thresh, num_classes, num_k
     Deliberate departures: with B > 1 every image is evaluated as the reference's own batch-1 call (the reference takes
     correspondingclass from image 0 and keeps its fallback maxima across the batch); a label with all 50 rows filled is evaluated
     in full, where the reference raises TypeError from range(None).  The reference's per-object corner_confidence and projected
-    corners are never used by it and are not computed."""
+    corners are never used by it and are not computed.
+
+    pnp="consensus" solves the G predicted poses with the consensus PnP (utils.pnp_consensus_batched, inliers within reproj_thresh
+    pixels) and adds `inliers` (G, K) bool and `hyp` (G,) int32; the ground-truth poses stay the plain solve.  projection_accuracy
+    of the pixel_err of both modes on one network output compares the two solves."""
+    pnp, reproj_thresh = check_pnp_args(pnp, reproj_thresh)
     if output.dim() == 3:
         output = output.unsqueeze(0)
     if not output.is_cuda:
@@ -408,13 +414,23 @@ def evaluate_multi_poses_batched(output, target, conf_thresh, num_classes, num_k
         R0 = torch.zeros(0, 3, 3, dtype=torch.float64, device=dev)
         t0 = torch.zeros(0, 3, dtype=torch.float64, device=dev)
         res = dict(res, R_gt=R0, t_gt=t0, R_pr=R0.clone(), t_pr=t0.clone(), pixel_err=torch.zeros(0, dtype=torch.float32, device=dev))
+        if pnp == "consensus":
+            res.update(inliers=torch.zeros(0, K, dtype=torch.bool, device=dev), hyp=torch.zeros(0, dtype=torch.int32, device=dev))
         if adds:
             res.update(vertex_dist=torch.zeros(0, dtype=torch.float64, device=dev), adds_dist=torch.zeros(0, dtype=torch.float64, device=dev))
         return res
     c3 = np.asarray(corners3D, dtype=np.float64)[:3]
     P3 = np.array(np.transpose(np.concatenate((np.zeros((3, 1)), c3), axis=1)), dtype="float32")          # valid_multi.py:135
     Kc = torch.as_tensor(np.asarray(internal_calibration, dtype=np.float32)).to(dev)
-    R, t = pnp_batched(torch.from_numpy(P3).to(dev), uv, Kc)                                                 # 2G problems, one launch
+    extra = {}
+    if pnp == "consensus":
+        P3d = torch.from_numpy(P3).to(dev)
+        R_gt, t_gt = pnp_batched(P3d, uv[:G], Kc)
+        R_pr, t_pr, _p, inl, hyp = pnp_consensus_batched(P3d, uv[G:], Kc, reproj_thresh)
+        R, t = torch.cat([R_gt, R_pr]), torch.cat([t_gt, t_pr])
+        extra = dict(inliers=inl, hyp=hyp)
+    else:
+        R, t = pnp_batched(torch.from_numpy(P3).to(dev), uv, Kc)                                             # 2G problems, one launch
     Rt = torch.cat([R, t.unsqueeze(2)], 2)
     V = torch.as_tensor(np.asarray(vertices, dtype=np.float32)).to(dev)
     if V.shape[0] == 3:
@@ -424,7 +440,7 @@ def evaluate_multi_poses_batched(output, target, conf_thresh, num_classes, num_k
     # valid_multi.py:143-149.  Elementwise distances, then an fp64 mean: the result of one object does not depend on how many
     # objects the batch holds (a batched fp32 reduction may change its summation order with the shape)
     pixel_err = torch.hypot(d[:, 0], d[:, 1]).double().mean(dim=1).float()
-    res = dict(res, R_gt=R[:G], t_gt=t[:G], R_pr=R[G:], t_pr=t[G:], pixel_err=pixel_err)
+    res = dict(res, R_gt=R[:G], t_gt=t[:G], R_pr=R[G:], t_pr=t[G:], pixel_err=pixel_err, **extra)
     if adds:
         res["adds_dist"], res["vertex_dist"] = adi_batched(vertices, Rt[G:], Rt[:G], with_add=True)
     return res
