@@ -67,7 +67,10 @@ int ssp_conv_gemm(int impl, const void* a_hi, const void* a_lo_or_null, long lon
 int ssp_conv_bandt_launches(void);
 /* ---- inference: nn.Conv2d + nn.BatchNorm2d(eval) + nn.LeakyReLU as ONE kernel (darknet.py:154-164 under model.eval()):
  *      z = leaky(conv * scale[c] + shift[c]) is written by the GEMM epilogue straight into the consumer's fp16 hi/lo operand
- *      planes (rows [row][d_ld], channel offset d_c0); scale/shift from ssp_bn_finalize(train=0).  fp16 hi/lo operands. ---- */
+ *      planes (rows [row][d_ld], channel offset d_c0); scale/shift from ssp_bn_finalize(train=0).  fp16 hi/lo operands.
+ *      The parts are saturating: hi = fp16(clamp(z, +-65504)), lo = fp16(clamp(z - hi, +-65504)), so a finite z never gives
+ *      an infinite part (ssp_bn_apply and ssp_pack_nchw split the same way).  SSP_ERR_ARG unless cout % 32 == 0, d_hi and d_lo
+ *      are 16-B aligned, d_ld % 8 == 0, d_c0 % 8 == 0 and d_ld >= d_c0 + cout. ---- */
 int ssp_conv_gemm_bnact(int impl, const void* a_hi, const void* a_lo, long long a_rows, int a_ld, int cin,
                         const void* b_hi, const void* b_lo, int b_rows, int b_ld, int N, int H, int W, int taps, int cout,
                         const float* scale, const float* shift, float slope, void* d_hi, void* d_lo, int d_ld, int d_c0,
@@ -119,7 +122,11 @@ int ssp_bn_finalize(double* stat_sum, double* stat_sq, double count, const float
 /* ypool (optional, max-pool destinations only): fp32 plane in the POOLED geometry receiving the conv output y at the arg-max
  * position of every 2x2 window.  With it the first pass of the BN backward of a pooled layer runs at a quarter of the
  * resolution: ssp_bn_bwd_reduce(y = ypool, H/2, W/2, g0 = pooled upstream gradient, SSP_ROUTE_DIRECT) accumulates the same
- * S1 / S2 as the full-resolution call (only arg-max positions receive gradient). */
+ * S1 / S2 as the full-resolution call (only arg-max positions receive gradient).
+ * Layout rules (4-channel vectors; SSP_ERR_ARG before any launch otherwise), for ssp_bn_apply, ssp_bn_apply_splitk and the
+ * ssp_bn_bwd_* calls: C % 4 == 0; y (and ypool) 16-B aligned with ld % 4 == 0 and ld >= C; every destination plane (hi, lo) 8-B
+ * aligned and every upstream gradient plane 16-B (fp32) or 8-B (SSP_ROUTE_F16) aligned, each with ld % 4 == 0, c0 % 4 == 0 and
+ * ld >= c0 + C (c0 + 4C behind SSP_ROUTE_REORG); dy of ssp_bn_bwd_apply 8-B aligned with dy_ld % 4 == 0 and dy_ld >= C. */
 int ssp_bn_apply(const float* y, int y_ld, const float* scale, const float* shift, int N, int C, int H, int W,
                  float slope, void* d0_hi, void* d0_lo, int d0_ld, int d0_c0, int d0_route, void* d1_hi, void* d1_lo,
                  int d1_ld, int d1_c0, int d1_route, float* ypool_or_null, int ypool_ld, void* stream);

@@ -224,12 +224,10 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
             uint32_t ph[16], pl[16];
 #pragma unroll
             for (int j = 0; j < 32; j += 2) {
-              uint16_t h0, l0, h1, l1;
               float z0 = fmaf(v[j], __ldg(p.fa.scale + c0 + j), __ldg(p.fa.shift + c0 + j));
               float z1 = fmaf(v[j + 1], __ldg(p.fa.scale + c0 + j + 1), __ldg(p.fa.shift + c0 + j + 1));
               z0 = z0 > 0.f ? z0 : z0 * p.fa.slope; z1 = z1 > 0.f ? z1 : z1 * p.fa.slope;
-              split_f16(z0, h0, l0); split_f16(z1, h1, l1);
-              ph[j >> 1] = h0 | ((uint32_t)h1 << 16); pl[j >> 1] = l0 | ((uint32_t)l1 << 16);
+              split_f16x2(z0, z1, ph[j >> 1], pl[j >> 1]);
             }
             uint4* dh = reinterpret_cast<uint4*>(p.fa.d_hi + m * p.fa.d_ld + p.fa.d_c0 + c0);
             uint4* dl = reinterpret_cast<uint4*>(p.fa.d_lo + m * p.fa.d_ld + p.fa.d_c0 + c0);
@@ -336,8 +334,10 @@ int conv_gemm_tc(const void* a_hi, const void* a_lo, long long a_rows, int a_ld,
     out_rows = flat_alloc_rows(N, H, W);
   }
   if (fa) {
-    if (!fa->scale || !fa->shift || !fa->d_hi || !fa->d_lo || (cout % 32) || (fa->d_ld % 8) || (fa->d_c0 % 8))
-      return fail_msg(SSP_ERR_ARG, "conv_gemm_tc: fused BN+activation epilogue needs cout % 32 == 0 and 16-B aligned destination rows");
+    if (!fa->scale || !fa->shift || !fa->d_hi || !fa->d_lo || (cout % 32) || (fa->d_ld % 8) || (fa->d_c0 % 8) || fa->d_c0 < 0 ||
+        ((uintptr_t)fa->d_hi % 16) || ((uintptr_t)fa->d_lo % 16) || fa->d_ld < fa->d_c0 + cout)
+      return fail_msg(SSP_ERR_ARG, "conv_gemm_tc: fused BN+activation epilogue needs cout % 32 == 0, 16-B aligned destination planes and "
+                                   "rows (d_ld % 8 == 0, d_c0 % 8 == 0) and d_ld >= d_c0 + cout");
     epi = EPI_BNACT;
   }
   if (!a_hi || !b_hi || (!out && !fa) || (taps != 1 && taps != 9) || cin <= 0 || cout <= 0) return fail_msg(SSP_ERR_ARG, "conv_gemm_tc: bad argument");

@@ -120,11 +120,11 @@ __device__ __forceinline__ float leaky(float v, float slope) { return v > 0.f ? 
 
 __device__ __forceinline__ void store4(const ActDst& d, long long row, int c, const float (&z)[4]) {
   const long long o = row * d.ld + d.c0 + c;
-  uint16_t h[4], l[4];
-#pragma unroll
-  for (int j = 0; j < 4; j++) split_f16(z[j], h[j], l[j]);
-  *reinterpret_cast<uint2*>(d.hi + o) = make_uint2(h[0] | ((uint32_t)h[1] << 16), h[2] | ((uint32_t)h[3] << 16));
-  if (d.lo) *reinterpret_cast<uint2*>(d.lo + o) = make_uint2(l[0] | ((uint32_t)l[1] << 16), l[2] | ((uint32_t)l[3] << 16));
+  uint32_t h01, l01, h23, l23;
+  split_f16x2(z[0], z[1], h01, l01);
+  split_f16x2(z[2], z[3], h23, l23);
+  *reinterpret_cast<uint2*>(d.hi + o) = make_uint2(h01, h23);
+  if (d.lo) *reinterpret_cast<uint2*>(d.lo + o) = make_uint2(l01, l23);
 }
 
 // Thread layout shared by the BN kernels: channel group cgi = tid % CG (4 channels each, consecutive threads on
@@ -508,6 +508,16 @@ __global__ void sgd_flat_kernel(float* __restrict__ p, const float* __restrict__
 
 // ================================================================================================ host launchers
 static inline unsigned nblk(long long total, int bs) { return (unsigned)((total + bs - 1) / bs); }
+static inline bool aligned(const void* p, int bytes) { return ((uintptr_t)p % bytes) == 0; }
+
+// Layout rules of the 4-channel vectors of the BN kernels, checked before any launch: a misaligned vector access would fault.
+// The fp32 conv output y is read in 16-B vectors at row * y_ld + c.
+static bool y_layout_ok(const float* y, int y_ld, int C) { return aligned(y, 16) && y_ld % 4 == 0 && y_ld >= C; }
+// A 16-bit destination (8-B stores) or an upstream gradient plane (8-B fp16 / 16-B fp32 loads) at row * ld + c0 + channel, with
+// channels [c0, c0 + C), or [c0, c0 + 4C) behind a reorg.
+static bool plane_layout_ok(const void* base, int elem_bytes, int ld, int c0, int route, int C) {
+  return aligned(base, 4 * elem_bytes) && ld % 4 == 0 && c0 % 4 == 0 && c0 >= 0 && ld >= c0 + (route == SSP_ROUTE_REORG ? 4 * C : C);
+}
 
 // ssp_bn_apply and ssp_bn_apply_splitk.  splits == 1 launches the plain kernel (the ssp_bn_apply path); splits > 1 the instantiation
 // that sums the partial slabs first
@@ -518,7 +528,13 @@ static int bn_apply_splitk(const float* y, int splits, long long slab, int y_ld,
   if (splits < 1 || (splits > 1 && (((uintptr_t)y % 16) || (y_ld % 4) || y_ld < C || (slab % 4) || slab < (long long)y_ld * flat_alloc_rows(N, H, W))))
     return fail_msg(SSP_ERR_ARG, "bn_apply_splitk: splits >= 1; partial slabs 16-B aligned, partial_ld % 4 == 0 and >= C, slab_elems % 4 == 0 and "
                                  ">= ssp_flat_alloc_rows(N, H, W) * partial_ld");
-  if (ypool && ((ypool_ld % 4) || ypool_ld < C)) return fail_msg(SSP_ERR_ARG, "bn_apply: arg-max plane needs ld % 4 == 0 and ld >= C");
+  if (!y_layout_ok(y, y_ld, C)) return fail_msg(SSP_ERR_ARG, "bn_apply: y must be 16-B aligned with y_ld % 4 == 0 and y_ld >= C");
+  if (ypool && !y_layout_ok(ypool, ypool_ld, C)) return fail_msg(SSP_ERR_ARG, "bn_apply: arg-max plane must be 16-B aligned with ld % 4 == 0 and ld >= C");
+  const struct { void* hi; void* lo; int ld, c0, kind; } dsts[2] = {{d0_hi, d0_lo, d0_ld, d0_c0, d0_kind}, {d1_hi, d1_lo, d1_ld, d1_c0, d1_kind}};
+  for (const auto& d : dsts)
+    if (d.hi && d.kind != DST_NONE && !(plane_layout_ok(d.hi, 2, d.ld, d.c0, d.kind, C) && (!d.lo || aligned(d.lo, 8))))
+      return fail_msg(SSP_ERR_ARG, "bn_apply: destination planes must be 8-B aligned with ld % 4 == 0, c0 % 4 == 0 and ld >= c0 + C "
+                                   "(c0 + 4C for a reorg)");
   BnApplyParams p;
   p.y = y; p.y_ld = y_ld; p.scale = scale; p.shift = shift; p.N = N; p.C = C; p.H = H; p.W = W; p.slope = slope;
   p.dst[0] = ActDst{(uint16_t*)d0_hi, (uint16_t*)d0_lo, d0_ld, d0_c0, d0_hi ? d0_kind : DST_NONE};
@@ -550,6 +566,15 @@ static int fill_bwd(BnBwdParams& p, const float* y, int y_ld, const float* scale
   p.src[1] = GradSrc{g1, g1_ld, g1_c0, g1 ? (g1_kind & 15) : SRC_NONE, (g1_kind & SSP_ROUTE_F16) ? 1 : 0};
   p.s1 = s1; p.s2 = s2; p.count = (double)N * H * W;
   p.dy = nullptr; p.dy_ld = 0; p.dy_fmt = 0; p.dy_scale = 1.f;
+  return SSP_OK;
+}
+// layout rules of y and of the upstream gradient planes, after fill_bwd has accepted the arguments
+static int check_bwd_layout(const BnBwdParams& p) {
+  if (!y_layout_ok(p.y, p.y_ld, p.C)) return fail_msg(SSP_ERR_ARG, "bn_bwd: y must be 16-B aligned with y_ld % 4 == 0 and y_ld >= C");
+  for (const GradSrc& gs : p.src)
+    if (gs.kind != SRC_NONE && !plane_layout_ok(gs.g, gs.f16 ? 2 : 4, gs.ld, gs.c0, gs.kind, p.C))
+      return fail_msg(SSP_ERR_ARG, "bn_bwd: gradient planes must be 16-B (fp32) / 8-B (fp16) aligned with ld % 4 == 0, c0 % 4 == 0 "
+                                   "and ld >= c0 + C (c0 + 4C for a reorg)");
   return SSP_OK;
 }
 
@@ -603,6 +628,7 @@ int ssp_bn_bwd_reduce(const float* y, int y_ld, const float* scale, const float*
   BnBwdParams p;
   if (fill_bwd(p, y, y_ld, scale, shift, mean, invstd, gamma, N, C, H, W, slope, g0, g0_ld, g0_c0, g0_kind, g1, g1_ld, g1_c0, g1_kind, s1, s2) || !s1 || !s2 || !p.has_bn)
     return fail_msg(SSP_ERR_ARG, "bn_bwd_reduce: bad argument");
+  if (const int rc = check_bwd_layout(p)) return rc;
   const bool pooled = p.src[0].kind == SRC_POOL || p.src[1].kind == SRC_POOL;
   const int cgs = C / 4, CG = cgs < 256 ? cgs : 256, PL = 256 / CG;
   const long long nunits = (long long)N * (pooled ? H / 2 : H) * (pooled ? W / 2 : W);
@@ -632,6 +658,8 @@ int ssp_bn_bwd_apply(const float* y, int y_ld, const float* scale, const float* 
   if (fill_bwd(p, y, y_ld, scale, shift, mean, invstd, gamma, N, C, H, W, slope, g0, g0_ld, g0_c0, g0_kind, g1, g1_ld, g1_c0, g1_kind, s1, s2) || !dy)
     return fail_msg(SSP_ERR_ARG, "bn_bwd_apply: bad argument");
   if (p.has_bn && (!s1 || !s2)) return fail_msg(SSP_ERR_ARG, "bn_bwd_apply: statistics buffers missing");
+  if (const int rc = check_bwd_layout(p)) return rc;
+  if (!aligned(dy, 8) || (dy_ld % 4) || dy_ld < C) return fail_msg(SSP_ERR_ARG, "bn_bwd_apply: dY must be 8-B aligned with dy_ld % 4 == 0 and dy_ld >= C");
   p.dy = (uint16_t*)dy; p.dy_ld = dy_ld; p.dy_fmt = dy_fmt; p.dy_scale = dy_scale;
   const bool pooled = p.src[0].kind == SRC_POOL || p.src[1].kind == SRC_POOL;
   const long long nunits = (long long)N * (pooled ? H / 2 : H) * (pooled ? W / 2 : W);

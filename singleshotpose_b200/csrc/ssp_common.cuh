@@ -74,11 +74,26 @@ __device__ __forceinline__ uint16_t cvt_f32_to_16(float f, int fmt) {
   return fmt == FMT_F16 ? __half_as_ushort(__float2half_rn(fminf(fmaxf(f, -65504.f), 65504.f)))
                         : __bfloat16_as_ushort(__float2bfloat16_rn(f));
 }
-// split an fp32 value into fp16 hi + fp16 lo (hi + lo carries ~22 mantissa bits)
+// fp16(clamp(f, +-65504)), round to nearest even: a conversion that would overflow gives the largest finite fp16 instead of an
+// infinity, NaN stays NaN (PTX cvt .satfinite: one instruction, like the plain conversion)
+__device__ __forceinline__ uint16_t f16_satfinite(float f) {
+  uint16_t h;
+  asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(h) : "f"(f));
+  return h;
+}
+// split an fp32 value into fp16 hi + fp16 lo (hi + lo carries ~22 mantissa bits).  Saturating: hi = fp16(clamp(f, +-65504)) and
+// lo = fp16(clamp(f - hi, +-65504)), so a finite f never yields an infinite part (an unclamped hi of +-inf for |f| >= 65520
+// would make lo = -+inf and hi + lo NaN).  f is represented to ~2^-11 relative up to |f| = 131008 and saturates beyond; for
+// |f| < 65520 both parts are the unclamped ones bit for bit.
 __device__ __forceinline__ void split_f16(float f, uint16_t& hi, uint16_t& lo) {
-  __half h = __float2half_rn(f);
-  hi = __half_as_ushort(h);
-  lo = __half_as_ushort(__float2half_rn(f - __half2float(h)));
+  hi = f16_satfinite(f);
+  lo = f16_satfinite(f - __half2float(__ushort_as_half(hi)));
+}
+// split_f16 of two values at once, packed (a in the low half): one paired conversion per plane, as the stores want them
+__device__ __forceinline__ void split_f16x2(float a, float b, uint32_t& hi2, uint32_t& lo2) {
+  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(hi2) : "f"(b), "f"(a));      // the first source goes to the upper half
+  const float2 h = __half22float2(*reinterpret_cast<const __half2*>(&hi2));
+  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(lo2) : "f"(b - h.y), "f"(a - h.x));
 }
 
 // ---------------------------------------------------------------------------------------------
