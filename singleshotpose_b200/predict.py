@@ -20,8 +20,8 @@ load_weights / optimiser updates (the planes are re-packed before the replay whe
 re-captured if the parameters were moved to new memory.  The predictor owns its activation buffers, so model(x) or a training
 step between two replays cannot write into memory the graph replays.
 
-Returned device tensors are the predictor's static outputs: the next call overwrites them.  Everything but the head lives in
-_FramePredictor, which predict_multi.MultiPosePredictor shares.
+Returned device tensors are the predictor's static outputs: the next call overwrites them.  Everything but the head's selection
+lives in _FramePredictor, which predict_multi.MultiPosePredictor and predict_instances.InstancePosePredictor share.
 
 Command line: python -m singleshotpose_b200.predict --datacfg cfg/ape.data --modelcfg cfg/yolo-pose.cfg --weightfile w.weights
               --out poses.npz img1.jpg img2.jpg ...
@@ -37,11 +37,12 @@ import torch
 from ._lib import SspError, call, load, ptr, stream_ptr
 from .engine import Buffers
 from .image import BICUBIC
-from .utils import check_pnp_args, consensus_subsets, consensus_work_bytes
+from .utils import check_pnp_args, consensus_subsets, consensus_work_bytes, inlier_bits, keypoint_bits, object_table
 
 
 class _Chain:
-    """static buffers (and the graph) of one (frame size, frame source); the head's buffers come from pred._head_buffers"""
+    """static buffers (and the graph) of one (frame size, frame source); the head's buffers come from pred._slot_buffers and
+    pred._head_buffers"""
 
     def __init__(self, pred, Wf, Hf, src):
         dev, B = pred.device, pred.batch
@@ -58,16 +59,23 @@ class _Chain:
         self.work = torch.empty(nb + 16, dtype=torch.uint8, device=dev)
         self.scale = torch.tensor([Wf, Hf], dtype=torch.float32, device=dev)
         self.logits = None
+        pred._slot_buffers(self)
         pred._head_buffers(self)
 
 
 class _FramePredictor:
     """What every pose predictor shares: input checks and the pinned staging buffer; JPEG, host and device frame sources; resize
     and ToTensor; the split-K eval forward on private Buffers; the per-(frame size, source) LRU of captured graphs; the re-pack
-    and re-capture after the weights change.  A subclass supplies the head: _head_buffers(chain) allocates its static buffers,
-    _head(chain, stream) launches it after the forward and _outputs(chain) names the returned tensors."""
+    and re-capture after the weights change; and the pose tail of the head.
 
-    def __init__(self, model, K, frame_size, shape, batch, graph, max_graphs):
+    Each frame's head selects into S slots.  With slots=None there is one slot per requested class and slot q holds the q-th
+    (PosePredictor: S = 1; MultiPosePredictor: S = Q).  With slots=M the selection detects: it fills c.cls, a device c.count and
+    each slot's PnP points c.P3 (utils_multi.detect_slots), and slots >= count[b] of frame b are empty.  The tail is _solve (PnP
+    of every slot: plain, counted or consensus) and _project (each slot's class's centroid and corners under its pose).
+    A subclass supplies the rest: _head_buffers(chain) allocates its selection's static buffers, _head(chain, stream) launches
+    the selection after the forward and then the tail, and _outputs(chain) names the returned tensors."""
+
+    def __init__(self, model, objects, K, frame_size, shape, batch, graph, max_graphs, pnp, reproj_thresh, slots=None):
         name = type(self).__name__
         if not torch.cuda.is_available():
             raise SspError("%s needs a CUDA device (no CPU fallback)" % name)
@@ -84,11 +92,30 @@ class _FramePredictor:
         dev = self.eng.device if self.eng.device is not None else torch.device("cuda", torch.cuda.current_device())
         self.device = dev
         self.eng.materialize(dev)
-        Km = np.asarray(K, dtype=np.float64)
-        if Km.shape != (3, 3):
-            raise SspError("K must be (3, 3), got %s" % (Km.shape,))
+        self.classes, points, Km = object_table(objects, self.num_classes, K)
+        self._cls_host = self.classes.astype(np.int32)                          # copied into the selection's launch
         self._K32 = torch.from_numpy(np.ascontiguousarray(Km, dtype=np.float32)).to(dev)       # PnP takes float32 K (valid.py:147)
         self._K64 = torch.from_numpy(np.ascontiguousarray(Km)).to(dev)
+        P3 = points[self.classes]                                                # (Q, 9, 3) PnP points of the requested classes
+        Q, B = len(P3), self.batch
+        # row-major copies: the kernels read raw pointers, and numpy keeps a transposed input's column-major order through
+        # concatenate / astype
+        X = np.concatenate([P3.reshape(-1, 3).T, np.ones((1, 9 * Q))], 0)
+        self._X = torch.from_numpy(np.ascontiguousarray(X, dtype=np.float32)).to(dev)                 # (4, 9Q)
+        self.pnp, self.reproj_thresh = check_pnp_args(pnp, reproj_thresh)
+        self._subsets = consensus_subsets(P3) if self.pnp == "consensus" else None
+        self._bits = keypoint_bits(self.num_keypoints, dev)
+        self.num_slots, self._detects = (Q if slots is None else int(slots)), slots is not None
+        if self._detects:
+            slot_of = np.zeros(self.num_classes, np.int64)                       # class id -> its column block in the projection
+            slot_of[self.classes] = np.arange(Q)
+            self._P3_table = torch.from_numpy(points.astype(np.float32)).to(dev)         # PnP points by class id
+            self._slot_of = torch.from_numpy(slot_of).to(dev)
+            self._slot_index = torch.arange(self.num_slots, device=dev)
+            self._rows = torch.arange(B * self.num_slots, device=dev)
+            self._zero = torch.zeros((), dtype=torch.float32, device=dev)
+        else:
+            self._P3 = torch.from_numpy(np.repeat(P3[None], B, 0).astype(np.float32)).to(dev)   # (B, Q, 9, 3): one per slot
         W, H = self.shape
         self.out_hw = self.eng.spatial(self.eng.layers[-1], H, W)               # raises for a shape off the pooling pyramid
         self._bufs = Buffers(self.eng, self.batch, H, W, False, split_k=True)
@@ -97,42 +124,58 @@ class _FramePredictor:
         self._jpeg = None
         self._last = None
 
-    # ------------------------------------------------------------------ PnP: plain (ssp_pnp_batched*) or consensus (ssp_pnp_consensus)
-    def _init_pnp(self, pnp, reproj_thresh, point_sets):
-        """point_sets: the (9, 3) PnP points of every class; all give the subset table (box points share their structure)"""
-        self.pnp, self.reproj_thresh = check_pnp_args(pnp, reproj_thresh)
-        self._subsets = consensus_subsets(np.stack(point_sets)) if self.pnp == "consensus" else None
-        self._bits = torch.tensor([1 << i for i in range(self.num_keypoints)], dtype=torch.int32, device=self.device)
+    # ------------------------------------------------------------------ the pose tail: slots -> PnP -> projection
+    def _slot_buffers(self, c):
+        dev, B, S, K, Q = self.device, self.batch, self.num_slots, self.num_keypoints, len(self.classes)
+        c.kp = torch.empty(B, S, K, 2, dtype=torch.float32, device=dev)
+        c.R = torch.empty(B, S, 3, 3, dtype=torch.float64, device=dev)
+        c.t = torch.empty(B, S, 3, dtype=torch.float64, device=dev)
+        c.Rt = torch.empty(B, S, 3, 4, dtype=torch.float64, device=dev)
+        c.proj = torch.empty(B * S, 2, Q * K, dtype=torch.float32, device=dev)
+        c.corners = torch.empty(B, S, K, 2, dtype=torch.float32, device=dev)
+        if self._detects:
+            c.valid = torch.empty(B, S, dtype=torch.bool, device=dev)
+        else:
+            c.P3, c.count = self._P3, None
+        if self.pnp == "consensus":
+            c.params = torch.empty(B, S, 6, dtype=torch.float64, device=dev)
+            c.inl_mask = torch.empty(B, S, dtype=torch.int32, device=dev)
+            c.hyp = torch.empty(B, S, dtype=torch.int32, device=dev)
+            c.inliers = torch.empty(B, S, K, dtype=torch.bool, device=dev)
+            wb = consensus_work_bytes(K, len(self._subsets), B * S)
+            c.pnp_work = torch.empty(max(wb, 8) // 8, dtype=torch.float64, device=dev)
 
-    def _consensus_buffers(self, c, lead):
-        """the consensus solve's outputs and workspace for the problems of shape `lead` (nothing for the plain solve)"""
-        if self.pnp != "consensus":
+    def _solve(self, c, s):
+        """PnP of every slot's keypoints c.kp against its points c.P3 with the fp32 K into c.R, c.t (the consensus solve: also
+        c.params, c.inliers, c.hyp); with a device c.count, frame b solves its first count[b] slots and the others get zeros"""
+        B, S, K = self.batch, self.num_slots, self.num_keypoints
+        if self.pnp == "consensus":
+            call("ssp_pnp_consensus", ptr(c.P3), 0, ptr(c.kp), ptr(self._K32), K, B, S, ptr(c.count), self._subsets.ctypes.data,
+                 len(self._subsets), self.reproj_thresh, 20, ptr(c.R), ptr(c.t), ptr(c.params), ptr(c.inl_mask), ptr(c.hyp),
+                 ptr(c.pnp_work), c.pnp_work.numel() * 8, s)
+            inlier_bits(c.inl_mask, self._bits, out=c.inliers)
+        elif c.count is None:
+            call("ssp_pnp_batched", ptr(c.P3), 0, ptr(c.kp), ptr(self._K32), K, B * S, 20, ptr(c.R), ptr(c.t), None, s)
+        else:
+            call("ssp_pnp_batched_counted", ptr(c.P3), ptr(c.kp), ptr(self._K32), K, B, S, ptr(c.count), 20, ptr(c.R), ptr(c.t), s)
+
+    def _project(self, c, s):
+        """c.corners: each slot's class's 9 points projected under the slot's pose (zero in empty slots)"""
+        B, S, K, Q = self.batch, self.num_slots, self.num_keypoints, len(self.classes)
+        c.Rt[..., :3].copy_(c.R)
+        c.Rt[..., 3].copy_(c.t)
+        # every requested class's points under every slot's pose (each point is projected on its own, so a slot's own columns are
+        # what ssp_project_points gives for its class's (4, 9) points alone); each slot keeps the columns of its class
+        call("ssp_project_points", ptr(self._X), 4, Q * K, ptr(c.Rt), ptr(self._K64), B * S, ptr(c.proj), s)
+        if not self._detects:                      # slot q: class q
+            c.corners.copy_(torch.diagonal(c.proj.view(B, S, 2, Q, K), dim1=1, dim2=3).permute(0, 3, 2, 1))
             return
-        dev, K, n = self.device, self.num_keypoints, int(np.prod(lead))
-        c.params = torch.empty(*lead, 6, dtype=torch.float64, device=dev)
-        c.inl_mask = torch.empty(*lead, dtype=torch.int32, device=dev)
-        c.hyp = torch.empty(*lead, dtype=torch.int32, device=dev)
-        c.inliers = torch.empty(*lead, K, dtype=torch.bool, device=dev)
-        wb = consensus_work_bytes(K, len(self._subsets), n)
-        c.pnp_work = torch.empty(max(wb, 8) // 8, dtype=torch.float64, device=dev)
-
-    def _consensus(self, c, s, P3, shared, groups, per_group, count):
-        """the consensus solve of groups x per_group problems into c.R, c.t, c.params, c.inliers, c.hyp (count: device int [groups] or None)"""
-        call("ssp_pnp_consensus", ptr(P3), shared, ptr(c.kp), ptr(self._K32), self.num_keypoints, groups, per_group, ptr(count),
-             self._subsets.ctypes.data, len(self._subsets), self.reproj_thresh, 20, ptr(c.R), ptr(c.t), ptr(c.params), ptr(c.inl_mask),
-             ptr(c.hyp), ptr(c.pnp_work), c.pnp_work.numel() * 8, s)
-        torch.ne(torch.bitwise_and(c.inl_mask.unsqueeze(-1), self._bits), 0, out=c.inliers)
+        own = c.proj.view(B * S, 2, Q, K)[self._rows, :, self._slot_of[c.cls0.view(-1)]]          # (B*S, 2, K)
+        torch.lt(self._slot_index, c.count.unsqueeze(1), out=c.valid)
+        torch.where(c.valid.view(B, S, 1, 1), own.view(B, S, 2, K).transpose(2, 3), self._zero, out=c.corners)
 
     def _consensus_outputs(self, c):
         return dict(inliers=c.inliers, hyp=c.hyp) if self.pnp == "consensus" else {}
-
-    @staticmethod
-    def _box_points(corners3D):
-        """(3|4, 8) box corners -> (3, 9) float64 [0; corners3D[:3]] as columns (valid.py:146, valid_multi.py:135)"""
-        c = np.asarray(corners3D, dtype=np.float64)
-        if c.ndim != 2 or c.shape[0] not in (3, 4) or c.shape[1] != 8:
-            raise SspError("corners3D must be (3|4, 8), got %s" % (c.shape,))
-        return np.concatenate([np.zeros((3, 1)), c[:3]], axis=1)
 
     # ------------------------------------------------------------------ inputs
     def _check(self, frames):
@@ -280,48 +323,30 @@ class PosePredictor(_FramePredictor):
 
     def __init__(self, model, corners3D, K, frame_size=(640, 480), shape=None, batch=1, graph=True, max_graphs=4, pnp="plain",
                  reproj_thresh=8.0):
-        P = self._box_points(corners3D)
-        super().__init__(model, K, frame_size, shape if shape is not None else (model.test_width, model.test_height), batch, graph,
-                         max_graphs)
-        self._init_pnp(pnp, reproj_thresh, [P.T])
-        dev = self.device
-        self._P3 = torch.from_numpy(np.ascontiguousarray(P.T, dtype=np.float32)).to(dev)           # (9, 3) PnP points
-        # row-major copies: the kernels read raw pointers, and numpy keeps a transposed input's column-major order through
-        # concatenate / astype
-        self._X = torch.from_numpy(np.ascontiguousarray(np.concatenate([P, np.ones((1, 9))], 0), dtype=np.float32)).to(dev)   # (4, 9)
+        super().__init__(model, {0: corners3D}, K, frame_size, shape if shape is not None else (model.test_width, model.test_height),
+                         batch, graph, max_graphs, pnp, reproj_thresh)
 
     def _head_buffers(self, c):
         dev, B, K = self.device, self.batch, self.num_keypoints
         c.boxes = torch.empty(B, 2 * K + 3, dtype=torch.float32, device=dev)
         c.conf = torch.empty(B, dtype=torch.float32, device=dev)
-        c.kp = torch.empty(B, K, 2, dtype=torch.float32, device=dev)
-        c.R = torch.empty(B, 3, 3, dtype=torch.float64, device=dev)
-        c.t = torch.empty(B, 3, dtype=torch.float64, device=dev)
-        c.Rt = torch.empty(B, 3, 4, dtype=torch.float64, device=dev)
-        c.proj = torch.empty(B, 2, K, dtype=torch.float32, device=dev)
-        c.corners = torch.empty(B, K, 2, dtype=torch.float32, device=dev)
-        self._consensus_buffers(c, (B,))
 
     def _head(self, c, s):
         B, K = self.batch, self.num_keypoints
         h, w = c.logits.shape[2:]
         call("ssp_region_decode_argmax", ptr(c.logits), B, K, self.num_classes, h, w, 1, ptr(c.boxes), ptr(c.conf), None, s)
-        torch.mul(c.boxes[:, :2 * K].view(B, K, 2), c.scale, out=c.kp)
-        if self.pnp == "consensus":
-            self._consensus(c, s, self._P3, 1, B, 1, None)
-        else:
-            call("ssp_pnp_batched", ptr(self._P3), 1, ptr(c.kp), ptr(self._K32), K, B, 20, ptr(c.R), ptr(c.t), None, s)
-        c.Rt[:, :, :3].copy_(c.R)
-        c.Rt[:, :, 3].copy_(c.t)
-        call("ssp_project_points", ptr(self._X), 4, K, ptr(c.Rt), ptr(self._K64), B, ptr(c.proj), s)
-        c.corners.copy_(c.proj.transpose(1, 2))
+        torch.mul(c.boxes[:, :2 * K].view(B, 1, K, 2), c.scale, out=c.kp)
+        self._solve(c, s)
+        self._project(c, s)
 
     def _outputs(self, c):
-        return dict(R=c.R, t=c.t, conf=c.conf, keypoints_px=c.kp, corners_px=c.corners, **self._consensus_outputs(c))
+        one = {k: v[:, 0] for k, v in self._consensus_outputs(c).items()}          # the one slot of each frame
+        return dict(R=c.R[:, 0], t=c.t[:, 0], conf=c.conf, keypoints_px=c.kp[:, 0], corners_px=c.corners[:, 0], **one)
 
 
 # ---------------------------------------------------------------------------------------------- command line
 CONSENSUS_KEYS = {"plain": (), "consensus": ("inliers", "hyp")}          # the .npz columns each --pnp adds
+SIZE_KEYS = (("width", "height"),)                                      # the frame size entries of a single-object .data file
 
 
 def add_pnp_args(ap):
@@ -330,19 +355,40 @@ def add_pnp_args(ap):
     ap.add_argument("--reproj-thresh", type=float, default=8.0, help="inlier threshold of --pnp consensus, frame pixels")
 
 
-def camera_from_data_cfg(datacfg):
-    """-> (mesh path, K (3, 3) float64, (width, height)) from a .data file (utils.py read_data_cfg keys mesh, fx, fy, u0, v0, width,
-    height; valid.py:26-35)"""
+def read_camera(datacfg, size_keys):
+    """-> (mesh path or None, K (3, 3) float64, (width, height)) from a .data file (utils.py read_data_cfg; valid.py:26-35,
+    valid_multi.py:30-35): fx, fy, u0, v0, and the size from the first (width key, height key) pair of size_keys of which the
+    file has either key (else the last pair)"""
     from .utils_host import read_data_cfg
     o = read_data_cfg(datacfg)
+    wk, hk = next((p for p in size_keys if p[0] in o or p[1] in o), size_keys[-1])
     try:
         fx, fy, u0, v0 = (float(o[k]) for k in ("fx", "fy", "u0", "v0"))
-        size = (int(o["width"]), int(o["height"]))
-        mesh = o["mesh"]
+        size = (int(o[wk]), int(o[hk]))
     except KeyError as e:
         raise SspError("%s has no %s entry" % (datacfg, e))
     K = np.array([[fx, 0.0, u0], [0.0, fy, v0], [0.0, 0.0, 1.0]])
-    return mesh, K, size
+    return o.get("mesh"), K, size
+
+
+def mesh_corners(path):
+    """(4, 8) box corners (utils.get_3D_corners) of the vertices of a PLY mesh"""
+    from .utils import get_3D_corners
+    from .utils_host import read_ply_vertices
+    V = read_ply_vertices(path)
+    return get_3D_corners(np.c_[V, np.ones((len(V), 1))].T)
+
+
+def predict_files(pred, paths):
+    """yields pred's host result for each image file, one frame per call: JPEG files go to the GPU decoder, others through Pillow"""
+    for path in paths:
+        with open(path, "rb") as f:
+            data = f.read()
+        if data[:2] == b"\xff\xd8":
+            yield pred([data], to_host=True)
+        else:
+            from PIL import Image
+            yield pred(np.asarray(Image.open(path).convert("RGB"))[None], to_host=True)
 
 
 def main(argv=None):
@@ -357,24 +403,16 @@ def main(argv=None):
     a = ap.parse_args(argv)
     check_pnp_args(a.pnp, a.reproj_thresh)
     from .darknet import Darknet
-    from .utils_host import read_ply_vertices
-    from .utils import get_3D_corners
-    mesh, K, size = camera_from_data_cfg(a.datacfg)
-    V = read_ply_vertices(mesh)
-    corners3D = get_3D_corners(np.c_[V, np.ones((len(V), 1))].T)
+    mesh, K, size = read_camera(a.datacfg, SIZE_KEYS)
+    if mesh is None:
+        raise SspError("%s has no mesh entry" % a.datacfg)
+    corners3D = mesh_corners(mesh)
     model = Darknet(a.modelcfg)
     model.load_weights(a.weightfile)
     model.cuda().eval()
     pred = PosePredictor(model, corners3D, K, frame_size=size, pnp=a.pnp, reproj_thresh=a.reproj_thresh)
     res = {k: [] for k in ("R", "t", "conf", "keypoints_px", "corners_px") + CONSENSUS_KEYS[a.pnp]}
-    for path in a.images:
-        with open(path, "rb") as f:
-            data = f.read()
-        if data[:2] == b"\xff\xd8":
-            r = pred([data], to_host=True)
-        else:
-            from PIL import Image
-            r = pred(np.asarray(Image.open(path).convert("RGB"))[None], to_host=True)
+    for r in predict_files(pred, a.images):
         for k in res:
             res[k].append(r[k][0])
     np.savez(a.out, paths=np.array(a.images), **{k: np.stack(v) for k, v in res.items()})

@@ -36,16 +36,16 @@ Command line: python -m singleshotpose_b200.predict_instances --datacfg cfg/occl
 from __future__ import annotations
 
 import argparse
-import ctypes as C
 
 import numpy as np
 import torch
 
-from ._lib import SspError, call, ptr
-from .predict import CONSENSUS_KEYS, _FramePredictor, add_pnp_args
-from .predict_multi import MAX_ENTRIES, parse_objects
+from . import predict, predict_multi
+from ._lib import SspError
+from .predict import CONSENSUS_KEYS, _FramePredictor, add_pnp_args, mesh_corners, predict_files, read_camera
+from .predict_multi import cfg_conf_thresh, check_grid, parse_objects
 from .utils import check_pnp_args
-from .utils_multi import MAX_TRACKS, InstanceTracker, check_track_args
+from .utils_multi import InstanceTracker, check_track_args, detect_buffers, detect_slots
 
 MAX_INSTANCES = 256         # largest max_instances (detect_core.h kMaxInstances)
 OUTPUT_KEYS = ("count", "kept", "cls", "R", "t", "conf", "cls_conf", "keypoints_px", "corners_px")
@@ -71,99 +71,22 @@ class InstancePosePredictor(_FramePredictor):
         self.num_anchors = int(getattr(model, "num_anchors", 0))
         if self.num_anchors < 1:
             raise SspError("InstancePosePredictor needs a model with a region head")
-        nC = int(model.num_classes)
-        if not isinstance(objects, dict):
-            objects = {0: objects}
-        if not objects:
-            raise SspError("objects must be a non-empty {class id: corners3D} dict")
-        ids = sorted(objects)
-        for c in ids:
-            if isinstance(c, bool) or not isinstance(c, (int, np.integer)) or not 0 <= c < nC:
-                raise SspError("class id %r is not in [0, %d)" % (c, nC))
-        pts = [self._box_points(objects[c]) for c in ids]
-        nms_thresh = float(nms_thresh)
-        if not 0.0 <= nms_thresh <= 1.0:
-            raise SspError("nms_thresh must be in [0, 1], got %r" % nms_thresh)
-        if isinstance(max_instances, bool) or not isinstance(max_instances, (int, np.integer)) or not 1 <= max_instances <= MAX_INSTANCES:
-            raise SspError("max_instances must be an integer in [1, %d], got %r" % (MAX_INSTANCES, max_instances))
-        if conf_thresh is None:
-            if "conf_thresh" not in model.blocks[0]:
-                raise SspError("the model's cfg has no conf_thresh in its [net] block: pass conf_thresh")
-            conf_thresh = float(model.blocks[0]["conf_thresh"])
-        self.conf_thresh, self.nms_thresh, self.max_instances = float(conf_thresh), nms_thresh, int(max_instances)
+        self.nms_thresh, self.max_instances = check_detect_args(nms_thresh, max_instances)
+        self.conf_thresh = cfg_conf_thresh(model, conf_thresh)
         if shape is None:
             shape = (model.test_width, model.test_height) if self.num_anchors == 1 else (model.width, model.height)
-        super().__init__(model, K, frame_size, shape, batch, graph, max_graphs)
-        self._init_pnp(pnp, reproj_thresh, [P.T for P in pts])
-        h, w = self.out_hw
-        if h * w * self.num_anchors > MAX_ENTRIES:
-            raise SspError("network shape %dx%d gives a %dx%d grid of %d anchors: more than the %d entries the detect kernel holds"
-                           % (self.shape[0], self.shape[1], h, w, self.num_anchors, MAX_ENTRIES))
-        dev, Q = self.device, len(ids)
-        self.classes = np.array(ids, dtype=np.int64)
-        self._cls_host = np.array(ids, dtype=np.int32)                            # copied into the detect kernel's launch
-        table = np.zeros((nC, 9, 3), np.float32)                                  # PnP points by class id (unrequested: zeros)
-        slot_of = np.zeros(nC, np.int64)                                          # class id -> its column block in the projection
-        for q, (c, P) in enumerate(zip(ids, pts)):
-            table[c] = P.T
-            slot_of[c] = q
-        self._P3_table = torch.from_numpy(table).to(dev)
-        self._slot_of = torch.from_numpy(slot_of).to(dev)
-        X = np.concatenate([np.concatenate([P, np.ones((1, 9))], 0) for P in pts], 1)                     # (4, 9Q)
-        self._X = torch.from_numpy(np.ascontiguousarray(X, dtype=np.float32)).to(dev)
-        self._slots = torch.arange(self.max_instances, device=dev)
-        self._rows = torch.arange(self.batch * self.max_instances, device=dev)
-        self._zero = torch.zeros((), dtype=torch.float32, device=dev)
-        self._Q = Q
+        super().__init__(model, objects if isinstance(objects, dict) else {0: objects}, K, frame_size, shape, batch, graph, max_graphs,
+                         pnp, reproj_thresh, slots=self.max_instances)
+        check_grid(self, "detect")
 
     def _head_buffers(self, c):
-        dev, B, K, M, Q = self.device, self.batch, self.num_keypoints, self.max_instances, self._Q
-        c.boxes = torch.empty(B, M, 2 * K + 3, dtype=torch.float32, device=dev)
-        c.cls = torch.empty(B, M, dtype=torch.int32, device=dev)
-        c.cls0 = torch.empty(B, M, dtype=torch.int32, device=dev)
-        c.count = torch.empty(B, dtype=torch.int32, device=dev)
-        c.kept = torch.empty(B, dtype=torch.int32, device=dev)
-        c.valid = torch.empty(B, M, dtype=torch.bool, device=dev)
-        c.kp = torch.empty(B, M, K, 2, dtype=torch.float32, device=dev)
-        c.P3 = torch.empty(B * M, K, 3, dtype=torch.float32, device=dev)
-        c.R = torch.empty(B, M, 3, 3, dtype=torch.float64, device=dev)
-        c.t = torch.empty(B, M, 3, dtype=torch.float64, device=dev)
-        c.Rt = torch.empty(B, M, 3, 4, dtype=torch.float64, device=dev)
-        c.proj = torch.empty(B * M, 2, Q * K, dtype=torch.float32, device=dev)
-        c.corners = torch.empty(B, M, K, 2, dtype=torch.float32, device=dev)
-        self._consensus_buffers(c, (B, M))
+        detect_buffers(c, self.batch, self.max_instances, self.device)
 
     def _head(self, c, s):
-        self._detect(c, s)
+        detect_slots(c, c.logits, self._cls_host, self._P3_table, self.num_classes, self.num_anchors, self.conf_thresh, self.nms_thresh,
+                     c.frame, s)
         self._solve(c, s)
         self._project(c, s)
-
-    def _detect(self, c, s):
-        B, K, M, Q = self.batch, self.num_keypoints, self.max_instances, self._Q
-        Wf, Hf = c.frame
-        h, w = c.logits.shape[2:]
-        call("ssp_detect_instances", ptr(c.logits), B, K, self.num_classes, self.num_anchors, h, w, C.c_void_p(self._cls_host.ctypes.data),
-             Q, self.conf_thresh, self.nms_thresh, M, float(Wf), float(Hf), ptr(c.boxes), ptr(c.cls), ptr(c.kp), ptr(c.count), ptr(c.kept), s)
-        torch.clamp(c.cls, min=0, out=c.cls0)                  # empty slots hold -1: any in-range index will do, PnP skips them
-        torch.index_select(self._P3_table, 0, c.cls0.view(-1), out=c.P3)
-
-    def _solve(self, c, s):
-        if self.pnp == "consensus":
-            self._consensus(c, s, c.P3, 0, self.batch, self.max_instances, c.count)
-            return
-        call("ssp_pnp_batched_counted", ptr(c.P3), ptr(c.kp), ptr(self._K32), self.num_keypoints, self.batch, self.max_instances,
-             ptr(c.count), 20, ptr(c.R), ptr(c.t), s)
-
-    def _project(self, c, s):
-        B, K, M, Q = self.batch, self.num_keypoints, self.max_instances, self._Q
-        c.Rt[..., :3].copy_(c.R)
-        c.Rt[..., 3].copy_(c.t)
-        # every requested class's points under every slot's pose (each point is projected on its own, so a slot's own columns are
-        # what ssp_project_points gives for its class's (4, 9) points alone); slot (b, m) keeps the columns of its class
-        call("ssp_project_points", ptr(self._X), 4, Q * K, ptr(c.Rt), ptr(self._K64), B * M, ptr(c.proj), s)
-        own = c.proj.view(B * M, 2, Q, K)[self._rows, :, self._slot_of[c.cls0.view(-1)]]          # (B*M, 2, K)
-        torch.lt(self._slots, c.count.unsqueeze(1), out=c.valid)
-        torch.where(c.valid.view(B, M, 1, 1), own.view(B, M, 2, K).transpose(2, 3), self._zero, out=c.corners)
 
     def _outputs(self, c):
         K = self.num_keypoints
@@ -190,8 +113,6 @@ class TrackingPosePredictor(InstancePosePredictor):
         check_tracking_pnp(pnp)
         check_track_args(max_tracks, match_iou, max_misses)
         super().__init__(model, objects, K, frame_size, shape, batch, conf_thresh, nms_thresh, max_instances, graph, max_graphs)
-        if not isinstance(objects, dict):
-            objects = {0: objects}
         self._tracker = InstanceTracker(objects, K, self.num_classes, self.num_anchors, self.frame_size, self.batch, self.conf_thresh,
                                         self.nms_thresh, self.max_instances, max_tracks, match_iou, max_misses, device=self.device)
         self.max_tracks, self.match_iou, self.max_misses = self._tracker.max_tracks, self._tracker.match_iou, self._tracker.max_misses
@@ -222,6 +143,16 @@ class TrackingPosePredictor(InstancePosePredictor):
         return dict(super()._outputs(c), track_id=c.track_id, warm=c.warm)
 
 
+def check_detect_args(nms_thresh, max_instances):
+    """-> (nms_thresh, max_instances) as float, int; SspError for nms_thresh outside [0, 1] or max_instances outside [1, 256]"""
+    nms_thresh = float(nms_thresh)
+    if not 0.0 <= nms_thresh <= 1.0:
+        raise SspError("nms_thresh must be in [0, 1], got %r" % nms_thresh)
+    if isinstance(max_instances, bool) or not isinstance(max_instances, (int, np.integer)) or not 1 <= max_instances <= MAX_INSTANCES:
+        raise SspError("max_instances must be an integer in [1, %d], got %r" % (MAX_INSTANCES, max_instances))
+    return nms_thresh, int(max_instances)
+
+
 def check_tracking_pnp(pnp):
     if pnp != "plain":
         raise SspError("tracking solves with pnp='plain' only, got %r: the consensus solve has no rule for how a track's warm guess "
@@ -229,21 +160,7 @@ def check_tracking_pnp(pnp):
 
 
 # ---------------------------------------------------------------------------------------------- command line
-def camera_from_any_data_cfg(datacfg):
-    """-> (mesh path or None, K (3, 3) float64, (width, height)) from a single-object .data file (mesh, width, height) or a
-    multi-object one (im_width, im_height); fx, fy, u0, v0 in both"""
-    from .utils_host import read_data_cfg
-    o = read_data_cfg(datacfg)
-    try:
-        fx, fy, u0, v0 = (float(o[k]) for k in ("fx", "fy", "u0", "v0"))
-        if "im_width" in o or "im_height" in o:
-            size = (int(o["im_width"]), int(o["im_height"]))
-        else:
-            size = (int(o["width"]), int(o["height"]))
-    except KeyError as e:
-        raise SspError("%s has no %s entry" % (datacfg, e))
-    K = np.array([[fx, 0.0, u0], [0.0, fy, v0], [0.0, 0.0, 1.0]])
-    return o.get("mesh"), K, size
+SIZE_KEYS = predict_multi.SIZE_KEYS + predict.SIZE_KEYS      # a multi-object .data file's frame size, else a single-object one's
 
 
 def parse_args(argv=None):
@@ -270,16 +187,8 @@ def parse_args(argv=None):
     check_pnp_args(a.pnp, a.reproj_thresh)
     if a.track:
         check_tracking_pnp(a.pnp)
-    if not 0.0 <= a.nms_thresh <= 1.0:
-        raise SspError("--nms-thresh must be in [0, 1], got %r" % a.nms_thresh)
-    if not 1 <= a.max_instances <= MAX_INSTANCES:
-        raise SspError("--max-instances must be in [1, %d], got %d" % (MAX_INSTANCES, a.max_instances))
-    if not 0.0 <= a.match_iou <= 1.0:
-        raise SspError("--match-iou must be in [0, 1], got %r" % a.match_iou)
-    if a.max_misses < 0:
-        raise SspError("--max-misses must be >= 0, got %d" % a.max_misses)
-    if not 1 <= a.max_tracks <= MAX_TRACKS:
-        raise SspError("--max-tracks must be in [1, %d], got %d" % (MAX_TRACKS, a.max_tracks))
+    check_detect_args(a.nms_thresh, a.max_instances)
+    check_track_args(a.max_tracks, a.match_iou, a.max_misses)
     a.objects = parse_objects(a.object) if a.object else None
     return a
 
@@ -294,18 +203,13 @@ def _region_anchors(modelcfg):
 
 def main(argv=None):
     a = parse_args(argv)
-    from .utils import get_3D_corners
-    from .utils_host import read_ply_vertices
-    mesh, K, size = camera_from_any_data_cfg(a.datacfg)
+    mesh, K, size = read_camera(a.datacfg, SIZE_KEYS)
     meshes = a.objects
     if meshes is None:
         if not mesh:
             raise SspError("%s has no mesh entry: give --object CLASS=MESH.ply" % a.datacfg)
         meshes = {0: mesh}
-    objects = {}
-    for c, path in meshes.items():
-        V = read_ply_vertices(path)
-        objects[c] = get_3D_corners(np.c_[V, np.ones((len(V), 1))].T)
+    objects = {c: mesh_corners(path) for c, path in meshes.items()}
     if _region_anchors(a.modelcfg) > 1:
         from .darknet_multi import Darknet
     else:
@@ -321,14 +225,7 @@ def main(argv=None):
                                      pnp=a.pnp, reproj_thresh=a.reproj_thresh)
     rows = {k: [] for k in ROW_KEYS + (("track_id",) if a.track else ()) + CONSENSUS_KEYS[a.pnp]}
     image = []
-    for i, path in enumerate(a.images):
-        with open(path, "rb") as f:
-            data = f.read()
-        if data[:2] == b"\xff\xd8":
-            r = pred([data], to_host=True)
-        else:
-            from PIL import Image
-            r = pred(np.asarray(Image.open(path).convert("RGB"))[None], to_host=True)
+    for i, r in enumerate(predict_files(pred, a.images)):
         n = int(r["count"][0])
         image += [i] * n
         for k in rows:

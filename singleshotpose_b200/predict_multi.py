@@ -32,7 +32,7 @@ import numpy as np
 import torch
 
 from ._lib import SspError, call, ptr
-from .predict import CONSENSUS_KEYS, _FramePredictor, add_pnp_args
+from .predict import CONSENSUS_KEYS, _FramePredictor, add_pnp_args, mesh_corners, predict_files, read_camera
 from .utils import check_pnp_args
 
 MAX_ENTRIES = 4096          # H*W*num_anchors the select kernel keeps in shared memory (eval_multi_core.h kMaxEntries)
@@ -56,64 +56,27 @@ class MultiPosePredictor(_FramePredictor):
         self.num_anchors = int(getattr(model, "num_anchors", 0))
         if self.num_anchors < 2:
             raise SspError("MultiPosePredictor needs a multi-anchor region head (yolo-pose-multi.cfg), got %d anchor(s)" % self.num_anchors)
-        nC = int(model.num_classes)
-        if not isinstance(objects, dict) or not objects:
-            raise SspError("objects must be a non-empty {class id: corners3D} dict")
-        ids = sorted(objects)
-        for c in ids:
-            if isinstance(c, bool) or not isinstance(c, (int, np.integer)) or not 0 <= c < nC:
-                raise SspError("class id %r is not in [0, %d)" % (c, nC))
-        pts = [self._box_points(objects[c]) for c in ids]
-        if conf_thresh is None:
-            if "conf_thresh" not in model.blocks[0]:
-                raise SspError("the model's cfg has no conf_thresh in its [net] block: pass conf_thresh")
-            conf_thresh = float(model.blocks[0]["conf_thresh"])
-        self.conf_thresh = float(conf_thresh)
-        super().__init__(model, K, frame_size, shape if shape is not None else (model.width, model.height), batch, graph, max_graphs)
-        self._init_pnp(pnp, reproj_thresh, [P.T for P in pts])
-        h, w = self.out_hw
-        if h * w * self.num_anchors > MAX_ENTRIES:
-            raise SspError("network shape %dx%d gives a %dx%d grid of %d anchors: more than the %d entries the select kernel holds"
-                           % (self.shape[0], self.shape[1], h, w, self.num_anchors, MAX_ENTRIES))
-        dev, B, Q = self.device, self.batch, len(ids)
-        self.classes = np.array(ids, dtype=np.int64)
-        self._cls_host = np.array(ids, dtype=np.int32)                            # copied into the select kernel's launch
-        self._classes = torch.from_numpy(self.classes).to(dev)
-        P3 = np.stack([P.T for P in pts]).astype(np.float32)                      # (Q, 9, 3) PnP points of each class
-        self._P3 = torch.from_numpy(np.repeat(P3[None], B, 0)).to(dev)              # (B, Q, 9, 3): one per slot
-        X = np.concatenate([np.concatenate([P, np.ones((1, 9))], 0) for P in pts], 1)                     # (4, 9Q)
-        self._X = torch.from_numpy(np.ascontiguousarray(X, dtype=np.float32)).to(dev)
+        self.conf_thresh = cfg_conf_thresh(model, conf_thresh)
+        super().__init__(model, objects, K, frame_size, shape if shape is not None else (model.width, model.height), batch, graph,
+                         max_graphs, pnp, reproj_thresh)
+        check_grid(self, "select")
+        self._classes = torch.from_numpy(self.classes).to(self.device)
 
     def _head_buffers(self, c):
-        dev, B, K, Q = self.device, self.batch, self.num_keypoints, len(self.classes)
-        c.boxes = torch.empty(B, Q, 2 * K + 3, dtype=torch.float32, device=dev)
+        dev, B, Q = self.device, self.batch, len(self.classes)
+        c.boxes = torch.empty(B, Q, 2 * self.num_keypoints + 3, dtype=torch.float32, device=dev)
         c.flags = torch.empty(B, Q, dtype=torch.int32, device=dev)
         c.detected = torch.empty(B, Q, dtype=torch.bool, device=dev)
-        c.kp = torch.empty(B, Q, K, 2, dtype=torch.float32, device=dev)
-        c.R = torch.empty(B, Q, 3, 3, dtype=torch.float64, device=dev)
-        c.t = torch.empty(B, Q, 3, dtype=torch.float64, device=dev)
-        c.Rt = torch.empty(B, Q, 3, 4, dtype=torch.float64, device=dev)
-        c.proj = torch.empty(B * Q, 2, Q * K, dtype=torch.float32, device=dev)
-        c.corners = torch.empty(B, Q, K, 2, dtype=torch.float32, device=dev)
-        self._consensus_buffers(c, (B, Q))
 
     def _head(self, c, s):
-        B, K, Q = self.batch, self.num_keypoints, len(self.classes)
         Wf, Hf = c.frame
         h, w = c.logits.shape[2:]
-        call("ssp_predict_multi_select", ptr(c.logits), B, K, self.num_classes, self.num_anchors, h, w, C.c_void_p(self._cls_host.ctypes.data),
-             Q, self.conf_thresh, float(Wf), float(Hf), ptr(c.boxes), ptr(c.flags), ptr(c.kp), s)
+        call("ssp_predict_multi_select", ptr(c.logits), self.batch, self.num_keypoints, self.num_classes, self.num_anchors, h, w,
+             C.c_void_p(self._cls_host.ctypes.data), len(self.classes), self.conf_thresh, float(Wf), float(Hf), ptr(c.boxes),
+             ptr(c.flags), ptr(c.kp), s)
         torch.eq(c.flags, 0, out=c.detected)
-        if self.pnp == "consensus":
-            self._consensus(c, s, self._P3, 0, B * Q, 1, None)
-        else:
-            call("ssp_pnp_batched", ptr(self._P3), 0, ptr(c.kp), ptr(self._K32), K, B * Q, 20, ptr(c.R), ptr(c.t), None, s)
-        c.Rt[..., :3].copy_(c.R)
-        c.Rt[..., 3].copy_(c.t)
-        # every class's points under every slot's pose (each point is projected on its own, so a slot's own columns are what
-        # ssp_project_points gives for that class's (4, 9) points alone); slot (b, q) keeps the columns of class q
-        call("ssp_project_points", ptr(self._X), 4, Q * K, ptr(c.Rt), ptr(self._K64), B * Q, ptr(c.proj), s)
-        c.corners.copy_(torch.diagonal(c.proj.view(B, Q, 2, Q, K), dim1=1, dim2=3).permute(0, 3, 2, 1))
+        self._solve(c, s)
+        self._project(c, s)
 
     def _outputs(self, c):
         K = self.num_keypoints
@@ -121,19 +84,25 @@ class MultiPosePredictor(_FramePredictor):
                     keypoints_px=c.kp, corners_px=c.corners, **self._consensus_outputs(c))
 
 
+def cfg_conf_thresh(model, conf_thresh):
+    """conf_thresh as a float, by default the model cfg's [net] conf_thresh (valid_multi.py:40)"""
+    if conf_thresh is None:
+        if "conf_thresh" not in model.blocks[0]:
+            raise SspError("the model's cfg has no conf_thresh in its [net] block: pass conf_thresh")
+        conf_thresh = model.blocks[0]["conf_thresh"]
+    return float(conf_thresh)
+
+
+def check_grid(pred, kernel):
+    """SspError unless the predictor's grid of anchors fits the MAX_ENTRIES the select and detect kernels hold in shared memory"""
+    h, w = pred.out_hw
+    if h * w * pred.num_anchors > MAX_ENTRIES:
+        raise SspError("network shape %dx%d gives a %dx%d grid of %d anchors: more than the %d entries the %s kernel holds"
+                       % (pred.shape[0], pred.shape[1], h, w, pred.num_anchors, MAX_ENTRIES, kernel))
+
+
 # ---------------------------------------------------------------------------------------------- command line
-def camera_from_multi_data_cfg(datacfg):
-    """-> (K (3, 3) float64, (width, height)) from a multi-object .data file (the keys valid_multi.py:30-35 reads: im_width,
-    im_height, fx, fy, u0, v0)"""
-    from .utils_host import read_data_cfg
-    o = read_data_cfg(datacfg)
-    try:
-        fx, fy, u0, v0 = (float(o[k]) for k in ("fx", "fy", "u0", "v0"))
-        size = (int(o["im_width"]), int(o["im_height"]))
-    except KeyError as e:
-        raise SspError("%s has no %s entry" % (datacfg, e))
-    K = np.array([[fx, 0.0, u0], [0.0, fy, v0], [0.0, 0.0, 1.0]])
-    return K, size
+SIZE_KEYS = (("im_width", "im_height"),)            # the frame size entries of a multi-object .data file (valid_multi.py:30-35)
 
 
 def parse_objects(specs):
@@ -169,26 +138,14 @@ def main(argv=None):
     a = ap.parse_args(argv)
     check_pnp_args(a.pnp, a.reproj_thresh)
     from .darknet_multi import Darknet
-    from .utils import get_3D_corners
-    from .utils_host import read_ply_vertices
-    K, size = camera_from_multi_data_cfg(a.datacfg)
-    objects = {}
-    for c, mesh in parse_objects(a.object).items():
-        V = read_ply_vertices(mesh)
-        objects[c] = get_3D_corners(np.c_[V, np.ones((len(V), 1))].T)
+    _mesh, K, size = read_camera(a.datacfg, SIZE_KEYS)
+    objects = {c: mesh_corners(mesh) for c, mesh in parse_objects(a.object).items()}
     model = Darknet(a.modelcfg)
     model.load_weights(a.weightfile)
     model.cuda().eval()
     pred = MultiPosePredictor(model, objects, K, frame_size=size, pnp=a.pnp, reproj_thresh=a.reproj_thresh)
     res = {k: [] for k in OUTPUT_KEYS + CONSENSUS_KEYS[a.pnp]}
-    for path in a.images:
-        with open(path, "rb") as f:
-            data = f.read()
-        if data[:2] == b"\xff\xd8":
-            r = pred([data], to_host=True)
-        else:
-            from PIL import Image
-            r = pred(np.asarray(Image.open(path).convert("RGB"))[None], to_host=True)
+    for r in predict_files(pred, a.images):
         for k in res:
             res[k].append(r[k][0])
     np.savez(a.out, paths=np.array(a.images), classes=pred.classes, **{k: np.stack(v) for k, v in res.items()})

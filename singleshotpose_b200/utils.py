@@ -90,15 +90,18 @@ def get_region_boxes(output, num_classes, num_keypoints, only_objectness=1, vali
 
 
 # ------------------------------------------------------------------------------------------ pose
+def _pnp_inputs(points_3D, points_2D, cameraMatrix):
+    """-> P3 (P,3) or (n,P,3), uv (n,P,2), K (3,3): contiguous float32 CUDA tensors"""
+    dev = _dev()
+    P3, uv, K = (torch.as_tensor(np.asarray(a, dtype=np.float32) if not torch.is_tensor(a) else a).to(dev, torch.float32).contiguous()
+                 for a in (points_3D, points_2D, cameraMatrix))
+    return P3, uv.unsqueeze(0) if uv.dim() == 2 else uv, K
+
+
 def pnp_batched(points_3D, points_2D, cameraMatrix, max_iter=20, return_iters=False):
     """points_3D (P,3) shared or (n,P,3); points_2D (n,P,2); K (3,3) -> R (n,3,3) f64, t (n,3) f64 CUDA tensors."""
-    dev = _dev()
-    P3 = torch.as_tensor(np.asarray(points_3D, dtype=np.float32) if not torch.is_tensor(points_3D) else points_3D)
-    uv = torch.as_tensor(np.asarray(points_2D, dtype=np.float32) if not torch.is_tensor(points_2D) else points_2D)
-    K = torch.as_tensor(np.asarray(cameraMatrix, dtype=np.float32) if not torch.is_tensor(cameraMatrix) else cameraMatrix)
-    P3 = P3.to(dev, torch.float32).contiguous(); uv = uv.to(dev, torch.float32).contiguous(); K = K.to(dev, torch.float32).contiguous()
-    if uv.dim() == 2:
-        uv = uv.unsqueeze(0)
+    P3, uv, K = _pnp_inputs(points_3D, points_2D, cameraMatrix)
+    dev = uv.device
     n, npts = uv.shape[0], uv.shape[1]
     shared = P3.dim() == 2
     assert P3.shape[-2] == npts and P3.shape[-1] == 3 and uv.shape[-1] == 2
@@ -107,6 +110,28 @@ def pnp_batched(points_3D, points_2D, cameraMatrix, max_iter=20, return_iters=Fa
     iters = torch.empty(n, dtype=torch.int32, device=dev) if return_iters else None
     call("ssp_pnp_batched", ptr(P3), 1 if shared else 0, ptr(uv), ptr(K), npts, n, max_iter, ptr(R), ptr(t), ptr(iters), stream_ptr())
     return (R, t, iters) if return_iters else (R, t)
+
+
+def object_table(objects, num_classes, K):
+    """The constants of a pose head, checked: objects {class id in [0, num_classes): (3|4, 8) box corners}, K (3, 3).
+    -> (classes (Q,) int64 sorted ids, points (num_classes, 9, 3) float64 PnP points [0; corners3D_c[:3]] of each requested class
+    by class id (valid.py:146, valid_multi.py:135; zeros for the others), K as (3, 3) float64)"""
+    if not isinstance(objects, dict) or not objects:
+        raise SspError("objects must be a non-empty {class id: corners3D} dict")
+    nC = int(num_classes)
+    classes = sorted(objects)
+    points = np.zeros((nC, 9, 3))
+    for c in classes:
+        if isinstance(c, bool) or not isinstance(c, (int, np.integer)) or not 0 <= c < nC:
+            raise SspError("class id %r is not in [0, %d)" % (c, nC))
+        corners = np.asarray(objects[c], dtype=np.float64)
+        if corners.ndim != 2 or corners.shape[0] not in (3, 4) or corners.shape[1] != 8:
+            raise SspError("corners3D must be (3|4, 8), got %s" % (corners.shape,))
+        points[c, 1:] = corners[:3].T
+    Km = np.asarray(K, dtype=np.float64)
+    if Km.shape != (3, 3):
+        raise SspError("K must be (3, 3), got %s" % (Km.shape,))
+    return np.array(classes, dtype=np.int64), points, Km
 
 
 def pnp(points_3D, points_2D, cameraMatrix):
@@ -166,14 +191,9 @@ def pnp_consensus_batched(points_3D, points_2D, cameraMatrix, reproj_thresh=8.0,
     default); subsets: (H,) uint16 masks, default consensus_subsets(points_3D).
     -> R (n,3,3) f64, t (n,3) f64, params (n,6) f64 (rvec, t), inliers (n,P) bool, hyp (n,) int32 (the chosen hypothesis: 0 the
     all-point solve, h the subset subsets[h-1], -1 none had an inlier), CUDA tensors."""
-    dev = _dev()
     _, thr = check_pnp_args("consensus", reproj_thresh)
-    P3 = torch.as_tensor(np.asarray(points_3D, dtype=np.float32) if not torch.is_tensor(points_3D) else points_3D)
-    uv = torch.as_tensor(np.asarray(points_2D, dtype=np.float32) if not torch.is_tensor(points_2D) else points_2D)
-    K = torch.as_tensor(np.asarray(cameraMatrix, dtype=np.float32) if not torch.is_tensor(cameraMatrix) else cameraMatrix)
-    P3 = P3.to(dev, torch.float32).contiguous(); uv = uv.to(dev, torch.float32).contiguous(); K = K.to(dev, torch.float32).contiguous()
-    if uv.dim() == 2:
-        uv = uv.unsqueeze(0)
+    P3, uv, K = _pnp_inputs(points_3D, points_2D, cameraMatrix)
+    dev = uv.device
     n, npts = uv.shape[0], uv.shape[1]
     shared = P3.dim() == 2
     if P3.shape[-2] != npts or P3.shape[-1] != 3 or uv.shape[-1] != 2 or (not shared and P3.shape[0] != n):
@@ -190,7 +210,7 @@ def pnp_consensus_batched(points_3D, points_2D, cameraMatrix, reproj_thresh=8.0,
     work = torch.empty(max(wb, 8) // 8, dtype=torch.float64, device=dev)
     call("ssp_pnp_consensus", ptr(P3), 1 if shared else 0, ptr(uv), ptr(K), npts, n, 1, None, tab.ctypes.data, len(tab), thr, max_iter,
          ptr(R), ptr(t), ptr(params), ptr(inl), ptr(hyp), ptr(work), work.numel() * 8, stream_ptr())
-    return R, t, params, inlier_bits(inl, npts), hyp
+    return R, t, params, inlier_bits(inl, keypoint_bits(npts, dev)), hyp
 
 
 def consensus_work_bytes(npts, n_subsets, n):
@@ -201,9 +221,15 @@ def consensus_work_bytes(npts, n_subsets, n):
     return out.value
 
 
-def inlier_bits(mask, npts):
-    """(...,) int32 bitmasks -> (..., npts) bool"""
-    return ((mask.unsqueeze(-1) >> torch.arange(npts, dtype=torch.int32, device=mask.device)) & 1) != 0
+def keypoint_bits(npts, device):
+    """(npts,) int32 1 << i: the bit of keypoint i in an inlier mask of ssp_pnp_consensus"""
+    return torch.tensor([1 << i for i in range(npts)], dtype=torch.int32, device=device)
+
+
+def inlier_bits(mask, bits, out=None):
+    """(...,) int32 inlier masks -> (..., npts) bool, with bits = keypoint_bits(npts, mask.device); out: the (..., npts) bool
+    tensor to write"""
+    return torch.ne(torch.bitwise_and(mask.unsqueeze(-1), bits), 0, out=out)
 
 
 def pnp_consensus(points_3D, points_2D, cameraMatrix, reproj_thresh=8.0):
@@ -337,6 +363,24 @@ def pose_label_rows(corners3D, Rt, K, width, height, class_id=0):
 
 
 # ------------------------------------------------------------------------------------------ batched evaluation tail
+def pnp_truth_and_prediction(P3, uv, K, pnp, reproj_thresh):
+    """The poses of n ground truths uv[:n] and n predictions uv[n:] (uv (2n, P, 2)) -> R (2n, 3, 3), t (2n, 3) fp64 and the
+    predictions' inliers (n, P) and hyp (n,) for pnp="consensus" ({} for "plain").  The ground truth is always the plain solve;
+    "plain" solves all 2n problems in one launch."""
+    dev, n = uv.device, len(uv) // 2
+    if n == 0:                                  # nothing to launch: the PnP entry points take no empty (null) buffers
+        R, t = torch.zeros(0, 3, 3, dtype=torch.float64, device=dev), torch.zeros(0, 3, dtype=torch.float64, device=dev)
+        if pnp != "consensus":
+            return R, t, {}
+        return R, t, dict(inliers=torch.zeros(0, uv.shape[1], dtype=torch.bool, device=dev), hyp=torch.zeros(0, dtype=torch.int32, device=dev))
+    if pnp != "consensus":
+        R, t = pnp_batched(P3, uv, K)
+        return R, t, {}
+    R_gt, t_gt = pnp_batched(P3, uv[:n], K)
+    R_pr, t_pr, _p, inl, hyp = pnp_consensus_batched(P3, uv[n:], K, reproj_thresh)
+    return torch.cat([R_gt, R_pr]), torch.cat([t_gt, t_pr]), dict(inliers=inl, hyp=hyp)
+
+
 def evaluate_poses_batched(output, target, vertices, points_3D, internal_calibration, num_classes=1, num_keypoints=9,
                            im_width=640, im_height=480, adds=False, pnp="plain", reproj_thresh=8.0):
     """GPU-resident version of the per-image evaluation loop of reference valid.py:123-183 (SURVEY 8f.1): per-image decode
@@ -361,14 +405,8 @@ def evaluate_poses_batched(output, target, vertices, points_3D, internal_calibra
     gt2d = torch.as_tensor(target)[:, 1:1 + 2 * K].to(dev, torch.float32).reshape(B, K, 2) * scale
     Kc = torch.as_tensor(np.asarray(internal_calibration, dtype=np.float32)).to(dev)
     P3 = torch.as_tensor(np.asarray(points_3D, dtype=np.float32)).to(dev)
-    extra = {}
-    if pnp == "consensus":
-        R_gt, t_gt = pnp_batched(P3, gt2d, Kc)
-        R_pr, t_pr, _p, inl, hyp = pnp_consensus_batched(P3, pr2d, Kc, reproj_thresh)
-        extra = dict(inliers=inl, hyp=hyp)
-    else:
-        R, t = pnp_batched(P3, torch.cat([gt2d, pr2d], 0), Kc)         # 2B problems in one launch
-        R_gt, R_pr, t_gt, t_pr = R[:B], R[B:], t[:B], t[B:]
+    R, t, extra = pnp_truth_and_prediction(P3, torch.cat([gt2d, pr2d], 0), Kc, pnp, reproj_thresh)
+    R_gt, R_pr, t_gt, t_pr = R[:B], R[B:], t[:B], t[B:]
     Rt_gt = torch.cat([R_gt, t_gt.unsqueeze(2)], 2)
     Rt_pr = torch.cat([R_pr, t_pr.unsqueeze(2)], 2)
     V = torch.as_tensor(np.asarray(vertices, dtype=np.float32)).to(dev)

@@ -11,7 +11,7 @@ import torch
 from ._lib import call, ptr, stream_ptr, SspError
 from .utils import (pnp, pnp_batched, compute_projection, compute_transformation, calcAngularDistance, get_3D_corners,  # noqa: F401
                     get_camera_intrinsic, convert2cpu, convert2cpu_long, project_points_batched, adi_batched, mesh_diameter,
-                    check_pnp_args, pnp_consensus_batched)
+                    check_pnp_args, object_table, pnp_truth_and_prediction)
 from .utils_host import (makedirs, get_all_files, calc_pts_diameter, adi, get_2d_bb, corner_confidences, corner_confidence,  # noqa: F401
                          sigmoid, softmax, read_truths, read_truths_args, read_pose, load_class_names, image2torch, scale_bboxes,
                          file_lines, get_image_size, logging)
@@ -154,6 +154,30 @@ def detect_instances(output, conf_thresh, nms_thresh, num_classes, num_keypoints
     return dict(count=count, kept=kept, cls=cls, conf=boxes[..., 2 * K], cls_conf=boxes[..., 2 * K + 1], keypoints_px=uv)
 
 
+def detect_buffers(c, batch, max_instances, device):
+    """the device buffers detect_slots writes for batch x max_instances slots, as attributes of c (c.kp is the caller's)"""
+    B, M, K = batch, max_instances, 9
+    c.boxes = torch.empty(B, M, 2 * K + 3, dtype=torch.float32, device=device)
+    c.cls = torch.empty(B, M, dtype=torch.int32, device=device)
+    c.cls0 = torch.empty(B, M, dtype=torch.int32, device=device)
+    c.count = torch.empty(B, dtype=torch.int32, device=device)
+    c.kept = torch.empty(B, dtype=torch.int32, device=device)
+    c.P3 = torch.empty(B * M, K, 3, dtype=torch.float32, device=device)
+
+
+def detect_slots(c, logits, classes, points, num_classes, num_anchors, conf_thresh, nms_thresh, frame_size, stream):
+    """detect_instances into the buffers of detect_buffers and c.kp (B, M, 9, 2), then each slot's PnP points c.P3 (B*M, 9, 3)
+    gathered from points (num_classes, 9, 3) by class.  logits: the contiguous fp32 network output; classes: the requested
+    class ids, a HOST int32 array copied into the launch."""
+    B, M = c.cls.shape
+    h, w = logits.shape[2:]
+    call("ssp_detect_instances", ptr(logits), B, 9, num_classes, num_anchors, h, w, _ctypes.c_void_p(classes.ctypes.data), len(classes),
+         conf_thresh, nms_thresh, M, float(frame_size[0]), float(frame_size[1]), ptr(c.boxes), ptr(c.cls), ptr(c.kp), ptr(c.count),
+         ptr(c.kept), stream)
+    torch.clamp(c.cls, min=0, out=c.cls0)                  # empty slots hold -1: any in-range index will do, PnP skips them
+    torch.index_select(points, 0, c.cls0.view(-1), out=c.P3)
+
+
 # ------------------------------------------------------------------------------------------ tracking across frames
 MAX_TRACKS = 256            # largest max_tracks (track_core.h kMaxTracks)
 
@@ -202,32 +226,19 @@ class InstanceTracker:
     def __init__(self, objects, K, num_classes, num_anchors, frame_size, batch=1, conf_thresh=0.05, nms_thresh=0.4, max_instances=32,
                  max_tracks=64, match_iou=0.3, max_misses=5, num_keypoints=9, device=None):
         self.max_tracks, self.match_iou, self.max_misses = check_track_args(max_tracks, match_iou, max_misses)
-        if not isinstance(objects, dict):
-            objects = {0: objects}
-        nC = int(num_classes)
-        if not objects or any(isinstance(c, bool) or not isinstance(c, (int, np.integer)) or not 0 <= c < nC for c in objects):
-            raise SspError("objects must be a non-empty {class id in [0, %d): corners3D} dict" % nC)
-        Km = np.asarray(K, dtype=np.float64)
-        if Km.shape != (3, 3):
-            raise SspError("K must be (3, 3), got %s" % (Km.shape,))
+        classes, points, Km = object_table(objects if isinstance(objects, dict) else {0: objects}, num_classes, K)
         if int(num_keypoints) != 9:
             raise SspError("tracking solves PnP on the centroid + 8 box corners: 9 keypoints, not %d" % int(num_keypoints))
         self.batch, self.max_instances = int(batch), int(max_instances)
         if self.batch < 1:
             raise SspError("batch must be >= 1")
-        self.num_classes, self.num_anchors, self.num_keypoints = nC, int(num_anchors), 9
+        self.num_classes, self.num_anchors, self.num_keypoints = int(num_classes), int(num_anchors), 9
         self.frame_size = (float(frame_size[0]), float(frame_size[1]))
         self.conf_thresh, self.nms_thresh = float(conf_thresh), float(nms_thresh)
-        self.classes = np.array(sorted(objects), np.int32)
+        self.classes = classes.astype(np.int32)
         dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
         self.device = dev
-        table = np.zeros((nC, 9, 3), np.float32)
-        for c in self.classes:
-            cc = np.asarray(objects[int(c)], dtype=np.float64)
-            if cc.ndim != 2 or cc.shape[0] not in (3, 4) or cc.shape[1] != 8:
-                raise SspError("corners3D must be (3|4, 8), got %s" % (cc.shape,))
-            table[c, 1:] = cc[:3].T
-        self._P3_table = torch.from_numpy(table).to(dev)
+        self._P3_table = torch.from_numpy(points.astype(np.float32)).to(dev)
         self._K32 = torch.from_numpy(np.ascontiguousarray(Km, dtype=np.float32)).to(dev)
         B, T = self.batch, self.max_tracks
         self.state_tracks = torch.zeros(B, T, 5, dtype=torch.int32, device=dev)
@@ -305,24 +316,14 @@ class InstanceTracker:
         c = self._bufs
         if c is None:
             import types
-            dev = self.device
             c = self._bufs = types.SimpleNamespace()
-            c.boxes = torch.empty(B, M, 2 * K + 3, dtype=torch.float32, device=dev)
-            c.cls = torch.empty(B, M, dtype=torch.int32, device=dev)
-            c.cls0 = torch.empty(B, M, dtype=torch.int32, device=dev)
-            c.kp = torch.empty(B, M, K, 2, dtype=torch.float32, device=dev)
-            c.count = torch.empty(B, dtype=torch.int32, device=dev)
-            c.kept = torch.empty(B, dtype=torch.int32, device=dev)
-            c.P3 = torch.empty(B * M, K, 3, dtype=torch.float32, device=dev)
-            c.R = torch.empty(B, M, 3, 3, dtype=torch.float64, device=dev)
-            c.t = torch.empty(B, M, 3, dtype=torch.float64, device=dev)
+            detect_buffers(c, B, M, self.device)
+            c.kp = torch.empty(B, M, K, 2, dtype=torch.float32, device=self.device)
+            c.R = torch.empty(B, M, 3, 3, dtype=torch.float64, device=self.device)
+            c.t = torch.empty(B, M, 3, dtype=torch.float64, device=self.device)
             self.buffers(c)
         s = stream_ptr()
-        call("ssp_detect_instances", ptr(out), B, K, nC, nA, H, W, _ctypes.c_void_p(self.classes.ctypes.data), len(self.classes),
-             self.conf_thresh, self.nms_thresh, M, self.frame_size[0], self.frame_size[1], ptr(c.boxes), ptr(c.cls), ptr(c.kp),
-             ptr(c.count), ptr(c.kept), s)
-        torch.clamp(c.cls, min=0, out=c.cls0)
-        torch.index_select(self._P3_table, 0, c.cls0.view(-1), out=c.P3)
+        detect_slots(c, out, self.classes, self._P3_table, nC, nA, self.conf_thresh, self.nms_thresh, self.frame_size, s)
         self.solve(c, s, c.P3, self._K32)
         return dict(count=c.count, kept=c.kept, cls=c.cls, track_id=c.track_id, warm=c.warm, conf=c.boxes[..., 2 * K],
                     cls_conf=c.boxes[..., 2 * K + 1], keypoints_px=c.kp, R=c.R, t=c.t, params=c.params)
@@ -410,27 +411,15 @@ def evaluate_multi_poses_batched(output, target, conf_thresh, num_classes, num_k
     rows = tgt_d.shape[1] // nl
     cls = tgt_d[:, :rows * nl].reshape(B, rows, nl)[image, gt_index, 0].long()
     res = dict(image=image, gt_index=gt_index, cls=cls, box=box, fallback=(flags & 1) != 0, carried=(flags & 2) != 0)
-    if G == 0:                                                  # nothing to solve: empty poses and errors
-        R0 = torch.zeros(0, 3, 3, dtype=torch.float64, device=dev)
-        t0 = torch.zeros(0, 3, dtype=torch.float64, device=dev)
-        res = dict(res, R_gt=R0, t_gt=t0, R_pr=R0.clone(), t_pr=t0.clone(), pixel_err=torch.zeros(0, dtype=torch.float32, device=dev))
-        if pnp == "consensus":
-            res.update(inliers=torch.zeros(0, K, dtype=torch.bool, device=dev), hyp=torch.zeros(0, dtype=torch.int32, device=dev))
-        if adds:
-            res.update(vertex_dist=torch.zeros(0, dtype=torch.float64, device=dev), adds_dist=torch.zeros(0, dtype=torch.float64, device=dev))
-        return res
     c3 = np.asarray(corners3D, dtype=np.float64)[:3]
     P3 = np.array(np.transpose(np.concatenate((np.zeros((3, 1)), c3), axis=1)), dtype="float32")          # valid_multi.py:135
     Kc = torch.as_tensor(np.asarray(internal_calibration, dtype=np.float32)).to(dev)
-    extra = {}
-    if pnp == "consensus":
-        P3d = torch.from_numpy(P3).to(dev)
-        R_gt, t_gt = pnp_batched(P3d, uv[:G], Kc)
-        R_pr, t_pr, _p, inl, hyp = pnp_consensus_batched(P3d, uv[G:], Kc, reproj_thresh)
-        R, t = torch.cat([R_gt, R_pr]), torch.cat([t_gt, t_pr])
-        extra = dict(inliers=inl, hyp=hyp)
-    else:
-        R, t = pnp_batched(torch.from_numpy(P3).to(dev), uv, Kc)                                             # 2G problems, one launch
+    R, t, extra = pnp_truth_and_prediction(torch.from_numpy(P3).to(dev), uv, Kc, pnp, reproj_thresh)       # 2G problems
+    if G == 0:                                                  # nothing to project: empty errors
+        res = dict(res, R_gt=R, t_gt=t, R_pr=R.clone(), t_pr=t.clone(), pixel_err=torch.zeros(0, dtype=torch.float32, device=dev), **extra)
+        if adds:
+            res.update(vertex_dist=torch.zeros(0, dtype=torch.float64, device=dev), adds_dist=torch.zeros(0, dtype=torch.float64, device=dev))
+        return res
     Rt = torch.cat([R, t.unsqueeze(2)], 2)
     V = torch.as_tensor(np.asarray(vertices, dtype=np.float32)).to(dev)
     if V.shape[0] == 3:

@@ -197,7 +197,8 @@ def test_oracle_listing_is_the_reference_listing(golden_dir):
 
 # ------------------------------------------------------------------------------------------------ command line
 def test_cli_checks(tmp_path):
-    from singleshotpose_b200.predict_instances import camera_from_any_data_cfg, parse_args
+    from singleshotpose_b200.predict import read_camera
+    from singleshotpose_b200.predict_instances import SIZE_KEYS, parse_args
     base = ["--datacfg", "d.data", "--modelcfg", "m.cfg", "--weightfile", "w"]
     a = parse_args(base + ["a.png", "b.png"])
     assert a.objects is None and a.nms_thresh == 0.4 and a.max_instances == 32 and a.images == ["a.png", "b.png"]
@@ -213,14 +214,14 @@ def test_cli_checks(tmp_path):
         parse_args(["--modelcfg", "m.cfg", "--weightfile", "w", "a.png"])   # --datacfg is required
     single = tmp_path / "ape.data"
     single.write_text("mesh = ape.ply\nwidth = 640\nheight = 480\nfx = 572.4114\nfy = 573.5704\nu0 = 325.2611\nv0 = 242.0489\n")
-    mesh, Km, size = camera_from_any_data_cfg(str(single))
+    mesh, Km, size = read_camera(str(single), SIZE_KEYS)
     assert mesh == "ape.ply" and size == (640, 480) and Km[0, 0] == 572.4114 and Km[1, 2] == 242.0489
     multi = tmp_path / "occlusion.data"
     multi.write_text("mesh1 = a.ply\nim_width = 320\nim_height = 240\nfx = 1\nfy = 2\nu0 = 3\nv0 = 4\n")
-    mesh, Km, size = camera_from_any_data_cfg(str(multi))
+    mesh, Km, size = read_camera(str(multi), SIZE_KEYS)
     assert mesh is None and size == (320, 240) and Km[1, 1] == 2
     for missing in ("fx", "height"):
         q = tmp_path / ("no_%s.data" % missing)
         q.write_text("".join(l + "\n" for l in single.read_text().splitlines() if not l.startswith(missing)))
         with pytest.raises(_lib.SspError, match=missing):
-            camera_from_any_data_cfg(str(q))
+            read_camera(str(q), SIZE_KEYS)

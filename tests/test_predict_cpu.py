@@ -152,16 +152,16 @@ def test_read_ply_vertices_refuses_binary(tmp_path):
 
 
 def test_cli_data_cfg_parsing(tmp_path):
-    from singleshotpose_b200.predict import camera_from_data_cfg, main
+    from singleshotpose_b200.predict import SIZE_KEYS, main, read_camera
     p = tmp_path / "ape.data"
     p.write_text("train  = LINEMOD/ape/train.txt\nmesh = LINEMOD/ape/ape.ply\nname = ape\ndiam = 0.103\nwidth = 640\nheight = 480\n"
                  "fx = 572.4114 \nfy = 573.5704\nu0 = 325.2611\nv0 = 242.0489\n")
-    mesh, K, size = camera_from_data_cfg(str(p))
+    mesh, K, size = read_camera(str(p), SIZE_KEYS)
     assert mesh == "LINEMOD/ape/ape.ply" and size == (640, 480)
     assert np.array_equal(K, np.array([[572.4114, 0, 325.2611], [0, 573.5704, 242.0489], [0, 0, 1]]))
     q = tmp_path / "bad.data"
     q.write_text("mesh = m.ply\nwidth = 640\n")
     with pytest.raises(_lib.SspError, match="height|fx"):
-        camera_from_data_cfg(str(q))
+        read_camera(str(q), SIZE_KEYS)
     with pytest.raises(SystemExit):
         main(["--datacfg", str(p)])                       # model cfg, weights and images are required

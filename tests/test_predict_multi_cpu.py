@@ -140,22 +140,23 @@ def test_host_build_pins_to_the_reference_run(golden, host):
 
 # ------------------------------------------------------------------------------------------------ command line
 def test_cli_parsing(tmp_path):
-    from singleshotpose_b200.predict_multi import camera_from_multi_data_cfg, parse_objects, main
+    from singleshotpose_b200.predict import read_camera
+    from singleshotpose_b200.predict_multi import SIZE_KEYS, parse_objects, main
     p = tmp_path / "occlusion.data"
     p.write_text("train  = cfg/train_occlusion.txt\nmesh1 = ../LINEMOD/ape/ape.ply\ngpus = 0\nim_width = 640\nim_height = 480\n"
                  "fx = 572.4114 \nfy = 573.5704\nu0 = 325.2611\nv0 = 242.0489\n")
-    Km, size = camera_from_multi_data_cfg(str(p))
+    _mesh, Km, size = read_camera(str(p), SIZE_KEYS)
     assert size == (640, 480)
     assert np.array_equal(Km, np.array([[572.4114, 0, 325.2611], [0, 573.5704, 242.0489], [0, 0, 1]]))
     for missing in ("im_width", "im_height", "fx", "v0"):
         q = tmp_path / ("no_%s.data" % missing)
         q.write_text("".join(l + "\n" for l in p.read_text().splitlines() if not l.startswith(missing)))
         with pytest.raises(_lib.SspError, match=missing):
-            camera_from_multi_data_cfg(str(q))
+            read_camera(str(q), SIZE_KEYS)
     q = tmp_path / "single.data"
     q.write_text("mesh = m.ply\nwidth = 640\nheight = 480\nfx = 1\nfy = 1\nu0 = 1\nv0 = 1\n")   # the single-object keys are not read
     with pytest.raises(_lib.SspError, match="im_width"):
-        camera_from_multi_data_cfg(str(q))
+        read_camera(str(q), SIZE_KEYS)
     assert parse_objects(["4=can.ply", "0=a=b.ply"]) == {4: "can.ply", 0: "a=b.ply"}
     for bad in (["ape.ply"], ["x=ape.ply"], ["1="], ["-1=ape.ply"], ["=ape.ply"], ["0=a.ply", "0=b.ply"], []):
         with pytest.raises(_lib.SspError):
