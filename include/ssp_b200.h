@@ -38,7 +38,7 @@ extern "C" {
 #define SSP_EPI_F32 0    /* store fp32 */
 #define SSP_EPI_STATS 1  /* store fp32 + per-channel sum / sum of squares over valid pixels (fp64) */
 #define SSP_EPI_BIAS 2   /* add bias, store fp32 */
-#define SSP_EPI_F16 8    /* store fp16 (saturating): `out` points to 16-bit elements, out_ld in elements; data gradients only (TC / TC2 / BANDT kernels) */
+#define SSP_EPI_F16 8    /* store fp16 (saturating to +-65504, NaN stays NaN): `out` points to 16-bit elements, out_ld in elements; data gradients only (TC / TC2 / BANDT kernels) */
 #define SSP_ROUTE_NONE 0
 #define SSP_ROUTE_DIRECT 1 /* consumer has the same geometry */
 #define SSP_ROUTE_POOL 2   /* consumer is behind MaxPool2d(2,2)          (darknet.py:168-176) */

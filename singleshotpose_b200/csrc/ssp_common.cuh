@@ -69,17 +69,17 @@ __host__ __device__ inline long long flat_alloc_rows(int N, int H, int W) {
 __device__ __forceinline__ float cvt16_to_f32(uint16_t v, int fmt) {
   return fmt == FMT_F16 ? __half2float(__ushort_as_half(v)) : __bfloat162float(__ushort_as_bfloat16(v));
 }
-__device__ __forceinline__ uint16_t cvt_f32_to_16(float f, int fmt) {
-  // fp16 saturates instead of overflowing to inf (loss-scaled gradients)
-  return fmt == FMT_F16 ? __half_as_ushort(__float2half_rn(fminf(fmaxf(f, -65504.f), 65504.f)))
-                        : __bfloat16_as_ushort(__float2bfloat16_rn(f));
-}
 // fp16(clamp(f, +-65504)), round to nearest even: a conversion that would overflow gives the largest finite fp16 instead of an
 // infinity, NaN stays NaN (PTX cvt .satfinite: one instruction, like the plain conversion)
 __device__ __forceinline__ uint16_t f16_satfinite(float f) {
   uint16_t h;
   asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(h) : "f"(f));
   return h;
+}
+// the single-term 16-bit store of the backward's planes (loss-scaled gradients, dgrad weights): fp16 saturates like f16_satfinite
+// instead of overflowing to inf, and a NaN stays NaN (a clamp through fmaxf would return its finite argument, -65504, for NaN)
+__device__ __forceinline__ uint16_t cvt_f32_to_16(float f, int fmt) {
+  return fmt == FMT_F16 ? f16_satfinite(f) : __bfloat16_as_ushort(__float2bfloat16_rn(f));
 }
 // split an fp32 value into fp16 hi + fp16 lo (hi + lo carries ~22 mantissa bits).  Saturating: hi = fp16(clamp(f, +-65504)) and
 // lo = fp16(clamp(f - hi, +-65504)), so a finite f never yields an infinite part (an unclamped hi of +-inf for |f| >= 65520

@@ -611,3 +611,133 @@ def test_fp16_range_edges_conv_gemm_bnact(nt3):
     assert np.array_equal(bits16(hi), want[0][0]) and np.array_equal(bits16(lo), want[0][1])
     idx = flat_index(N, H, W)
     _check_split_planes(bits16(hi)[idx], bits16(lo)[idx], leaky(fmaf(y, scale.cpu().numpy(), shift.cpu().numpy()), 0.1).reshape(-1, cout))
+
+
+# ------------------------------------------------------------------------------------------------ NaN and saturation, single-term fp16
+# The backward's fp16 planes are stored by one conversion each (no hi/lo): the data-gradient epilogue SSP_EPI_F16 of the per-tap and
+# the operand-swapped kernels, ssp_pack_nchw without a lo plane (the loss gradient), the dY store of ssp_bn_bwd_apply and the W_d
+# planes of ssp_pack_weights and ssp_sgd_pack_step.  Each must give fp16(clamp(x, +-65504)) bit for bit and keep NaN a NaN.
+NAN_EDGES = np.array([np.nan, np.inf, -np.inf, 65519, -65519, 65520, -65520, 1e6, -1e6, 65504, -65504, 65503, -0.0, 1.5, 6e-8,
+                      -131008], F32)
+
+
+def _check_f16_sat(got_bits, x):
+    """device fp16 bits against numpy fp16(clip(x, +-65504)): NaN must come back as a NaN, everything else bit for bit"""
+    x = np.asarray(x, F32)
+    want = np.clip(x, F32(-65504), F32(65504)).astype(np.float16).view(np.uint16)
+    got = np.asarray(got_bits, np.uint16)
+    nan = np.isnan(x)
+    assert np.isnan(got[nan].view(np.float16)).all(), "NaN did not survive the fp16 conversion: %s" % got[nan].view(np.float16)
+    assert np.array_equal(got[~nan], want[~nan]), (x[~nan][got[~nan] != want[~nan]], got[~nan][got[~nan] != want[~nan]].view(np.float16))
+
+
+def _fp16_parts(v, k):
+    """k fp16 values whose exact sum is v (v a NaN / an infinity: that value, then zeros); the partial sums are integers or
+    short dyadic values well inside fp32, so a tensor-core fp32 accumulation of them is exact in any order"""
+    parts = np.zeros(k, np.float64)
+    if not np.isfinite(v):
+        parts[0] = v
+        return parts
+    r = float(v)
+    for i in range(k):
+        parts[i] = float(np.float16(np.clip(r, -65504, 65504)))
+        r -= parts[i]
+    assert r == 0.0, v
+    return parts
+
+
+@pytest.mark.parametrize("impl", [_lib.IMPL_TC2, _lib.IMPL_BANDT])
+@pytest.mark.parametrize("tail_rows", [False, True])
+def test_fp16_nan_and_saturation_data_gradient_epilogue(impl, tail_rows):
+    """SSP_EPI_F16: dX[m][c] = sum_k dY[m][k] * W_d[c][k] with dY = 1 and W_d[c] the fp16 parts of an edge value.  48 channels: the
+    per-tap kernel's packed 32-channel store and its channel tail; tail_rows: an output row count that ends inside the operand-swapped
+    kernel's last 32-row chunk (its per-row tail store)"""
+    N, H, W, K, cout = 2, 5, 7, 64, 48
+    vals = np.resize(NAN_EDGES[(NAN_EDGES != 0) & (NAN_EDGES != F32(6e-8))], cout).astype(F32)   # -0 is not a sum of products, 6e-8 not one of fp16 values
+    wd = torch.from_numpy(np.stack([_fp16_parts(v, K) for v in vals])).half().to(DEV)
+    dy, _, rows = pack_nchw(torch.ones(N, K, H, W), split=False)
+    out_rows = N * (H + 1) * (W + 1) + 5 if tail_rows else rows
+    ld = (cout + 7) // 8 * 8
+    dx = sentinel16(rows, ld)
+    call("ssp_conv_gemm", impl, ptr(dy), None, rows, K, K, ptr(wd), None, cout, K, _lib.FMT_F16, _lib.FMT_F16,
+         N, H, W, 1, cout, ptr(dx), ld, out_rows, _lib.EPI_F16, None, None, None, stream_ptr())
+    torch.cuda.synchronize()
+    idx = flat_index(N, H, W)
+    got = bits16(dx)[idx, :cout]
+    _check_f16_sat(got, np.broadcast_to(vals, got.shape))
+
+
+def test_fp16_nan_and_saturation_pack_single_term():
+    """ssp_pack_nchw with lo = NULL (the engine packs the loss gradient this way), loss scale 1 and 256"""
+    C = NAN_EDGES.size
+    x = np.ascontiguousarray(np.stack([NAN_EDGES, NAN_EDGES[::-1]]).T.reshape(1, C, 2, 1).astype(F32))
+    for scale in (1.0, 256.0):
+        hi = sentinel16(rows_of(1, 2, 1), C)
+        xd = torch.from_numpy(x).to(DEV)
+        call("ssp_pack_nchw", ptr(xd), ptr(hi), None, 1, C, 2, 1, C, 0, _lib.FMT_F16, scale, stream_ptr())
+        torch.cuda.synchronize()
+        got = bits16(hi)[flat_index(1, 2, 1)]
+        _check_f16_sat(got, x.transpose(0, 2, 3, 1).reshape(-1, C) * F32(scale))
+
+
+def test_fp16_nan_and_saturation_bn_backward_dy():
+    """ssp_bn_bwd_apply's dY store: y = 1, scale 1, shift 0 (z > 0: leaky' = 1), mean 0, invstd 1, gamma 1 and zero sums, so
+    dY = 1 * ((g + 0) - 0 - 1 * 0) = g + 0 (the second, absent source adds +0: -0 becomes +0)"""
+    N, H, W, C = 1, 2, 3, NAN_EDGES.size
+    g = np.resize(NAN_EDGES, (N, H, W, C)).astype(F32)
+    g[0, 1] = g[0, 1, :, ::-1]
+    yf, gf = flat_f32(np.ones((N, H, W, C), F32)), flat_f32(g)
+    one, zero = torch.ones(C, device=DEV), torch.zeros(C, device=DEV)
+    s1 = torch.zeros(C, dtype=torch.float64, device=DEV); s2 = torch.zeros_like(s1)
+    dy = sentinel16(rows_of(N, H, W), C)
+    call("ssp_bn_bwd_apply", ptr(yf), C, ptr(one), ptr(zero), ptr(zero), ptr(one), ptr(one), N, C, H, W, 0.1,
+         ptr(gf), C, 0, DIRECT, None, 0, 0, _lib.ROUTE_NONE, ptr(s1), ptr(s2), ptr(dy), C, _lib.FMT_F16, 1.0, stream_ptr())
+    torch.cuda.synchronize()
+    got = bits16(dy)[flat_index(N, H, W)]
+    _check_f16_sat(got, g.reshape(-1, C) + F32(0))
+
+
+def test_fp16_nan_and_saturation_weight_planes():
+    """the W_d plane [cin][taps*cout] of ssp_pack_weights and of the fused SGD + re-pack pass (vector path: cin % 4 == 0; scalar
+    path: cin = 3), with a zero step (lr = momentum = weight decay = 0): p stays p except where 0 * p is a NaN (p = +-inf)"""
+    for cout, taps, cin in [(16, 1, 64), (16, 9, 3)]:
+        n = cout * taps * cin
+        w = np.random.default_rng(cin).permutation(np.resize(NAN_EDGES, n)).reshape(cout, taps, cin).astype(F32)
+        ld_f, ld_d = (taps * cin + 7) // 8 * 8, (taps * cout + 7) // 8 * 8
+        d_want = lambda m: m.transpose(2, 1, 0)[:, ::-1, :].reshape(cin, taps * cout)       # k = (taps-1-tap)*cout + co
+        master = torch.from_numpy(w).to(DEV)
+        fh = torch.zeros(cout, ld_f, dtype=torch.float16, device=DEV); fl = torch.zeros_like(fh)
+        d = sentinel16(cin, ld_d)
+        call("ssp_pack_weights", ptr(master), cout, taps, cin, ptr(fh), ptr(fl), ld_f, ptr(d), ld_d, _lib.FMT_F16, stream_ptr())
+        torch.cuda.synchronize()
+        _check_f16_sat(bits16(d)[:, :taps * cout], d_want(w))
+        # the same plane from ssp_sgd_pack_step
+        tab = np.zeros(1, dtype=np.dtype(_lib.STRUCTS["ssp_sgd_segment"]))
+        e = tab[0]
+        d2 = sentinel16(cin, ld_d)
+        e["off"], e["n"], e["cout"], e["taps"], e["cin"], e["ld_f"], e["ld_d"], e["d_fmt"] = 0, n, cout, taps, cin, ld_f, ld_d, _lib.FMT_F16
+        e["f_hi"], e["f_lo"], e["d"], e["block0"] = fh.data_ptr(), fl.data_ptr(), d2.data_ptr(), 0
+        nb = int(_lib.load().ssp_sgd_segment_blocks(cout, taps, cin, n))
+        table = torch.from_numpy(tab.view(np.uint8).reshape(-1).copy()).to(DEV)
+        p = master.clone().reshape(-1); gz = torch.zeros_like(p); v = torch.zeros_like(p)
+        call("ssp_sgd_pack_step", ptr(table), 1, 0, nb, ptr(p), ptr(gz), ptr(v), 0.0, 0.0, 0.0, 1.0, stream_ptr())
+        torch.cuda.synchronize()
+        pw = p.cpu().numpy().reshape(cout, taps, cin)
+        assert np.isnan(pw[np.isinf(w)]).all() and np.array_equal(pw[np.isfinite(w)].view(np.uint32), w[np.isfinite(w)].view(np.uint32))
+        _check_f16_sat(bits16(d2)[:, :taps * cout], d_want(pw))
+
+
+def test_nan_in_loss_gradient_reaches_head_weight_gradient(cfg_path):
+    """end to end: one NaN element in the gradient of the logits must give NaN in the head's weight gradient (as autograd would)
+    for the output channel it belongs to, and leave the other channels finite -- not a finite gradient of arbitrary sign"""
+    from singleshotpose_b200 import Darknet, synth
+    torch.manual_seed(0)
+    m = Darknet(cfg_path).cuda().train()
+    out = m(synth.images(2, 128, 128, seed=3).cuda())
+    g = torch.zeros_like(out)
+    g[1, 0, 2, 3] = float("nan")
+    out.backward(g)
+    head = m._engine.conv_modules()[-1][0]
+    dw = head.weight.grad                                           # (20, 1024, 1, 1)
+    assert torch.isnan(dw[0]).all(), "a NaN logit gradient gave a finite weight gradient: %s" % dw[0].flatten()[:4].tolist()
+    assert torch.isfinite(dw[1:]).all()
