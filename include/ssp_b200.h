@@ -288,6 +288,31 @@ int ssp_track_commit(int B, int max_tracks, int max_det, const int* count, const
 int ssp_project_points(const float* X, int rows, int nv, const double* Rt, const double* K3x3, long long n,
                        float* out, void* stream);
 
+/* ---- cameras with lens distortion (utils.py:86-100 with pnp.distCoeffs -> cv2.solvePnP(..., distCoeffs); csrc/pnp_dist.cu).
+ *      dist8: DEVICE double [8] = OpenCV's (k1, k2, p1, p2, k3, k4, k5, k6), read in place (a graph replay sees its current values);
+ *      NULL is SSP_ERR_ARG: zero distortion is the entry points above.  The PnP undistorts the keypoints as cv2.undistortPoints does
+ *      (5 fixed-point iterations) for the DLT and fits the raw keypoints with cv2.projectPoints' distorted model in the LM.
+ *  ssp_pnp_dist: groups x per_group problems, points3d shared or [n][num_points][3] as ssp_pnp_batched.  count_or_null: DEVICE int
+ *      [groups] as ssp_pnp_batched_counted (empty slots get zeros, also in params and work), NULL to solve all.  guess_or_null with
+ *      use_guess_or_null (both or neither): warm starts as ssp_pnp_batched_guess, which need params_out.  params_out_or_null [n][6]
+ *      the final LM vector; work_out_or_null [n][3] as ssp_pnp_batched_work.  SSP_ERR_ARG for a null required pointer, num_points
+ *      outside 6..16, groups < 0, per_group < 1, guess without use_guess (or the reverse) or guess without params_out.
+ *  ssp_pnp_consensus_dist: ssp_pnp_consensus with every solve and the scoring distorted; same workspace (ssp_pnp_consensus_work_bytes),
+ *      same checks, plus a null dist8.
+ *  ssp_project_points_dist: cv2.projectPoints(X, R, t, K, dist) in ssp_project_points' layout (fp64 math, fp32 out [n][2][nv]; with
+ *      rows == 4 the translation is scaled by the homogeneous coordinate).  SSP_ERR_ARG for a null pointer, rows not 3 or 4, nv < 0
+ *      or n < 0. ---- */
+int ssp_pnp_dist(const float* points3d, int points3d_shared, const float* points2d, const float* K3x3, const double* dist8,
+                 int num_points, int groups, int per_group, const int* count_or_null, const double* guess_or_null,
+                 const int* use_guess_or_null, int max_iter, double* R_out, double* t_out, double* params_out_or_null,
+                 int* work_out_or_null, void* stream);
+int ssp_pnp_consensus_dist(const float* points3d, int points3d_shared, const float* points2d, const float* K3x3, const double* dist8,
+                           int num_points, int groups, int per_group, const int* count_or_null, const unsigned short* subsets_host,
+                           int n_subsets, double reproj_thresh, int max_iter, double* R_out, double* t_out, double* params_out,
+                           int* inliers_out, int* hyp_out, void* work, long long work_bytes, void* stream);
+int ssp_project_points_dist(const float* X, int rows, int nv, const double* Rt, const double* K3x3, const double* dist8,
+                            long long n, float* out, void* stream);
+
 /* ---- pose errors over the mesh (utils.py:50-64, valid.py:69-72, 173-177), fp64 throughout (csrc/adds.cu, csrc/adds_core.h).
  *      X [nv][3] fp64 vertices; Rt_est, Rt_gt [n][3][4] fp64 poses [R | t].
  *  ssp_adds_batched: adds_out[p] = mean_i min_j |Rt_gt[p] x_i - Rt_est[p] x_j|, the reference's adi(pts_est, pts_gt) (ADD-S, for

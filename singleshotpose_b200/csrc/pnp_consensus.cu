@@ -12,10 +12,6 @@
 
 namespace ssp {
 
-struct SubsetTable { unsigned short m[ssp_pnpc::kMaxSubsets]; };
-
-// workspace: slots [n][H+1][15] fp64, then masks [n][H+1] uint32; a multiple of 8 B, so that a buffer of fp64 elements fits it exactly
-static long long consensus_work_bytes(int H, long long n) { return (n * (H + 1) * (ssp_pnpc::kSlotDoubles * 8 + 4) + 7) / 8 * 8; }
 
 __global__ void __launch_bounds__(128) pnp_hyp_kernel(const float* __restrict__ P3, long long p3_stride, const float* __restrict__ uv,
                                                       const float* __restrict__ Kmat, int np, long long n, int max_iter, double thr2,
@@ -65,7 +61,7 @@ extern "C" {
 int ssp_pnp_consensus_work_bytes(int num_points, int n_subsets, long long n, long long* bytes_out) {
   if (!bytes_out || num_points < ssp_pnpc::kMinPoints || num_points > ssp_pnpc::kMaxPoints || n_subsets < 1 || n_subsets > ssp_pnpc::kMaxSubsets || n < 0)
     return fail_msg(SSP_ERR_ARG, "pnp_consensus_work_bytes: bad size (7 <= points <= 10, 1 <= subsets <= 210, n >= 0)");
-  *bytes_out = consensus_work_bytes(n_subsets, n);
+  *bytes_out = ssp_pnpc::work_bytes(n_subsets, n);
   return SSP_OK;
 }
 
@@ -80,7 +76,7 @@ int ssp_pnp_consensus(const float* P3, int shared, const float* uv, const float*
   if (!(thr > 0.0) || !isfinite(thr)) return fail_msg(SSP_ERR_ARG, "pnp_consensus: the threshold must be > 0 and finite");
   if (max_iter < 1) return fail_msg(SSP_ERR_ARG, "pnp_consensus: max_iter must be >= 1");
   const long long n = (long long)groups * per_group;
-  if (work_bytes < consensus_work_bytes(H, n) || ((unsigned long long)work & 7u))
+  if (work_bytes < ssp_pnpc::work_bytes(H, n) || ((unsigned long long)work & 7u))
     return fail_msg(SSP_ERR_ARG, "pnp_consensus: workspace smaller than ssp_pnp_consensus_work_bytes or not 8-B aligned");
   if (n == 0) return SSP_OK;
   SubsetTable tab = {};

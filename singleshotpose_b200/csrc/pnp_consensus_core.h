@@ -20,6 +20,8 @@
 //      cv2.solvePnP(P[inl], uv[inl], K, None, rvec, tvec, useExtrinsicGuess=True).  Otherwise: the hypothesis's pose, unrefined.
 //   Out: R, t, the final LM vector, the inlier mask of the chosen hypothesis (bit i = point i) and hyp.
 // Invariant: when hypothesis 0 has all np points as inliers, the result is bit-identical to ssp_pnp_batched.
+// With distortion coefficients (dist, 8 values, or null) every solve is cv2.solvePnP(..., distCoeffs) (pnp_solve_one's dist) and step
+// 2 scores the distorted reprojection (score); the rule is otherwise the same.
 #pragma once
 #include "pnp_core.h"
 
@@ -27,6 +29,9 @@ namespace ssp_pnpc {
 
 constexpr int kMinPoints = 7, kMaxPoints = 10, kSubsetSize = 6, kMaxSubsets = 210;
 constexpr int kSlotDoubles = 15;        // per hypothesis in the workspace: R[9], then the final LM vector (rvec, t)
+
+// workspace: slots [n][H+1][15] fp64, then masks [n][H+1] uint32; a multiple of 8 B, so that a buffer of fp64 elements fits it exactly
+SSP_HD long long work_bytes(int H, long long n) { return (n * (H + 1) * (kSlotDoubles * 8 + 4) + 7) / 8 * 8; }
 
 SSP_HD double mul(double a, double b) {
 #if defined(__CUDA_ARCH__)
@@ -86,8 +91,20 @@ SSP_HD int gather(const float* p3, const float* uv, int np, unsigned set, float*
   return n;
 }
 
-// step 2: the inlier mask of the pose (R, t) over all np points, 0 if a point has z <= 0
-SSP_HD unsigned score(const double R[9], const double t[3], const float* p3, const float* uv, const float* Kmat, int np, double thr2) {
+// cv2.projectPoints' lens model (ssp_pnp::distort) with every operation rounded on its own, in the written order
+SSP_HD void distort_rn(const double* k, double x, double y, double* xd, double* yd) {
+  const double r2 = add(mul(x, x), mul(y, y)), r4 = mul(r2, r2), r6 = mul(r4, r2);
+  const double a1 = mul(mul(2.0, x), y), a2 = add(r2, mul(mul(2.0, x), x)), a3 = add(r2, mul(mul(2.0, y), y));
+  const double cdist = add(add(add(1.0, mul(k[0], r2)), mul(k[1], r4)), mul(k[4], r6));
+  const double icdist2 = rcp(add(add(add(1.0, mul(k[5], r2)), mul(k[6], r4)), mul(k[7], r6)));
+  *xd = add(add(mul(mul(x, cdist), icdist2), mul(k[2], a1)), mul(k[3], a2));
+  *yd = add(add(mul(mul(y, cdist), icdist2), mul(k[2], a3)), mul(k[3], a1));
+}
+
+// step 2: the inlier mask of the pose (R, t) over all np points, 0 if a point has z <= 0.  dist (8, or null): the distorted
+// reprojection, xn = x*iz, yn = y*iz, (xd, yd) = distort_rn(xn, yn), du = (xd*fx + cx) - u, dv = (yd*fy + cy) - v
+SSP_HD unsigned score(const double R[9], const double t[3], const float* p3, const float* uv, const float* Kmat, int np, double thr2,
+                      const double* dist = nullptr) {
   const double fx = Kmat[0], fy = Kmat[4], cx = Kmat[2], cy = Kmat[5];
   unsigned mask = 0;
   for (int i = 0; i < np; i++) {
@@ -97,6 +114,14 @@ SSP_HD unsigned score(const double R[9], const double t[3], const float* p3, con
     const double z = add(add(add(mul(R[6], X), mul(R[7], Y)), mul(R[8], Z)), t[2]);
     if (!(z > 0.0)) return 0u;
     const double iz = rcp(z);
+    if (dist) {
+      double xd, yd;
+      distort_rn(dist, mul(x, iz), mul(y, iz), &xd, &yd);
+      const double du = sub(add(mul(xd, fx), cx), (double)uv[2 * i]);
+      const double dv = sub(add(mul(yd, fy), cy), (double)uv[2 * i + 1]);
+      if (add(mul(du, du), mul(dv, dv)) <= thr2) mask |= 1u << i;
+      continue;
+    }
     const double du = sub(add(mul(mul(fx, x), iz), cx), (double)uv[2 * i]);
     const double dv = sub(add(mul(mul(fy, y), iz), cy), (double)uv[2 * i + 1]);
     if (add(mul(du, du), mul(dv, dv)) <= thr2) mask |= 1u << i;
@@ -106,15 +131,15 @@ SSP_HD unsigned score(const double R[9], const double t[3], const float* p3, con
 
 // steps 1-2 for hypothesis h: slot [15] = R, (rvec, t); returns its inlier mask
 SSP_HD unsigned solve_hypothesis(int h, const unsigned short* masks, const float* p3, const float* uv, const float* Kmat, int np,
-                                 double thr2, int max_iter, double* slot) {
+                                 double thr2, int max_iter, double* slot, const double* dist = nullptr) {
   int work[3];
   double* R = slot;
   double* p = slot + 9;
   // one call site for every h (hypothesis 0 gathers all points, the same values): two inlined solves would double the spills
   float p3s[3 * kMaxPoints], uvs[2 * kMaxPoints];
   const int n = gather(p3, uv, np, hyp_set(h, masks, np), p3s, uvs);
-  ssp_pnp::pnp_solve_one(p3s, uvs, Kmat, n, max_iter, R, p + 3, work, nullptr, nullptr, p);
-  return score(R, p + 3, p3, uv, Kmat, np, thr2);
+  ssp_pnp::pnp_solve_one(p3s, uvs, Kmat, n, max_iter, R, p + 3, work, nullptr, nullptr, p, dist);
+  return score(R, p + 3, p3, uv, Kmat, np, thr2, dist);
 }
 
 // step 3 over the H + 1 masks of the hypotheses (stride apart)
@@ -130,13 +155,14 @@ SSP_HD int select(const unsigned* hmask, int stride, int H1) {
 // step 4 for the chosen hypothesis `hyp` (its inlier mask `inl`, slot = its workspace entry; slot0 = hypothesis 0's).
 // Writes R [9], t [3], params [6]
 SSP_HD void finish(int hyp, unsigned inl, const double* slot, const double* slot0, const unsigned short* masks, const float* p3,
-                   const float* uv, const float* Kmat, int np, int max_iter, double* R_out, double* t_out, double* params_out) {
+                   const float* uv, const float* Kmat, int np, int max_iter, double* R_out, double* t_out, double* params_out,
+                   const double* dist = nullptr) {
   const double* src = hyp < 0 ? slot0 : slot;
   if (hyp >= 0 && inl != hyp_set(hyp, masks, np) && popc(inl) >= kSubsetSize) {
     float p3s[3 * kMaxPoints], uvs[2 * kMaxPoints];
     const int n = gather(p3, uv, np, inl, p3s, uvs);
     int work[3];
-    ssp_pnp::pnp_solve_one(p3s, uvs, Kmat, n, max_iter, R_out, t_out, work, nullptr, slot + 9, params_out);
+    ssp_pnp::pnp_solve_one(p3s, uvs, Kmat, n, max_iter, R_out, t_out, work, nullptr, slot + 9, params_out, dist);
     return;
   }
   for (int i = 0; i < 9; i++) R_out[i] = src[i];
@@ -145,3 +171,7 @@ SSP_HD void finish(int hyp, unsigned inl, const double* slot, const double* slot
 }
 
 }  // namespace ssp_pnpc
+
+namespace ssp {
+struct SubsetTable { unsigned short m[ssp_pnpc::kMaxSubsets]; };       // the subset table, by value in the kernels' launch parameters
+}  // namespace ssp

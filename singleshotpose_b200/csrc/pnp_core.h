@@ -1,7 +1,7 @@
 // PnP pose recovery of ONE problem -- cv2.solvePnP(SOLVEPNP_ITERATIVE) + cv2.Rodrigues restated in fp64 (reference utils.py:86-100).
 // SSP_HD: the same source is compiled by nvcc into pnp_kernel (pnp.cu, one problem per thread) and by g++ into the CPU test harness
 // (tests/helpers/pnp_host.cpp), where it is checked against the reference-generated goldens without a GPU.
-//   1. normalise the 2-D points with K (zero distortion);
+//   1. normalise the 2-D points with K (with distortion coefficients: cv2.undistortPoints, see `undistort`);
 //   2. DLT initialisation exactly as cvFindExtrinsicCameraParams2 poses it: the 2N x 12 system on the RAW 3-D coordinates,
 //      unit-norm constraint over all 12 entries, i.e. the eigenvector of the smallest eigenvalue of the 12x12 normal matrix
 //      L^T L = [[S, 0, -Sx], [0, S, -Sy], [-Sx, -Sy, Sq]] (S = sum XX^T, Sx = sum x XX^T, ..., X = [X Y Z 1]); cyclic Jacobi in fp64;
@@ -311,12 +311,63 @@ SSP_HD bool chol_solve(double A[n][n], double b[n]) {
   return true;
 }
 
-SSP_HD double reproj_err(const double* M, const double* m, int np, const double p[6], double fx, double fy, double cx, double cy) {
+// ---- OpenCV's lens distortion, k = (k1, k2, p1, p2, k3, k4, k5, k6) as cv2 orders distCoeffs ----
+// cv2.projectPoints' model (cvProjectPoints2Internal): normalised (x', y') = (x/z, y/z) -> distorted (xd, yd); the pixel is
+// (xd*fx + cx, yd*fy + cy).  J (4, or null): d(xd, yd)/d(x', y') row-major (the matrix is symmetric: J[1] == J[2]).
+SSP_HD void distort(const double* k, double x, double y, double* xd, double* yd, double* J) {
+  const double r2 = x * x + y * y, r4 = r2 * r2, r6 = r4 * r2;
+  const double a1 = 2 * x * y, a2 = r2 + 2 * x * x, a3 = r2 + 2 * y * y;
+  const double cdist = 1 + k[0] * r2 + k[1] * r4 + k[4] * r6;
+  const double icdist2 = 1. / (1 + k[5] * r2 + k[6] * r4 + k[7] * r6);
+  *xd = x * cdist * icdist2 + k[2] * a1 + k[3] * a2;
+  *yd = y * cdist * icdist2 + k[2] * a3 + k[3] * a1;
+  if (!J) return;
+  const double g = cdist * icdist2;                 // radial factor and its derivative in r2
+  const double dg = (k[0] + 2 * k[1] * r2 + 3 * k[4] * r4) * icdist2 - g * icdist2 * (k[5] + 2 * k[6] * r2 + 3 * k[7] * r4);
+  J[0] = g + 2 * x * x * dg + 2 * k[2] * y + 6 * k[3] * x;
+  J[1] = J[2] = 2 * x * y * dg + 2 * k[2] * x + 2 * k[3] * y;
+  J[3] = g + 2 * y * y * dg + 6 * k[2] * y + 2 * k[3] * x;
+}
+
+// cv2.undistortPoints(uv, K, k) of one pixel (cvUndistortPointsInternal with its default criteria): exactly 5 fixed-point
+// iterations, not "to convergence" -- cv2's DLT starts from what 5 iterations give.  icdist < 0 gives the plain normalised point.
+SSP_HD void undistort(const double* k, double u, double v, double fx, double fy, double cx, double cy, double* xo, double* yo) {
+  const double x0 = (u - cx) * (1. / fx), y0 = (v - cy) * (1. / fy);
+  double x = x0, y = y0;
+  for (int j = 0; j < 5; j++) {
+    const double r2 = x * x + y * y;
+    const double icdist = (1 + ((k[7] * r2 + k[6]) * r2 + k[5]) * r2) / (1 + ((k[4] * r2 + k[1]) * r2 + k[0]) * r2);
+    if (icdist < 0) { x = x0; y = y0; break; }
+    const double deltaX = 2 * k[2] * x * y + k[3] * (r2 + 2 * x * x);
+    const double deltaY = k[2] * (r2 + 2 * y * y) + 2 * k[3] * x * y;
+    x = (x0 - deltaX) * icdist;
+    y = (y0 - deltaY) * icdist;
+  }
+  *xo = x; *yo = y;
+}
+
+// cv2.projectPoints of one camera-frame point (x, y, z) with distortion k -> pixel (u, v)
+SSP_HD void project_distorted(const double* k, double x, double y, double z, double fx, double fy, double cx, double cy, double* u, double* v) {
+  const double iz = 1.0 / z;
+  double xd, yd;
+  distort(k, x * iz, y * iz, &xd, &yd, nullptr);
+  *u = xd * fx + cx; *v = yd * fy + cy;
+}
+
+SSP_HD double reproj_err(const double* M, const double* m, int np, const double p[6], double fx, double fy, double cx, double cy,
+                         const double* dist = nullptr) {
   double R[9]; rodrigues(p, R, nullptr);
   double e = 0.0;
   for (int i = 0; i < np; i++) {
     const double X = M[3 * i], Y = M[3 * i + 1], Z = M[3 * i + 2];
     const double x = R[0] * X + R[1] * Y + R[2] * Z + p[3], y = R[3] * X + R[4] * Y + R[5] * Z + p[4], z = R[6] * X + R[7] * Y + R[8] * Z + p[5];
+    if (dist) {
+      double u, v;
+      project_distorted(dist, x, y, z, fx, fy, cx, cy, &u, &v);
+      const double du = u - m[2 * i], dv = v - m[2 * i + 1];
+      e += du * du + dv * dv;
+      continue;
+    }
     const double iz = 1.0 / z;
     const double du = fx * x * iz + cx - m[2 * i], dv = fy * y * iz + cy - m[2 * i + 1];
     e += du * du + dv * dv;
@@ -330,9 +381,12 @@ SSP_HD double reproj_err(const double* M, const double* m, int np, const double 
 // (rvec, t) and the DLT is skipped, as cvFindExtrinsicCameraParams2 does with useExtrinsicGuess (same LM, same max_iter, same
 // FLT_EPSILON stop).  params_out (6, or null): the final LM vector, what cv2.solvePnP returns as rvec, tvec.  Both stay in this one
 // function (not two called ones) because that keeps the code nvcc generates for guess == params_out == null unchanged.
+// dist (8, or null): OpenCV's distortion coefficients (k1, k2, p1, p2, k3, k4, k5, k6), cv2.solvePnP's distCoeffs: the DLT runs on
+// cv2.undistortPoints' normalised points (undistort), the LM residual stays in pixels against the raw points with cv2.projectPoints'
+// distorted model (distort) and its chain-rule Jacobian.  With dist == null the code is the zero-distortion solve, unchanged.
 SSP_HD void pnp_solve_one(const float* p3, const float* q, const float* Kmat, int np, int max_iter, double* R_out, double* t_out, int* work,
                           double* dbg = nullptr /*[20]: smallest eigenvalue, its eigenvector, det, initial (rvec, t) -- probes only*/,
-                          const double* guess = nullptr, double* params_out = nullptr) {
+                          const double* guess = nullptr, double* params_out = nullptr, const double* dist = nullptr) {
   const double fx = Kmat[0], fy = Kmat[4], cx = Kmat[2], cy = Kmat[5];
   double M[3 * PNP_MAXP], m[2 * PNP_MAXP];
   for (int i = 0; i < 3 * np; i++) M[i] = (double)p3[i];
@@ -350,7 +404,10 @@ SSP_HD void pnp_solve_one(const float* p3, const float* q, const float* Kmat, in
     for (int a = 0; a < 4; a++) for (int b = 0; b < 4; b++) { Bk.S[a][b] = 0.0; Bk.Sx[a][b] = 0.0; Bk.Sy[a][b] = 0.0; Bk.Sq[a][b] = 0.0; }
     for (int i = 0; i < np; i++) {
       const double X[4] = {M[3 * i], M[3 * i + 1], M[3 * i + 2], 1.0};
-      const double x = (m[2 * i] - cx) / fx, y = (m[2 * i + 1] - cy) / fy, qq = x * x + y * y;
+      double x, y;
+      if (dist) undistort(dist, m[2 * i], m[2 * i + 1], fx, fy, cx, cy, &x, &y);
+      else { x = (m[2 * i] - cx) / fx; y = (m[2 * i + 1] - cy) / fy; }
+      const double qq = x * x + y * y;
       for (int a = 0; a < 4; a++)
         for (int b = 0; b < 4; b++) {
           const double xx = X[a] * X[b];
@@ -433,16 +490,32 @@ SSP_HD void pnp_solve_one(const float* p3, const float* q, const float* Kmat, in
       const double X = M[3 * i], Y = M[3 * i + 1], Z = M[3 * i + 2];
       const double x = R[0] * X + R[1] * Y + R[2] * Z + p[3], y = R[3] * X + R[4] * Y + R[5] * Z + p[4], z = R[6] * X + R[7] * Y + R[8] * Z + p[5];
       const double iz = 1.0 / z, xn = x * iz, yn = y * iz;
-      const double eu = fx * xn + cx - m[2 * i], ev = fy * yn + cy - m[2 * i + 1];
-      err2 += eu * eu + ev * ev;
-      double ju[6], jv[6];
-      for (int j = 0; j < 3; j++) {
-        const double* d = dR + 9 * j;
-        const double dx = d[0] * X + d[1] * Y + d[2] * Z, dy = d[3] * X + d[4] * Y + d[5] * Z, dz = d[6] * X + d[7] * Y + d[8] * Z;
-        ju[j] = fx * (dx - xn * dz) * iz; jv[j] = fy * (dy - yn * dz) * iz;
+      double ju[6], jv[6], eu, ev;
+      if (dist) {
+        // d(u, v)/dp = diag(fx, fy) . d(xd, yd)/d(x', y') . d(x', y')/dp
+        double xd, yd, D[4], gx[6], gy[6];
+        distort(dist, xn, yn, &xd, &yd, D);
+        eu = xd * fx + cx - m[2 * i]; ev = yd * fy + cy - m[2 * i + 1];
+        err2 += eu * eu + ev * ev;
+        for (int j = 0; j < 3; j++) {
+          const double* d = dR + 9 * j;
+          const double dx = d[0] * X + d[1] * Y + d[2] * Z, dy = d[3] * X + d[4] * Y + d[5] * Z, dz = d[6] * X + d[7] * Y + d[8] * Z;
+          gx[j] = (dx - xn * dz) * iz; gy[j] = (dy - yn * dz) * iz;
+        }
+        gx[3] = iz; gx[4] = 0.0; gx[5] = -xn * iz;
+        gy[3] = 0.0; gy[4] = iz; gy[5] = -yn * iz;
+        for (int a = 0; a < 6; a++) { ju[a] = fx * (D[0] * gx[a] + D[1] * gy[a]); jv[a] = fy * (D[2] * gx[a] + D[3] * gy[a]); }
+      } else {
+        eu = fx * xn + cx - m[2 * i]; ev = fy * yn + cy - m[2 * i + 1];
+        err2 += eu * eu + ev * ev;
+        for (int j = 0; j < 3; j++) {
+          const double* d = dR + 9 * j;
+          const double dx = d[0] * X + d[1] * Y + d[2] * Z, dy = d[3] * X + d[4] * Y + d[5] * Z, dz = d[6] * X + d[7] * Y + d[8] * Z;
+          ju[j] = fx * (dx - xn * dz) * iz; jv[j] = fy * (dy - yn * dz) * iz;
+        }
+        ju[3] = fx * iz; ju[4] = 0.0; ju[5] = -fx * xn * iz;
+        jv[3] = 0.0; jv[4] = fy * iz; jv[5] = -fy * yn * iz;
       }
-      ju[3] = fx * iz; ju[4] = 0.0; ju[5] = -fx * xn * iz;
-      jv[3] = 0.0; jv[4] = fy * iz; jv[5] = -fy * yn * iz;
       for (int a = 0; a < 6; a++) {
         Jte[a] += ju[a] * eu + jv[a] * ev;
         for (int b = a; b < 6; b++) JtJ[a][b] += ju[a] * ju[b] + jv[a] * jv[b];
@@ -462,7 +535,7 @@ SSP_HD void pnp_solve_one(const float* p3, const float* q, const float* Kmat, in
       if (!chol_solve<6>(A, d)) { for (int a = 0; a < 6; a++) d[a] = 0.0; }
       solves++;
       for (int a = 0; a < 6; a++) p[a] = prev[a] - d[a];
-      e = reproj_err(M, m, np, p, fx, fy, cx, cy);
+      e = reproj_err(M, m, np, p, fx, fy, cx, cy, dist);
       if (!(e > prev_err)) break;
     }
     lam_lg10 = lam_lg10 - 1 < -16 ? -16 : lam_lg10 - 1;

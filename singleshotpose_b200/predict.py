@@ -37,7 +37,8 @@ import torch
 from ._lib import SspError, call, load, ptr, stream_ptr
 from .engine import Buffers
 from .image import BICUBIC
-from .utils import check_pnp_args, consensus_subsets, consensus_work_bytes, inlier_bits, keypoint_bits, object_table
+from .utils import (camera_distortion, check_pnp_args, consensus_subsets, consensus_work_bytes, distortion_tensor, inlier_bits,
+                    keypoint_bits, object_table)
 
 
 class _Chain:
@@ -71,11 +72,14 @@ class _FramePredictor:
     Each frame's head selects into S slots.  With slots=None there is one slot per requested class and slot q holds the q-th
     (PosePredictor: S = 1; MultiPosePredictor: S = Q).  With slots=M the selection detects: it fills c.cls, a device c.count and
     each slot's PnP points c.P3 (utils_multi.detect_slots), and slots >= count[b] of frame b are empty.  The tail is _solve (PnP
-    of every slot: plain, counted or consensus) and _project (each slot's class's centroid and corners under its pose).
+    of every slot: plain, counted or consensus) and _project (each slot's class's centroid and corners under its pose).  With lens
+    distortion coefficients (dist_coeffs, utils.camera_distortion) both are cv2's distorted model: the PnP fits the raw keypoints
+    (ssp_pnp_dist / ssp_pnp_consensus_dist) and the corners land on the raw frame (ssp_project_points_dist).  The coefficients are
+    a device constant read by the replay; the selection (NMS, track association) works on the raw keypoints either way.
     A subclass supplies the rest: _head_buffers(chain) allocates its selection's static buffers, _head(chain, stream) launches
     the selection after the forward and then the tail, and _outputs(chain) names the returned tensors."""
 
-    def __init__(self, model, objects, K, frame_size, shape, batch, graph, max_graphs, pnp, reproj_thresh, slots=None):
+    def __init__(self, model, objects, K, frame_size, shape, batch, graph, max_graphs, pnp, reproj_thresh, slots=None, dist_coeffs=None):
         name = type(self).__name__
         if not torch.cuda.is_available():
             raise SspError("%s needs a CUDA device (no CPU fallback)" % name)
@@ -93,6 +97,9 @@ class _FramePredictor:
         self.device = dev
         self.eng.materialize(dev)
         self.classes, points, Km = object_table(objects, self.num_classes, K)
+        dist = camera_distortion(dist_coeffs)
+        self.dist_coeffs = dist                                                  # (8,) float64, or None: no distortion
+        self._dist = None if dist is None else distortion_tensor(dist, dev)
         self._cls_host = self.classes.astype(np.int32)                          # copied into the selection's launch
         self._K32 = torch.from_numpy(np.ascontiguousarray(Km, dtype=np.float32)).to(dev)       # PnP takes float32 K (valid.py:147)
         self._K64 = torch.from_numpy(np.ascontiguousarray(Km)).to(dev)
@@ -150,10 +157,18 @@ class _FramePredictor:
         c.params, c.inliers, c.hyp); with a device c.count, frame b solves its first count[b] slots and the others get zeros"""
         B, S, K = self.batch, self.num_slots, self.num_keypoints
         if self.pnp == "consensus":
-            call("ssp_pnp_consensus", ptr(c.P3), 0, ptr(c.kp), ptr(self._K32), K, B, S, ptr(c.count), self._subsets.ctypes.data,
-                 len(self._subsets), self.reproj_thresh, 20, ptr(c.R), ptr(c.t), ptr(c.params), ptr(c.inl_mask), ptr(c.hyp),
-                 ptr(c.pnp_work), c.pnp_work.numel() * 8, s)
+            if self._dist is None:
+                call("ssp_pnp_consensus", ptr(c.P3), 0, ptr(c.kp), ptr(self._K32), K, B, S, ptr(c.count), self._subsets.ctypes.data,
+                     len(self._subsets), self.reproj_thresh, 20, ptr(c.R), ptr(c.t), ptr(c.params), ptr(c.inl_mask), ptr(c.hyp),
+                     ptr(c.pnp_work), c.pnp_work.numel() * 8, s)
+            else:
+                call("ssp_pnp_consensus_dist", ptr(c.P3), 0, ptr(c.kp), ptr(self._K32), ptr(self._dist), K, B, S, ptr(c.count),
+                     self._subsets.ctypes.data, len(self._subsets), self.reproj_thresh, 20, ptr(c.R), ptr(c.t), ptr(c.params),
+                     ptr(c.inl_mask), ptr(c.hyp), ptr(c.pnp_work), c.pnp_work.numel() * 8, s)
             inlier_bits(c.inl_mask, self._bits, out=c.inliers)
+        elif self._dist is not None:                # plain or counted (c.count None: every slot)
+            call("ssp_pnp_dist", ptr(c.P3), 0, ptr(c.kp), ptr(self._K32), ptr(self._dist), K, B, S, ptr(c.count), None, None, 20, ptr(c.R),
+                 ptr(c.t), None, None, s)
         elif c.count is None:
             call("ssp_pnp_batched", ptr(c.P3), 0, ptr(c.kp), ptr(self._K32), K, B * S, 20, ptr(c.R), ptr(c.t), None, s)
         else:
@@ -166,7 +181,10 @@ class _FramePredictor:
         c.Rt[..., 3].copy_(c.t)
         # every requested class's points under every slot's pose (each point is projected on its own, so a slot's own columns are
         # what ssp_project_points gives for its class's (4, 9) points alone); each slot keeps the columns of its class
-        call("ssp_project_points", ptr(self._X), 4, Q * K, ptr(c.Rt), ptr(self._K64), B * S, ptr(c.proj), s)
+        if self._dist is None:
+            call("ssp_project_points", ptr(self._X), 4, Q * K, ptr(c.Rt), ptr(self._K64), B * S, ptr(c.proj), s)
+        else:
+            call("ssp_project_points_dist", ptr(self._X), 4, Q * K, ptr(c.Rt), ptr(self._K64), ptr(self._dist), B * S, ptr(c.proj), s)
         if not self._detects:                      # slot q: class q
             c.corners.copy_(torch.diagonal(c.proj.view(B, S, 2, Q, K), dim1=1, dim2=3).permute(0, 3, 2, 1))
             return
@@ -319,12 +337,14 @@ class PosePredictor(_FramePredictor):
     graph=False runs the same launches eagerly (no capture).
     pnp="consensus" solves each pose with the consensus PnP (utils.pnp_consensus_batched): a pose that survives one or two wrong
     keypoints, with inlier keypoints within reproj_thresh frame pixels; the outputs then add inliers (B, 9) bool and hyp (B,) int32.
-    pnp="plain" (default) is the all-point solve."""
+    pnp="plain" (default) is the all-point solve.
+    dist_coeffs: the camera's OpenCV distortion coefficients (k1, k2, p1, p2[, k3[, k4, k5, k6]]): the pose is cv2.solvePnP(...,
+    distCoeffs) of the raw keypoints and corners_px is cv2.projectPoints with them, on the raw frame; None or all zeros: no distortion."""
 
     def __init__(self, model, corners3D, K, frame_size=(640, 480), shape=None, batch=1, graph=True, max_graphs=4, pnp="plain",
-                 reproj_thresh=8.0):
+                 reproj_thresh=8.0, dist_coeffs=None):
         super().__init__(model, {0: corners3D}, K, frame_size, shape if shape is not None else (model.test_width, model.test_height),
-                         batch, graph, max_graphs, pnp, reproj_thresh)
+                         batch, graph, max_graphs, pnp, reproj_thresh, dist_coeffs=dist_coeffs)
 
     def _head_buffers(self, c):
         dev, B, K = self.device, self.batch, self.num_keypoints
@@ -353,6 +373,29 @@ def add_pnp_args(ap):
     ap.add_argument("--pnp", choices=("plain", "consensus"), default="plain",
                     help="consensus: a pose that survives wrong keypoints (PnP over keypoint subsets); adds inliers and hyp columns")
     ap.add_argument("--reproj-thresh", type=float, default=8.0, help="inlier threshold of --pnp consensus, frame pixels")
+
+
+def add_dist_arg(ap):
+    ap.add_argument("--dist", type=float, nargs="+", metavar="K",
+                    help="the camera's OpenCV distortion coefficients k1 k2 p1 p2 [k3 [k4 k5 k6]] (cv2.calibrateCamera's distCoeffs); "
+                         "overrides the .data file's dist entry.  End the list with -- when the images follow it")
+
+
+def camera_dist(args):
+    """the distortion coefficients of a command line: --dist if given, else the .data file's optional `dist = k1 k2 p1 p2 [k3 [k4 k5
+    k6]]` entry (the flag's values, separated by spaces or commas) -> utils.camera_distortion's (8,) float64 array, or None for
+    neither (or all zeros).  SspError for a count other than 4, 5 or 8 or a value that is not a finite number."""
+    if args.dist is not None:
+        return camera_distortion(args.dist)
+    from .utils_host import read_data_cfg
+    text = read_data_cfg(args.datacfg).get("dist")
+    if text is None:
+        return None
+    try:
+        values = [float(v) for v in text.replace(",", " ").split()]
+    except ValueError:
+        raise SspError("%s: dist must be numbers k1 k2 p1 p2 [k3 [k4 k5 k6]], got %r" % (args.datacfg, text))
+    return camera_distortion(values)
 
 
 def read_camera(datacfg, size_keys):
@@ -399,9 +442,11 @@ def main(argv=None):
     ap.add_argument("--weightfile", required=True)
     ap.add_argument("--out", default="poses.npz")
     add_pnp_args(ap)
+    add_dist_arg(ap)
     ap.add_argument("images", nargs="+")
     a = ap.parse_args(argv)
     check_pnp_args(a.pnp, a.reproj_thresh)
+    dist = camera_dist(a)
     from .darknet import Darknet
     mesh, K, size = read_camera(a.datacfg, SIZE_KEYS)
     if mesh is None:
@@ -410,7 +455,7 @@ def main(argv=None):
     model = Darknet(a.modelcfg)
     model.load_weights(a.weightfile)
     model.cuda().eval()
-    pred = PosePredictor(model, corners3D, K, frame_size=size, pnp=a.pnp, reproj_thresh=a.reproj_thresh)
+    pred = PosePredictor(model, corners3D, K, frame_size=size, pnp=a.pnp, reproj_thresh=a.reproj_thresh, dist_coeffs=dist)
     res = {k: [] for k in ("R", "t", "conf", "keypoints_px", "corners_px") + CONSENSUS_KEYS[a.pnp]}
     for r in predict_files(pred, a.images):
         for k in res:

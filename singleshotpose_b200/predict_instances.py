@@ -42,9 +42,9 @@ import torch
 
 from . import predict, predict_multi
 from ._lib import SspError
-from .predict import CONSENSUS_KEYS, _FramePredictor, add_pnp_args, mesh_corners, predict_files, read_camera
+from .predict import CONSENSUS_KEYS, _FramePredictor, add_dist_arg, add_pnp_args, camera_dist, mesh_corners, predict_files, read_camera
 from .predict_multi import cfg_conf_thresh, check_grid, parse_objects
-from .utils import check_pnp_args
+from .utils import camera_distortion, check_pnp_args
 from .utils_multi import InstanceTracker, check_track_args, detect_buffers, detect_slots
 
 MAX_INSTANCES = 256         # largest max_instances (detect_core.h kMaxInstances)
@@ -64,10 +64,11 @@ class InstancePosePredictor(_FramePredictor):
     cls_conf (B, M), keypoints_px (B, M, 9, 2), corners_px (B, M, 9, 2)): device tensors, or numpy with to_host=True.
     pnp="consensus" solves each slot with the consensus PnP (utils.pnp_consensus_batched, inliers within reproj_thresh frame
     pixels) and adds inliers (B, M, 9) bool and hyp (B, M) int32 (empty slots: False and 0); pnp="plain" (default) is the all-point
-    solve."""
+    solve.  dist_coeffs: the camera's OpenCV distortion coefficients, as predict.PosePredictor takes them (the suppression still
+    compares the raw keypoints' rectangles)."""
 
     def __init__(self, model, objects, K, frame_size=(640, 480), shape=None, batch=1, conf_thresh=None, nms_thresh=0.4, max_instances=32,
-                 graph=True, max_graphs=4, pnp="plain", reproj_thresh=8.0):
+                 graph=True, max_graphs=4, pnp="plain", reproj_thresh=8.0, dist_coeffs=None):
         self.num_anchors = int(getattr(model, "num_anchors", 0))
         if self.num_anchors < 1:
             raise SspError("InstancePosePredictor needs a model with a region head")
@@ -76,7 +77,7 @@ class InstancePosePredictor(_FramePredictor):
         if shape is None:
             shape = (model.test_width, model.test_height) if self.num_anchors == 1 else (model.width, model.height)
         super().__init__(model, objects if isinstance(objects, dict) else {0: objects}, K, frame_size, shape, batch, graph, max_graphs,
-                         pnp, reproj_thresh, slots=self.max_instances)
+                         pnp, reproj_thresh, slots=self.max_instances, dist_coeffs=dist_coeffs)
         check_grid(self, "detect")
 
     def _head_buffers(self, c):
@@ -106,15 +107,19 @@ class TrackingPosePredictor(InstancePosePredictor):
     Returns InstancePosePredictor's dict plus track_id (B, M) int32 (-1 in empty and untracked slots) and warm (B, M) bool (the
     slot's solve started from its track's pose).  The track state is shared by every frame size and source (one set of device
     arrays, zeroed in place by reset); the warm-up runs before a graph capture do not advance it.
-    Only pnp="plain": the consensus solve has no rule yet for how a track's warm guess competes with its subset hypotheses."""
+    Only pnp="plain": the consensus solve has no rule yet for how a track's warm guess competes with its subset hypotheses.
+    dist_coeffs: the camera's OpenCV distortion coefficients; the warm and the cold solves both use them, the association compares
+    the raw keypoints' rectangles."""
 
     def __init__(self, model, objects, K, frame_size=(640, 480), shape=None, batch=1, conf_thresh=None, nms_thresh=0.4, max_instances=32,
-                 max_tracks=64, match_iou=0.3, max_misses=5, graph=True, max_graphs=4, pnp="plain"):
+                 max_tracks=64, match_iou=0.3, max_misses=5, graph=True, max_graphs=4, pnp="plain", dist_coeffs=None):
         check_tracking_pnp(pnp)
         check_track_args(max_tracks, match_iou, max_misses)
-        super().__init__(model, objects, K, frame_size, shape, batch, conf_thresh, nms_thresh, max_instances, graph, max_graphs)
+        super().__init__(model, objects, K, frame_size, shape, batch, conf_thresh, nms_thresh, max_instances, graph, max_graphs,
+                         dist_coeffs=dist_coeffs)
         self._tracker = InstanceTracker(objects, K, self.num_classes, self.num_anchors, self.frame_size, self.batch, self.conf_thresh,
-                                        self.nms_thresh, self.max_instances, max_tracks, match_iou, max_misses, device=self.device)
+                                        self.nms_thresh, self.max_instances, max_tracks, match_iou, max_misses, device=self.device,
+                                        dist_coeffs=dist_coeffs)
         self.max_tracks, self.match_iou, self.max_misses = self._tracker.max_tracks, self._tracker.match_iou, self._tracker.max_misses
 
     def reset(self, streams=None):
@@ -165,7 +170,7 @@ SIZE_KEYS = predict_multi.SIZE_KEYS + predict.SIZE_KEYS      # a multi-object .d
 
 def parse_args(argv=None):
     """the command line, checked before any model is built: raises SspError for a bad --object, --nms-thresh, --max-instances,
-    --match-iou, --max-misses, --max-tracks or --reproj-thresh, and for --track with --pnp consensus"""
+    --match-iou, --max-misses, --max-tracks, --reproj-thresh or --dist, and for --track with --pnp consensus"""
     ap = argparse.ArgumentParser(prog="python -m singleshotpose_b200.predict_instances",
                                  description="6-D pose of every detected instance of the requested objects in each image")
     ap.add_argument("--datacfg", required=True, help=".data file: fx fy u0 v0 and width height (or im_width im_height); mesh")
@@ -182,6 +187,7 @@ def parse_args(argv=None):
     ap.add_argument("--max-misses", type=int, default=5)
     ap.add_argument("--max-tracks", type=int, default=64)
     add_pnp_args(ap)
+    add_dist_arg(ap)
     ap.add_argument("images", nargs="+")
     a = ap.parse_args(argv)
     check_pnp_args(a.pnp, a.reproj_thresh)
@@ -190,6 +196,8 @@ def parse_args(argv=None):
     check_detect_args(a.nms_thresh, a.max_instances)
     check_track_args(a.max_tracks, a.match_iou, a.max_misses)
     a.objects = parse_objects(a.object) if a.object else None
+    if a.dist is not None:
+        camera_distortion(a.dist)
     return a
 
 
@@ -204,6 +212,7 @@ def _region_anchors(modelcfg):
 def main(argv=None):
     a = parse_args(argv)
     mesh, K, size = read_camera(a.datacfg, SIZE_KEYS)
+    dist = camera_dist(a)
     meshes = a.objects
     if meshes is None:
         if not mesh:
@@ -219,10 +228,10 @@ def main(argv=None):
     model.cuda().eval()
     if a.track:
         pred = TrackingPosePredictor(model, objects, K, frame_size=size, nms_thresh=a.nms_thresh, max_instances=a.max_instances,
-                                     max_tracks=a.max_tracks, match_iou=a.match_iou, max_misses=a.max_misses)
+                                     max_tracks=a.max_tracks, match_iou=a.match_iou, max_misses=a.max_misses, dist_coeffs=dist)
     else:
         pred = InstancePosePredictor(model, objects, K, frame_size=size, nms_thresh=a.nms_thresh, max_instances=a.max_instances,
-                                     pnp=a.pnp, reproj_thresh=a.reproj_thresh)
+                                     pnp=a.pnp, reproj_thresh=a.reproj_thresh, dist_coeffs=dist)
     rows = {k: [] for k in ROW_KEYS + (("track_id",) if a.track else ()) + CONSENSUS_KEYS[a.pnp]}
     image = []
     for i, r in enumerate(predict_files(pred, a.images)):

@@ -32,7 +32,7 @@ import numpy as np
 import torch
 
 from ._lib import SspError, call, ptr
-from .predict import CONSENSUS_KEYS, _FramePredictor, add_pnp_args, mesh_corners, predict_files, read_camera
+from .predict import CONSENSUS_KEYS, _FramePredictor, add_dist_arg, add_pnp_args, camera_dist, mesh_corners, predict_files, read_camera
 from .utils import check_pnp_args
 
 MAX_ENTRIES = 4096          # H*W*num_anchors the select kernel keeps in shared memory (eval_multi_core.h kMaxEntries)
@@ -49,16 +49,17 @@ class MultiPosePredictor(_FramePredictor):
     Returns dict(classes (Q,), R (B, Q, 3, 3) fp64, t (B, Q, 3) fp64, conf (B, Q) det_conf of the box, cls_conf (B, Q),
     detected (B, Q) bool, keypoints_px (B, Q, 9, 2), corners_px (B, Q, 9, 2)): device tensors, or numpy with to_host=True.
     pnp="consensus" solves each slot with the consensus PnP (utils.pnp_consensus_batched, inliers within reproj_thresh frame
-    pixels) and adds inliers (B, Q, 9) bool and hyp (B, Q) int32; pnp="plain" (default) is the all-point solve."""
+    pixels) and adds inliers (B, Q, 9) bool and hyp (B, Q) int32; pnp="plain" (default) is the all-point solve.
+    dist_coeffs: the camera's OpenCV distortion coefficients, as predict.PosePredictor takes them."""
 
     def __init__(self, model, objects, K, frame_size=(640, 480), shape=None, batch=1, conf_thresh=None, graph=True, max_graphs=4,
-                 pnp="plain", reproj_thresh=8.0):
+                 pnp="plain", reproj_thresh=8.0, dist_coeffs=None):
         self.num_anchors = int(getattr(model, "num_anchors", 0))
         if self.num_anchors < 2:
             raise SspError("MultiPosePredictor needs a multi-anchor region head (yolo-pose-multi.cfg), got %d anchor(s)" % self.num_anchors)
         self.conf_thresh = cfg_conf_thresh(model, conf_thresh)
         super().__init__(model, objects, K, frame_size, shape if shape is not None else (model.width, model.height), batch, graph,
-                         max_graphs, pnp, reproj_thresh)
+                         max_graphs, pnp, reproj_thresh, dist_coeffs=dist_coeffs)
         check_grid(self, "select")
         self._classes = torch.from_numpy(self.classes).to(self.device)
 
@@ -134,16 +135,18 @@ def main(argv=None):
                     help="a class id of the model and the mesh of its object; repeat for every object to predict")
     ap.add_argument("--out", default="poses.npz")
     add_pnp_args(ap)
+    add_dist_arg(ap)
     ap.add_argument("images", nargs="+")
     a = ap.parse_args(argv)
     check_pnp_args(a.pnp, a.reproj_thresh)
+    dist = camera_dist(a)
     from .darknet_multi import Darknet
     _mesh, K, size = read_camera(a.datacfg, SIZE_KEYS)
     objects = {c: mesh_corners(mesh) for c, mesh in parse_objects(a.object).items()}
     model = Darknet(a.modelcfg)
     model.load_weights(a.weightfile)
     model.cuda().eval()
-    pred = MultiPosePredictor(model, objects, K, frame_size=size, pnp=a.pnp, reproj_thresh=a.reproj_thresh)
+    pred = MultiPosePredictor(model, objects, K, frame_size=size, pnp=a.pnp, reproj_thresh=a.reproj_thresh, dist_coeffs=dist)
     res = {k: [] for k in OUTPUT_KEYS + CONSENSUS_KEYS[a.pnp]}
     for r in predict_files(pred, a.images):
         for k in res:

@@ -98,8 +98,42 @@ def _pnp_inputs(points_3D, points_2D, cameraMatrix):
     return P3, uv.unsqueeze(0) if uv.dim() == 2 else uv, K
 
 
-def pnp_batched(points_3D, points_2D, cameraMatrix, max_iter=20, return_iters=False):
-    """points_3D (P,3) shared or (n,P,3); points_2D (n,P,2); K (3,3) -> R (n,3,3) f64, t (n,3) f64 CUDA tensors."""
+def camera_distortion(d):
+    """OpenCV distortion coefficients (k1, k2, p1, p2[, k3[, k4, k5, k6]]), as cv2.calibrateCamera returns them -> (8,) float64
+    numpy array, zero-padded; None for None, an empty input or all zeros (the zero-distortion solve).  Any shape that flattens to
+    4, 5 or 8 values; float32 input keeps its float32 values, as cv2 does.  SspError for 12 or 14 coefficients (the thin-prism and
+    tilted models), any other count, or a value that is not finite."""
+    if d is None:
+        return None
+    a = d.detach().cpu().numpy() if torch.is_tensor(d) else np.asarray(d)
+    a = a.reshape(-1)
+    if a.size == 0:
+        return None
+    if a.size in (12, 14):
+        raise SspError("%d distortion coefficients: the thin-prism / tilted models are not supported (4, 5 or 8)" % a.size)
+    if a.size not in (4, 5, 8):
+        raise SspError("distortion coefficients are (k1, k2, p1, p2[, k3[, k4, k5, k6]]): 4, 5 or 8 values, got %d" % a.size)
+    try:
+        a = a.astype(np.float64)
+    except (TypeError, ValueError):
+        raise SspError("distortion coefficients must be numbers, got %r" % (d,))
+    if not np.isfinite(a).all():
+        raise SspError("distortion coefficients must be finite, got %s" % (a,))
+    if not a.any():
+        return None
+    return np.concatenate([a, np.zeros(8 - a.size)])
+
+
+def distortion_tensor(k, dev):
+    """camera_distortion's (8,) array -> the DEVICE double[8] the *_dist entry points read"""
+    return torch.from_numpy(np.ascontiguousarray(k, np.float64)).to(dev)
+
+
+def pnp_batched(points_3D, points_2D, cameraMatrix, max_iter=20, return_iters=False, dist_coeffs=None):
+    """points_3D (P,3) shared or (n,P,3); points_2D (n,P,2); K (3,3) -> R (n,3,3) f64, t (n,3) f64 CUDA tensors.
+    dist_coeffs: OpenCV distortion coefficients (camera_distortion), cv2.solvePnP's distCoeffs (ssp_pnp_dist); None or all zeros
+    is the zero-distortion solve (ssp_pnp_batched)."""
+    k = camera_distortion(dist_coeffs)
     P3, uv, K = _pnp_inputs(points_3D, points_2D, cameraMatrix)
     dev = uv.device
     n, npts = uv.shape[0], uv.shape[1]
@@ -107,6 +141,11 @@ def pnp_batched(points_3D, points_2D, cameraMatrix, max_iter=20, return_iters=Fa
     assert P3.shape[-2] == npts and P3.shape[-1] == 3 and uv.shape[-1] == 2
     R = torch.empty(n, 3, 3, dtype=torch.float64, device=dev)
     t = torch.empty(n, 3, dtype=torch.float64, device=dev)
+    if k is not None:
+        work = torch.empty(n, 3, dtype=torch.int32, device=dev) if return_iters else None
+        call("ssp_pnp_dist", ptr(P3), 1 if shared else 0, ptr(uv), ptr(K), ptr(distortion_tensor(k, dev)), npts, n, 1, None, None, None,
+             max_iter, ptr(R), ptr(t), None, ptr(work), stream_ptr())
+        return (R, t, work[:, 1]) if return_iters else (R, t)
     iters = torch.empty(n, dtype=torch.int32, device=dev) if return_iters else None
     call("ssp_pnp_batched", ptr(P3), 1 if shared else 0, ptr(uv), ptr(K), npts, n, max_iter, ptr(R), ptr(t), ptr(iters), stream_ptr())
     return (R, t, iters) if return_iters else (R, t)
@@ -134,11 +173,18 @@ def object_table(objects, num_classes, K):
     return np.array(classes, dtype=np.int64), points, Km
 
 
-def pnp(points_3D, points_2D, cameraMatrix):
-    """Same contract as utils.py:86-100: numpy in, R (3,3) float64 and t (3,1) float64 out."""
+def pnp_one(points_3D, points_2D, cameraMatrix, distCoeffs=None):
+    """one problem of pnp_batched: numpy in, R (3,3) float64 and t (3,1) float64 out"""
     assert points_3D.shape[0] == points_2D.shape[0], "points 3D and points 2D must have same number of vertices"
-    R, t = pnp_batched(points_3D, np.ascontiguousarray(points_2D[:, :2]), cameraMatrix)
+    R, t = pnp_batched(points_3D, np.ascontiguousarray(points_2D[:, :2]), cameraMatrix, dist_coeffs=distCoeffs)
     return R[0].cpu().numpy(), t[0].cpu().numpy().reshape(3, 1)
+
+
+def pnp(points_3D, points_2D, cameraMatrix):
+    """Same contract as utils.py:86-100: numpy in, R (3,3) float64 and t (3,1) float64 out.  Like the reference, the distortion
+    coefficients are the function attribute pnp.distCoeffs (cv2's 4, 5 or 8 values, camera_distortion); unset or all zeros is the
+    zero-distortion solve."""
+    return pnp_one(points_3D, points_2D, cameraMatrix, getattr(pnp, "distCoeffs", None))
 
 
 # ------------------------------------------------------------------------------------------ consensus pose (csrc/pnp_consensus_core.h)
@@ -182,7 +228,7 @@ def consensus_subsets(point_sets, size=6):
     return np.array(out, np.uint16)
 
 
-def pnp_consensus_batched(points_3D, points_2D, cameraMatrix, reproj_thresh=8.0, max_iter=20, subsets=None):
+def pnp_consensus_batched(points_3D, points_2D, cameraMatrix, reproj_thresh=8.0, max_iter=20, subsets=None, dist_coeffs=None):
     """Consensus PnP of n problems on the GPU (ssp_pnp_consensus, rule: csrc/pnp_consensus_core.h): the plain all-point solve and
     one cold solve per 6-point subset, each scored by its inliers (squared reprojection error <= reproj_thresh^2 px^2, none if a
     point lies behind the camera); the best is refined on its inliers.  A pose that survives one or two wrong keypoints; where
@@ -190,8 +236,11 @@ def pnp_consensus_batched(points_3D, points_2D, cameraMatrix, reproj_thresh=8.0,
     points_3D (P,3) shared or (n,P,3), 7 <= P <= 10; points_2D (n,P,2); K (3,3); reproj_thresh in pixels (8, cv2.solvePnPRansac's
     default); subsets: (H,) uint16 masks, default consensus_subsets(points_3D).
     -> R (n,3,3) f64, t (n,3) f64, params (n,6) f64 (rvec, t), inliers (n,P) bool, hyp (n,) int32 (the chosen hypothesis: 0 the
-    all-point solve, h the subset subsets[h-1], -1 none had an inlier), CUDA tensors."""
+    all-point solve, h the subset subsets[h-1], -1 none had an inlier), CUDA tensors.
+    dist_coeffs: OpenCV distortion coefficients (camera_distortion): every solve is cv2.solvePnP(..., distCoeffs) and the inliers
+    are scored on the distorted reprojection (ssp_pnp_consensus_dist); None or all zeros is ssp_pnp_consensus."""
     _, thr = check_pnp_args("consensus", reproj_thresh)
+    k = camera_distortion(dist_coeffs)
     P3, uv, K = _pnp_inputs(points_3D, points_2D, cameraMatrix)
     dev = uv.device
     n, npts = uv.shape[0], uv.shape[1]
@@ -208,8 +257,13 @@ def pnp_consensus_batched(points_3D, points_2D, cameraMatrix, reproj_thresh=8.0,
     hyp = torch.empty(n, dtype=torch.int32, device=dev)
     wb = consensus_work_bytes(npts, len(tab), n)
     work = torch.empty(max(wb, 8) // 8, dtype=torch.float64, device=dev)
-    call("ssp_pnp_consensus", ptr(P3), 1 if shared else 0, ptr(uv), ptr(K), npts, n, 1, None, tab.ctypes.data, len(tab), thr, max_iter,
-         ptr(R), ptr(t), ptr(params), ptr(inl), ptr(hyp), ptr(work), work.numel() * 8, stream_ptr())
+    if k is None:
+        call("ssp_pnp_consensus", ptr(P3), 1 if shared else 0, ptr(uv), ptr(K), npts, n, 1, None, tab.ctypes.data, len(tab), thr, max_iter,
+             ptr(R), ptr(t), ptr(params), ptr(inl), ptr(hyp), ptr(work), work.numel() * 8, stream_ptr())
+    else:
+        call("ssp_pnp_consensus_dist", ptr(P3), 1 if shared else 0, ptr(uv), ptr(K), ptr(distortion_tensor(k, dev)), npts, n, 1, None,
+             tab.ctypes.data, len(tab), thr, max_iter, ptr(R), ptr(t), ptr(params), ptr(inl), ptr(hyp), ptr(work), work.numel() * 8,
+             stream_ptr())
     return R, t, params, inlier_bits(inl, keypoint_bits(npts, dev)), hyp
 
 
@@ -232,16 +286,20 @@ def inlier_bits(mask, bits, out=None):
     return torch.ne(torch.bitwise_and(mask.unsqueeze(-1), bits), 0, out=out)
 
 
-def pnp_consensus(points_3D, points_2D, cameraMatrix, reproj_thresh=8.0):
+def pnp_consensus(points_3D, points_2D, cameraMatrix, reproj_thresh=8.0, dist_coeffs=None):
     """pnp's contract (numpy in, R (3,3) and t (3,1) float64 out) with the consensus solve of pnp_consensus_batched, plus the
-    indices of the inlier keypoints (int64, ascending)."""
+    indices of the inlier keypoints (int64, ascending).  dist_coeffs: as pnp_consensus_batched."""
     assert points_3D.shape[0] == points_2D.shape[0], "points 3D and points 2D must have same number of vertices"
-    R, t, _p, inl, _h = pnp_consensus_batched(points_3D, np.ascontiguousarray(points_2D[:, :2]), cameraMatrix, reproj_thresh)
+    R, t, _p, inl, _h = pnp_consensus_batched(points_3D, np.ascontiguousarray(points_2D[:, :2]), cameraMatrix, reproj_thresh,
+                                              dist_coeffs=dist_coeffs)
     return R[0].cpu().numpy(), t[0].cpu().numpy().reshape(3, 1), np.nonzero(inl[0].cpu().numpy())[0]
 
 
-def project_points_batched(points_3D, Rt, internal_calibration):
-    """points_3D (3|4, Nv); Rt (n,3,4) -> (n, 2, Nv) float32 CUDA tensor (compute_projection for n poses)."""
+def project_points_batched(points_3D, Rt, internal_calibration, dist_coeffs=None):
+    """points_3D (3|4, Nv); Rt (n,3,4) -> (n, 2, Nv) float32 CUDA tensor (compute_projection for n poses).  dist_coeffs: OpenCV
+    distortion coefficients (camera_distortion): cv2.projectPoints with them (ssp_project_points_dist), the pixels of the raw,
+    distorted frame; None or all zeros is compute_projection."""
+    k = camera_distortion(dist_coeffs)
     dev = _dev()
     X = torch.as_tensor(points_3D).to(dev, torch.float32).contiguous()
     T = torch.as_tensor(Rt).to(dev, torch.float64).contiguous()
@@ -250,7 +308,10 @@ def project_points_batched(points_3D, Rt, internal_calibration):
         T = T.unsqueeze(0)
     n, nv = T.shape[0], X.shape[1]
     out = torch.empty(n, 2, nv, dtype=torch.float32, device=dev)
-    call("ssp_project_points", ptr(X), X.shape[0], nv, ptr(T), ptr(K), n, ptr(out), stream_ptr())
+    if k is None:
+        call("ssp_project_points", ptr(X), X.shape[0], nv, ptr(T), ptr(K), n, ptr(out), stream_ptr())
+    else:
+        call("ssp_project_points_dist", ptr(X), X.shape[0], nv, ptr(T), ptr(K), ptr(distortion_tensor(k, dev)), n, ptr(out), stream_ptr())
     return out
 
 
@@ -363,10 +424,10 @@ def pose_label_rows(corners3D, Rt, K, width, height, class_id=0):
 
 
 # ------------------------------------------------------------------------------------------ batched evaluation tail
-def pnp_truth_and_prediction(P3, uv, K, pnp, reproj_thresh):
+def pnp_truth_and_prediction(P3, uv, K, pnp, reproj_thresh, dist_coeffs=None):
     """The poses of n ground truths uv[:n] and n predictions uv[n:] (uv (2n, P, 2)) -> R (2n, 3, 3), t (2n, 3) fp64 and the
     predictions' inliers (n, P) and hyp (n,) for pnp="consensus" ({} for "plain").  The ground truth is always the plain solve;
-    "plain" solves all 2n problems in one launch."""
+    "plain" solves all 2n problems in one launch.  dist_coeffs: both solves with these distortion coefficients (pnp_batched)."""
     dev, n = uv.device, len(uv) // 2
     if n == 0:                                  # nothing to launch: the PnP entry points take no empty (null) buffers
         R, t = torch.zeros(0, 3, 3, dtype=torch.float64, device=dev), torch.zeros(0, 3, dtype=torch.float64, device=dev)
@@ -374,15 +435,15 @@ def pnp_truth_and_prediction(P3, uv, K, pnp, reproj_thresh):
             return R, t, {}
         return R, t, dict(inliers=torch.zeros(0, uv.shape[1], dtype=torch.bool, device=dev), hyp=torch.zeros(0, dtype=torch.int32, device=dev))
     if pnp != "consensus":
-        R, t = pnp_batched(P3, uv, K)
+        R, t = pnp_batched(P3, uv, K, dist_coeffs=dist_coeffs)
         return R, t, {}
-    R_gt, t_gt = pnp_batched(P3, uv[:n], K)
-    R_pr, t_pr, _p, inl, hyp = pnp_consensus_batched(P3, uv[n:], K, reproj_thresh)
+    R_gt, t_gt = pnp_batched(P3, uv[:n], K, dist_coeffs=dist_coeffs)
+    R_pr, t_pr, _p, inl, hyp = pnp_consensus_batched(P3, uv[n:], K, reproj_thresh, dist_coeffs=dist_coeffs)
     return torch.cat([R_gt, R_pr]), torch.cat([t_gt, t_pr]), dict(inliers=inl, hyp=hyp)
 
 
 def evaluate_poses_batched(output, target, vertices, points_3D, internal_calibration, num_classes=1, num_keypoints=9,
-                           im_width=640, im_height=480, adds=False, pnp="plain", reproj_thresh=8.0):
+                           im_width=640, im_height=480, adds=False, pnp="plain", reproj_thresh=8.0, dist_coeffs=None):
     """GPU-resident version of the per-image evaluation loop of reference valid.py:123-183 (SURVEY 8f.1): per-image decode
     (arg-max cell of EACH image, not the whole batch), PnP of the ground-truth and the predicted keypoints, reprojection of
     all mesh vertices, pixel / 3-D / angular / translation errors -- no Python loop over images.
@@ -394,8 +455,12 @@ def evaluate_poses_batched(output, target, vertices, points_3D, internal_calibra
     so an exact pose gives 0 where the reference's calcAngularDistance can give NaN.
     pnp="consensus" solves the predicted pose with the consensus PnP (pnp_consensus_batched, inliers within reproj_thresh pixels of
     the im_width x im_height image) and adds `inliers` (B, K) bool and `hyp` (B,) int32; the ground-truth pose stays the plain
-    solve.  Passing the results of both modes of one network output to pose_accuracy compares the two solves."""
+    solve.  Passing the results of both modes of one network output to pose_accuracy compares the two solves.
+    dist_coeffs: OpenCV distortion coefficients of the camera (camera_distortion): the ground-truth and the predicted poses are both
+    solved with them, as valid.py does when pnp.distCoeffs is set; the pixel and vertex errors stay the undistorted projection
+    (compute_projection), which is also what valid.py computes then."""
     pnp, reproj_thresh = check_pnp_args(pnp, reproj_thresh)
+    camera_distortion(dist_coeffs)
     dev = output.device
     K = num_keypoints
     boxes, best, _ = region_boxes_batched(output, num_classes, K)
@@ -405,7 +470,7 @@ def evaluate_poses_batched(output, target, vertices, points_3D, internal_calibra
     gt2d = torch.as_tensor(target)[:, 1:1 + 2 * K].to(dev, torch.float32).reshape(B, K, 2) * scale
     Kc = torch.as_tensor(np.asarray(internal_calibration, dtype=np.float32)).to(dev)
     P3 = torch.as_tensor(np.asarray(points_3D, dtype=np.float32)).to(dev)
-    R, t, extra = pnp_truth_and_prediction(P3, torch.cat([gt2d, pr2d], 0), Kc, pnp, reproj_thresh)
+    R, t, extra = pnp_truth_and_prediction(P3, torch.cat([gt2d, pr2d], 0), Kc, pnp, reproj_thresh, dist_coeffs)
     R_gt, R_pr, t_gt, t_pr = R[:B], R[B:], t[:B], t[B:]
     Rt_gt = torch.cat([R_gt, t_gt.unsqueeze(2)], 2)
     Rt_pr = torch.cat([R_pr, t_pr.unsqueeze(2)], 2)

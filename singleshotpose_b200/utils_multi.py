@@ -9,13 +9,19 @@ import numpy as np
 import torch
 
 from ._lib import call, ptr, stream_ptr, SspError
-from .utils import (pnp, pnp_batched, compute_projection, compute_transformation, calcAngularDistance, get_3D_corners,  # noqa: F401
+from .utils import (pnp_batched, compute_projection, compute_transformation, calcAngularDistance, get_3D_corners,  # noqa: F401
                     get_camera_intrinsic, convert2cpu, convert2cpu_long, project_points_batched, adi_batched, mesh_diameter,
-                    check_pnp_args, object_table, pnp_truth_and_prediction)
+                    check_pnp_args, object_table, pnp_truth_and_prediction, pnp_one, camera_distortion, distortion_tensor)
 from .utils_host import (makedirs, get_all_files, calc_pts_diameter, adi, get_2d_bb, corner_confidences, corner_confidence,  # noqa: F401
                          sigmoid, softmax, read_truths, read_truths_args, read_pose, load_class_names, image2torch, scale_bboxes,
                          file_lines, get_image_size, logging)
 from . import utils_host as _host
+
+
+def pnp(points_3D, points_2D, cameraMatrix):
+    """utils.pnp for valid_multi.py (utils_multi.py:95-109).  A function of its own, as in the reference: its distortion coefficients
+    are ITS attribute pnp.distCoeffs, independent of utils.pnp.distCoeffs; unset or all zeros is the zero-distortion solve."""
+    return pnp_one(points_3D, points_2D, cameraMatrix, getattr(pnp, "distCoeffs", None))
 
 
 def read_data_cfg(datacfg):
@@ -219,12 +225,13 @@ class InstanceTracker:
     TrackingPosePredictor issues the same launches inside its graph replay.
 
     objects: {class id: (3|4, 8) box corners}; K (3, 3); frame_size (width, height); batch = streams; max_tracks in [1, 256] slots
-    per stream, match_iou in [0, 1], max_misses >= 0.  The state lives in four device arrays allocated once (graphs bake their
+    per stream, match_iou in [0, 1], max_misses >= 0; dist_coeffs: the camera's OpenCV distortion coefficients (utils.camera_distortion),
+    for the warm and the cold solves (ssp_pnp_dist); the association compares the raw keypoints' rectangles.  The state lives in four device arrays allocated once (graphs bake their
     addresses in): tracks (B, T, 5) int32 = alive, id, cls, misses, hits; rects (B, T, 4) fp32; poses (B, T, 6) fp64 = (rvec, t);
     next_id (B,) int32.  reset() zeroes them in place."""
 
     def __init__(self, objects, K, num_classes, num_anchors, frame_size, batch=1, conf_thresh=0.05, nms_thresh=0.4, max_instances=32,
-                 max_tracks=64, match_iou=0.3, max_misses=5, num_keypoints=9, device=None):
+                 max_tracks=64, match_iou=0.3, max_misses=5, num_keypoints=9, device=None, dist_coeffs=None):
         self.max_tracks, self.match_iou, self.max_misses = check_track_args(max_tracks, match_iou, max_misses)
         classes, points, Km = object_table(objects if isinstance(objects, dict) else {0: objects}, num_classes, K)
         if int(num_keypoints) != 9:
@@ -240,6 +247,8 @@ class InstanceTracker:
         self.device = dev
         self._P3_table = torch.from_numpy(points.astype(np.float32)).to(dev)
         self._K32 = torch.from_numpy(np.ascontiguousarray(Km, dtype=np.float32)).to(dev)
+        dist = camera_distortion(dist_coeffs)
+        self._dist = None if dist is None else distortion_tensor(dist, dev)
         B, T = self.batch, self.max_tracks
         self.state_tracks = torch.zeros(B, T, 5, dtype=torch.int32, device=dev)
         self.state_rects = torch.zeros(B, T, 4, dtype=torch.float32, device=dev)
@@ -294,8 +303,12 @@ class InstanceTracker:
         call("ssp_track_associate", B, T, M, ptr(c.count), ptr(c.cls), ptr(c.kp), self.match_iou, self.max_misses, ptr(self.state_tracks),
              ptr(self.state_rects), ptr(self.state_poses), ptr(self.state_next_id), ptr(c.slot), ptr(c.track_id), ptr(c.guess),
              ptr(c.use_guess), s)
-        call("ssp_pnp_batched_guess", ptr(P3), ptr(c.kp), ptr(K32), 9, B, M, ptr(c.count), ptr(c.guess), ptr(c.use_guess), 20, ptr(c.R),
-             ptr(c.t), ptr(c.params), None, s)
+        if self._dist is None:
+            call("ssp_pnp_batched_guess", ptr(P3), ptr(c.kp), ptr(K32), 9, B, M, ptr(c.count), ptr(c.guess), ptr(c.use_guess), 20, ptr(c.R),
+                 ptr(c.t), ptr(c.params), None, s)
+        else:
+            call("ssp_pnp_dist", ptr(P3), 0, ptr(c.kp), ptr(K32), ptr(self._dist), 9, B, M, ptr(c.count), ptr(c.guess), ptr(c.use_guess), 20,
+                 ptr(c.R), ptr(c.t), ptr(c.params), None, s)
         call("ssp_track_commit", B, T, M, ptr(c.count), ptr(c.kp), ptr(c.slot), ptr(c.params), ptr(self.state_tracks), ptr(self.state_rects),
              ptr(self.state_poses), s)
         torch.ne(c.use_guess, 0, out=c.warm)
@@ -353,7 +366,8 @@ def projection_accuracy(pixel_err, thresholds=ACCURACY_THRESHOLDS):
 
 
 def evaluate_multi_poses_batched(output, target, conf_thresh, num_classes, num_keypoints, num_anchors, vertices, corners3D,
-                                 internal_calibration, im_width=640, im_height=480, adds=False, pnp="plain", reproj_thresh=8.0):
+                                 internal_calibration, im_width=640, im_height=480, adds=False, pnp="plain", reproj_thresh=8.0,
+                                 dist_coeffs=None):
     """GPU version of the multi-object evaluation loop (valid_multi.py:97-149, train_multi.py:196-240) for a whole batch.
 
     output (B, (2K+1+C)*A, H, W) CUDA network output; target (B, 50*(2K+3)) label of dataset_multi.listDataset in test mode, host
@@ -379,8 +393,13 @@ def evaluate_multi_poses_batched(output, target, conf_thresh, num_classes, num_k
 
     pnp="consensus" solves the G predicted poses with the consensus PnP (utils.pnp_consensus_batched, inliers within reproj_thresh
     pixels) and adds `inliers` (G, K) bool and `hyp` (G,) int32; the ground-truth poses stay the plain solve.  projection_accuracy
-    of the pixel_err of both modes on one network output compares the two solves."""
+    of the pixel_err of both modes on one network output compares the two solves.
+
+    dist_coeffs: OpenCV distortion coefficients of the camera (utils.camera_distortion): the ground-truth and the predicted poses are
+    both solved with them, as valid_multi.py does when pnp.distCoeffs is set; pixel_err stays the undistorted projection
+    (compute_projection), which is also what valid_multi.py computes then."""
     pnp, reproj_thresh = check_pnp_args(pnp, reproj_thresh)
+    camera_distortion(dist_coeffs)
     if output.dim() == 3:
         output = output.unsqueeze(0)
     if not output.is_cuda:
@@ -414,7 +433,7 @@ def evaluate_multi_poses_batched(output, target, conf_thresh, num_classes, num_k
     c3 = np.asarray(corners3D, dtype=np.float64)[:3]
     P3 = np.array(np.transpose(np.concatenate((np.zeros((3, 1)), c3), axis=1)), dtype="float32")          # valid_multi.py:135
     Kc = torch.as_tensor(np.asarray(internal_calibration, dtype=np.float32)).to(dev)
-    R, t, extra = pnp_truth_and_prediction(torch.from_numpy(P3).to(dev), uv, Kc, pnp, reproj_thresh)       # 2G problems
+    R, t, extra = pnp_truth_and_prediction(torch.from_numpy(P3).to(dev), uv, Kc, pnp, reproj_thresh, dist_coeffs)       # 2G problems
     if G == 0:                                                  # nothing to project: empty errors
         res = dict(res, R_gt=R, t_gt=t, R_pr=R.clone(), t_pr=t.clone(), pixel_err=torch.zeros(0, dtype=torch.float32, device=dev), **extra)
         if adds:
