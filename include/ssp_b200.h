@@ -313,6 +313,43 @@ int ssp_pnp_consensus_dist(const float* points3d, int points3d_shared, const flo
 int ssp_project_points_dist(const float* X, int rows, int nv, const double* Rt, const double* K3x3, const double* dist8,
                             long long n, float* out, void* stream);
 
+/* ---- pose covariance and the constant-velocity pose filter of tracked instances (rules: csrc/pose_filter_core.h; csrc/pose_filter.cu),
+ *      fp64.  A pose is perturbed on the left, x_cam = exp([dth]x) R X + t + dt_, and a 6 x 6 covariance is over (dth, dt_).
+ *  ssp_pose_covariance: Sigma = sigma^2 (J^T J)^-1 of the pose (R, t) of each problem, J the pixel projection of its points with
+ *      respect to (dth, dt_) (distorted with dist8_or_null, a DEVICE double [8] as ssp_pnp_dist takes it; NULL: no distortion).  The
+ *      keypoints do not enter: J is taken at the solved pose.  points3d shared or [n][num_points][3], K3x3 fp32, count_or_null as
+ *      ssp_pnp_dist; R [n][9], t [n][3] the solutions (ssp_pnp_* outputs).  Out: cov_out [n][6][6], status_out [n] = 0 (usable) or
+ *      SSP_POSE_COV_SINGULAR (a Cholesky pivot <= 1e-12 x the largest diagonal entry of J^T J) | SSP_POSE_COV_DEPTH (a point at
+ *      depth <= 0); an unusable or empty slot gets zeros.  SSP_ERR_ARG for a null required pointer, num_points outside 3..16,
+ *      groups < 0, per_group < 1 or sigma not > 0 and finite.
+ *  The filter of each (stream, track slot) is filter [B][max_tracks][SSP_FILTER_DOUBLES] fp64 = R [9], t [3], w [3] (rad/s, camera
+ *      frame), v [3] (mesh units / s), P [12][12] over (dth, dt_, dw, dv), valid; zeros for a fresh start.
+ *  ssp_track_predict: for every alive slot whose filter has started, moves the filter by dt [B] seconds (DEVICE fp64, one per stream)
+ *      in place, and writes the predicted LM vector (log R, t) to pred_poses [B][max_tracks][6] and the predicted corner rectangle to
+ *      pred_rects [B][max_tracks][4]: the 8 corners points3d_table [cls][1..8] (fp32 [num_classes][9][3]) of the slot's class
+ *      projected with K3x3 (fp64; distorted with dist8_or_null) and rounded to fp32.  Any other slot, and a slot with a predicted
+ *      corner at depth <= 0, passes its rects / poses on.  The two outputs take the place of rects / poses in ssp_track_associate.
+ *      SSP_ERR_ARG for a null required pointer, B < 0, max_tracks outside [1, 256], num_classes < 1 or an accel sigma not > 0 and finite.
+ *  ssp_track_filter_update: after ssp_track_commit, per detection slot with a track slot (slot >= 0, m < count[b]): a new track
+ *      (use_guess 0) starts its filter from the measurement R, t (the frame's PnP) with covariance cov / cov_status
+ *      (ssp_pose_covariance), a matched one is gated (y^T S^-1 y > gate restarts it) and updated.  Out per detection slot: R_filt
+ *      [9], t_filt [3], pose_cov [6][6], velocity [6] = (w, v), reinit (1: the filter was started from this measurement); zeros
+ *      elsewhere.  SSP_ERR_ARG for a null pointer, B < 0, max_tracks or max_det outside [1, 256], or an init velocity sigma or the
+ *      gate not > 0 and finite. ---- */
+#define SSP_POSE_COV_SINGULAR 1
+#define SSP_POSE_COV_DEPTH 2
+#define SSP_FILTER_DOUBLES 163
+int ssp_pose_covariance(const float* points3d, int points3d_shared, const float* K3x3, const double* dist8_or_null, int num_points,
+                        int groups, int per_group, const int* count_or_null, const double* R, const double* t, double sigma,
+                        double* cov_out, int* status_out, void* stream);
+int ssp_track_predict(int B, int max_tracks, const int* tracks, const float* rects, const double* poses, double* filter, const double* dt,
+                      const float* points3d_table, int num_classes, const double* K3x3, const double* dist8_or_null,
+                      double accel_sigma_rot, double accel_sigma_trans, double* pred_poses, float* pred_rects, void* stream);
+int ssp_track_filter_update(int B, int max_tracks, int max_det, const int* count, const int* slot, const int* use_guess,
+                            const double* R, const double* t, const double* cov, const int* cov_status, double* filter,
+                            double init_velocity_sigma_rot, double init_velocity_sigma_trans, double gate, double* R_filt,
+                            double* t_filt, double* pose_cov, double* velocity, int* reinit, void* stream);
+
 /* ---- pose errors over the mesh (utils.py:50-64, valid.py:69-72, 173-177), fp64 throughout (csrc/adds.cu, csrc/adds_core.h).
  *      X [nv][3] fp64 vertices; Rt_est, Rt_gt [n][3][4] fp64 poses [R | t].
  *  ssp_adds_batched: adds_out[p] = mean_i min_j |Rt_gt[p] x_i - Rt_est[p] x_j|, the reference's adi(pts_est, pts_gt) (ADD-S, for

@@ -31,6 +31,8 @@ Command line: python -m singleshotpose_b200.predict_instances --datacfg cfg/occl
               --weightfile w.weights --object 0=../LINEMOD/ape/ape.ply --object 4=../LINEMOD/can/can.ply --out det.npz img...
               [--track [--match-iou 0.3 --max-misses 5 --max-tracks 64]]: the images, in the order given, as one stream, with a
               track_id column
+              [--track --motion cv [--keypoint-sigma 2 --fps 30]]: with the constant-velocity pose filter, adding the columns
+              R_filt, t_filt, velocity and pose_cov
               [--pnp consensus [--reproj-thresh 8]]: the consensus PnP, with inliers and hyp columns (not with --track)
 """
 from __future__ import annotations
@@ -44,12 +46,13 @@ from . import predict, predict_multi
 from ._lib import SspError
 from .predict import CONSENSUS_KEYS, _FramePredictor, add_dist_arg, add_pnp_args, camera_dist, mesh_corners, predict_files, read_camera
 from .predict_multi import cfg_conf_thresh, check_grid, parse_objects
-from .utils import camera_distortion, check_pnp_args
-from .utils_multi import InstanceTracker, check_track_args, detect_buffers, detect_slots
+from .utils import camera_distortion, check_pnp_args, check_sigma
+from .utils_multi import InstanceTracker, check_motion_args, check_track_args, detect_buffers, detect_slots
 
 MAX_INSTANCES = 256         # largest max_instances (detect_core.h kMaxInstances)
 OUTPUT_KEYS = ("count", "kept", "cls", "R", "t", "conf", "cls_conf", "keypoints_px", "corners_px")
 ROW_KEYS = ("cls", "R", "t", "conf", "cls_conf", "keypoints_px", "corners_px")
+MOTION_KEYS = ("R_filt", "t_filt", "velocity", "pose_cov")          # the --motion columns
 
 
 class InstancePosePredictor(_FramePredictor):
@@ -99,7 +102,8 @@ class TrackingPosePredictor(InstancePosePredictor):
     """InstancePosePredictor whose instances keep their identity across calls: each row b of a batch is its own camera stream, and
     each instance is matched to a track of its class (utils_multi.InstanceTracker, rules: csrc/track_core.h).  A matched instance's
     PnP starts Levenberg-Marquardt from its track's last pose (cv2.solvePnP's useExtrinsicGuess), the others are solved cold.
-    No motion model: a track is matched against its last corner rectangle, and the guess is its last pose.
+    With motion=None (the default) there is no motion model: a track is matched against its last corner rectangle, and the guess
+    is its last pose; motion="constant_velocity" matches and warm-starts on predictions (below).
 
     max_tracks in [1, 256] track slots per stream, match_iou in [0, 1] (a match needs IoU > match_iou), max_misses >= 0 (a track
     dies after max_misses + 1 frames in a row without a match); the other arguments are InstancePosePredictor's.
@@ -109,18 +113,41 @@ class TrackingPosePredictor(InstancePosePredictor):
     arrays, zeroed in place by reset); the warm-up runs before a graph capture do not advance it.
     Only pnp="plain": the consensus solve has no rule yet for how a track's warm guess competes with its subset hypotheses.
     dist_coeffs: the camera's OpenCV distortion coefficients; the warm and the cold solves both use them, the association compares
-    the raw keypoints' rectangles."""
+    the raw keypoints' rectangles.
+
+    motion="constant_velocity" smooths and predicts each track's pose with a constant-velocity pose filter
+    (utils_multi.InstanceTracker, rules: csrc/pose_filter_core.h): the association compares each detection with its track's
+    predicted rectangle, the warm start is the predicted pose, and the outputs add R_filt (B, M, 3, 3), t_filt (B, M, 3),
+    pose_cov (B, M, 6, 6), velocity (B, M, 6) and reinit (B, M) bool; R and t stay this frame's PnP.  keypoint_sigma (px),
+    accel_sigma, init_velocity_sigma, gate and frame_dt (s) are InstanceTracker's, and their defaults are not tuned on real data.
+    __call__ then takes timestamps= (B,) seconds per stream (default: the stream's last + frame_dt), checked before any launch."""
 
     def __init__(self, model, objects, K, frame_size=(640, 480), shape=None, batch=1, conf_thresh=None, nms_thresh=0.4, max_instances=32,
-                 max_tracks=64, match_iou=0.3, max_misses=5, graph=True, max_graphs=4, pnp="plain", dist_coeffs=None):
+                 max_tracks=64, match_iou=0.3, max_misses=5, graph=True, max_graphs=4, pnp="plain", dist_coeffs=None, motion=None,
+                 keypoint_sigma=2.0, accel_sigma=(2.0, 1.0), init_velocity_sigma=(1.0, 0.5), gate=22.46, frame_dt=1 / 30):
         check_tracking_pnp(pnp)
         check_track_args(max_tracks, match_iou, max_misses)
+        check_motion_args(motion, keypoint_sigma, accel_sigma, init_velocity_sigma, gate, frame_dt)
         super().__init__(model, objects, K, frame_size, shape, batch, conf_thresh, nms_thresh, max_instances, graph, max_graphs,
                          dist_coeffs=dist_coeffs)
         self._tracker = InstanceTracker(objects, K, self.num_classes, self.num_anchors, self.frame_size, self.batch, self.conf_thresh,
                                         self.nms_thresh, self.max_instances, max_tracks, match_iou, max_misses, device=self.device,
-                                        dist_coeffs=dist_coeffs)
+                                        dist_coeffs=dist_coeffs, motion=motion, keypoint_sigma=keypoint_sigma, accel_sigma=accel_sigma,
+                                        init_velocity_sigma=init_velocity_sigma, gate=gate, frame_dt=frame_dt)
         self.max_tracks, self.match_iou, self.max_misses = self._tracker.max_tracks, self._tracker.match_iou, self._tracker.max_misses
+        self.motion = self._tracker.motion
+
+    def __call__(self, frames, to_host=False, events=None, timestamps=None):
+        """InstancePosePredictor's call; timestamps (B,) seconds of the frames, per stream, for the motion model (ignored without it)"""
+        if not self.motion:
+            return super().__call__(frames, to_host, events)
+        self._check(frames)                        # the frames' errors before the timestamps change anything
+        with torch.cuda.device(self.device):
+            self._tracker.stage_times(timestamps)
+        out = super().__call__(frames, to_host, events)
+        with torch.cuda.device(self.device):
+            self._tracker.staged()
+        return out
 
     def reset(self, streams=None):
         """forget the tracks of the given streams (default: all); their ids start again from 0"""
@@ -128,7 +155,8 @@ class TrackingPosePredictor(InstancePosePredictor):
             self._tracker.reset(streams)
 
     def tracks(self, to_host=False):
-        """the alive tracks (utils_multi.InstanceTracker.tracks): stream, slot, id, cls, misses, hits, rvec, R, t, rect"""
+        """the alive tracks (utils_multi.InstanceTracker.tracks): stream, slot, id, cls, misses, hits, rvec, R, t, rect; with motion
+        also R_filt, t_filt, velocity, pose_cov and filter_valid"""
         with torch.cuda.device(self.device):
             return self._tracker.tracks(to_host)
 
@@ -145,7 +173,7 @@ class TrackingPosePredictor(InstancePosePredictor):
         self._tracker.restore(saved)
 
     def _outputs(self, c):
-        return dict(super()._outputs(c), track_id=c.track_id, warm=c.warm)
+        return dict(super()._outputs(c), track_id=c.track_id, warm=c.warm, **self._tracker.outputs(c))
 
 
 def check_detect_args(nms_thresh, max_instances):
@@ -170,7 +198,8 @@ SIZE_KEYS = predict_multi.SIZE_KEYS + predict.SIZE_KEYS      # a multi-object .d
 
 def parse_args(argv=None):
     """the command line, checked before any model is built: raises SspError for a bad --object, --nms-thresh, --max-instances,
-    --match-iou, --max-misses, --max-tracks, --reproj-thresh or --dist, and for --track with --pnp consensus"""
+    --match-iou, --max-misses, --max-tracks, --reproj-thresh, --dist, --keypoint-sigma or --fps, for --track with --pnp consensus
+    and for --motion without --track"""
     ap = argparse.ArgumentParser(prog="python -m singleshotpose_b200.predict_instances",
                                  description="6-D pose of every detected instance of the requested objects in each image")
     ap.add_argument("--datacfg", required=True, help=".data file: fx fy u0 v0 and width height (or im_width im_height); mesh")
@@ -186,6 +215,11 @@ def parse_args(argv=None):
     ap.add_argument("--match-iou", type=float, default=0.3)
     ap.add_argument("--max-misses", type=int, default=5)
     ap.add_argument("--max-tracks", type=int, default=64)
+    ap.add_argument("--motion", choices=("cv",), default=None,
+                    help="with --track: smooth each track's pose with the constant-velocity pose filter, adding the columns R_filt, "
+                         "t_filt, velocity and pose_cov")
+    ap.add_argument("--keypoint-sigma", type=float, default=2.0, help="--motion: the keypoint noise in pixels")
+    ap.add_argument("--fps", type=float, default=30.0, help="--motion: the frame rate of the image sequence")
     add_pnp_args(ap)
     add_dist_arg(ap)
     ap.add_argument("images", nargs="+")
@@ -195,6 +229,10 @@ def parse_args(argv=None):
         check_tracking_pnp(a.pnp)
     check_detect_args(a.nms_thresh, a.max_instances)
     check_track_args(a.max_tracks, a.match_iou, a.max_misses)
+    if a.motion and not a.track:
+        raise SspError("--motion filters tracks: it needs --track")
+    check_sigma("--keypoint-sigma", a.keypoint_sigma)
+    check_sigma("--fps", a.fps)
     a.objects = parse_objects(a.object) if a.object else None
     if a.dist is not None:
         camera_distortion(a.dist)
@@ -226,13 +264,15 @@ def main(argv=None):
     model = Darknet(a.modelcfg)
     model.load_weights(a.weightfile)
     model.cuda().eval()
+    motion = "constant_velocity" if a.motion else None
     if a.track:
         pred = TrackingPosePredictor(model, objects, K, frame_size=size, nms_thresh=a.nms_thresh, max_instances=a.max_instances,
-                                     max_tracks=a.max_tracks, match_iou=a.match_iou, max_misses=a.max_misses, dist_coeffs=dist)
+                                     max_tracks=a.max_tracks, match_iou=a.match_iou, max_misses=a.max_misses, dist_coeffs=dist,
+                                     motion=motion, keypoint_sigma=a.keypoint_sigma, frame_dt=1.0 / a.fps)
     else:
         pred = InstancePosePredictor(model, objects, K, frame_size=size, nms_thresh=a.nms_thresh, max_instances=a.max_instances,
                                      pnp=a.pnp, reproj_thresh=a.reproj_thresh, dist_coeffs=dist)
-    rows = {k: [] for k in ROW_KEYS + (("track_id",) if a.track else ()) + CONSENSUS_KEYS[a.pnp]}
+    rows = {k: [] for k in ROW_KEYS + (("track_id",) if a.track else ()) + (MOTION_KEYS if motion else ()) + CONSENSUS_KEYS[a.pnp]}
     image = []
     for i, r in enumerate(predict_files(pred, a.images)):
         n = int(r["count"][0])

@@ -151,6 +151,45 @@ def pnp_batched(points_3D, points_2D, cameraMatrix, max_iter=20, return_iters=Fa
     return (R, t, iters) if return_iters else (R, t)
 
 
+def check_sigma(name, value):
+    """-> float(value); SspError unless it is > 0 and finite"""
+    try:
+        v = float(value)
+    except (TypeError, ValueError):
+        raise SspError("%s must be a number, got %r" % (name, value))
+    if not (v > 0.0 and np.isfinite(v)):
+        raise SspError("%s must be > 0 and finite, got %r" % (name, value))
+    return v
+
+
+def pose_covariance_batched(points_3D, cameraMatrix, R, t, keypoint_sigma, dist_coeffs=None):
+    """Covariance of PnP poses (ssp_pose_covariance, rules: csrc/pose_filter_core.h): points_3D (P,3) shared or (n,P,3); K (3,3);
+    R (n,3,3), t (n,3) the solved poses (pnp_batched's outputs); keypoint_sigma: the keypoint noise in pixels (> 0).
+    -> (cov (n,6,6) fp64, status (n,) int32) CUDA tensors.  cov = keypoint_sigma^2 (J^T J)^-1 over (dth, dt_), the pose perturbed
+    on the left (x_cam = exp([dth]x) R X + t + dt_), J the keypoints' pixel Jacobian at the pose: the covariance of the pose to
+    first order when the keypoints carry independent Gaussian noise of keypoint_sigma px.  It depends on the points, the camera and
+    the pose, not on the keypoints.  status: 0, or SSP_POSE_COV_SINGULAR (1: J^T J is singular to 1e-12 of its largest diagonal
+    entry) | SSP_POSE_COV_DEPTH (2: a point at depth <= 0); such a cov is zero.  dist_coeffs: as pnp_batched (the distorted
+    projection's Jacobian)."""
+    sigma = check_sigma("keypoint_sigma", keypoint_sigma)
+    k = camera_distortion(dist_coeffs)
+    dev = _dev()
+    P3, K = (torch.as_tensor(np.asarray(a, dtype=np.float32) if not torch.is_tensor(a) else a).to(dev, torch.float32).contiguous()
+             for a in (points_3D, cameraMatrix))
+    R, t = (torch.as_tensor(a).to(dev, torch.float64).contiguous() for a in (R, t))
+    R, t = R.reshape(-1, 3, 3), t.reshape(-1, 3)
+    n, npts = R.shape[0], P3.shape[-2]
+    shared = P3.dim() == 2
+    if t.shape[0] != n or P3.shape[-1] != 3 or (not shared and P3.shape[0] != n):
+        raise SspError("pose_covariance_batched: R (n,3,3), t (n,3) and points_3D (P,3) or (n,P,3) disagree: %s, %s, %s"
+                       % (tuple(R.shape), tuple(t.shape), tuple(P3.shape)))
+    cov = torch.empty(n, 6, 6, dtype=torch.float64, device=dev)
+    status = torch.empty(n, dtype=torch.int32, device=dev)
+    call("ssp_pose_covariance", ptr(P3), 1 if shared else 0, ptr(K), None if k is None else ptr(distortion_tensor(k, dev)), npts, n, 1,
+         None, ptr(R), ptr(t), sigma, ptr(cov), ptr(status), stream_ptr())
+    return cov, status
+
+
 def object_table(objects, num_classes, K):
     """The constants of a pose head, checked: objects {class id in [0, num_classes): (3|4, 8) box corners}, K (3, 3).
     -> (classes (Q,) int64 sorted ids, points (num_classes, 9, 3) float64 PnP points [0; corners3D_c[:3]] of each requested class

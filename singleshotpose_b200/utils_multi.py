@@ -8,10 +8,10 @@ import ctypes as _ctypes
 import numpy as np
 import torch
 
-from ._lib import call, ptr, stream_ptr, SspError
+from ._lib import CONSTANTS, call, ptr, stream_ptr, SspError
 from .utils import (pnp_batched, compute_projection, compute_transformation, calcAngularDistance, get_3D_corners,  # noqa: F401
                     get_camera_intrinsic, convert2cpu, convert2cpu_long, project_points_batched, adi_batched, mesh_diameter,
-                    check_pnp_args, object_table, pnp_truth_and_prediction, pnp_one, camera_distortion, distortion_tensor)
+                    check_pnp_args, object_table, pnp_truth_and_prediction, pnp_one, camera_distortion, distortion_tensor, check_sigma)
 from .utils_host import (makedirs, get_all_files, calc_pts_diameter, adi, get_2d_bb, corner_confidences, corner_confidence,  # noqa: F401
                          sigmoid, softmax, read_truths, read_truths_args, read_pose, load_class_names, image2torch, scale_bboxes,
                          file_lines, get_image_size, logging)
@@ -186,6 +186,7 @@ def detect_slots(c, logits, classes, points, num_classes, num_anchors, conf_thre
 
 # ------------------------------------------------------------------------------------------ tracking across frames
 MAX_TRACKS = 256            # largest max_tracks (track_core.h kMaxTracks)
+FILTER_DOUBLES = CONSTANTS["SSP_FILTER_DOUBLES"]            # one track's pose filter (pose_filter_core.h kFilterDoubles)
 
 
 def check_track_args(max_tracks, match_iou, max_misses):
@@ -199,6 +200,23 @@ def check_track_args(max_tracks, match_iou, max_misses):
     if isinstance(max_misses, bool) or not isinstance(max_misses, (int, np.integer)) or max_misses < 0:
         raise SspError("max_misses must be an integer >= 0, got %r" % (max_misses,))
     return int(max_tracks), match_iou, int(max_misses)
+
+
+MOTIONS = (None, "constant_velocity")
+
+
+def check_motion_args(motion, keypoint_sigma, accel_sigma, init_velocity_sigma, gate, frame_dt):
+    """-> (motion, keypoint_sigma, accel_sigma (rot, trans), init_velocity_sigma (rot, trans), gate, frame_dt) checked: motion None or
+    'constant_velocity', every sigma, the gate and frame_dt > 0 and finite; SspError otherwise"""
+    if not any(motion is m or motion == m for m in MOTIONS):
+        raise SspError("motion must be None or 'constant_velocity', got %r" % (motion,))
+
+    def pair(name, v):
+        if isinstance(v, (str, bytes)) or np.ndim(v) != 1 or len(v) != 2:
+            raise SspError("%s must be a pair (rotation, translation), got %r" % (name, v))
+        return tuple(check_sigma("%s[%d]" % (name, i), x) for i, x in enumerate(v))
+    return (motion, check_sigma("keypoint_sigma", keypoint_sigma), pair("accel_sigma", accel_sigma),
+            pair("init_velocity_sigma", init_velocity_sigma), check_sigma("gate", gate), check_sigma("frame_dt", frame_dt))
 
 
 def rodrigues_batched(r):
@@ -220,19 +238,35 @@ class InstanceTracker:
     class (highest IoU of the corner rectangles > match_iou, in det_conf order), ages the unmatched tracks (a track dies after
     max_misses + 1 missed frames in a row) and gives the other detections the lowest free slot and the stream's next id;
     ssp_pnp_batched_guess starts Levenberg-Marquardt from the matched track's pose (no DLT) and solves the others cold;
-    ssp_track_commit stores each track's rectangle and final LM vector.  No motion model: a track is matched against its last
-    rectangle and the guess is its last pose.  update(logits) is the eager, logits-level surface; predict_instances.
+    ssp_track_commit stores each track's rectangle and final LM vector.  With motion=None (the default) there is no motion model: a
+    track is matched against its last rectangle and the guess is its last pose (motion="constant_velocity": see below).  update(logits) is the eager, logits-level surface; predict_instances.
     TrackingPosePredictor issues the same launches inside its graph replay.
 
     objects: {class id: (3|4, 8) box corners}; K (3, 3); frame_size (width, height); batch = streams; max_tracks in [1, 256] slots
     per stream, match_iou in [0, 1], max_misses >= 0; dist_coeffs: the camera's OpenCV distortion coefficients (utils.camera_distortion),
     for the warm and the cold solves (ssp_pnp_dist); the association compares the raw keypoints' rectangles.  The state lives in four device arrays allocated once (graphs bake their
     addresses in): tracks (B, T, 5) int32 = alive, id, cls, misses, hits; rects (B, T, 4) fp32; poses (B, T, 6) fp64 = (rvec, t);
-    next_id (B,) int32.  reset() zeroes them in place."""
+    next_id (B,) int32.  reset() zeroes them in place.
+
+    motion="constant_velocity" adds a pose filter per track (rules: csrc/pose_filter_core.h): an error-state Kalman filter of the
+    pose, the angular velocity and the linear velocity, fed by each frame's PnP with its covariance (utils.pose_covariance_batched
+    with keypoint_sigma px).  Each frame, ssp_track_predict moves every alive track's filter to the frame's time first, and the
+    association then compares each detection with the track's PREDICTED corner rectangle and warm-starts its PnP from the
+    predicted pose, so an object that moves more than about half its width per frame keeps its id.  After the PnP,
+    ssp_track_filter_update starts the filter of a new track and gates and updates a matched one: a measurement with
+    y^T S^-1 y > gate (default 22.46, chi^2 with 6 degrees of freedom at 99.9 %) restarts the filter instead, as a mirrored PnP
+    solution would.  accel_sigma = (rad/s^2, mesh units/s^2): the white-noise acceleration; init_velocity_sigma = (rad/s, mesh
+    units/s): the velocity prior of a new track; frame_dt: the frame interval in seconds when update() is given no timestamps.
+    These defaults are not tuned on real data: set keypoint_sigma to the network's keypoint error in pixels and the
+    accelerations to how fast the objects can change their motion.  The filter state is one more device array, filter (B, T, 163)
+    fp64 (csrc/pose_filter_core.h's layout), and each stream's last timestamp stays on the host."""
 
     def __init__(self, objects, K, num_classes, num_anchors, frame_size, batch=1, conf_thresh=0.05, nms_thresh=0.4, max_instances=32,
-                 max_tracks=64, match_iou=0.3, max_misses=5, num_keypoints=9, device=None, dist_coeffs=None):
+                 max_tracks=64, match_iou=0.3, max_misses=5, num_keypoints=9, device=None, dist_coeffs=None, motion=None,
+                 keypoint_sigma=2.0, accel_sigma=(2.0, 1.0), init_velocity_sigma=(1.0, 0.5), gate=22.46, frame_dt=1 / 30):
         self.max_tracks, self.match_iou, self.max_misses = check_track_args(max_tracks, match_iou, max_misses)
+        (self.motion, self.keypoint_sigma, self.accel_sigma, self.init_velocity_sigma, self.gate,
+         self.frame_dt) = check_motion_args(motion, keypoint_sigma, accel_sigma, init_velocity_sigma, gate, frame_dt)
         classes, points, Km = object_table(objects if isinstance(objects, dict) else {0: objects}, num_classes, K)
         if int(num_keypoints) != 9:
             raise SspError("tracking solves PnP on the centroid + 8 box corners: 9 keypoints, not %d" % int(num_keypoints))
@@ -247,6 +281,7 @@ class InstanceTracker:
         self.device = dev
         self._P3_table = torch.from_numpy(points.astype(np.float32)).to(dev)
         self._K32 = torch.from_numpy(np.ascontiguousarray(Km, dtype=np.float32)).to(dev)
+        self._K64 = torch.from_numpy(np.ascontiguousarray(Km, dtype=np.float64)).to(dev)
         dist = camera_distortion(dist_coeffs)
         self._dist = None if dist is None else distortion_tensor(dist, dev)
         B, T = self.batch, self.max_tracks
@@ -254,33 +289,88 @@ class InstanceTracker:
         self.state_rects = torch.zeros(B, T, 4, dtype=torch.float32, device=dev)
         self.state_poses = torch.zeros(B, T, 6, dtype=torch.float64, device=dev)
         self.state_next_id = torch.zeros(B, dtype=torch.int32, device=dev)
+        if self.motion:
+            self.state_filter = torch.zeros(B, T, FILTER_DOUBLES, dtype=torch.float64, device=dev)
+            self._dt = torch.zeros(B, dtype=torch.float64, device=dev)        # this frame's interval per stream, read by the replay
+            self._dt_pin = torch.zeros(B, dtype=torch.float64).pin_memory()
+            self._dt_copied = torch.cuda.Event()      # the launches that last read _dt_pin have been enqueued before this
+            self._last_time = np.full(B, np.nan)      # each stream's last timestamp (NaN: none since the start or a reset)
         self._bufs = None
 
     # ------------------------------------------------------------------ state
     def _state(self):
-        return (self.state_tracks, self.state_rects, self.state_poses, self.state_next_id)
+        base = (self.state_tracks, self.state_rects, self.state_poses, self.state_next_id)
+        return base + (self.state_filter,) if self.motion else base
 
     def reset(self, streams=None):
-        """forget every track of the given streams (default: all), in place: ids start again from 0"""
-        idx = slice(None) if streams is None else torch.as_tensor(np.asarray(streams, np.int64).reshape(-1), device=self.device)
+        """forget every track of the given streams (default: all), in place: ids start again from 0; with motion, their filters
+        and last timestamps too (the next frame of such a stream has dt = 0)"""
+        sel = slice(None) if streams is None else np.asarray(streams, np.int64).reshape(-1)
+        idx = sel if streams is None else torch.as_tensor(sel, device=self.device)
         for t in self._state():
             t[idx] = 0
+        if self.motion:
+            self._last_time[sel] = np.nan
 
     def snapshot(self):
-        return tuple(t.clone() for t in self._state())
+        saved = tuple(t.clone() for t in self._state())
+        return saved + (self._last_time.copy(),) if self.motion else saved
 
     def restore(self, saved):
         for t, s in zip(self._state(), saved):
             t.copy_(s)
+        if self.motion:
+            self._last_time[:] = saved[-1]
+
+    def stage_times(self, timestamps=None):
+        """with motion: this frame's interval per stream into the pinned buffer the next launches copy from.  timestamps: (B,)
+        seconds, or None for each stream's last timestamp + frame_dt (a stream's first frame is at 0); dt = 0 for a stream's first
+        frame.  SspError, before anything changes, for a timestamp that is not finite or not after the stream's last one."""
+        if not self.motion:
+            return
+        last = self._last_time
+        if timestamps is None:
+            now = np.where(np.isnan(last), 0.0, last + self.frame_dt)
+        else:
+            try:
+                now = np.asarray(timestamps, np.float64).reshape(-1)
+            except (TypeError, ValueError):
+                raise SspError("timestamps must be %d numbers (seconds), got %r" % (self.batch, timestamps))
+            if now.shape != (self.batch,) or not np.isfinite(now).all():
+                raise SspError("timestamps must be %d finite numbers (seconds), one per stream, got %r" % (self.batch, timestamps))
+            bad = ~np.isnan(last) & ~(now > last)
+            if bad.any():
+                b = int(np.nonzero(bad)[0][0])
+                raise SspError("stream %d: timestamp %r is not after the stream's last one, %r" % (b, float(now[b]), float(last[b])))
+        # the last frame's copy out of the pinned buffer has run.  The event is recorded after ALL of that frame's launches (the copy
+        # is a node inside the captured graph, where no host-visible event can follow it alone), so this waits until the previous
+        # frame has finished.  Host frames already wait for their own staging buffer this way; for device and JPEG frames it is a
+        # host synchronisation per frame that motion=None does not have.
+        self._dt_copied.synchronize()
+        self._dt_pin.numpy()[:] = np.where(np.isnan(last), 0.0, now - last)
+        self._last_time = now
+
+    def staged(self):
+        """after the launches of a frame are enqueued: the pinned interval buffer may be rewritten once they have run"""
+        if self.motion:
+            self._dt_copied.record()
 
     def tracks(self, to_host=False):
         """the alive tracks of every stream, ordered by (stream, slot): stream, slot, id, cls, misses, hits (n,) int32; rvec (n, 3),
-        R (n, 3, 3) (Rodrigues of rvec), t (n, 3) fp64 = the track's last pose; rect (n, 4) fp32 = its last corner rectangle"""
+        R (n, 3, 3) (Rodrigues of rvec), t (n, 3) fp64 = the track's last pose; rect (n, 4) fp32 = its last corner rectangle.
+        With motion also the filter's R_filt (n, 3, 3), t_filt (n, 3), velocity (n, 6) = (w, v) and pose_cov (n, 6, 6) at the last
+        frame's time (a track that missed the frame reports its prediction) and filter_valid (n,) bool (False while the track has
+        had no measurement with a usable covariance)."""
         st = self.state_tracks
         b, s = torch.nonzero(st[..., 0] != 0, as_tuple=True)
         f, pose = st[b, s], self.state_poses[b, s]
         out = dict(stream=b.int(), slot=s.int(), id=f[:, 1], cls=f[:, 2], misses=f[:, 3], hits=f[:, 4], rvec=pose[:, :3],
                    R=rodrigues_batched(pose[:, :3]), t=pose[:, 3:], rect=self.state_rects[b, s])
+        if self.motion:             # the filter: this frame's estimate, or its prediction for a track that missed the frame
+            fs = self.state_filter[b, s]
+            P = fs[:, 18:162].reshape(-1, 12, 12)
+            out.update(R_filt=fs[:, :9].reshape(-1, 3, 3), t_filt=fs[:, 9:12], velocity=fs[:, 12:18], pose_cov=P[:, :6, :6].contiguous(),
+                       filter_valid=fs[:, 162] == 1.0)
         if to_host:
             return {k: v.cpu().numpy() for k, v in out.items()}
         return out
@@ -295,14 +385,40 @@ class InstanceTracker:
         c.use_guess = torch.empty(B, M, dtype=torch.int32, device=dev)
         c.params = torch.empty(B, M, 6, dtype=torch.float64, device=dev)
         c.warm = torch.empty(B, M, dtype=torch.bool, device=dev)
+        if self.motion:
+            T = self.max_tracks
+            c.pred_poses = torch.empty(B, T, 6, dtype=torch.float64, device=dev)
+            c.pred_rects = torch.empty(B, T, 4, dtype=torch.float32, device=dev)
+            c.cov_m = torch.empty(B, M, 6, 6, dtype=torch.float64, device=dev)
+            c.cov_status = torch.empty(B, M, dtype=torch.int32, device=dev)
+            c.R_filt = torch.empty(B, M, 3, 3, dtype=torch.float64, device=dev)
+            c.t_filt = torch.empty(B, M, 3, dtype=torch.float64, device=dev)
+            c.pose_cov = torch.empty(B, M, 6, 6, dtype=torch.float64, device=dev)
+            c.velocity = torch.empty(B, M, 6, dtype=torch.float64, device=dev)
+            c.reinit_i = torch.empty(B, M, dtype=torch.int32, device=dev)
+            c.reinit = torch.empty(B, M, dtype=torch.bool, device=dev)
+
+    def outputs(self, c):
+        """the filter's outputs per detection slot (empty with motion None)"""
+        if not self.motion:
+            return {}
+        return dict(R_filt=c.R_filt, t_filt=c.t_filt, pose_cov=c.pose_cov, velocity=c.velocity, reinit=c.reinit)
 
     def solve(self, c, s, P3, K32):
         """associate, warm-started PnP, commit: reads c.count, c.cls, c.kp (ssp_detect_instances' outputs) and P3 (B*M, 9, 3) the
-        slots' PnP points; writes c.R, c.t, c.params, c.slot, c.track_id, c.guess, c.use_guess, c.warm"""
+        slots' PnP points; writes c.R, c.t, c.params, c.slot, c.track_id, c.guess, c.use_guess, c.warm.  With motion the tracks are
+        predicted first and associated on the predictions, and the filters are updated last (outputs())."""
         B, T, M = self.batch, self.max_tracks, self.max_instances
+        rects, poses = self.state_rects, self.state_poses
+        dist = None if self._dist is None else ptr(self._dist)
+        if self.motion:
+            self._dt.copy_(self._dt_pin, non_blocking=True)
+            call("ssp_track_predict", B, T, ptr(self.state_tracks), ptr(rects), ptr(poses), ptr(self.state_filter), ptr(self._dt),
+                 ptr(self._P3_table), self.num_classes, ptr(self._K64), dist, self.accel_sigma[0], self.accel_sigma[1], ptr(c.pred_poses),
+                 ptr(c.pred_rects), s)
+            rects, poses = c.pred_rects, c.pred_poses
         call("ssp_track_associate", B, T, M, ptr(c.count), ptr(c.cls), ptr(c.kp), self.match_iou, self.max_misses, ptr(self.state_tracks),
-             ptr(self.state_rects), ptr(self.state_poses), ptr(self.state_next_id), ptr(c.slot), ptr(c.track_id), ptr(c.guess),
-             ptr(c.use_guess), s)
+             ptr(rects), ptr(poses), ptr(self.state_next_id), ptr(c.slot), ptr(c.track_id), ptr(c.guess), ptr(c.use_guess), s)
         if self._dist is None:
             call("ssp_pnp_batched_guess", ptr(P3), ptr(c.kp), ptr(K32), 9, B, M, ptr(c.count), ptr(c.guess), ptr(c.use_guess), 20, ptr(c.R),
                  ptr(c.t), ptr(c.params), None, s)
@@ -312,11 +428,22 @@ class InstanceTracker:
         call("ssp_track_commit", B, T, M, ptr(c.count), ptr(c.kp), ptr(c.slot), ptr(c.params), ptr(self.state_tracks), ptr(self.state_rects),
              ptr(self.state_poses), s)
         torch.ne(c.use_guess, 0, out=c.warm)
+        if self.motion:
+            call("ssp_pose_covariance", ptr(P3), 0, ptr(K32), dist, 9, B, M, ptr(c.count), ptr(c.R), ptr(c.t), self.keypoint_sigma, ptr(c.cov_m),
+                 ptr(c.cov_status), s)
+            call("ssp_track_filter_update", B, T, M, ptr(c.count), ptr(c.slot), ptr(c.use_guess), ptr(c.R), ptr(c.t), ptr(c.cov_m),
+                 ptr(c.cov_status), ptr(self.state_filter), self.init_velocity_sigma[0], self.init_velocity_sigma[1], self.gate,
+                 ptr(c.R_filt), ptr(c.t_filt), ptr(c.pose_cov), ptr(c.velocity), ptr(c.reinit_i), s)
+            torch.ne(c.reinit_i, 0, out=c.reinit)
 
-    def update(self, logits):
+    def update(self, logits, timestamps=None):
         """one frame of every stream from the network output (B, (2K+1+C)*A, H, W) -> dict of device tensors: count, kept (B,);
         cls, track_id (B, M) int32 (-1 in empty and untracked slots); warm (B, M) bool; conf, cls_conf (B, M); keypoints_px
-        (B, M, 9, 2); R (B, M, 3, 3), t (B, M, 3), params (B, M, 6) fp64 (zero in empty slots).  Returned tensors are reused."""
+        (B, M, 9, 2); R (B, M, 3, 3), t (B, M, 3), params (B, M, 6) fp64 (zero in empty slots).  Returned tensors are reused.
+        With motion: timestamps (B,) seconds of this frame per stream (stage_times), and the outputs add, per detection slot with a
+        track, the filtered pose R_filt (B, M, 3, 3), t_filt (B, M, 3), its covariance pose_cov (B, M, 6, 6) over (dth, dt_), the
+        velocity (B, M, 6) = (w rad/s, v mesh units/s) and reinit (B, M) bool (the filter was started from this frame's PnP: a new
+        track, a measurement outside the gate or one without a usable covariance); zeros elsewhere.  R, t stay this frame's PnP."""
         if not logits.is_cuda:
             raise SspError("InstanceTracker.update runs on CUDA tensors only")
         out = logits.detach().contiguous().float()
@@ -326,6 +453,7 @@ class InstanceTracker:
             raise SspError("this tracker follows %d streams, got a batch of %d" % (self.batch, B))
         if Cn != (2 * K + 1 + nC) * nA:
             raise SspError("output has %d channels, expected (2K+1+C)*A = %d" % (Cn, (2 * K + 1 + nC) * nA))
+        self.stage_times(timestamps)
         c = self._bufs
         if c is None:
             import types
@@ -338,8 +466,9 @@ class InstanceTracker:
         s = stream_ptr()
         detect_slots(c, out, self.classes, self._P3_table, nC, nA, self.conf_thresh, self.nms_thresh, self.frame_size, s)
         self.solve(c, s, c.P3, self._K32)
+        self.staged()
         return dict(count=c.count, kept=c.kept, cls=c.cls, track_id=c.track_id, warm=c.warm, conf=c.boxes[..., 2 * K],
-                    cls_conf=c.boxes[..., 2 * K + 1], keypoints_px=c.kp, R=c.R, t=c.t, params=c.params)
+                    cls_conf=c.boxes[..., 2 * K + 1], keypoints_px=c.kp, R=c.R, t=c.t, params=c.params, **self.outputs(c))
 
 
 # ------------------------------------------------------------------------------------------ batched evaluation tail
