@@ -186,7 +186,12 @@ class Engine:
         # backward operands: one 16-bit format for dY, W and X (wgmma takes both 16-bit operands in one format).  fp16 + a static
         # loss scale (saturating conversion) is 8x more precise than bf16, and the activation planes are fp16 anyway.
         self.grad_scale = float(os.environ.get("SSP_GRAD_SCALE", "256"))
-        self.fast = os.environ.get("SSP_PRECISION", "parity").lower() == "fast"   # single-term forward (no hi/lo)
+        # SSP_PRECISION: "exact" (default: split-fp16 hi + lo forward, three products) or "fast" (single-term fp16 forward, no lo
+        # planes), case-insensitive; anything else is refused, so that a misspelt value cannot silently select the default
+        precision = os.environ.get("SSP_PRECISION", "exact").lower()
+        if precision not in ("exact", "fast"):
+            raise _lib.SspError("SSP_PRECISION=%r: expected 'exact' (the default) or 'fast'" % os.environ["SSP_PRECISION"])
+        self.fast = precision == "fast"
         self.launches = 0
         # inference split-K (forward(split_k=True)): launches of ssp_conv_gemm_splitk so far; split_override (internal, for tests and
         # tools/bench_predict.py): None = ssp_conv_splitk_count's rule, 0 = split-K off, k >= 1 = k splits (at most the k-block

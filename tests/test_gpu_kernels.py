@@ -74,20 +74,31 @@ CONV_CASES = [
     (2, 26, 26, 256, 128, 1, False),
     (2, 13, 13, 1024, 20, 1, True),
     (1, 13, 13, 1280, 512, 3, False),
+    (2, 13, 13, 1024, 160, 1, True),         # multi-object head: 160 channels, two N tiles of the per-tap kernel
 ]
 
 
-@pytest.mark.parametrize("case", CONV_CASES)
+def _operands(x, w, terms):
+    """x (NCHW), w (OIHW) fp32 on the CPU -> padded-flat planes, weight planes and the fp64 reference operands of a forward with
+    `terms` products: 3 = split fp16 (x_hi + x_lo, w_hi + w_lo; the reference takes the unrounded values), 1 = single term (no lo
+    planes; the reference takes the fp16-rounded values, whose products are exact in the fp32 accumulator)"""
+    xh, xl, rows = flat_from_nchw(x.to(DEV), split=terms == 3)
+    wh, wl, _ = _pack_w(w.to(DEV), split=terms == 3)
+    if terms == 1:
+        x, w = x.half(), w.half()
+    return xh, xl, rows, wh, wl, x.double(), w.double()
+
+
+@pytest.mark.parametrize("case", [c + (3,) for c in CONV_CASES] + [c + (1,) for c in CONV_CASES])      # last field: operand terms
 @pytest.mark.parametrize("impl", [_lib.IMPL_SIMT, _lib.IMPL_TC, _lib.IMPL_TC2, _lib.IMPL_BAND, _lib.IMPL_BANDT])
 def test_conv_gemm_matches_torch(case, impl):
-    N, H, W, cin, cout, k, use_bias = case
-    g = torch.Generator().manual_seed(hash(case) % 1000)
+    N, H, W, cin, cout, k, use_bias, terms = case
+    g = torch.Generator().manual_seed(hash(case[:7]) % 1000)
     x = torch.randn(N, cin, H, W, generator=g)
     w = torch.randn(cout, cin, k, k, generator=g) / (cin * k * k) ** 0.5
     b = torch.randn(cout, generator=g) if use_bias else None
-    ref = F.conv2d(x.double(), w.double(), None if b is None else b.double(), padding=(k - 1) // 2).float()
-    xh, xl, rows = flat_from_nchw(x.to(DEV))
-    wh, wl, _ = _pack_w(w.to(DEV))
+    xh, xl, rows, wh, wl, x64, w64 = _operands(x, w, terms)
+    ref = F.conv2d(x64, w64, None if b is None else b.double(), padding=(k - 1) // 2).float()
     ldo = (cout + 3) // 4 * 4
     y = torch.zeros(rows, ldo, device=DEV)
     ssum = torch.zeros(cout, dtype=torch.float64, device=DEV); ssq = torch.zeros_like(ssum)
@@ -490,12 +501,19 @@ def test_l0_fused_blocks_match_torch(shape):
 
 
 BANDT_FWD = [
-    # N, H, W, cin, cout, k   (split-fp16 forward with BN statistics; cout <= 64: W_hi / W_lo stacked on the M side)
-    (2, 40, 24, 32, 64, 3),        # block-2 class: 128-pixel tiles (nine resident 16 KB tiles leave room for two 136-row bands only)
-    (4, 104, 104, 32, 64, 3),      # 345 tiles: several tiles per CTA, every ring phase in use
-    (2, 26, 26, 128, 64, 1),       # 1x1, two K chunks
-    (3, 5, 7, 64, 32, 3),          # cout 32: half of each stacked plane is zero fill
-    (1, 13, 13, 64, 24, 3),        # cout not a multiple of 32
+    # N, H, W, cin, cout, k, operand terms   (forward with BN statistics; split fp16, cout <= 64: W_hi / W_lo stacked on the M side;
+    # single term, cout <= 128: channels 64-127 in the upper half (UP) of the M side)
+    (2, 40, 24, 32, 64, 3, 3),     # block-2 class: 128-pixel tiles (nine resident 16 KB tiles leave room for two 136-row bands only)
+    (4, 104, 104, 32, 64, 3, 3),   # 345 tiles: several tiles per CTA, every ring phase in use
+    (2, 26, 26, 128, 64, 1, 3),    # 1x1, two K chunks
+    (3, 5, 7, 64, 32, 3, 3),       # cout 32: half of each stacked plane is zero fill
+    (1, 13, 13, 64, 24, 3, 3),     # cout not a multiple of 32
+    (2, 40, 24, 32, 64, 3, 1),     # block 2 of the fast forward: the overlapping-row variant, single term
+    (4, 104, 104, 64, 128, 3, 1),  # blocks 4 / 6 of the fast forward: UP 3x3, nine resident tiles, many tiles per CTA, every ring phase
+    (2, 26, 26, 256, 128, 1, 1),   # block 9: UP 1x1, four K chunks
+    (1, 13, 13, 64, 100, 3, 1),    # cout > 64 and not a multiple of 8: the weight tile's row count rounds up to 104
+    (2, 26, 26, 512, 64, 1, 1),    # block 26: eight K chunks
+    (2, 13, 13, 128, 64, 1, 1),    # block 5 class
 ]
 BANDT_DGRAD = [
     # N, H, W, channels of dY (K per tap), channels of dX (<= 128), k      (single-term fp16)
@@ -510,14 +528,15 @@ BANDT_DGRAD = [
 @pytest.mark.parametrize("case", BANDT_FWD)
 def test_conv_bandt_forward_runs_and_matches_torch(case):
     """operand-swapped kernel (csrc/conv_bandt.cu): the kernel itself must have run (launch counter), outputs / BN statistics
-    against the fp64 torch convolution at the tolerance of the other tensor-core kernels."""
-    N, H, W, cin, cout, k = case
+    against the fp64 torch convolution at the tolerance of the other tensor-core kernels.  The statistics are checked per 64-channel
+    half of the M side: channels 64-127 come from the upper half of the accumulator, and only the valid pixel rows of each tile
+    (its ballot mask) may contribute."""
+    N, H, W, cin, cout, k, terms = case
     g = torch.Generator().manual_seed(31 + cin + cout + H)
     x = torch.randn(N, cin, H, W, generator=g)
     w = torch.randn(cout, cin, k, k, generator=g) / (cin * k * k) ** 0.5
-    ref = F.conv2d(x.double(), w.double(), None, padding=(k - 1) // 2).float()
-    xh, xl, rows = flat_from_nchw(x.to(DEV))
-    wh, wl, _ = _pack_w(w.to(DEV))
+    xh, xl, rows, wh, wl, x64, w64 = _operands(x, w, terms)
+    ref = F.conv2d(x64, w64, None, padding=(k - 1) // 2).float()
     ldo = (cout + 3) // 4 * 4
     y = torch.full((rows, ldo), float("nan"), device=DEV)
     ssum = torch.zeros(cout, dtype=torch.float64, device=DEV); ssq = torch.zeros_like(ssum)
@@ -530,8 +549,10 @@ def test_conv_bandt_forward_runs_and_matches_torch(case):
     tol = 2e-5 + 5e-9 * cin * k * k
     assert (out - ref).abs().max() / ref.abs().max() < tol
     s_ref = ref.double().sum(dim=(0, 2, 3)); q_ref = (ref.double() ** 2).sum(dim=(0, 2, 3))
-    assert (ssum.cpu() - s_ref).abs().max() < 1e-4 * q_ref.max().sqrt() * (N * H * W) ** 0.5
-    assert ((ssq.cpu() - q_ref).abs() / q_ref).max() < 1e-4
+    for c0 in range(0, cout, 64):
+        c = slice(c0, min(cout, c0 + 64))
+        assert (ssum.cpu()[c] - s_ref[c]).abs().max() < 1e-4 * q_ref[c].max().sqrt() * (N * H * W) ** 0.5, c0
+        assert ((ssq.cpu()[c] - q_ref[c]).abs() / q_ref[c]).max() < 1e-4, c0
 
 
 @pytest.mark.parametrize("out16", [False, True])              # fp32 plane, or the fp16 plane of SSP_EPI_F16

@@ -104,21 +104,26 @@ def _split_run(xh, xl, rows, wh, wl, S, H, W, cin, cout, k, dests, scale, shift)
     return planes
 
 
-@pytest.mark.parametrize("smode", ["two", "rule", "per_kblock"])
+# "_fast": the single-term forward of SSP_PRECISION=fast (no lo planes), against the convolution of the fp16-rounded operands
+@pytest.mark.parametrize("smode", ["two", "rule", "per_kblock", "rule_fast", "per_kblock_fast"])
 @pytest.mark.parametrize("block", sorted(LAYERS))
 def test_splitk_gemm_and_reduction_match_fp64_and_repeat_bitwise(block, smode):
     H, W, cin, cout, k, dests, rule = LAYERS[block]
     kblocks = k * k * ((cin + 63) // 64)
-    S = {"two": 2, "rule": rule, "per_kblock": kblocks}[smode]
+    fast = smode.endswith("_fast")
+    S = {"two": 2, "rule": rule, "per_kblock": kblocks}[smode[:-5] if fast else smode]
     g = torch.Generator().manual_seed(block * 7 + S)
     x = torch.randn(1, cin, H, W, generator=g)
     w = torch.randn(cout, cin, k, k, generator=g) / (cin * k * k) ** 0.5
     scale = torch.rand(cout, generator=g) + 0.5
     shift = torch.randn(cout, generator=g) * 0.1
-    y = F.conv2d(x.double(), w.double(), None, padding=(k - 1) // 2) * scale.double().view(1, -1, 1, 1) + shift.double().view(1, -1, 1, 1)
+    xr, wr = (x.half(), w.half()) if fast else (x, w)
+    y = F.conv2d(xr.double(), wr.double(), None, padding=(k - 1) // 2) * scale.double().view(1, -1, 1, 1) + shift.double().view(1, -1, 1, 1)
     z = torch.where(y > 0, y, 0.1 * y)
     xh, xl, rows = _flat(x.to(DEV))
     wh, wl = _pack_w(w.to(DEV))
+    if fast:
+        xl = wl = None
     sc, sh = scale.to(DEV), shift.to(DEV)
     assert _lib.load().ssp_conv_splitk_count(1, H, W, k * k, cin, cout, 132) == rule
     first = _split_run(xh, xl, rows, wh, wl, S, H, W, cin, cout, k, dests, sc, sh)
