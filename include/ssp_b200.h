@@ -350,6 +350,32 @@ int ssp_track_filter_update(int B, int max_tracks, int max_det, const int* count
                             double init_velocity_sigma_rot, double init_velocity_sigma_trans, double gate, double* R_filt,
                             double* t_filt, double* pose_cov, double* velocity, int* reinit, void* stream);
 
+/* ---- refinement of poses against registered depth frames: projective point-to-plane ICP (rules: csrc/refine_depth_core.h;
+ *      csrc/refine_depth.cu), fp64, one 256-thread CTA per problem, every iteration in one launch.
+ *  ssp_refine_depth: groups x per_group problems, group g = depth frame depth [g][H][W] (uint16, 0 = no measurement; depth_scale
+ *      mesh units per depth unit, 0.001 for millimetre depth and metre meshes), registered to the camera K3x3 (DEVICE fp64) with
+ *      dist8_or_null (a DEVICE double [8] as ssp_pnp_dist takes it; NULL: no distortion).  model [total][6] fp64 = (x, y, z, nx,
+ *      ny, nz) of every class's points with unit outward normals, class c's rows offsets[c] .. offsets[c + 1] - 1 (DEVICE int
+ *      [num_classes + 1]), diam [num_classes] (DEVICE fp64) its diameter; cls [groups][per_group] (DEVICE int) each problem's class.
+ *      count_or_null: DEVICE int [groups] as ssp_pnp_batched_counted (problems at m >= count[g] get zeros and status 0).  R [n][9],
+ *      t [n][3] the input poses (camera from model).  iters fixed iterations at the gates diam * g_k, g_k = gate_start *
+ *      (gate_end / gate_start)^(k / (iters - 1)): a pair whose depths differ by more is dropped.  Out: R_out, t_out the refined
+ *      pose; points_out [n] the pair count and rmse_out [n] the point-to-plane RMS residual of the last iteration (before its
+ *      update); status_out [n] 0 or SSP_REFINE_FEW_POINTS (an iteration had fewer than SSP_REFINE_MIN_POINTS pairs; also a class
+ *      outside [0, num_classes)) | SSP_REFINE_SINGULAR (a Cholesky pivot of J^T J <= 1e-12 x its largest diagonal entry) |
+ *      SSP_REFINE_BAD_POSE (the input pose is not finite or has t_z <= 0).  With a status bit the output pose is the input pose.
+ *      SSP_ERR_ARG for a null required pointer, W or H outside [1, 16384], num_classes < 1, groups < 0, per_group < 1, iters
+ *      outside [1, SSP_REFINE_MAX_ITERS], a gate not > 0 and finite or gate_end > gate_start, or depth_scale not > 0 and finite. ---- */
+#define SSP_REFINE_MIN_POINTS 50
+#define SSP_REFINE_MAX_ITERS 100
+#define SSP_REFINE_FEW_POINTS 1
+#define SSP_REFINE_SINGULAR 2
+#define SSP_REFINE_BAD_POSE 4
+int ssp_refine_depth(const unsigned short* depth, int W, int H, double depth_scale, const double* K3x3, const double* dist8_or_null,
+                     const double* model, const int* offsets, const double* diam, int num_classes, const int* cls, int groups,
+                     int per_group, const int* count_or_null, const double* R, const double* t, int iters, double gate_start,
+                     double gate_end, double* R_out, double* t_out, int* points_out, double* rmse_out, int* status_out, void* stream);
+
 /* ---- pose errors over the mesh (utils.py:50-64, valid.py:69-72, 173-177), fp64 throughout (csrc/adds.cu, csrc/adds_core.h).
  *      X [nv][3] fp64 vertices; Rt_est, Rt_gt [n][3][4] fp64 poses [R | t].
  *  ssp_adds_batched: adds_out[p] = mean_i min_j |Rt_gt[p] x_i - Rt_est[p] x_j|, the reference's adi(pts_est, pts_gt) (ADD-S, for

@@ -25,11 +25,14 @@ lives in _FramePredictor, which predict_multi.MultiPosePredictor and predict_ins
 
 Command line: python -m singleshotpose_b200.predict --datacfg cfg/ape.data --modelcfg cfg/yolo-pose.cfg --weightfile w.weights
               --out poses.npz img1.jpg img2.jpg ...
+              [--depth-dir DIR [--depth-scale 0.001 --refine-iters 10]]: refine each pose against DIR/<image stem>.png, a 16-bit
+              depth PNG registered to the image, adding the columns R_ref t_ref corners_ref_px refine_points refine_rmse refine_status
 """
 from __future__ import annotations
 
 import argparse
 import collections
+import os
 
 import numpy as np
 import torch
@@ -37,21 +40,24 @@ import torch
 from ._lib import SspError, call, load, ptr, stream_ptr
 from .engine import Buffers
 from .image import BICUBIC
-from .utils import (camera_distortion, check_pnp_args, consensus_subsets, consensus_work_bytes, distortion_tensor, inlier_bits,
-                    keypoint_bits, object_table)
+from .utils import (camera_distortion, check_pnp_args, check_refine_args, consensus_subsets, consensus_work_bytes, distortion_tensor,
+                    inlier_bits, keypoint_bits, object_table, refine_model_table)
 
 
 class _Chain:
-    """static buffers (and the graph) of one (frame size, frame source); the head's buffers come from pred._slot_buffers and
-    pred._head_buffers"""
+    """static buffers (and the graph) of one (frame size, frame source, depth source); the head's buffers come from
+    pred._slot_buffers and pred._head_buffers"""
 
-    def __init__(self, pred, Wf, Hf, src):
+    def __init__(self, pred, Wf, Hf, src, dsrc=None):
         dev, B = pred.device, pred.batch
         W, H = pred.shape
-        self.frame, self.src, self.graph = (Wf, Hf), src, None
+        self.frame, self.src, self.dsrc, self.graph = (Wf, Hf), src, dsrc, None
         self.u8 = torch.zeros(B, Hf, Wf, 3, dtype=torch.uint8, device=dev)
         self.pin = torch.zeros(B, Hf, Wf, 3, dtype=torch.uint8).pin_memory() if src == "host" else None
-        self.copied = torch.cuda.Event()          # the replay that last read `pin` has been enqueued after this
+        # depth frames (uint16 bits in int16 storage), staged like the frames when they come from the host
+        self.depth = torch.zeros(B, Hf, Wf, dtype=torch.int16, device=dev) if dsrc else None
+        self.dpin = torch.zeros(B, Hf, Wf, dtype=torch.int16).pin_memory() if dsrc == "host" else None
+        self.copied = torch.cuda.Event()          # the replay that last read `pin` / `dpin` has been enqueued after this
         self.rs = torch.empty(B, H, W, 3, dtype=torch.uint8, device=dev)
         self.x = torch.empty(B, 3, H, W, dtype=torch.float32, device=dev)
         nb = int(load().ssp_aug_resize_work_bytes(Wf, Hf, W, H, BICUBIC))
@@ -76,10 +82,14 @@ class _FramePredictor:
     distortion coefficients (dist_coeffs, utils.camera_distortion) both are cv2's distorted model: the PnP fits the raw keypoints
     (ssp_pnp_dist / ssp_pnp_consensus_dist) and the corners land on the raw frame (ssp_project_points_dist).  The coefficients are
     a device constant read by the replay; the selection (NMS, track association) works on the raw keypoints either way.
+    With meshes ({class id: (vertices, faces)}, one for every requested class) the tail ends with _refine: one ssp_refine_depth
+    launch refines every slot's pose against the call's registered depth frames (rule: csrc/refine_depth_core.h) into c.R_ref,
+    c.t_ref, and a second _project of the refined poses gives c.corners_ref.  _tail runs the whole tail; every head calls it.
     A subclass supplies the rest: _head_buffers(chain) allocates its selection's static buffers, _head(chain, stream) launches
     the selection after the forward and then the tail, and _outputs(chain) names the returned tensors."""
 
-    def __init__(self, model, objects, K, frame_size, shape, batch, graph, max_graphs, pnp, reproj_thresh, slots=None, dist_coeffs=None):
+    def __init__(self, model, objects, K, frame_size, shape, batch, graph, max_graphs, pnp, reproj_thresh, slots=None, dist_coeffs=None,
+                 meshes=None, depth_scale=0.001, refine_iters=10, refine_gate=(0.5, 0.02)):
         name = type(self).__name__
         if not torch.cuda.is_available():
             raise SspError("%s needs a CUDA device (no CPU fallback)" % name)
@@ -123,6 +133,15 @@ class _FramePredictor:
             self._zero = torch.zeros((), dtype=torch.float32, device=dev)
         else:
             self._P3 = torch.from_numpy(np.repeat(P3[None], B, 0).astype(np.float32)).to(dev)   # (B, Q, 9, 3): one per slot
+        self._refines = meshes is not None
+        if self._refines:
+            self.depth_scale, self.refine_iters, self.refine_gate = check_refine_args(depth_scale, refine_iters, refine_gate)
+            if not isinstance(meshes, dict) or sorted(meshes) != self.classes.tolist():
+                raise SspError("meshes must hold one (vertices, faces) mesh for every requested class %s, got %s"
+                               % (self.classes.tolist(), sorted(meshes) if isinstance(meshes, dict) else type(meshes).__name__))
+            self._model, self._offsets, self._diam = refine_model_table(meshes, self.num_classes, dev)
+            if not self._detects:                  # slot q: class classes[q]
+                self._slot_cls = torch.from_numpy(np.tile(self.classes.astype(np.int32), (B, 1))).to(dev)
         W, H = self.shape
         self.out_hw = self.eng.spatial(self.eng.layers[-1], H, W)               # raises for a shape off the pooling pyramid
         self._bufs = Buffers(self.eng, self.batch, H, W, False, split_k=True)
@@ -151,6 +170,13 @@ class _FramePredictor:
             c.inliers = torch.empty(B, S, K, dtype=torch.bool, device=dev)
             wb = consensus_work_bytes(K, len(self._subsets), B * S)
             c.pnp_work = torch.empty(max(wb, 8) // 8, dtype=torch.float64, device=dev)
+        if self._refines:
+            c.R_ref = torch.empty(B, S, 3, 3, dtype=torch.float64, device=dev)
+            c.t_ref = torch.empty(B, S, 3, dtype=torch.float64, device=dev)
+            c.corners_ref = torch.empty(B, S, K, 2, dtype=torch.float32, device=dev)
+            c.ref_points = torch.empty(B, S, dtype=torch.int32, device=dev)
+            c.ref_rmse = torch.empty(B, S, dtype=torch.float64, device=dev)
+            c.ref_status = torch.empty(B, S, dtype=torch.int32, device=dev)
 
     def _solve(self, c, s):
         """PnP of every slot's keypoints c.kp against its points c.P3 with the fp32 K into c.R, c.t (the consensus solve: also
@@ -174,11 +200,13 @@ class _FramePredictor:
         else:
             call("ssp_pnp_batched_counted", ptr(c.P3), ptr(c.kp), ptr(self._K32), K, B, S, ptr(c.count), 20, ptr(c.R), ptr(c.t), s)
 
-    def _project(self, c, s):
-        """c.corners: each slot's class's 9 points projected under the slot's pose (zero in empty slots)"""
+    def _project(self, c, s, R=None, t=None, corners=None):
+        """corners (default c.corners): each slot's class's 9 points projected under the slot's pose R, t (default c.R, c.t), zero
+        in empty slots"""
         B, S, K, Q = self.batch, self.num_slots, self.num_keypoints, len(self.classes)
-        c.Rt[..., :3].copy_(c.R)
-        c.Rt[..., 3].copy_(c.t)
+        R, t, corners = (c.R, c.t, c.corners) if R is None else (R, t, corners)
+        c.Rt[..., :3].copy_(R)
+        c.Rt[..., 3].copy_(t)
         # every requested class's points under every slot's pose (each point is projected on its own, so a slot's own columns are
         # what ssp_project_points gives for its class's (4, 9) points alone); each slot keeps the columns of its class
         if self._dist is None:
@@ -186,14 +214,37 @@ class _FramePredictor:
         else:
             call("ssp_project_points_dist", ptr(self._X), 4, Q * K, ptr(c.Rt), ptr(self._K64), ptr(self._dist), B * S, ptr(c.proj), s)
         if not self._detects:                      # slot q: class q
-            c.corners.copy_(torch.diagonal(c.proj.view(B, S, 2, Q, K), dim1=1, dim2=3).permute(0, 3, 2, 1))
+            corners.copy_(torch.diagonal(c.proj.view(B, S, 2, Q, K), dim1=1, dim2=3).permute(0, 3, 2, 1))
             return
         own = c.proj.view(B * S, 2, Q, K)[self._rows, :, self._slot_of[c.cls0.view(-1)]]          # (B*S, 2, K)
         torch.lt(self._slot_index, c.count.unsqueeze(1), out=c.valid)
-        torch.where(c.valid.view(B, S, 1, 1), own.view(B, S, 2, K).transpose(2, 3), self._zero, out=c.corners)
+        torch.where(c.valid.view(B, S, 1, 1), own.view(B, S, 2, K).transpose(2, 3), self._zero, out=corners)
+
+    def _refine(self, c, s):
+        """c.R_ref, c.t_ref, c.ref_points, c.ref_rmse, c.ref_status: every slot's pose refined against its frame's depth c.depth;
+        c.corners_ref its projection (empty slots: zeros)"""
+        Wf, Hf = c.frame
+        cls = self._slot_cls if not self._detects else c.cls
+        call("ssp_refine_depth", ptr(c.depth), Wf, Hf, self.depth_scale, ptr(self._K64), ptr(self._dist), ptr(self._model), ptr(self._offsets),
+             ptr(self._diam), self.num_classes, ptr(cls), self.batch, self.num_slots, ptr(c.count), ptr(c.R), ptr(c.t), self.refine_iters,
+             self.refine_gate[0], self.refine_gate[1], ptr(c.R_ref), ptr(c.t_ref), ptr(c.ref_points), ptr(c.ref_rmse), ptr(c.ref_status), s)
+        self._project(c, s, c.R_ref, c.t_ref, c.corners_ref)
+
+    def _tail(self, c, s):
+        """the pose tail every head runs after its selection: PnP, projection and, with meshes, the depth refinement"""
+        self._solve(c, s)
+        self._project(c, s)
+        if self._refines:
+            self._refine(c, s)
 
     def _consensus_outputs(self, c):
         return dict(inliers=c.inliers, hyp=c.hyp) if self.pnp == "consensus" else {}
+
+    def _refine_outputs(self, c):
+        if not self._refines:
+            return {}
+        return dict(R_ref=c.R_ref, t_ref=c.t_ref, corners_ref_px=c.corners_ref, refine_points=c.ref_points, refine_rmse=c.ref_rmse,
+                    refine_status=c.ref_status)
 
     # ------------------------------------------------------------------ inputs
     def _check(self, frames):
@@ -228,6 +279,35 @@ class _FramePredictor:
             raise SspError("empty frames %s" % (tuple(frames.shape),))
         return kind, frames
 
+    def _check_depth(self, depth, kind, frames):
+        """-> (depth source kind or None, array / tensor) for the frames checked by _check; raises SspError before anything is
+        launched: depth without meshes, no depth with meshes, or depth that is not (B, H, W) uint16 at the frames' own size"""
+        if not self._refines:
+            if depth is not None:
+                raise SspError("depth= is read by the refinement only: build the predictor with a mesh (mesh= / meshes=)")
+            return None, None
+        if depth is None:
+            raise SspError("this predictor refines its poses against depth: pass depth=(B, H, W) uint16 frames registered to the frames")
+        if kind == "jpeg":
+            from .jpeg import read_jpeg_size
+            Wf, Hf = read_jpeg_size(frames[0])
+        else:
+            Hf, Wf = int(frames.shape[1]), int(frames.shape[2])
+        if isinstance(depth, np.ndarray):
+            dkind, ok = "host", depth.dtype == np.uint16
+        elif torch.is_tensor(depth):
+            if not depth.is_cuda:
+                raise SspError("depth given as a torch tensor must be on the GPU (pass host depth as a numpy array)")
+            dkind, ok = "device", depth.dtype == torch.uint16
+        else:
+            raise SspError("depth must be a (B, H, W) uint16 numpy array or CUDA tensor, got %s" % type(depth).__name__)
+        if not ok:
+            raise SspError("depth must be uint16, got %s" % depth.dtype)
+        if tuple(depth.shape) != (self.batch, Hf, Wf):
+            raise SspError("depth must be (B, H, W) = (%d, %d, %d), registered to the frames at their own size; got %s"
+                           % (self.batch, Hf, Wf, tuple(depth.shape)))
+        return dkind, depth
+
     # ------------------------------------------------------------------ the chain
     def _body(self, c, events=None):
         """every launch of one prediction, in stream order; events (4 CUDA events, eager runs only) bracket image / forward / head"""
@@ -239,6 +319,8 @@ class _FramePredictor:
             events[0].record()
         if c.src == "host":
             c.u8.copy_(c.pin, non_blocking=True)
+        if c.dsrc == "host":
+            c.depth.copy_(c.dpin, non_blocking=True)
         for i in range(B):
             call("ssp_aug_resize_u8", ptr(c.u8[i]), Wf, Hf, 0, 0, Wf, Hf, ptr(c.rs[i]), W, H, BICUBIC, ptr(c.work), c.work.numel(), s)
             call("ssp_aug_to_tensor_u8", ptr(c.rs[i]), H * W, ptr(c.x[i]), s)
@@ -278,19 +360,20 @@ class _FramePredictor:
             self._chains.clear()
             self._sig = sig
 
-    def _chain(self, Wf, Hf, src):
-        key = (Wf, Hf, src)
+    def _chain(self, Wf, Hf, src, dsrc=None):
+        key = (Wf, Hf, src, dsrc)
         c = self._chains.get(key)
         if c is None:
-            c = _Chain(self, Wf, Hf, src)
+            c = _Chain(self, Wf, Hf, src, dsrc)
             self._chains[key] = c
             while len(self._chains) > self.max_graphs:
                 self._chains.popitem(last=False)
         self._chains.move_to_end(key)
         return c
 
-    def __call__(self, frames, to_host=False, events=None):
+    def __call__(self, frames, to_host=False, events=None, depth=None):
         kind, arr = self._check(frames)
+        dkind, darr = self._check_depth(depth, kind, arr)
         with torch.cuda.device(self.device):
             if kind == "jpeg":
                 if self._jpeg is None:
@@ -299,19 +382,25 @@ class _FramePredictor:
                 arr, kind = torch.stack(self._jpeg(arr)), "device"
             Hf, Wf = int(arr.shape[1]), int(arr.shape[2])
             self._ensure_current()
-            c = self._chain(Wf, Hf, kind)
+            c = self._chain(Wf, Hf, kind, dkind)
+            staged = kind == "host" or dkind == "host"
+            if staged:
+                c.copied.synchronize()            # the previous replay's copies out of the staging buffers have run
             if kind == "host":
-                c.copied.synchronize()            # the previous replay's copy out of the staging buffer has run
                 np.copyto(c.pin.numpy(), arr, casting="no")
             else:
                 c.u8.copy_(arr)
+            if dkind == "host":
+                np.copyto(c.dpin.numpy(), darr.view(np.int16), casting="no")
+            elif dkind == "device":
+                c.depth.copy_(darr.view(torch.int16))
             if self.use_graph and not events:
                 if c.graph is None:
                     self._capture(c)
                 c.graph.replay()
             else:
                 self._body(c, events)
-            if kind == "host":
+            if staged:
                 c.copied.record()
             self._last = c
         out = self._outputs(c)
@@ -339,12 +428,20 @@ class PosePredictor(_FramePredictor):
     keypoints, with inlier keypoints within reproj_thresh frame pixels; the outputs then add inliers (B, 9) bool and hyp (B,) int32.
     pnp="plain" (default) is the all-point solve.
     dist_coeffs: the camera's OpenCV distortion coefficients (k1, k2, p1, p2[, k3[, k4, k5, k6]]): the pose is cv2.solvePnP(...,
-    distCoeffs) of the raw keypoints and corners_px is cv2.projectPoints with them, on the raw frame; None or all zeros: no distortion."""
+    distCoeffs) of the raw keypoints and corners_px is cv2.projectPoints with them, on the raw frame; None or all zeros: no distortion.
+    mesh=(vertices (Nv, 3), faces (Nf, 3)): refine each pose against a depth frame registered to the colour frame, which every call
+    then takes as depth=(B, H, W) uint16 at the frames' size (host numpy or CUDA tensor): projective point-to-plane ICP of the mesh's
+    vertices (utils.refine_depth_batched; depth_scale mesh units per depth unit, refine_iters iterations, refine_gate the pair gate
+    range as fractions of the mesh's diameter).  The outputs add R_ref (B, 3, 3), t_ref (B, 3), corners_ref_px (B, 9, 2),
+    refine_points (B,), refine_rmse (B,) and refine_status (B,) (utils.REFINE_STATUS bits; with a bit set R_ref, t_ref are R, t);
+    R, t and the other outputs are the same bits as without a mesh."""
 
     def __init__(self, model, corners3D, K, frame_size=(640, 480), shape=None, batch=1, graph=True, max_graphs=4, pnp="plain",
-                 reproj_thresh=8.0, dist_coeffs=None):
+                 reproj_thresh=8.0, dist_coeffs=None, mesh=None, depth_scale=0.001, refine_iters=10, refine_gate=(0.5, 0.02)):
         super().__init__(model, {0: corners3D}, K, frame_size, shape if shape is not None else (model.test_width, model.test_height),
-                         batch, graph, max_graphs, pnp, reproj_thresh, dist_coeffs=dist_coeffs)
+                         batch, graph, max_graphs, pnp, reproj_thresh, dist_coeffs=dist_coeffs,
+                         meshes=None if mesh is None else {0: mesh}, depth_scale=depth_scale, refine_iters=refine_iters,
+                         refine_gate=refine_gate)
 
     def _head_buffers(self, c):
         dev, B, K = self.device, self.batch, self.num_keypoints
@@ -356,16 +453,16 @@ class PosePredictor(_FramePredictor):
         h, w = c.logits.shape[2:]
         call("ssp_region_decode_argmax", ptr(c.logits), B, K, self.num_classes, h, w, 1, ptr(c.boxes), ptr(c.conf), None, s)
         torch.mul(c.boxes[:, :2 * K].view(B, 1, K, 2), c.scale, out=c.kp)
-        self._solve(c, s)
-        self._project(c, s)
+        self._tail(c, s)
 
     def _outputs(self, c):
-        one = {k: v[:, 0] for k, v in self._consensus_outputs(c).items()}          # the one slot of each frame
+        one = {k: v[:, 0] for k, v in dict(self._consensus_outputs(c), **self._refine_outputs(c)).items()}   # the one slot of each frame
         return dict(R=c.R[:, 0], t=c.t[:, 0], conf=c.conf, keypoints_px=c.kp[:, 0], corners_px=c.corners[:, 0], **one)
 
 
 # ---------------------------------------------------------------------------------------------- command line
 CONSENSUS_KEYS = {"plain": (), "consensus": ("inliers", "hyp")}          # the .npz columns each --pnp adds
+REFINE_KEYS = ("R_ref", "t_ref", "corners_ref_px", "refine_points", "refine_rmse", "refine_status")     # the --depth-dir columns
 SIZE_KEYS = (("width", "height"),)                                      # the frame size entries of a single-object .data file
 
 
@@ -379,6 +476,46 @@ def add_dist_arg(ap):
     ap.add_argument("--dist", type=float, nargs="+", metavar="K",
                     help="the camera's OpenCV distortion coefficients k1 k2 p1 p2 [k3 [k4 k5 k6]] (cv2.calibrateCamera's distCoeffs); "
                          "overrides the .data file's dist entry.  End the list with -- when the images follow it")
+
+
+def add_depth_args(ap):
+    ap.add_argument("--depth-dir", metavar="DIR",
+                    help="refine each pose against DIR/<image stem>.png, a 16-bit depth PNG registered to the image (same size); adds "
+                         "the columns " + " ".join(REFINE_KEYS))
+    ap.add_argument("--depth-scale", type=float, default=0.001,
+                    help="--depth-dir: mesh units per depth unit (0.001 for millimetre depth and metre meshes)")
+    ap.add_argument("--refine-iters", type=int, default=10, help="--depth-dir: iterations of the refinement")
+
+
+def check_depth_args(args):
+    """SspError for a bad --depth-scale or --refine-iters given with --depth-dir"""
+    if args.depth_dir is not None:
+        check_refine_args(args.depth_scale, args.refine_iters, (0.5, 0.02))
+
+
+def refine_kwargs(args):
+    """the predictor keywords of --depth-scale and --refine-iters"""
+    return dict(depth_scale=args.depth_scale, refine_iters=args.refine_iters)
+
+
+def read_depth_png(path, size):
+    """(H, W) uint16 depth of a 16-bit grayscale PNG; SspError naming the file when it is missing, not 16-bit or not of
+    size (width, height)"""
+    from PIL import Image
+    if not os.path.isfile(path):
+        raise SspError("depth file %s does not exist" % path)
+    with Image.open(path) as im:
+        if im.mode not in ("I;16", "I;16B", "I;16L", "I"):
+            raise SspError("depth file %s is not a 16-bit grayscale PNG (mode %s)" % (path, im.mode))
+        d = np.asarray(im)
+    if d.dtype != np.uint16:
+        if d.size and (d.min() < 0 or d.max() > 65535):
+            raise SspError("depth file %s holds values outside 0..65535" % path)
+        d = d.astype(np.uint16)
+    if (d.shape[1], d.shape[0]) != tuple(size):
+        raise SspError("depth file %s is %dx%d, its image %dx%d: the depth must be registered to the image at its size"
+                       % (path, d.shape[1], d.shape[0], size[0], size[1]))
+    return d
 
 
 def camera_dist(args):
@@ -414,6 +551,12 @@ def read_camera(datacfg, size_keys):
     return o.get("mesh"), K, size
 
 
+def read_mesh(path):
+    """(vertices, faces) of a PLY mesh (utils_host.read_ply_mesh)"""
+    from .utils_host import read_ply_mesh
+    return read_ply_mesh(path)
+
+
 def mesh_corners(path):
     """(4, 8) box corners (utils.get_3D_corners) of the vertices of a PLY mesh"""
     from .utils import get_3D_corners
@@ -422,16 +565,24 @@ def mesh_corners(path):
     return get_3D_corners(np.c_[V, np.ones((len(V), 1))].T)
 
 
-def predict_files(pred, paths):
-    """yields pred's host result for each image file, one frame per call: JPEG files go to the GPU decoder, others through Pillow"""
+def predict_files(pred, paths, depth_dir=None):
+    """yields pred's host result for each image file, one frame per call: JPEG files go to the GPU decoder, others through Pillow.
+    depth_dir: each call also takes depth_dir/<image stem>.png (read_depth_png)"""
     for path in paths:
         with open(path, "rb") as f:
             data = f.read()
         if data[:2] == b"\xff\xd8":
-            yield pred([data], to_host=True)
+            from .jpeg import read_jpeg_size
+            frames, size = [data], read_jpeg_size(data)
         else:
             from PIL import Image
-            yield pred(np.asarray(Image.open(path).convert("RGB"))[None], to_host=True)
+            frames = np.asarray(Image.open(path).convert("RGB"))[None]
+            size = (frames.shape[2], frames.shape[1])
+        kw = {}
+        if depth_dir is not None:
+            stem = os.path.splitext(os.path.basename(path))[0]
+            kw["depth"] = read_depth_png(os.path.join(depth_dir, stem + ".png"), size)[None]
+        yield pred(frames, to_host=True, **kw)
 
 
 def main(argv=None):
@@ -443,9 +594,11 @@ def main(argv=None):
     ap.add_argument("--out", default="poses.npz")
     add_pnp_args(ap)
     add_dist_arg(ap)
+    add_depth_args(ap)
     ap.add_argument("images", nargs="+")
     a = ap.parse_args(argv)
     check_pnp_args(a.pnp, a.reproj_thresh)
+    check_depth_args(a)
     dist = camera_dist(a)
     from .darknet import Darknet
     mesh, K, size = read_camera(a.datacfg, SIZE_KEYS)
@@ -455,9 +608,10 @@ def main(argv=None):
     model = Darknet(a.modelcfg)
     model.load_weights(a.weightfile)
     model.cuda().eval()
-    pred = PosePredictor(model, corners3D, K, frame_size=size, pnp=a.pnp, reproj_thresh=a.reproj_thresh, dist_coeffs=dist)
-    res = {k: [] for k in ("R", "t", "conf", "keypoints_px", "corners_px") + CONSENSUS_KEYS[a.pnp]}
-    for r in predict_files(pred, a.images):
+    refine = dict(mesh=read_mesh(mesh), **refine_kwargs(a)) if a.depth_dir is not None else {}
+    pred = PosePredictor(model, corners3D, K, frame_size=size, pnp=a.pnp, reproj_thresh=a.reproj_thresh, dist_coeffs=dist, **refine)
+    res = {k: [] for k in ("R", "t", "conf", "keypoints_px", "corners_px") + CONSENSUS_KEYS[a.pnp] + (REFINE_KEYS if refine else ())}
+    for r in predict_files(pred, a.images, a.depth_dir):
         for k in res:
             res[k].append(r[k][0])
     np.savez(a.out, paths=np.array(a.images), **{k: np.stack(v) for k, v in res.items()})

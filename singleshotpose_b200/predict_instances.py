@@ -34,6 +34,8 @@ Command line: python -m singleshotpose_b200.predict_instances --datacfg cfg/occl
               [--track --motion cv [--keypoint-sigma 2 --fps 30]]: with the constant-velocity pose filter, adding the columns
               R_filt, t_filt, velocity and pose_cov
               [--pnp consensus [--reproj-thresh 8]]: the consensus PnP, with inliers and hyp columns (not with --track)
+              [--depth-dir DIR [--depth-scale 0.001 --refine-iters 10]]: refine against 16-bit depth PNGs, as predict's command line
+              (not with --track)
 """
 from __future__ import annotations
 
@@ -44,7 +46,8 @@ import torch
 
 from . import predict, predict_multi
 from ._lib import SspError
-from .predict import CONSENSUS_KEYS, _FramePredictor, add_dist_arg, add_pnp_args, camera_dist, mesh_corners, predict_files, read_camera
+from .predict import (CONSENSUS_KEYS, REFINE_KEYS, _FramePredictor, add_depth_args, add_dist_arg, add_pnp_args, camera_dist, check_depth_args,
+                      mesh_corners, predict_files, read_camera, read_mesh, refine_kwargs)
 from .predict_multi import cfg_conf_thresh, check_grid, parse_objects
 from .utils import camera_distortion, check_pnp_args, check_sigma
 from .utils_multi import InstanceTracker, check_motion_args, check_track_args, detect_buffers, detect_slots
@@ -68,10 +71,14 @@ class InstancePosePredictor(_FramePredictor):
     pnp="consensus" solves each slot with the consensus PnP (utils.pnp_consensus_batched, inliers within reproj_thresh frame
     pixels) and adds inliers (B, M, 9) bool and hyp (B, M) int32 (empty slots: False and 0); pnp="plain" (default) is the all-point
     solve.  dist_coeffs: the camera's OpenCV distortion coefficients, as predict.PosePredictor takes them (the suppression still
-    compares the raw keypoints' rectangles)."""
+    compares the raw keypoints' rectangles).
+    meshes={class id: (vertices, faces)}, one for every requested class: refine every instance's pose against the call's
+    depth=(B, H, W) uint16 frames, as predict.PosePredictor's mesh= does, adding R_ref (B, M, 3, 3), t_ref (B, M, 3),
+    corners_ref_px (B, M, 9, 2), refine_points, refine_rmse and refine_status (B, M) (empty slots: zeros)."""
 
     def __init__(self, model, objects, K, frame_size=(640, 480), shape=None, batch=1, conf_thresh=None, nms_thresh=0.4, max_instances=32,
-                 graph=True, max_graphs=4, pnp="plain", reproj_thresh=8.0, dist_coeffs=None):
+                 graph=True, max_graphs=4, pnp="plain", reproj_thresh=8.0, dist_coeffs=None, meshes=None, depth_scale=0.001, refine_iters=10,
+                 refine_gate=(0.5, 0.02)):
         self.num_anchors = int(getattr(model, "num_anchors", 0))
         if self.num_anchors < 1:
             raise SspError("InstancePosePredictor needs a model with a region head")
@@ -80,7 +87,8 @@ class InstancePosePredictor(_FramePredictor):
         if shape is None:
             shape = (model.test_width, model.test_height) if self.num_anchors == 1 else (model.width, model.height)
         super().__init__(model, objects if isinstance(objects, dict) else {0: objects}, K, frame_size, shape, batch, graph, max_graphs,
-                         pnp, reproj_thresh, slots=self.max_instances, dist_coeffs=dist_coeffs)
+                         pnp, reproj_thresh, slots=self.max_instances, dist_coeffs=dist_coeffs, meshes=meshes, depth_scale=depth_scale,
+                         refine_iters=refine_iters, refine_gate=refine_gate)
         check_grid(self, "detect")
 
     def _head_buffers(self, c):
@@ -89,13 +97,12 @@ class InstancePosePredictor(_FramePredictor):
     def _head(self, c, s):
         detect_slots(c, c.logits, self._cls_host, self._P3_table, self.num_classes, self.num_anchors, self.conf_thresh, self.nms_thresh,
                      c.frame, s)
-        self._solve(c, s)
-        self._project(c, s)
+        self._tail(c, s)
 
     def _outputs(self, c):
         K = self.num_keypoints
         return dict(count=c.count, kept=c.kept, cls=c.cls, R=c.R, t=c.t, conf=c.boxes[..., 2 * K], cls_conf=c.boxes[..., 2 * K + 1],
-                    keypoints_px=c.kp, corners_px=c.corners, **self._consensus_outputs(c))
+                    keypoints_px=c.kp, corners_px=c.corners, **self._consensus_outputs(c), **self._refine_outputs(c))
 
 
 class TrackingPosePredictor(InstancePosePredictor):
@@ -120,12 +127,14 @@ class TrackingPosePredictor(InstancePosePredictor):
     predicted rectangle, the warm start is the predicted pose, and the outputs add R_filt (B, M, 3, 3), t_filt (B, M, 3),
     pose_cov (B, M, 6, 6), velocity (B, M, 6) and reinit (B, M) bool; R and t stay this frame's PnP.  keypoint_sigma (px),
     accel_sigma, init_velocity_sigma, gate and frame_dt (s) are InstanceTracker's, and their defaults are not tuned on real data.
-    __call__ then takes timestamps= (B,) seconds per stream (default: the stream's last + frame_dt), checked before any launch."""
+    __call__ then takes timestamps= (B,) seconds per stream (default: the stream's last + frame_dt), checked before any launch.
+    meshes= (the depth refinement) is refused: how a refined pose should feed the tracks and the pose filter is not defined yet."""
 
     def __init__(self, model, objects, K, frame_size=(640, 480), shape=None, batch=1, conf_thresh=None, nms_thresh=0.4, max_instances=32,
                  max_tracks=64, match_iou=0.3, max_misses=5, graph=True, max_graphs=4, pnp="plain", dist_coeffs=None, motion=None,
-                 keypoint_sigma=2.0, accel_sigma=(2.0, 1.0), init_velocity_sigma=(1.0, 0.5), gate=22.46, frame_dt=1 / 30):
+                 keypoint_sigma=2.0, accel_sigma=(2.0, 1.0), init_velocity_sigma=(1.0, 0.5), gate=22.46, frame_dt=1 / 30, meshes=None):
         check_tracking_pnp(pnp)
+        check_tracking_meshes(meshes)
         check_track_args(max_tracks, match_iou, max_misses)
         check_motion_args(motion, keypoint_sigma, accel_sigma, init_velocity_sigma, gate, frame_dt)
         super().__init__(model, objects, K, frame_size, shape, batch, conf_thresh, nms_thresh, max_instances, graph, max_graphs,
@@ -186,6 +195,12 @@ def check_detect_args(nms_thresh, max_instances):
     return nms_thresh, int(max_instances)
 
 
+def check_tracking_meshes(meshes):
+    if meshes is not None:
+        raise SspError("tracking does not refine against depth (meshes=): how a refined pose should feed the tracks and the pose "
+                       "filter is not defined yet")
+
+
 def check_tracking_pnp(pnp):
     if pnp != "plain":
         raise SspError("tracking solves with pnp='plain' only, got %r: the consensus solve has no rule for how a track's warm guess "
@@ -198,8 +213,8 @@ SIZE_KEYS = predict_multi.SIZE_KEYS + predict.SIZE_KEYS      # a multi-object .d
 
 def parse_args(argv=None):
     """the command line, checked before any model is built: raises SspError for a bad --object, --nms-thresh, --max-instances,
-    --match-iou, --max-misses, --max-tracks, --reproj-thresh, --dist, --keypoint-sigma or --fps, for --track with --pnp consensus
-    and for --motion without --track"""
+    --match-iou, --max-misses, --max-tracks, --reproj-thresh, --dist, --keypoint-sigma, --fps, --depth-scale or --refine-iters, for
+    --track with --pnp consensus or --depth-dir and for --motion without --track"""
     ap = argparse.ArgumentParser(prog="python -m singleshotpose_b200.predict_instances",
                                  description="6-D pose of every detected instance of the requested objects in each image")
     ap.add_argument("--datacfg", required=True, help=".data file: fx fy u0 v0 and width height (or im_width im_height); mesh")
@@ -222,11 +237,15 @@ def parse_args(argv=None):
     ap.add_argument("--fps", type=float, default=30.0, help="--motion: the frame rate of the image sequence")
     add_pnp_args(ap)
     add_dist_arg(ap)
+    add_depth_args(ap)
     ap.add_argument("images", nargs="+")
     a = ap.parse_args(argv)
     check_pnp_args(a.pnp, a.reproj_thresh)
+    check_depth_args(a)
     if a.track:
         check_tracking_pnp(a.pnp)
+        if a.depth_dir is not None:
+            raise SspError("--depth-dir does not combine with --track: how a refined pose should feed the tracks is not defined yet")
     check_detect_args(a.nms_thresh, a.max_instances)
     check_track_args(a.max_tracks, a.match_iou, a.max_misses)
     if a.motion and not a.track:
@@ -257,6 +276,7 @@ def main(argv=None):
             raise SspError("%s has no mesh entry: give --object CLASS=MESH.ply" % a.datacfg)
         meshes = {0: mesh}
     objects = {c: mesh_corners(path) for c, path in meshes.items()}
+    refine = dict(meshes={c: read_mesh(p) for c, p in meshes.items()}, **refine_kwargs(a)) if a.depth_dir is not None else {}
     if _region_anchors(a.modelcfg) > 1:
         from .darknet_multi import Darknet
     else:
@@ -271,10 +291,11 @@ def main(argv=None):
                                      motion=motion, keypoint_sigma=a.keypoint_sigma, frame_dt=1.0 / a.fps)
     else:
         pred = InstancePosePredictor(model, objects, K, frame_size=size, nms_thresh=a.nms_thresh, max_instances=a.max_instances,
-                                     pnp=a.pnp, reproj_thresh=a.reproj_thresh, dist_coeffs=dist)
-    rows = {k: [] for k in ROW_KEYS + (("track_id",) if a.track else ()) + (MOTION_KEYS if motion else ()) + CONSENSUS_KEYS[a.pnp]}
+                                     pnp=a.pnp, reproj_thresh=a.reproj_thresh, dist_coeffs=dist, **refine)
+    rows = {k: [] for k in ROW_KEYS + (("track_id",) if a.track else ()) + (MOTION_KEYS if motion else ()) + CONSENSUS_KEYS[a.pnp]
+            + (REFINE_KEYS if refine else ())}
     image = []
-    for i, r in enumerate(predict_files(pred, a.images)):
+    for i, r in enumerate(predict_files(pred, a.images, a.depth_dir)):
         n = int(r["count"][0])
         image += [i] * n
         for k in rows:

@@ -10,7 +10,7 @@ from __future__ import annotations
 import numpy as np
 import torch
 
-from ._lib import call, load, ptr, stream_ptr, SspError
+from ._lib import CONSTANTS, call, load, ptr, stream_ptr, SspError
 from .utils_host import (makedirs, get_all_files, calc_pts_diameter, adi, get_2d_bb, compute_2d_bb, compute_2d_bb_from_orig_pix,  # noqa: F401
                          corner_confidences, corner_confidence, sigmoid, softmax, fix_corner_order, read_truths, read_truths_args,
                          read_pose, load_class_names, image2torch, read_data_cfg, scale_bboxes, file_lines, get_image_size, logging,
@@ -409,6 +409,116 @@ def mesh_diameter(pts):
     out = torch.empty(1, dtype=torch.float64, device=dev)
     call("ssp_mesh_diameter", ptr(P), P.shape[0], ptr(out), stream_ptr())
     return float(out.item())
+
+
+# ------------------------------------------------------------------------------------------ refinement against depth frames
+REFINE_STATUS = {"few_points": 1, "singular": 2, "bad_pose": 4}         # ssp_refine_depth's status bits (SSP_REFINE_*)
+
+
+def vertex_normals(vertices, faces):
+    """Unit outward normals (Nv, 3) float64 of a triangle mesh: each vertex sums the unnormalised cross products (b - a) x (c - a)
+    of its faces (normals weighted by area), the sum is normalised, and every normal is flipped when the mesh's signed volume is
+    negative, so a closed mesh of either winding gets outward normals.  A vertex whose sum is zero gets a zero normal (the
+    refinement never pairs it).  vertices (Nv, 3); faces (Nf, 3) indices in [0, Nv)."""
+    V = np.asarray(vertices, np.float64)
+    F = np.asarray(faces)
+    if V.ndim != 2 or V.shape[1] != 3:
+        raise SspError("vertices must be (Nv, 3), got %s" % (V.shape,))
+    if F.ndim != 2 or F.shape[1] != 3 or not np.issubdtype(F.dtype, np.integer):
+        raise SspError("faces must be (Nf, 3) integers, got %s %s" % (F.shape, F.dtype))
+    if F.size and (F.min() < 0 or F.max() >= len(V)):
+        raise SspError("a face index lies outside [0, %d)" % len(V))
+    a, b, c = V[F[:, 0]], V[F[:, 1]], V[F[:, 2]]
+    cr = np.cross(b - a, c - a)
+    N = np.zeros_like(V)
+    for k in range(3):
+        np.add.at(N, F[:, k], cr)
+    if (a * np.cross(b, c)).sum() < 0:                  # 6 x the signed volume
+        N = -N
+    norm = np.linalg.norm(N, axis=1, keepdims=True)
+    return np.divide(N, norm, out=np.zeros_like(N), where=norm > 0)
+
+
+def check_refine_args(depth_scale, iters, gate):
+    """-> (depth_scale, iters, (gate_start, gate_end)); SspError for a depth_scale not > 0 and finite, iters outside [1, 100] or a
+    gate range that is not 0 < gate_end <= gate_start < inf (fractions of the object's diameter)"""
+    depth_scale = check_sigma("depth_scale", depth_scale)
+    maxit = CONSTANTS["SSP_REFINE_MAX_ITERS"]
+    if isinstance(iters, bool) or not isinstance(iters, (int, np.integer)) or not 1 <= iters <= maxit:
+        raise SspError("refine iters must be an integer in [1, %d], got %r" % (maxit, iters))
+    try:
+        s, e = (float(g) for g in gate)
+    except (TypeError, ValueError):
+        raise SspError("the refine gate is (start, end) as fractions of the diameter, got %r" % (gate,))
+    if not (0.0 < e <= s < np.inf):
+        raise SspError("the refine gate needs 0 < end <= start < inf, got %r" % (gate,))
+    return depth_scale, int(iters), (s, e)
+
+
+def refine_model_table(meshes, num_classes, dev):
+    """{class id: (vertices, faces)} -> device (model [total][6] fp64 points and outward normals, offsets [num_classes + 1] int32,
+    diam [num_classes] fp64): the tables ssp_refine_depth reads, class c's rows at offsets[c] .. offsets[c + 1] - 1 (no rows for the
+    classes not given).  The diameter is mesh_diameter of the vertices."""
+    if not isinstance(meshes, dict) or not meshes:
+        raise SspError("meshes must be a non-empty {class id: (vertices, faces)} dict")
+    rows, counts, diam = [], np.zeros(num_classes, np.int64), np.zeros(num_classes)
+    for c in sorted(meshes):
+        if isinstance(c, bool) or not isinstance(c, (int, np.integer)) or not 0 <= c < num_classes:
+            raise SspError("class id %r is not in [0, %d)" % (c, num_classes))
+        try:
+            V, F = meshes[c]
+        except (TypeError, ValueError):
+            raise SspError("the mesh of class %d must be (vertices, faces)" % c)
+        V = np.asarray(V, np.float64)
+        N = vertex_normals(V, F)
+        rows.append(np.concatenate([V, N], 1))
+        counts[c], diam[c] = len(V), mesh_diameter(V)
+    offsets = np.concatenate([[0], np.cumsum(counts)]).astype(np.int32)
+    model = np.concatenate(rows) if rows else np.zeros((0, 6))
+    return (torch.from_numpy(np.ascontiguousarray(model)).to(dev), torch.from_numpy(offsets).to(dev), torch.from_numpy(diam).to(dev))
+
+
+def refine_depth_batched(depth, vertices, faces, K, R, t, depth_scale=0.001, iters=10, gate=(0.5, 0.02), dist_coeffs=None):
+    """Refine n poses of one mesh against n registered depth frames on the GPU (ssp_refine_depth, rule: csrc/refine_depth_core.h):
+    projective point-to-plane ICP of the mesh's vertices, with the outward normals of vertex_normals, against the depth pixel
+    each front-facing vertex projects to, over `iters` fixed iterations whose pair gate |p_z - q_z| shrinks geometrically from
+    gate[0] to gate[1] times the mesh's diameter (mesh_diameter).
+    depth (n, H, W) uint16 numpy array or CUDA tensor (0: no measurement), registered to the camera K (3, 3) with dist_coeffs
+    (camera_distortion); depth_scale: mesh units per depth unit (0.001 for millimetre depth and metre meshes); R (n, 3, 3), t (n, 3)
+    camera from model.  -> (R (n, 3, 3) fp64, t (n, 3) fp64, points (n,) int32 pairs of the last iteration, rmse (n,) fp64 its RMS
+    point-to-plane residual before the update, status (n,) int32: 0, or REFINE_STATUS bits, with which the pose is the input
+    pose), CUDA tensors."""
+    depth_scale, iters, (s, e) = check_refine_args(depth_scale, iters, gate)
+    k = camera_distortion(dist_coeffs)
+    dev = _dev()
+    if torch.is_tensor(depth):
+        if not depth.is_cuda or depth.dtype != torch.uint16:
+            raise SspError("depth given as a torch tensor must be a CUDA uint16 tensor, got %s %s" % (depth.device, depth.dtype))
+        D = depth.to(dev).view(torch.int16).contiguous()
+    else:
+        D = np.asarray(depth)
+        if D.dtype != np.uint16:
+            raise SspError("depth must be uint16, got %s" % D.dtype)
+        D = torch.from_numpy(np.ascontiguousarray(D).view(np.int16)).to(dev)
+    if D.dim() != 3:
+        raise SspError("depth must be (n, H, W), got %s" % (tuple(D.shape),))
+    n, H, W = D.shape
+    R, t = (torch.as_tensor(a).to(dev, torch.float64).contiguous() for a in (R, t))
+    R, t = R.reshape(-1, 3, 3), t.reshape(-1, 3)
+    if R.shape[0] != n or t.shape[0] != n:
+        raise SspError("refine_depth_batched: %d depth frames but R %s, t %s" % (n, tuple(R.shape), tuple(t.shape)))
+    model, offsets, diam = refine_model_table({0: (vertices, faces)}, 1, dev)
+    if n == 0:
+        return R.clone(), t.clone(), *(torch.zeros(0, dtype=d, device=dev) for d in (torch.int32, torch.float64, torch.int32))
+    Kd = torch.as_tensor(np.asarray(K, np.float64)).to(dev).contiguous()
+    cls = torch.zeros(n, dtype=torch.int32, device=dev)
+    R_out, t_out = torch.empty_like(R), torch.empty_like(t)
+    points, status = torch.empty(n, dtype=torch.int32, device=dev), torch.empty(n, dtype=torch.int32, device=dev)
+    rmse = torch.empty(n, dtype=torch.float64, device=dev)
+    call("ssp_refine_depth", ptr(D), W, H, depth_scale, ptr(Kd), None if k is None else ptr(distortion_tensor(k, dev)), ptr(model),
+         ptr(offsets), ptr(diam), 1, ptr(cls), n, 1, None, ptr(R), ptr(t), iters, s, e, ptr(R_out), ptr(t_out), ptr(points), ptr(rmse),
+         ptr(status), stream_ptr())
+    return R_out, t_out, points, rmse, status
 
 
 # ------------------------------------------------------------------------------------------ training-set creation

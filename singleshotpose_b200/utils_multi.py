@@ -259,11 +259,15 @@ class InstanceTracker:
     units/s): the velocity prior of a new track; frame_dt: the frame interval in seconds when update() is given no timestamps.
     These defaults are not tuned on real data: set keypoint_sigma to the network's keypoint error in pixels and the
     accelerations to how fast the objects can change their motion.  The filter state is one more device array, filter (B, T, 163)
-    fp64 (csrc/pose_filter_core.h's layout), and each stream's last timestamp stays on the host."""
+    fp64 (csrc/pose_filter_core.h's layout), and each stream's last timestamp stays on the host.
+    meshes= (the predictors' depth refinement) is refused: how a refined pose should feed the tracks and the filter is not defined."""
 
     def __init__(self, objects, K, num_classes, num_anchors, frame_size, batch=1, conf_thresh=0.05, nms_thresh=0.4, max_instances=32,
                  max_tracks=64, match_iou=0.3, max_misses=5, num_keypoints=9, device=None, dist_coeffs=None, motion=None,
-                 keypoint_sigma=2.0, accel_sigma=(2.0, 1.0), init_velocity_sigma=(1.0, 0.5), gate=22.46, frame_dt=1 / 30):
+                 keypoint_sigma=2.0, accel_sigma=(2.0, 1.0), init_velocity_sigma=(1.0, 0.5), gate=22.46, frame_dt=1 / 30, meshes=None):
+        if meshes is not None:
+            raise SspError("InstanceTracker does not refine against depth (meshes=): how a refined pose should feed the tracks and the "
+                           "pose filter is not defined yet")
         self.max_tracks, self.match_iou, self.max_misses = check_track_args(max_tracks, match_iou, max_misses)
         (self.motion, self.keypoint_sigma, self.accel_sigma, self.init_velocity_sigma, self.gate,
          self.frame_dt) = check_motion_args(motion, keypoint_sigma, accel_sigma, init_velocity_sigma, gate, frame_dt)
