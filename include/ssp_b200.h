@@ -376,6 +376,38 @@ int ssp_refine_depth(const unsigned short* depth, int W, int H, double depth_sca
                      int per_group, const int* count_or_null, const double* R, const double* t, int iters, double gate_start,
                      double gate_end, double* R_out, double* t_out, int* points_out, double* rmse_out, int* status_out, void* stream);
 
+/* ---- fusing the poses of several calibrated cameras (rules: csrc/multiview_core.h; csrc/multiview_rows.cu, csrc/multiview.cu), fp64.
+ *      A rig is `views` = C cameras (1..SSP_RIG_MAX_VIEWS): K3x3_f32 [C][9] (DEVICE fp32, the PnP's K), K3x3 [C][9] (DEVICE fp64, the
+ *      projection's K), dist8_or_null [C][8] (DEVICE fp64; a camera whose 8 values are all zero, or NULL, is the pinhole model) and
+ *      extrinsics camera-from-world x_c = R_rig[c] x_w + t_rig[c] (DEVICE fp64 [C][9], [C][3]).  Rows b = g * C + c (g < groups) are
+ *      camera c of capture g, each with `slots` objects: points3d [rows][slots][num_points][3] (or one shared [num_points][3]),
+ *      points2d [rows][slots][num_points][2] raw pixels, valid [rows][slots] (DEVICE bytes, nonzero: the view takes part).
+ *  ssp_fuse_views: step 1 solves every (row, slot) with its camera (max_iter LM iterations) into R_out [rows][slots][9], t_out
+ *      [rows][slots][3] and projects its points into corners_out [rows][slots][num_points][2]: the bits of ssp_pnp_batched /
+ *      ssp_pnp_dist and ssp_project_points / ssp_project_points_dist with that camera.  Per (capture, slot): each valid view's pose in
+ *      the world frame is a hypothesis; the views that agree with it (mean squared reprojection error <= gate^2, every point in
+ *      front) are fused by LM (at most max_iter steps), the views that agree with the result at reproj_thresh are fused again, and
+ *      while a fused view lies beyond reproj_thresh it leaves and the rest is refitted; the
+ *      hypothesis with the most views, then the lowest cost, then the lowest index wins.  Out: R_world [groups][slots][9], t_world
+ *      [3], world_cov [36] (keypoint_sigma^2 (J^T J)^-1 over the final views, world axes, left perturbation), views_out [C] bytes,
+ *      view_err [C] (RMS px of every valid view under the fused pose, -1 for the others), fuse_hyp (the winning view, -1 for none),
+ *      fuse_status (SSP_FUSE_NO_VALID | SSP_FUSE_NO_VIEW: zero pose, no views, view_err -1; SSP_FUSE_SINGULAR: world_cov zeros) and
+ *      corners_world [rows][slots][num_points][2] (the fused pose in each row's camera; zeros without one).  work: DEVICE scratch
+ *      (8-B aligned) of at least the *bytes_out that ssp_fuse_views_work_bytes(groups, views, slots, bytes_out) writes.  SSP_ERR_ARG
+ *      for a null pointer, views outside 1..16, num_points outside 7..10, groups < 0, slots < 1, max_iter < 1, a threshold or sigma
+ *      not > 0 and finite, gate < reproj_thresh or a short workspace. ---- */
+#define SSP_RIG_MAX_VIEWS 16
+#define SSP_FUSE_NO_VALID 1
+#define SSP_FUSE_NO_VIEW 2
+#define SSP_FUSE_SINGULAR 4
+int ssp_fuse_views_work_bytes(int groups, int views, int slots, long long* bytes_out);
+int ssp_fuse_views(const float* points3d, int points3d_shared, const float* points2d, const unsigned char* valid, int num_points, int groups,
+                   int views, int slots, const float* K3x3_f32, const double* K3x3, const double* dist8_or_null, const double* R_rig,
+                   const double* t_rig, double gate, double reproj_thresh, double keypoint_sigma, int max_iter, double* R_out,
+                   double* t_out, float* corners_out, double* R_world, double* t_world, double* world_cov, unsigned char* views_out,
+                   double* view_err, int* fuse_hyp, int* fuse_status, float* corners_world, void* work, long long work_bytes,
+                   void* stream);
+
 /* ---- pose errors over the mesh (utils.py:50-64, valid.py:69-72, 173-177), fp64 throughout (csrc/adds.cu, csrc/adds_core.h).
  *      X [nv][3] fp64 vertices; Rt_est, Rt_gt [n][3][4] fp64 poses [R | t].
  *  ssp_adds_batched: adds_out[p] = mean_i min_j |Rt_gt[p] x_i - Rt_est[p] x_j|, the reference's adi(pts_est, pts_gt) (ADD-S, for

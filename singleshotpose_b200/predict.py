@@ -27,6 +27,8 @@ Command line: python -m singleshotpose_b200.predict --datacfg cfg/ape.data --mod
               --out poses.npz img1.jpg img2.jpg ...
               [--depth-dir DIR [--depth-scale 0.001 --refine-iters 10]]: refine each pose against DIR/<image stem>.png, a 16-bit
               depth PNG registered to the image, adding the columns R_ref t_ref corners_ref_px refine_points refine_rmse refine_status
+              [--rig rig.npz]: the images come in groups of C calibrated cameras (image i is camera i % C; utils_host.read_rig), adding
+              the per-capture columns R_world t_world world_cov views view_err fuse_hyp fuse_status and the per-image corners_world_px
 """
 from __future__ import annotations
 
@@ -40,8 +42,8 @@ import torch
 from ._lib import SspError, call, load, ptr, stream_ptr
 from .engine import Buffers
 from .image import BICUBIC
-from .utils import (camera_distortion, check_pnp_args, check_refine_args, consensus_subsets, consensus_work_bytes, distortion_tensor,
-                    inlier_bits, keypoint_bits, object_table, refine_model_table)
+from .utils import (CameraRig, camera_distortion, check_fuse_args, check_pnp_args, check_refine_args, consensus_subsets, consensus_work_bytes,
+                    distortion_tensor, fuse_work_bytes, inlier_bits, keypoint_bits, object_table, refine_model_table, rig_tensors)
 
 
 class _Chain:
@@ -84,12 +86,15 @@ class _FramePredictor:
     a device constant read by the replay; the selection (NMS, track association) works on the raw keypoints either way.
     With meshes ({class id: (vertices, faces)}, one for every requested class) the tail ends with _refine: one ssp_refine_depth
     launch refines every slot's pose against the call's registered depth frames (rule: csrc/refine_depth_core.h) into c.R_ref,
-    c.t_ref, and a second _project of the refined poses gives c.corners_ref.  _tail runs the whole tail; every head calls it.
+    c.t_ref, and a second _project of the refined poses gives c.corners_ref.  With a rig (utils.camera_rig of C cameras;
+    row b = g C + c is camera c of capture g) the tail is _fuse instead: one ssp_fuse_views (rule: csrc/multiview_core.h) solves
+    every row with its own camera into c.R, c.t, c.corners and fuses each capture's valid views (the head's flags) into one world
+    pose per slot.  _tail runs the whole tail; every head calls it.
     A subclass supplies the rest: _head_buffers(chain) allocates its selection's static buffers, _head(chain, stream) launches
     the selection after the forward and then the tail, and _outputs(chain) names the returned tensors."""
 
     def __init__(self, model, objects, K, frame_size, shape, batch, graph, max_graphs, pnp, reproj_thresh, slots=None, dist_coeffs=None,
-                 meshes=None, depth_scale=0.001, refine_iters=10, refine_gate=(0.5, 0.02)):
+                 meshes=None, depth_scale=0.001, refine_iters=10, refine_gate=(0.5, 0.02), rig=None, fuse=(40.0, 8.0, 2.0)):
         name = type(self).__name__
         if not torch.cuda.is_available():
             raise SspError("%s needs a CUDA device (no CPU fallback)" % name)
@@ -106,6 +111,11 @@ class _FramePredictor:
         dev = self.eng.device if self.eng.device is not None else torch.device("cuda", torch.cuda.current_device())
         self.device = dev
         self.eng.materialize(dev)
+        self.rig = rig
+        if rig is not None:
+            check_rig_predictor(name, rig, K, dist_coeffs, pnp, meshes, slots, self.batch)
+            self.fuse_gate, self.fuse_thresh, self.keypoint_sigma = check_fuse_args(*fuse)
+            K = rig.K[0]                        # object_table's check only: each row is solved and projected with its camera's K
         self.classes, points, Km = object_table(objects, self.num_classes, K)
         dist = camera_distortion(dist_coeffs)
         self.dist_coeffs = dist                                                  # (8,) float64, or None: no distortion
@@ -133,6 +143,8 @@ class _FramePredictor:
             self._zero = torch.zeros((), dtype=torch.float32, device=dev)
         else:
             self._P3 = torch.from_numpy(np.repeat(P3[None], B, 0).astype(np.float32)).to(dev)   # (B, Q, 9, 3): one per slot
+        if rig is not None:
+            self._rig = rig_tensors(rig, dev)
         self._refines = meshes is not None
         if self._refines:
             self.depth_scale, self.refine_iters, self.refine_gate = check_refine_args(depth_scale, refine_iters, refine_gate)
@@ -177,6 +189,18 @@ class _FramePredictor:
             c.ref_points = torch.empty(B, S, dtype=torch.int32, device=dev)
             c.ref_rmse = torch.empty(B, S, dtype=torch.float64, device=dev)
             c.ref_status = torch.empty(B, S, dtype=torch.int32, device=dev)
+        if self.rig is not None:
+            G, Cn = B // len(self.rig.K), len(self.rig.K)
+            c.R_world = torch.empty(G, S, 3, 3, dtype=torch.float64, device=dev)
+            c.t_world = torch.empty(G, S, 3, dtype=torch.float64, device=dev)
+            c.world_cov = torch.empty(G, S, 6, 6, dtype=torch.float64, device=dev)
+            c.views = torch.empty(G, S, Cn, dtype=torch.bool, device=dev)
+            c.view_err = torch.empty(G, S, Cn, dtype=torch.float64, device=dev)
+            c.fuse_hyp = torch.empty(G, S, dtype=torch.int32, device=dev)
+            c.fuse_status = torch.empty(G, S, dtype=torch.int32, device=dev)
+            c.corners_world = torch.empty(B, S, K, 2, dtype=torch.float32, device=dev)
+            c.row_valid = torch.empty(B, S, dtype=torch.bool, device=dev)
+            c.fuse_work = torch.empty(max(fuse_work_bytes(G, Cn, S), 8) // 8, dtype=torch.float64, device=dev)
 
     def _solve(self, c, s):
         """PnP of every slot's keypoints c.kp against its points c.P3 with the fp32 K into c.R, c.t (the consensus solve: also
@@ -230,8 +254,22 @@ class _FramePredictor:
              self.refine_gate[0], self.refine_gate[1], ptr(c.R_ref), ptr(c.t_ref), ptr(c.ref_points), ptr(c.ref_rmse), ptr(c.ref_status), s)
         self._project(c, s, c.R_ref, c.t_ref, c.corners_ref)
 
-    def _tail(self, c, s):
-        """the pose tail every head runs after its selection: PnP, projection and, with meshes, the depth refinement"""
+    def _fuse(self, c, s, valid):
+        """with a rig: every row's PnP and projection with its camera into c.R, c.t, c.corners, and each capture's valid views
+        (valid (B, S) bool) fused into c.R_world, c.t_world, ... (ssp_fuse_views)"""
+        K32, K64, D, Rr, tr = self._rig
+        Cn = len(self.rig.K)
+        call("ssp_fuse_views", ptr(c.P3), 0, ptr(c.kp), ptr(valid), self.num_keypoints, self.batch // Cn, Cn, self.num_slots, ptr(K32), ptr(K64),
+             ptr(D), ptr(Rr), ptr(tr), self.fuse_gate, self.fuse_thresh, self.keypoint_sigma, 20, ptr(c.R), ptr(c.t), ptr(c.corners),
+             ptr(c.R_world), ptr(c.t_world), ptr(c.world_cov), ptr(c.views), ptr(c.view_err), ptr(c.fuse_hyp), ptr(c.fuse_status),
+             ptr(c.corners_world), ptr(c.fuse_work), c.fuse_work.numel() * 8, s)
+
+    def _tail(self, c, s, valid=None):
+        """the pose tail every head runs after its selection: PnP, projection and, with meshes, the depth refinement; with a rig
+        the fusion of the views whose slots are valid (B, S) bool"""
+        if self.rig is not None:
+            self._fuse(c, s, valid)
+            return
         self._solve(c, s)
         self._project(c, s)
         if self._refines:
@@ -239,6 +277,12 @@ class _FramePredictor:
 
     def _consensus_outputs(self, c):
         return dict(inliers=c.inliers, hyp=c.hyp) if self.pnp == "consensus" else {}
+
+    def _fuse_outputs(self, c):
+        if self.rig is None:
+            return {}
+        return dict(R_world=c.R_world, t_world=c.t_world, world_cov=c.world_cov, views=c.views, view_err=c.view_err, fuse_hyp=c.fuse_hyp,
+                    fuse_status=c.fuse_status, corners_world_px=c.corners_world)
 
     def _refine_outputs(self, c):
         if not self._refines:
@@ -434,14 +478,24 @@ class PosePredictor(_FramePredictor):
     vertices (utils.refine_depth_batched; depth_scale mesh units per depth unit, refine_iters iterations, refine_gate the pair gate
     range as fractions of the mesh's diameter).  The outputs add R_ref (B, 3, 3), t_ref (B, 3), corners_ref_px (B, 9, 2),
     refine_points (B,), refine_rmse (B,) and refine_status (B,) (utils.REFINE_STATUS bits; with a bit set R_ref, t_ref are R, t);
-    R, t and the other outputs are the same bits as without a mesh."""
+    R, t and the other outputs are the same bits as without a mesh.
+    rig=utils.camera_rig(...) of C calibrated cameras (K=None; no dist_coeffs, each camera brings its own): batch is a multiple of
+    C and frame g C + c is camera c of capture g.  R, t, corners_px are each frame's pose with its own camera; a frame's view takes
+    part in the fusion when conf > conf_thresh (default the cfg's [net] conf_thresh).  The outputs add, per capture, R_world (G, 3, 3),
+    t_world (G, 3) world-from-object, world_cov (G, 6, 6), views (G, C) bool, view_err (G, C), fuse_hyp (G,), fuse_status (G,)
+    (utils.fuse_views_batched, fuse = (gate, reproj_thresh, keypoint_sigma)), and per frame corners_world_px (B, 9, 2), the fused
+    pose in the frame's camera.  Not with pnp="consensus" or a mesh."""
 
     def __init__(self, model, corners3D, K, frame_size=(640, 480), shape=None, batch=1, graph=True, max_graphs=4, pnp="plain",
-                 reproj_thresh=8.0, dist_coeffs=None, mesh=None, depth_scale=0.001, refine_iters=10, refine_gate=(0.5, 0.02)):
+                 reproj_thresh=8.0, dist_coeffs=None, mesh=None, depth_scale=0.001, refine_iters=10, refine_gate=(0.5, 0.02), rig=None,
+                 conf_thresh=None, fuse=(40.0, 8.0, 2.0)):
+        if rig is not None:
+            from .predict_multi import cfg_conf_thresh
+            self.conf_thresh = cfg_conf_thresh(model, conf_thresh)
         super().__init__(model, {0: corners3D}, K, frame_size, shape if shape is not None else (model.test_width, model.test_height),
                          batch, graph, max_graphs, pnp, reproj_thresh, dist_coeffs=dist_coeffs,
                          meshes=None if mesh is None else {0: mesh}, depth_scale=depth_scale, refine_iters=refine_iters,
-                         refine_gate=refine_gate)
+                         refine_gate=refine_gate, rig=rig, fuse=fuse)
 
     def _head_buffers(self, c):
         dev, B, K = self.device, self.batch, self.num_keypoints
@@ -453,14 +507,34 @@ class PosePredictor(_FramePredictor):
         h, w = c.logits.shape[2:]
         call("ssp_region_decode_argmax", ptr(c.logits), B, K, self.num_classes, h, w, 1, ptr(c.boxes), ptr(c.conf), None, s)
         torch.mul(c.boxes[:, :2 * K].view(B, 1, K, 2), c.scale, out=c.kp)
-        self._tail(c, s)
+        if self.rig is not None:
+            torch.gt(c.conf.view(B, 1), self.conf_thresh, out=c.row_valid)
+        self._tail(c, s, c.row_valid if self.rig is not None else None)
 
     def _outputs(self, c):
-        one = {k: v[:, 0] for k, v in dict(self._consensus_outputs(c), **self._refine_outputs(c)).items()}   # the one slot of each frame
+        one = {k: v[:, 0] for k, v in dict(self._consensus_outputs(c), **self._refine_outputs(c), **self._fuse_outputs(c)).items()}   # the one slot of each frame
         return dict(R=c.R[:, 0], t=c.t[:, 0], conf=c.conf, keypoints_px=c.kp[:, 0], corners_px=c.corners[:, 0], **one)
 
 
+def check_rig_predictor(name, rig, K, dist_coeffs, pnp, meshes, slots, batch):
+    """SspError for what a predictor with a rig refuses: a rig that is not a utils.CameraRig, K or dist_coeffs given as well
+    (each camera brings its own), pnp="consensus", meshes, a detecting head, or a batch that is not whole captures"""
+    if not isinstance(rig, CameraRig):
+        raise SspError("rig must be a CameraRig (utils.camera_rig)")
+    if K is not None or dist_coeffs is not None:
+        raise SspError("%s with a rig takes K=None and no dist_coeffs: each camera of the rig brings its own" % name)
+    if pnp != "plain":
+        raise SspError("%s with a rig fuses the plain per-view solves: pnp=%r is not supported with a rig" % (name, pnp))
+    if meshes is not None:
+        raise SspError("%s: depth refinement (mesh= / meshes=) is not supported with a rig" % name)
+    if slots is not None:
+        raise SspError("%s detects instances: associating instances across the views of a rig is not supported" % name)
+    if batch % len(rig.K):
+        raise SspError("batch %d is not a multiple of the rig's %d cameras" % (batch, len(rig.K)))
+
+
 # ---------------------------------------------------------------------------------------------- command line
+FUSE_KEYS = ("R_world", "t_world", "world_cov", "views", "view_err", "fuse_hyp", "fuse_status", "corners_world_px")     # the --rig columns
 CONSENSUS_KEYS = {"plain": (), "consensus": ("inliers", "hyp")}          # the .npz columns each --pnp adds
 REFINE_KEYS = ("R_ref", "t_ref", "corners_ref_px", "refine_points", "refine_rmse", "refine_status")     # the --depth-dir columns
 SIZE_KEYS = (("width", "height"),)                                      # the frame size entries of a single-object .data file
@@ -485,6 +559,31 @@ def add_depth_args(ap):
     ap.add_argument("--depth-scale", type=float, default=0.001,
                     help="--depth-dir: mesh units per depth unit (0.001 for millimetre depth and metre meshes)")
     ap.add_argument("--refine-iters", type=int, default=10, help="--depth-dir: iterations of the refinement")
+
+
+def add_rig_arg(ap):
+    ap.add_argument("--rig", metavar="RIG.npz",
+                    help="fuse the views of several calibrated cameras (utils_host.read_rig: K, R, t[, dist] per camera): the images come "
+                         "in groups of C, image i is camera i %% C; adds the columns " + " ".join(FUSE_KEYS))
+
+
+def check_rig_args(args):
+    """-> the --rig file's CameraRig, or None; SspError for --rig with --dist, --depth-dir or --pnp consensus, or an image count
+    that is not a multiple of the rig's cameras"""
+    if args.rig is None:
+        return None
+    if args.dist is not None:
+        raise SspError("--dist and --rig: each camera of the rig brings its own distortion coefficients (the rig's dist)")
+    if args.depth_dir is not None:
+        raise SspError("--depth-dir is not supported with --rig")
+    if args.pnp != "plain":
+        raise SspError("--pnp %s is not supported with --rig" % args.pnp)
+    from .utils_host import read_rig
+    rig = read_rig(args.rig)
+    if len(args.images) % len(rig.K):
+        raise SspError("%d images are not whole captures of the rig's %d cameras: give the images in groups of %d"
+                       % (len(args.images), len(rig.K), len(rig.K)))
+    return rig
 
 
 def check_depth_args(args):
@@ -565,23 +664,29 @@ def mesh_corners(path):
     return get_3D_corners(np.c_[V, np.ones((len(V), 1))].T)
 
 
-def predict_files(pred, paths, depth_dir=None):
-    """yields pred's host result for each image file, one frame per call: JPEG files go to the GPU decoder, others through Pillow.
-    depth_dir: each call also takes depth_dir/<image stem>.png (read_depth_png)"""
-    for path in paths:
-        with open(path, "rb") as f:
-            data = f.read()
-        if data[:2] == b"\xff\xd8":
+def predict_files(pred, paths, depth_dir=None, group=1):
+    """yields pred's host result for each group of `group` image files, one call per group: JPEG files go to the GPU decoder, others
+    (or a group that mixes them) through Pillow.  depth_dir: each call also takes depth_dir/<image stem>.png (read_depth_png)"""
+    for i in range(0, len(paths), group):
+        chunk = paths[i:i + group]
+        datas = []
+        for path in chunk:
+            with open(path, "rb") as f:
+                datas.append(f.read())
+        if all(d[:2] == b"\xff\xd8" for d in datas):
             from .jpeg import read_jpeg_size
-            frames, size = [data], read_jpeg_size(data)
+            frames, size = datas, read_jpeg_size(datas[0])
         else:
             from PIL import Image
-            frames = np.asarray(Image.open(path).convert("RGB"))[None]
+            arrays = [np.asarray(Image.open(path).convert("RGB")) for path in chunk]
+            if len({a.shape for a in arrays}) != 1:
+                raise SspError("the images of one capture must have one size: %s" % ", ".join(chunk))
+            frames = np.stack(arrays)
             size = (frames.shape[2], frames.shape[1])
         kw = {}
         if depth_dir is not None:
-            stem = os.path.splitext(os.path.basename(path))[0]
-            kw["depth"] = read_depth_png(os.path.join(depth_dir, stem + ".png"), size)[None]
+            stems = [os.path.splitext(os.path.basename(p))[0] for p in chunk]
+            kw["depth"] = np.stack([read_depth_png(os.path.join(depth_dir, st + ".png"), size) for st in stems])
         yield pred(frames, to_host=True, **kw)
 
 
@@ -595,11 +700,13 @@ def main(argv=None):
     add_pnp_args(ap)
     add_dist_arg(ap)
     add_depth_args(ap)
+    add_rig_arg(ap)
     ap.add_argument("images", nargs="+")
     a = ap.parse_args(argv)
     check_pnp_args(a.pnp, a.reproj_thresh)
     check_depth_args(a)
-    dist = camera_dist(a)
+    rig = check_rig_args(a)
+    dist = camera_dist(a) if rig is None else None
     from .darknet import Darknet
     mesh, K, size = read_camera(a.datacfg, SIZE_KEYS)
     if mesh is None:
@@ -609,11 +716,13 @@ def main(argv=None):
     model.load_weights(a.weightfile)
     model.cuda().eval()
     refine = dict(mesh=read_mesh(mesh), **refine_kwargs(a)) if a.depth_dir is not None else {}
-    pred = PosePredictor(model, corners3D, K, frame_size=size, pnp=a.pnp, reproj_thresh=a.reproj_thresh, dist_coeffs=dist, **refine)
-    res = {k: [] for k in ("R", "t", "conf", "keypoints_px", "corners_px") + CONSENSUS_KEYS[a.pnp] + (REFINE_KEYS if refine else ())}
-    for r in predict_files(pred, a.images, a.depth_dir):
+    cams = dict(K=K) if rig is None else dict(K=None, rig=rig, batch=len(rig.K))
+    pred = PosePredictor(model, corners3D, frame_size=size, pnp=a.pnp, reproj_thresh=a.reproj_thresh, dist_coeffs=dist, **cams, **refine)
+    res = {k: [] for k in ("R", "t", "conf", "keypoints_px", "corners_px") + CONSENSUS_KEYS[a.pnp] + (REFINE_KEYS if refine else ())
+           + (FUSE_KEYS if rig is not None else ())}
+    for r in predict_files(pred, a.images, a.depth_dir, pred.batch):
         for k in res:
-            res[k].append(r[k][0])
+            res[k].extend(r[k])
     np.savez(a.out, paths=np.array(a.images), **{k: np.stack(v) for k, v in res.items()})
     print("%d poses -> %s" % (len(a.images), a.out))
 

@@ -23,6 +23,7 @@ Returned device tensors are the predictor's static outputs: the next call overwr
 Command line: python -m singleshotpose_b200.predict_multi --datacfg cfg/occlusion.data --modelcfg cfg/yolo-pose-multi.cfg
               --weightfile w.weights --object 0=../LINEMOD/ape/ape.ply --object 4=../LINEMOD/can/can.ply --out poses.npz img...
               [--depth-dir DIR [--depth-scale 0.001 --refine-iters 10]]: refine against 16-bit depth PNGs, as predict's command line
+              [--rig rig.npz]: fuse the views of several calibrated cameras, as predict's command line
 """
 from __future__ import annotations
 
@@ -33,8 +34,8 @@ import numpy as np
 import torch
 
 from ._lib import SspError, call, ptr
-from .predict import (CONSENSUS_KEYS, REFINE_KEYS, _FramePredictor, add_depth_args, add_dist_arg, add_pnp_args, camera_dist, check_depth_args,
-                      mesh_corners, predict_files, read_camera, read_mesh, refine_kwargs)
+from .predict import (CONSENSUS_KEYS, FUSE_KEYS, REFINE_KEYS, _FramePredictor, add_depth_args, add_dist_arg, add_pnp_args, add_rig_arg, camera_dist,
+                      check_depth_args, check_rig_args, mesh_corners, predict_files, read_camera, read_mesh, refine_kwargs)
 from .utils import check_pnp_args
 
 MAX_ENTRIES = 4096          # H*W*num_anchors the select kernel keeps in shared memory (eval_multi_core.h kMaxEntries)
@@ -55,17 +56,22 @@ class MultiPosePredictor(_FramePredictor):
     dist_coeffs: the camera's OpenCV distortion coefficients, as predict.PosePredictor takes them.
     meshes={class id: (vertices, faces)}, one for every requested class: refine every slot's pose against the call's depth=(B, H, W)
     uint16 frames, as predict.PosePredictor's mesh= does, adding R_ref (B, Q, 3, 3), t_ref (B, Q, 3), corners_ref_px (B, Q, 9, 2),
-    refine_points, refine_rmse and refine_status (B, Q)."""
+    refine_points, refine_rmse and refine_status (B, Q).
+    rig=utils.camera_rig(...) of C calibrated cameras (K=None, no dist_coeffs): frame g C + c is camera c of capture g, and each
+    class's detected views are fused into one world pose, as predict.PosePredictor's rig= does; the outputs add R_world (G, Q, 3, 3),
+    t_world (G, Q, 3), world_cov (G, Q, 6, 6), views (G, Q, C), view_err (G, Q, C), fuse_hyp, fuse_status (G, Q) and
+    corners_world_px (B, Q, 9, 2)."""
 
     def __init__(self, model, objects, K, frame_size=(640, 480), shape=None, batch=1, conf_thresh=None, graph=True, max_graphs=4,
-                 pnp="plain", reproj_thresh=8.0, dist_coeffs=None, meshes=None, depth_scale=0.001, refine_iters=10, refine_gate=(0.5, 0.02)):
+                 pnp="plain", reproj_thresh=8.0, dist_coeffs=None, meshes=None, depth_scale=0.001, refine_iters=10, refine_gate=(0.5, 0.02),
+                 rig=None, fuse=(40.0, 8.0, 2.0)):
         self.num_anchors = int(getattr(model, "num_anchors", 0))
         if self.num_anchors < 2:
             raise SspError("MultiPosePredictor needs a multi-anchor region head (yolo-pose-multi.cfg), got %d anchor(s)" % self.num_anchors)
         self.conf_thresh = cfg_conf_thresh(model, conf_thresh)
         super().__init__(model, objects, K, frame_size, shape if shape is not None else (model.width, model.height), batch, graph,
                          max_graphs, pnp, reproj_thresh, dist_coeffs=dist_coeffs, meshes=meshes, depth_scale=depth_scale,
-                         refine_iters=refine_iters, refine_gate=refine_gate)
+                         refine_iters=refine_iters, refine_gate=refine_gate, rig=rig, fuse=fuse)
         check_grid(self, "select")
         self._classes = torch.from_numpy(self.classes).to(self.device)
 
@@ -82,12 +88,12 @@ class MultiPosePredictor(_FramePredictor):
              C.c_void_p(self._cls_host.ctypes.data), len(self.classes), self.conf_thresh, float(Wf), float(Hf), ptr(c.boxes),
              ptr(c.flags), ptr(c.kp), s)
         torch.eq(c.flags, 0, out=c.detected)
-        self._tail(c, s)
+        self._tail(c, s, c.detected)
 
     def _outputs(self, c):
         K = self.num_keypoints
         return dict(classes=self._classes, R=c.R, t=c.t, conf=c.boxes[..., 2 * K], cls_conf=c.boxes[..., 2 * K + 1], detected=c.detected,
-                    keypoints_px=c.kp, corners_px=c.corners, **self._consensus_outputs(c), **self._refine_outputs(c))
+                    keypoints_px=c.kp, corners_px=c.corners, **self._consensus_outputs(c), **self._refine_outputs(c), **self._fuse_outputs(c))
 
 
 def cfg_conf_thresh(model, conf_thresh):
@@ -142,11 +148,13 @@ def main(argv=None):
     add_pnp_args(ap)
     add_dist_arg(ap)
     add_depth_args(ap)
+    add_rig_arg(ap)
     ap.add_argument("images", nargs="+")
     a = ap.parse_args(argv)
     check_pnp_args(a.pnp, a.reproj_thresh)
     check_depth_args(a)
-    dist = camera_dist(a)
+    rig = check_rig_args(a)
+    dist = camera_dist(a) if rig is None else None
     from .darknet_multi import Darknet
     _mesh, K, size = read_camera(a.datacfg, SIZE_KEYS)
     paths = parse_objects(a.object)
@@ -155,11 +163,12 @@ def main(argv=None):
     model = Darknet(a.modelcfg)
     model.load_weights(a.weightfile)
     model.cuda().eval()
-    pred = MultiPosePredictor(model, objects, K, frame_size=size, pnp=a.pnp, reproj_thresh=a.reproj_thresh, dist_coeffs=dist, **refine)
-    res = {k: [] for k in OUTPUT_KEYS + CONSENSUS_KEYS[a.pnp] + (REFINE_KEYS if refine else ())}
-    for r in predict_files(pred, a.images, a.depth_dir):
+    cams = dict(K=K) if rig is None else dict(K=None, rig=rig, batch=len(rig.K))
+    pred = MultiPosePredictor(model, objects, frame_size=size, pnp=a.pnp, reproj_thresh=a.reproj_thresh, dist_coeffs=dist, **cams, **refine)
+    res = {k: [] for k in OUTPUT_KEYS + CONSENSUS_KEYS[a.pnp] + (REFINE_KEYS if refine else ()) + (FUSE_KEYS if rig is not None else ())}
+    for r in predict_files(pred, a.images, a.depth_dir, pred.batch):
         for k in res:
-            res[k].append(r[k][0])
+            res[k].extend(r[k])
     np.savez(a.out, paths=np.array(a.images), classes=pred.classes, **{k: np.stack(v) for k, v in res.items()})
     print("%d images x %d objects -> %s" % (len(a.images), len(pred.classes), a.out))
 

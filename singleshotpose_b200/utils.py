@@ -7,6 +7,8 @@ pnp_batched, project_points_batched) expose the same kernels without the per-ima
 """
 from __future__ import annotations
 
+import collections
+
 import numpy as np
 import torch
 
@@ -519,6 +521,113 @@ def refine_depth_batched(depth, vertices, faces, K, R, t, depth_scale=0.001, ite
          ptr(offsets), ptr(diam), 1, ptr(cls), n, 1, None, ptr(R), ptr(t), iters, s, e, ptr(R_out), ptr(t_out), ptr(points), ptr(rmse),
          ptr(status), stream_ptr())
     return R_out, t_out, points, rmse, status
+
+
+# ------------------------------------------------------------------------------------------ several calibrated cameras
+FUSE_STATUS = {"no_valid": 1, "no_view": 2, "singular": 4}              # ssp_fuse_views' status bits (SSP_FUSE_*)
+CameraRig = collections.namedtuple("CameraRig", "K R t dist")
+
+
+def camera_rig(K, R, t, dist=None):
+    """A rig of C calibrated cameras (1 <= C <= 16), checked -> CameraRig(K (C, 3, 3), R (C, 3, 3), t (C, 3) float64, dist (C, 8)
+    float64 or None).  K: each camera's intrinsics; R, t: its extrinsics camera-from-world, x_c = R_c x_w + t_c, in the mesh's
+    units; dist: None, or one set of OpenCV coefficients per camera (4, 5 or 8 values each, camera_distortion; None or zeros for a
+    pinhole camera).  SspError for a value that is not finite, fx or fy <= 0, an R_c that is not a rotation (|R^T R - I| > 1e-6 or
+    det < 0), C outside 1..16 or shapes that disagree.  cv2.stereoCalibrate's (K1, d1, K2, d2, R, T) is camera_rig([K1, K2],
+    [I, R], [0, T], [d1, d2]): the world frame is camera 0's."""
+    try:
+        K, R, t = (np.asarray(a, np.float64) for a in (K, R, t))
+    except (TypeError, ValueError):
+        raise SspError("the rig's K, R and t must be numeric arrays")
+    C = len(K) if K.ndim == 3 else -1
+    maxv = CONSTANTS["SSP_RIG_MAX_VIEWS"]
+    if not 1 <= C <= maxv:
+        raise SspError("a rig has 1..%d cameras: K must be (C, 3, 3), got %s" % (maxv, K.shape))
+    if K.shape != (C, 3, 3) or R.shape != (C, 3, 3) or t.shape != (C, 3):
+        raise SspError("the rig's shapes disagree: K %s, R %s, t %s for (C, 3, 3), (C, 3, 3), (C, 3)" % (K.shape, R.shape, t.shape))
+    if not (np.isfinite(K).all() and np.isfinite(R).all() and np.isfinite(t).all()):
+        raise SspError("the rig's K, R and t must be finite")
+    if not ((K[:, 0, 0] > 0).all() and (K[:, 1, 1] > 0).all()):
+        raise SspError("every camera needs fx > 0 and fy > 0")
+    for c in range(C):
+        if np.abs(R[c].T @ R[c] - np.eye(3)).max() > 1e-6 or np.linalg.det(R[c]) < 0:
+            raise SspError("R of camera %d is not a rotation" % c)
+    D = None
+    if dist is not None:
+        if len(dist) != C:
+            raise SspError("dist must hold one set of coefficients per camera: %d for %d cameras" % (len(dist), C))
+        rows = [camera_distortion(d) for d in dist]
+        if any(r is not None for r in rows):
+            D = np.stack([np.zeros(8) if r is None else r for r in rows])
+    return CameraRig(K, R, t, D)
+
+
+def rig_tensors(rig, dev):
+    """the device tables ssp_fuse_views reads: K (C, 3, 3) fp32 and fp64, dist (C, 8) or None, R (C, 3, 3), t (C, 3)"""
+    to = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a, dt)).to(dev)
+    return (to(rig.K, np.float32), to(rig.K, np.float64), None if rig.dist is None else to(rig.dist, np.float64), to(rig.R, np.float64),
+            to(rig.t, np.float64))
+
+
+def check_fuse_args(gate, reproj_thresh, keypoint_sigma):
+    """-> the three as floats; SspError for a value not > 0 and finite or gate < reproj_thresh"""
+    gate, thr, sigma = (check_sigma(n, v) for n, v in (("gate", gate), ("reproj_thresh", reproj_thresh), ("keypoint_sigma", keypoint_sigma)))
+    if gate < thr:
+        raise SspError("the gate (%g px) must be >= reproj_thresh (%g px)" % (gate, thr))
+    return gate, thr, sigma
+
+
+def fuse_work_bytes(groups, views, slots):
+    """bytes of device workspace ssp_fuse_views needs"""
+    import ctypes
+    out = ctypes.c_longlong(0)
+    call("ssp_fuse_views_work_bytes", int(groups), int(views), int(slots), ctypes.byref(out))
+    return out.value
+
+
+def fuse_views_batched(points_3D, keypoints_px, rig, valid=None, gate=40.0, reproj_thresh=8.0, keypoint_sigma=2.0, max_iter=20):
+    """Fuse the poses of several calibrated cameras on the GPU (ssp_fuse_views, rule: csrc/multiview_core.h).  rig: camera_rig's
+    CameraRig of C cameras.  keypoints_px (B, P, 2) or (B, S, P, 2) raw pixels, 7 <= P <= 10: row b = g C + c is camera c's view of
+    capture g (B a multiple of C), S objects per row; points_3D (P, 3) shared, or one set per row (and slot); valid (B,) or (B, S)
+    bool, default all: the views that take part.  Every row gets its own cold PnP with its camera; each valid view's pose in the
+    world frame is a hypothesis; the views that agree with it within `gate` px (mean squared reprojection error) are fused by LM,
+    then the views within `reproj_thresh` px of that fit; the hypothesis with the most views wins.
+    -> dict of CUDA tensors: per row R (B[, S], 3, 3), t, corners_px (B[, S], P, 2) (the per-view solve); per capture R_world (G[, S],
+    3, 3), t_world (G[, S], 3) world-from-object, world_cov (G[, S], 6, 6) (keypoint_sigma^2 (J^T J)^-1, left perturbation, world
+    axes), views (G[, S], C) bool, view_err (G[, S], C) (RMS px of each valid view under the fused pose, -1 for the others),
+    fuse_hyp (G[, S]) int32 (the winning view, -1 for none), fuse_status (G[, S]) int32 (FUSE_STATUS bits); per row
+    corners_world_px (B[, S], P, 2), the fused pose in each row's camera."""
+    gate, thr, sigma = check_fuse_args(gate, reproj_thresh, keypoint_sigma)
+    if not isinstance(rig, CameraRig):
+        raise SspError("rig must be a CameraRig (utils.camera_rig)")
+    dev = _dev()
+    uv = torch.as_tensor(np.asarray(keypoints_px, np.float32) if not torch.is_tensor(keypoints_px) else keypoints_px).to(dev, torch.float32)
+    slotted = uv.dim() == 4
+    uv = (uv if slotted else uv.unsqueeze(1)).contiguous()
+    if uv.dim() != 4 or uv.shape[-1] != 2:
+        raise SspError("keypoints_px must be (B, P, 2) or (B, S, P, 2), got %s" % (tuple(uv.shape),))
+    B, S, npts = uv.shape[:3]
+    C = len(rig.K)
+    if B % C:
+        raise SspError("%d rows are not whole captures of the rig's %d cameras" % (B, C))
+    P3 = torch.as_tensor(np.asarray(points_3D, np.float32) if not torch.is_tensor(points_3D) else points_3D).to(dev, torch.float32).contiguous()
+    shared = P3.dim() == 2
+    if P3.shape[-2:] != (npts, 3) or (not shared and P3.numel() != B * S * npts * 3):
+        raise SspError("points_3D %s does not match keypoints_px %s" % (tuple(P3.shape), tuple(uv.shape)))
+    ok = torch.ones(B, S, dtype=torch.bool, device=dev) if valid is None else torch.as_tensor(valid).to(dev, torch.bool).reshape(B, S).contiguous()
+    K32, K64, D, Rr, tr = rig_tensors(rig, dev)
+    G = B // C
+    f64 = lambda *s: torch.empty(*s, dtype=torch.float64, device=dev)
+    o = dict(R=f64(B, S, 3, 3), t=f64(B, S, 3), corners_px=torch.empty(B, S, npts, 2, dtype=torch.float32, device=dev), R_world=f64(G, S, 3, 3),
+             t_world=f64(G, S, 3), world_cov=f64(G, S, 6, 6), views=torch.empty(G, S, C, dtype=torch.bool, device=dev), view_err=f64(G, S, C),
+             fuse_hyp=torch.empty(G, S, dtype=torch.int32, device=dev), fuse_status=torch.empty(G, S, dtype=torch.int32, device=dev),
+             corners_world_px=torch.empty(B, S, npts, 2, dtype=torch.float32, device=dev))
+    work = f64(max(fuse_work_bytes(G, C, S), 8) // 8)
+    call("ssp_fuse_views", ptr(P3), 1 if shared else 0, ptr(uv), ptr(ok), npts, G, C, S, ptr(K32), ptr(K64), ptr(D), ptr(Rr), ptr(tr), gate,
+         thr, sigma, max_iter, ptr(o["R"]), ptr(o["t"]), ptr(o["corners_px"]), ptr(o["R_world"]), ptr(o["t_world"]), ptr(o["world_cov"]),
+         ptr(o["views"]), ptr(o["view_err"]), ptr(o["fuse_hyp"]), ptr(o["fuse_status"]), ptr(o["corners_world_px"]), ptr(work),
+         work.numel() * 8, stream_ptr())
+    return o if slotted else {k: v[:, 0] for k, v in o.items()}
 
 
 # ------------------------------------------------------------------------------------------ training-set creation

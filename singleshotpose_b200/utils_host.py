@@ -324,3 +324,17 @@ def get_image_size(fname):
 def logging(message):
     """utils.py:416-417"""
     print('%s %s' % (time.strftime("%Y-%m-%d %H:%M:%S", time.localtime()), message))
+
+
+def read_rig(path):
+    """utils.camera_rig of a .npz with the keys K (C, 3, 3), R (C, 3, 3), t (C, 3) and optionally dist (C, n), n in 4, 5, 8
+    (camera-from-world extrinsics, x_c = R_c x_w + t_c); SspError naming the file for a missing file or key"""
+    from ._lib import SspError
+    from .utils import camera_rig
+    if not os.path.isfile(path):
+        raise SspError("rig file %s does not exist" % path)
+    with np.load(path) as z:
+        missing = [k for k in ("K", "R", "t") if k not in z.files]
+        if missing:
+            raise SspError("rig file %s has no %s" % (path, ", ".join(missing)))
+        return camera_rig(z["K"], z["R"], z["t"], z["dist"] if "dist" in z.files else None)
