@@ -408,6 +408,35 @@ int ssp_fuse_views(const float* points3d, int points3d_shared, const float* poin
                    double* view_err, int* fuse_hyp, int* fuse_status, float* corners_world, void* work, long long work_bytes,
                    void* stream);
 
+/* ---- fusing every detected instance across the cameras of a rig (rules: csrc/multiview_instances_core.h; csrc/multiview_rows.cu,
+ *      csrc/multiview_instances.cu), fp64.  The rig, the rows b = g * C + c and max_iter are ssp_fuse_views'; each row has `slots` = M
+ *      detection slots (1..SSP_FUSE_MAX_SLOTS): points3d_table [num_classes][num_points][3] (DEVICE fp32, the PnP points of each class
+ *      id), points2d [rows][M][num_points][2] raw pixels, cls [rows][M] and count [rows] (DEVICE int32; slot m of row b is a detection
+ *      when m < count[b] and 0 <= cls < num_classes; ssp_detect_instances' outputs).
+ *  ssp_fuse_instances: step 1 solves and projects every (row, slot) with m < count[b] as ssp_fuse_views does (the bits of
+ *      ssp_pnp_batched_counted / ssp_pnp_dist and ssp_project_points(_dist) with that camera) into R_out [rows][M][9], t_out [3],
+ *      corners_out [num_points][2]; empty slots get zeros.  Per capture: each detection's pose in the world frame is a hypothesis;
+ *      in each view the closest available detection of its class within gate px joins, the set is fused by LM, and again with the
+ *      detections within reproj_thresh px of that fit, members beyond reproj_thresh leave; the hypothesis with the most views, then
+ *      the lowest cost, then the lowest index is emitted as a world instance and its detections leave; repeated until no hypothesis
+ *      keeps a view or M instances are out.  Out per capture: world_count, unfused (the detections left) [groups]; per world slot
+ *      w < M: world_cls [groups][M] (-1 for an empty slot), R_world [groups][M][9], t_world [3], world_cov [36] (keypoint_sigma^2
+ *      (J^T J)^-1 over the members), members [groups][M][C] int32 (view c's fused slot, -1 for none), view_err [groups][M][C] (RMS px
+ *      of the members, -1 for the others), fuse_hyp [groups][M] (the winning detection's index c * M + m, -1 for an empty slot),
+ *      fuse_status [groups][M] (SSP_FUSE_SINGULAR: world_cov zeros); empty world slots are zeros.  Per row: world_index [rows][M]
+ *      (the world slot each detection joined, -1 for none) and corners_world [rows][M][num_points][2] (world instance w of the row's
+ *      capture drawn in the row's camera, zeros past world_count).  work: DEVICE scratch (8-B aligned) of at least the *bytes_out
+ *      that ssp_fuse_instances_work_bytes(groups, views, slots, bytes_out) writes.  SSP_ERR_ARG as ssp_fuse_views, and for slots
+ *      outside 1..256 or num_classes < 1. ---- */
+#define SSP_FUSE_MAX_SLOTS 256
+int ssp_fuse_instances_work_bytes(int groups, int views, int slots, long long* bytes_out);
+int ssp_fuse_instances(const float* points3d_table, int num_classes, const float* points2d, const int* cls, const int* count, int num_points,
+                       int groups, int views, int slots, const float* K3x3_f32, const double* K3x3, const double* dist8_or_null,
+                       const double* R_rig, const double* t_rig, double gate, double reproj_thresh, double keypoint_sigma, int max_iter,
+                       double* R_out, double* t_out, float* corners_out, int* world_count, int* unfused, int* world_cls, double* R_world,
+                       double* t_world, double* world_cov, int* members, double* view_err, int* fuse_hyp, int* fuse_status,
+                       int* world_index, float* corners_world, void* work, long long work_bytes, void* stream);
+
 /* ---- pose errors over the mesh (utils.py:50-64, valid.py:69-72, 173-177), fp64 throughout (csrc/adds.cu, csrc/adds_core.h).
  *      X [nv][3] fp64 vertices; Rt_est, Rt_gt [n][3][4] fp64 poses [R | t].
  *  ssp_adds_batched: adds_out[p] = mean_i min_j |Rt_gt[p] x_i - Rt_est[p] x_j|, the reference's adi(pts_est, pts_gt) (ADD-S, for

@@ -43,7 +43,7 @@ from ._lib import SspError, call, load, ptr, stream_ptr
 from .engine import Buffers
 from .image import BICUBIC
 from .utils import (CameraRig, camera_distortion, check_fuse_args, check_pnp_args, check_refine_args, consensus_subsets, consensus_work_bytes,
-                    distortion_tensor, fuse_work_bytes, inlier_bits, keypoint_bits, object_table, refine_model_table, rig_tensors)
+                    distortion_tensor, fuse_instances_outputs, fuse_instances_work_bytes, fuse_work_bytes, inlier_bits, keypoint_bits, object_table, refine_model_table, rig_tensors)
 
 
 class _Chain:
@@ -89,7 +89,9 @@ class _FramePredictor:
     c.t_ref, and a second _project of the refined poses gives c.corners_ref.  With a rig (utils.camera_rig of C cameras;
     row b = g C + c is camera c of capture g) the tail is _fuse instead: one ssp_fuse_views (rule: csrc/multiview_core.h) solves
     every row with its own camera into c.R, c.t, c.corners and fuses each capture's valid views (the head's flags) into one world
-    pose per slot.  _tail runs the whole tail; every head calls it.
+    pose per slot; a detecting head's slots are instead associated across the views by one ssp_fuse_instances (rule:
+    csrc/multiview_instances_core.h), which solves every row likewise and fuses each capture's detections into world instances.
+    _tail runs the whole tail; every head calls it.
     A subclass supplies the rest: _head_buffers(chain) allocates its selection's static buffers, _head(chain, stream) launches
     the selection after the forward and then the tail, and _outputs(chain) names the returned tensors."""
 
@@ -113,7 +115,7 @@ class _FramePredictor:
         self.eng.materialize(dev)
         self.rig = rig
         if rig is not None:
-            check_rig_predictor(name, rig, K, dist_coeffs, pnp, meshes, slots, self.batch)
+            check_rig_predictor(name, rig, K, dist_coeffs, pnp, meshes, self.batch)
             self.fuse_gate, self.fuse_thresh, self.keypoint_sigma = check_fuse_args(*fuse)
             K = rig.K[0]                        # object_table's check only: each row is solved and projected with its camera's K
         self.classes, points, Km = object_table(objects, self.num_classes, K)
@@ -189,7 +191,11 @@ class _FramePredictor:
             c.ref_points = torch.empty(B, S, dtype=torch.int32, device=dev)
             c.ref_rmse = torch.empty(B, S, dtype=torch.float64, device=dev)
             c.ref_status = torch.empty(B, S, dtype=torch.int32, device=dev)
-        if self.rig is not None:
+        if self.rig is not None and self._detects:
+            Cn = len(self.rig.K)
+            c.fi = {k: v for k, v in fuse_instances_outputs(B, Cn, S, K, dev).items() if k not in ("R", "t", "corners_px")}
+            c.fuse_work = torch.empty(max(fuse_instances_work_bytes(B // Cn, Cn, S), 8) // 8, dtype=torch.float64, device=dev)
+        elif self.rig is not None:
             G, Cn = B // len(self.rig.K), len(self.rig.K)
             c.R_world = torch.empty(G, S, 3, 3, dtype=torch.float64, device=dev)
             c.t_world = torch.empty(G, S, 3, dtype=torch.float64, device=dev)
@@ -264,9 +270,22 @@ class _FramePredictor:
              ptr(c.R_world), ptr(c.t_world), ptr(c.world_cov), ptr(c.views), ptr(c.view_err), ptr(c.fuse_hyp), ptr(c.fuse_status),
              ptr(c.corners_world), ptr(c.fuse_work), c.fuse_work.numel() * 8, s)
 
+    def _fuse_instances(self, c, s):
+        """with a rig and a detecting head: every row's PnP and projection with its camera into c.R, c.t, c.corners (zeros in empty
+        slots), and each capture's detections (c.cls, c.count, c.kp) associated across the views into world instances
+        (ssp_fuse_instances) in c.fi"""
+        K32, K64, D, Rr, tr = self._rig
+        Cn = len(self.rig.K)
+        call("ssp_fuse_instances", ptr(self._P3_table), self.num_classes, ptr(c.kp), ptr(c.cls), ptr(c.count), self.num_keypoints, self.batch // Cn,
+             Cn, self.num_slots, ptr(K32), ptr(K64), ptr(D), ptr(Rr), ptr(tr), self.fuse_gate, self.fuse_thresh, self.keypoint_sigma, 20,
+             ptr(c.R), ptr(c.t), ptr(c.corners), *(ptr(v) for v in c.fi.values()), ptr(c.fuse_work), c.fuse_work.numel() * 8, s)
+
     def _tail(self, c, s, valid=None):
         """the pose tail every head runs after its selection: PnP, projection and, with meshes, the depth refinement; with a rig
         the fusion of the views whose slots are valid (B, S) bool"""
+        if self.rig is not None and self._detects:
+            self._fuse_instances(c, s)
+            return
         if self.rig is not None:
             self._fuse(c, s, valid)
             return
@@ -281,6 +300,8 @@ class _FramePredictor:
     def _fuse_outputs(self, c):
         if self.rig is None:
             return {}
+        if self._detects:
+            return dict(c.fi)
         return dict(R_world=c.R_world, t_world=c.t_world, world_cov=c.world_cov, views=c.views, view_err=c.view_err, fuse_hyp=c.fuse_hyp,
                     fuse_status=c.fuse_status, corners_world_px=c.corners_world)
 
@@ -516,9 +537,10 @@ class PosePredictor(_FramePredictor):
         return dict(R=c.R[:, 0], t=c.t[:, 0], conf=c.conf, keypoints_px=c.kp[:, 0], corners_px=c.corners[:, 0], **one)
 
 
-def check_rig_predictor(name, rig, K, dist_coeffs, pnp, meshes, slots, batch):
+def check_rig_predictor(name, rig, K, dist_coeffs, pnp, meshes, batch):
     """SspError for what a predictor with a rig refuses: a rig that is not a utils.CameraRig, K or dist_coeffs given as well
-    (each camera brings its own), pnp="consensus", meshes, a detecting head, or a batch that is not whole captures"""
+    (each camera brings its own), pnp="consensus", meshes, or a batch that is not whole captures.  A detecting head
+    is let through: its detections are associated across the views (ssp_fuse_instances)"""
     if not isinstance(rig, CameraRig):
         raise SspError("rig must be a CameraRig (utils.camera_rig)")
     if K is not None or dist_coeffs is not None:
@@ -527,8 +549,6 @@ def check_rig_predictor(name, rig, K, dist_coeffs, pnp, meshes, slots, batch):
         raise SspError("%s with a rig fuses the plain per-view solves: pnp=%r is not supported with a rig" % (name, pnp))
     if meshes is not None:
         raise SspError("%s: depth refinement (mesh= / meshes=) is not supported with a rig" % name)
-    if slots is not None:
-        raise SspError("%s detects instances: associating instances across the views of a rig is not supported" % name)
     if batch % len(rig.K):
         raise SspError("batch %d is not a multiple of the rig's %d cameras" % (batch, len(rig.K)))
 

@@ -36,6 +36,10 @@ Command line: python -m singleshotpose_b200.predict_instances --datacfg cfg/occl
               [--pnp consensus [--reproj-thresh 8]]: the consensus PnP, with inliers and hyp columns (not with --track)
               [--depth-dir DIR [--depth-scale 0.001 --refine-iters 10]]: refine against 16-bit depth PNGs, as predict's command line
               (not with --track)
+              [--rig rig.npz]: the images come in groups of C calibrated cameras (image i is camera i % C; utils_host.read_rig)
+              and each capture's detections are associated into world instances, adding the per-detection column world_index and
+              the per-world-instance rows capture world_cls R_world t_world world_cov members view_err fuse_hyp fuse_status
+              (not with --track, --dist, --depth-dir or --pnp consensus)
 """
 from __future__ import annotations
 
@@ -47,7 +51,7 @@ import torch
 from . import predict, predict_multi
 from ._lib import SspError
 from .predict import (CONSENSUS_KEYS, REFINE_KEYS, _FramePredictor, add_depth_args, add_dist_arg, add_pnp_args, camera_dist, check_depth_args,
-                      mesh_corners, predict_files, read_camera, read_mesh, refine_kwargs)
+                      check_rig_args, mesh_corners, predict_files, read_camera, read_mesh, refine_kwargs)
 from .predict_multi import cfg_conf_thresh, check_grid, parse_objects
 from .utils import camera_distortion, check_pnp_args, check_sigma
 from .utils_multi import InstanceTracker, check_motion_args, check_track_args, detect_buffers, detect_slots
@@ -56,6 +60,7 @@ MAX_INSTANCES = 256         # largest max_instances (detect_core.h kMaxInstances
 OUTPUT_KEYS = ("count", "kept", "cls", "R", "t", "conf", "cls_conf", "keypoints_px", "corners_px")
 ROW_KEYS = ("cls", "R", "t", "conf", "cls_conf", "keypoints_px", "corners_px")
 MOTION_KEYS = ("R_filt", "t_filt", "velocity", "pose_cov")          # the --motion columns
+WORLD_KEYS = ("world_cls", "R_world", "t_world", "world_cov", "members", "view_err", "fuse_hyp", "fuse_status")   # --rig: per world instance
 
 
 class InstancePosePredictor(_FramePredictor):
@@ -74,11 +79,17 @@ class InstancePosePredictor(_FramePredictor):
     compares the raw keypoints' rectangles).
     meshes={class id: (vertices, faces)}, one for every requested class: refine every instance's pose against the call's
     depth=(B, H, W) uint16 frames, as predict.PosePredictor's mesh= does, adding R_ref (B, M, 3, 3), t_ref (B, M, 3),
-    corners_ref_px (B, M, 9, 2), refine_points, refine_rmse and refine_status (B, M) (empty slots: zeros)."""
+    corners_ref_px (B, M, 9, 2), refine_points, refine_rmse and refine_status (B, M) (empty slots: zeros).
+    rig=utils.camera_rig(...) of C calibrated cameras (K=None; no dist_coeffs, each camera brings its own): batch is a multiple of
+    C and frame g C + c is camera c of capture g.  Every per-frame output is what a one-camera predictor with that camera's K and
+    distortion gives; the detections are then associated across the views into world instances (utils.fuse_instances_batched,
+    fuse = (gate, reproj_thresh, keypoint_sigma)), adding per capture world_count (G,), unfused (G,), world_cls (G, M), R_world
+    (G, M, 3, 3), t_world (G, M, 3), world_cov (G, M, 6, 6), members (G, M, C), view_err (G, M, C), fuse_hyp (G, M), fuse_status
+    (G, M), and per frame world_index (B, M) and corners_world_px (B, M, 9, 2).  Not with pnp="consensus" or meshes."""
 
     def __init__(self, model, objects, K, frame_size=(640, 480), shape=None, batch=1, conf_thresh=None, nms_thresh=0.4, max_instances=32,
                  graph=True, max_graphs=4, pnp="plain", reproj_thresh=8.0, dist_coeffs=None, meshes=None, depth_scale=0.001, refine_iters=10,
-                 refine_gate=(0.5, 0.02)):
+                 refine_gate=(0.5, 0.02), rig=None, fuse=(40.0, 8.0, 2.0)):
         self.num_anchors = int(getattr(model, "num_anchors", 0))
         if self.num_anchors < 1:
             raise SspError("InstancePosePredictor needs a model with a region head")
@@ -88,7 +99,7 @@ class InstancePosePredictor(_FramePredictor):
             shape = (model.test_width, model.test_height) if self.num_anchors == 1 else (model.width, model.height)
         super().__init__(model, objects if isinstance(objects, dict) else {0: objects}, K, frame_size, shape, batch, graph, max_graphs,
                          pnp, reproj_thresh, slots=self.max_instances, dist_coeffs=dist_coeffs, meshes=meshes, depth_scale=depth_scale,
-                         refine_iters=refine_iters, refine_gate=refine_gate)
+                         refine_iters=refine_iters, refine_gate=refine_gate, rig=rig, fuse=fuse)
         check_grid(self, "detect")
 
     def _head_buffers(self, c):
@@ -102,7 +113,7 @@ class InstancePosePredictor(_FramePredictor):
     def _outputs(self, c):
         K = self.num_keypoints
         return dict(count=c.count, kept=c.kept, cls=c.cls, R=c.R, t=c.t, conf=c.boxes[..., 2 * K], cls_conf=c.boxes[..., 2 * K + 1],
-                    keypoints_px=c.kp, corners_px=c.corners, **self._consensus_outputs(c), **self._refine_outputs(c))
+                    keypoints_px=c.kp, corners_px=c.corners, **self._consensus_outputs(c), **self._refine_outputs(c), **self._fuse_outputs(c))
 
 
 class TrackingPosePredictor(InstancePosePredictor):
@@ -214,7 +225,8 @@ SIZE_KEYS = predict_multi.SIZE_KEYS + predict.SIZE_KEYS      # a multi-object .d
 def parse_args(argv=None):
     """the command line, checked before any model is built: raises SspError for a bad --object, --nms-thresh, --max-instances,
     --match-iou, --max-misses, --max-tracks, --reproj-thresh, --dist, --keypoint-sigma, --fps, --depth-scale or --refine-iters, for
-    --track with --pnp consensus or --depth-dir and for --motion without --track"""
+    --track with --pnp consensus or --depth-dir, for --motion without --track, and for --rig with --track, --dist, --depth-dir, --pnp
+    consensus or an image count that is not whole captures (a.rig_cams is then the rig's CameraRig, else None)"""
     ap = argparse.ArgumentParser(prog="python -m singleshotpose_b200.predict_instances",
                                  description="6-D pose of every detected instance of the requested objects in each image")
     ap.add_argument("--datacfg", required=True, help=".data file: fx fy u0 v0 and width height (or im_width im_height); mesh")
@@ -238,8 +250,14 @@ def parse_args(argv=None):
     add_pnp_args(ap)
     add_dist_arg(ap)
     add_depth_args(ap)
+    ap.add_argument("--rig", metavar="RIG.npz",
+                    help="associate the detections of several calibrated cameras (utils_host.read_rig: K, R, t[, dist] per camera) into "
+                         "world instances: the images come in groups of C, image i is camera i %% C; adds the column world_index and the "
+                         "per-world-instance rows capture " + " ".join(WORLD_KEYS))
     ap.add_argument("images", nargs="+")
     a = ap.parse_args(argv)
+    if a.rig is not None and a.track:
+        raise SspError("--track is not supported with --rig: world instances are not tracked over time yet")
     check_pnp_args(a.pnp, a.reproj_thresh)
     check_depth_args(a)
     if a.track:
@@ -255,6 +273,7 @@ def parse_args(argv=None):
     a.objects = parse_objects(a.object) if a.object else None
     if a.dist is not None:
         camera_distortion(a.dist)
+    a.rig_cams = check_rig_args(a)
     return a
 
 
@@ -269,7 +288,7 @@ def _region_anchors(modelcfg):
 def main(argv=None):
     a = parse_args(argv)
     mesh, K, size = read_camera(a.datacfg, SIZE_KEYS)
-    dist = camera_dist(a)
+    dist = camera_dist(a) if a.rig_cams is None else None
     meshes = a.objects
     if meshes is None:
         if not mesh:
@@ -285,6 +304,9 @@ def main(argv=None):
     model.load_weights(a.weightfile)
     model.cuda().eval()
     motion = "constant_velocity" if a.motion else None
+    rig = a.rig_cams
+    if rig is not None:
+        return _main_rig(a, model, objects, size, rig)
     if a.track:
         pred = TrackingPosePredictor(model, objects, K, frame_size=size, nms_thresh=a.nms_thresh, max_instances=a.max_instances,
                                      max_tracks=a.max_tracks, match_iou=a.match_iou, max_misses=a.max_misses, dist_coeffs=dist,
@@ -302,6 +324,29 @@ def main(argv=None):
             rows[k].append(r[k][0, :n])
     np.savez(a.out, paths=np.array(a.images), image=np.array(image, dtype=np.int64), **{k: np.concatenate(v) for k, v in rows.items()})
     print("%d images -> %d detections -> %s" % (len(a.images), len(image), a.out))
+
+
+def _main_rig(a, model, objects, size, rig):
+    """the --rig command line: one call per capture of C images"""
+    Cn = len(rig.K)
+    pred = InstancePosePredictor(model, objects, None, frame_size=size, batch=Cn, nms_thresh=a.nms_thresh, max_instances=a.max_instances,
+                                 rig=rig)
+    rows = {k: [] for k in ROW_KEYS + ("world_index",)}
+    world = {k: [] for k in WORLD_KEYS}
+    image, capture = [], []
+    for g, r in enumerate(predict_files(pred, a.images, None, Cn)):
+        for b in range(Cn):
+            n = int(r["count"][b])
+            image += [g * Cn + b] * n
+            for k in rows:
+                rows[k].append(r[k][b, :n])
+        n = int(r["world_count"][0])
+        capture += [g] * n
+        for k in world:
+            world[k].append(r[k][0, :n])
+    np.savez(a.out, paths=np.array(a.images), image=np.array(image, dtype=np.int64), capture=np.array(capture, dtype=np.int64),
+             **{k: np.concatenate(v) for k, v in rows.items()}, **{k: np.concatenate(v) for k, v in world.items()})
+    print("%d images -> %d detections -> %d world instances -> %s" % (len(a.images), len(image), len(capture), a.out))
 
 
 if __name__ == "__main__":

@@ -630,6 +630,64 @@ def fuse_views_batched(points_3D, keypoints_px, rig, valid=None, gate=40.0, repr
     return o if slotted else {k: v[:, 0] for k, v in o.items()}
 
 
+def fuse_instances_work_bytes(groups, views, slots):
+    """bytes of device workspace ssp_fuse_instances needs"""
+    import ctypes
+    out = ctypes.c_longlong(0)
+    call("ssp_fuse_instances_work_bytes", int(groups), int(views), int(slots), ctypes.byref(out))
+    return out.value
+
+
+def fuse_instances_outputs(B, C, M, npts, dev):
+    """the device outputs of ssp_fuse_instances for B rows of a C-camera rig with M slots, in its argument order"""
+    G = B // C
+    f64 = lambda *s: torch.empty(*s, dtype=torch.float64, device=dev)
+    i32 = lambda *s: torch.empty(*s, dtype=torch.int32, device=dev)
+    return dict(R=f64(B, M, 3, 3), t=f64(B, M, 3), corners_px=torch.empty(B, M, npts, 2, dtype=torch.float32, device=dev), world_count=i32(G),
+                unfused=i32(G), world_cls=i32(G, M), R_world=f64(G, M, 3, 3), t_world=f64(G, M, 3), world_cov=f64(G, M, 6, 6),
+                members=i32(G, M, C), view_err=f64(G, M, C), fuse_hyp=i32(G, M), fuse_status=i32(G, M), world_index=i32(B, M),
+                corners_world_px=torch.empty(B, M, npts, 2, dtype=torch.float32, device=dev))
+
+
+def fuse_instances_batched(points3D_table, keypoints_px, cls, count, rig, gate=40.0, reproj_thresh=8.0, keypoint_sigma=2.0, max_iter=20):
+    """Fuse every detected instance across the cameras of a rig on the GPU (ssp_fuse_instances, rule:
+    csrc/multiview_instances_core.h).  points3D_table (num_classes, P, 3): the PnP points of each class id, 7 <= P <= 10;
+    keypoints_px (B, M, P, 2) raw pixels, cls (B, M) int class ids and count (B,) int: row b = g C + c is camera c's detections of
+    capture g (B a multiple of C), slot m < count[b] a detection (InstancePosePredictor's count, cls and keypoints_px).  Every
+    detection gets its own cold PnP with its camera; each detection's pose in the world frame is a hypothesis; in each view the
+    closest detection of its class within `gate` px joins, the set is fused by LM, then again with the detections within
+    `reproj_thresh` px of that fit; the best-supported hypothesis becomes a world instance, its detections leave, and so on.
+    -> dict of CUDA tensors: per row R (B, M, 3, 3), t (B, M, 3), corners_px (B, M, P, 2) (the per-row solve, zeros in empty slots),
+    world_index (B, M) (the world slot each detection joined, -1 for none), corners_world_px (B, M, P, 2) (world instance m of the
+    row's capture in the row's camera, zeros past world_count); per capture world_count (G,), unfused (G,) (detections in no world
+    instance), world_cls (G, M) (-1 for an empty slot), R_world (G, M, 3, 3), t_world (G, M, 3) world-from-object, world_cov
+    (G, M, 6, 6), members (G, M, C) (view c's fused slot, -1 for none), view_err (G, M, C) (RMS px of the members, -1 for the
+    others), fuse_hyp (G, M) (the winning detection c M + m, -1 for an empty slot), fuse_status (G, M) (FUSE_STATUS bits)."""
+    gate, thr, sigma = check_fuse_args(gate, reproj_thresh, keypoint_sigma)
+    if not isinstance(rig, CameraRig):
+        raise SspError("rig must be a CameraRig (utils.camera_rig)")
+    dev = _dev()
+    t32 = lambda a, dt: (a if torch.is_tensor(a) else torch.as_tensor(np.asarray(a))).to(dev, dt).contiguous()
+    uv, table = t32(keypoints_px, torch.float32), t32(points3D_table, torch.float32)
+    cls, count = t32(cls, torch.int32), t32(count, torch.int32)
+    if uv.dim() != 4 or uv.shape[-1] != 2:
+        raise SspError("keypoints_px must be (B, M, P, 2), got %s" % (tuple(uv.shape),))
+    B, M, npts = uv.shape[:3]
+    if table.dim() != 3 or table.shape[1:] != (npts, 3):
+        raise SspError("points3D_table %s does not match keypoints_px %s: (num_classes, P, 3)" % (tuple(table.shape), tuple(uv.shape)))
+    if tuple(cls.shape) != (B, M) or tuple(count.shape) != (B,):
+        raise SspError("cls must be (B, M) and count (B,) for keypoints_px %s, got %s and %s" % (tuple(uv.shape), tuple(cls.shape), tuple(count.shape)))
+    C = len(rig.K)
+    if B % C:
+        raise SspError("%d rows are not whole captures of the rig's %d cameras" % (B, C))
+    K32, K64, D, Rr, tr = rig_tensors(rig, dev)
+    o = fuse_instances_outputs(B, C, M, npts, dev)
+    work = torch.empty(max(fuse_instances_work_bytes(B // C, C, M), 8) // 8, dtype=torch.float64, device=dev)
+    call("ssp_fuse_instances", ptr(table), table.shape[0], ptr(uv), ptr(cls), ptr(count), npts, B // C, C, M, ptr(K32), ptr(K64), ptr(D), ptr(Rr),
+         ptr(tr), gate, thr, sigma, max_iter, *(ptr(v) for v in o.values()), ptr(work), work.numel() * 8, stream_ptr())
+    return o
+
+
 # ------------------------------------------------------------------------------------------ training-set creation
 RENDER_CHUNK_BYTES = 1 << 30           # device scratch of one ssp_render_masks launch; larger batches go in chunks
 
