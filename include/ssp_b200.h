@@ -437,6 +437,38 @@ int ssp_fuse_instances(const float* points3d_table, int num_classes, const float
                        double* t_world, double* world_cov, int* members, double* view_err, int* fuse_hyp, int* fuse_status,
                        int* world_index, float* corners_world, void* work, long long work_bytes, void* stream);
 
+/* ---- tracking the world instances of a rig over time (rules: csrc/world_track_core.h; csrc/world_track.cu), fp64.  Each capture g
+ *      of ssp_fuse_instances (rows g * views .. g * views + views - 1, M = slots world slots) is its own stream with T = max_tracks
+ *      (1..256) slots, state in DEVICE arrays the caller keeps between calls (zeros for a fresh start):
+ *        tracks  int    [groups][T][5]   alive, id, cls, misses, hits (as ssp_track_associate's)
+ *        poses   double [groups][T][12]  R (row-major), t of the track's last fused world pose
+ *        next_id int    [groups]
+ *        filter  double [groups][T][SSP_FILTER_DOUBLES] or NULL: the pose filter of ssp_track_filter_update, in world axes.
+ *      The inputs are ssp_fuse_instances' world_count, world_cls, R_world, t_world, world_cov, fuse_status and world_index.
+ *  ssp_world_track_associate: with a filter, every alive slot whose filter has started moves by dt [groups] seconds (DEVICE fp64)
+ *      in place (dt is NULL exactly when filter is).  Then the world instances, in slot order, each take the alive, not yet taken
+ *      track of their class whose position (the started filter's t, else the last fused t) lies nearest, strictly within
+ *      match_dist * class_size[cls] (class_size: DEVICE fp64 [num_classes], the largest distance between two of the class's 8 box
+ *      corners), the lower slot on ties; unmatched tracks age (they die at misses > max_misses) and unmatched instances take the
+ *      lowest free slot and the next id.  Out per world slot: wslot [groups][M] (the track slot, -1 for an empty or untracked world
+ *      slot), world_track_id [groups][M] (-1 likewise), matched [groups][M] (1: an existing track); per detection: track_id
+ *      [groups * views][M] = its world instance's world_track_id through world_index (-1 for none).
+ *  ssp_world_track_commit: each matched or born track stores its instance's R_world, t_world, misses 0, hits + 1; with a filter, a
+ *      new track starts it from (R_world, t_world, world_cov) and a matched one is gated and updated (world_cov is unusable when
+ *      fuse_status has SSP_FUSE_SINGULAR).  Out per world slot with a filter: R_filt [9], t_filt [3], pose_cov [6][6], velocity
+ *      [6] = (w rad/s, v mesh units/s, world axes), reinit (1: the filter was started from this measurement); zeros elsewhere.
+ *  SSP_ERR_ARG for a null required pointer, groups < 0, max_tracks or slots outside 1..256, views outside 1..16, num_classes < 1,
+ *  max_misses < 0, or match_dist, an acceleration or initial velocity sigma or the gate not > 0 and finite. ---- */
+int ssp_world_track_associate(int groups, int views, int max_tracks, int slots, const int* world_count, const int* world_cls,
+                              const double* t_world, const int* world_index, const double* class_size, int num_classes, double match_dist,
+                              int max_misses, int* tracks, const double* poses, double* filter, const double* dt, double accel_sigma_rot,
+                              double accel_sigma_trans, int* next_id, int* wslot, int* world_track_id, int* matched, int* track_id,
+                              void* stream);
+int ssp_world_track_commit(int groups, int max_tracks, int slots, const int* world_count, const double* R_world, const double* t_world,
+                           const double* world_cov, const int* fuse_status, const int* wslot, const int* matched, int* tracks, double* poses,
+                           double* filter, double init_velocity_sigma_rot, double init_velocity_sigma_trans, double gate, double* R_filt,
+                           double* t_filt, double* pose_cov, double* velocity, int* reinit, void* stream);
+
 /* ---- pose errors over the mesh (utils.py:50-64, valid.py:69-72, 173-177), fp64 throughout (csrc/adds.cu, csrc/adds_core.h).
  *      X [nv][3] fp64 vertices; Rt_est, Rt_gt [n][3][4] fp64 poses [R | t].
  *  ssp_adds_batched: adds_out[p] = mean_i min_j |Rt_gt[p] x_i - Rt_est[p] x_j|, the reference's adi(pts_est, pts_gt) (ADD-S, for

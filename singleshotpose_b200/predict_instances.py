@@ -25,7 +25,10 @@ class's columns, masked to zero in the empty slots.
 Returned device tensors are the predictor's static outputs: the next call overwrites them.
 
 TrackingPosePredictor adds stable track ids across calls (each batch row is a camera stream) and PnP warm-started from each
-track's last pose (utils_multi.InstanceTracker, rules: csrc/track_core.h).
+track's last pose (utils_multi.InstanceTracker, rules: csrc/track_core.h).  WorldTrackingPosePredictor tracks the fused world
+instances of a rig instead: each capture is a stream, and every world instance is matched to the nearest track of its class in
+the world frame (utils_multi.WorldInstanceTracker, rules: csrc/world_track_core.h), after ssp_fuse_instances in the same graph
+replay.
 
 Command line: python -m singleshotpose_b200.predict_instances --datacfg cfg/occlusion.data --modelcfg cfg/yolo-pose-multi.cfg
               --weightfile w.weights --object 0=../LINEMOD/ape/ape.ply --object 4=../LINEMOD/can/can.ply --out det.npz img...
@@ -39,11 +42,16 @@ Command line: python -m singleshotpose_b200.predict_instances --datacfg cfg/occl
               [--rig rig.npz]: the images come in groups of C calibrated cameras (image i is camera i % C; utils_host.read_rig)
               and each capture's detections are associated into world instances, adding the per-detection column world_index and
               the per-world-instance rows capture world_cls R_world t_world world_cov members view_err fuse_hyp fuse_status
-              (not with --track, --dist, --depth-dir or --pnp consensus)
+              (not with --dist, --depth-dir or --pnp consensus)
+              [--rig rig.npz --track [--match-dist 0.5 --max-misses 5 --max-tracks 64] [--motion cv --keypoint-sigma 2 --fps 30]]:
+              the captures, in order, as one stream of tracked world instances, adding the per-detection column track_id, the
+              per-world-instance column world_track_id and, with --motion, the per-world-instance columns R_filt t_filt velocity
+              pose_cov (--keypoint-sigma is then the fusion's keypoint noise, which sets world_cov)
 """
 from __future__ import annotations
 
 import argparse
+import os
 
 import numpy as np
 import torch
@@ -53,8 +61,8 @@ from ._lib import SspError
 from .predict import (CONSENSUS_KEYS, REFINE_KEYS, _FramePredictor, add_depth_args, add_dist_arg, add_pnp_args, camera_dist, check_depth_args,
                       check_rig_args, mesh_corners, predict_files, read_camera, read_mesh, refine_kwargs)
 from .predict_multi import cfg_conf_thresh, check_grid, parse_objects
-from .utils import camera_distortion, check_pnp_args, check_sigma
-from .utils_multi import InstanceTracker, check_motion_args, check_track_args, detect_buffers, detect_slots
+from .utils import CameraRig, camera_distortion, check_pnp_args, check_sigma
+from .utils_multi import InstanceTracker, WorldInstanceTracker, check_motion_args, check_track_args, detect_buffers, detect_slots
 
 MAX_INSTANCES = 256         # largest max_instances (detect_core.h kMaxInstances)
 OUTPUT_KEYS = ("count", "kept", "cls", "R", "t", "conf", "cls_conf", "keypoints_px", "corners_px")
@@ -116,7 +124,40 @@ class InstancePosePredictor(_FramePredictor):
                     keypoints_px=c.kp, corners_px=c.corners, **self._consensus_outputs(c), **self._refine_outputs(c), **self._fuse_outputs(c))
 
 
-class TrackingPosePredictor(InstancePosePredictor):
+class _TrackedCalls:
+    """What a tracking predictor adds around InstancePosePredictor's call, for its tracker self._tracker (utils_multi.InstanceTracker
+    or WorldInstanceTracker): with motion, each stream's timestamp staged before the launches (checked before any launch, after the
+    frames); reset and tracks; and the track state put back after the warm-up runs of a graph capture, which advance it."""
+
+    def __call__(self, frames, to_host=False, events=None, timestamps=None):
+        """InstancePosePredictor's call; timestamps: one per stream, seconds, for the motion model (ignored without it)"""
+        if not self.motion:
+            return super().__call__(frames, to_host, events)
+        self._check(frames)                        # the frames' errors before the timestamps change anything
+        with torch.cuda.device(self.device):
+            self._tracker.stage_times(timestamps)
+        out = super().__call__(frames, to_host, events)
+        with torch.cuda.device(self.device):
+            self._tracker.staged()
+        return out
+
+    def reset(self, streams=None):
+        """forget the tracks of the given streams (default: all); their ids start again from 0"""
+        with torch.cuda.device(self.device):
+            self._tracker.reset(streams)
+
+    def tracks(self, to_host=False):
+        """the alive tracks (the tracker's tracks())"""
+        with torch.cuda.device(self.device):
+            return self._tracker.tracks(to_host)
+
+    def _capture(self, c, warmup=2):
+        saved = self._tracker.snapshot()          # the warm-up runs advance the tracks: put them back before the first replay
+        super()._capture(c, warmup)
+        self._tracker.restore(saved)
+
+
+class TrackingPosePredictor(_TrackedCalls, InstancePosePredictor):
     """InstancePosePredictor whose instances keep their identity across calls: each row b of a batch is its own camera stream, and
     each instance is matched to a track of its class (utils_multi.InstanceTracker, rules: csrc/track_core.h).  A matched instance's
     PnP starts Levenberg-Marquardt from its track's last pose (cv2.solvePnP's useExtrinsicGuess), the others are solved cold.
@@ -139,6 +180,7 @@ class TrackingPosePredictor(InstancePosePredictor):
     pose_cov (B, M, 6, 6), velocity (B, M, 6) and reinit (B, M) bool; R and t stay this frame's PnP.  keypoint_sigma (px),
     accel_sigma, init_velocity_sigma, gate and frame_dt (s) are InstanceTracker's, and their defaults are not tuned on real data.
     __call__ then takes timestamps= (B,) seconds per stream (default: the stream's last + frame_dt), checked before any launch.
+    reset(streams) forgets the tracks of some streams; tracks() lists the alive ones (utils_multi.InstanceTracker.tracks).
     meshes= (the depth refinement) is refused: how a refined pose should feed the tracks and the pose filter is not defined yet."""
 
     def __init__(self, model, objects, K, frame_size=(640, 480), shape=None, batch=1, conf_thresh=None, nms_thresh=0.4, max_instances=32,
@@ -157,29 +199,6 @@ class TrackingPosePredictor(InstancePosePredictor):
         self.max_tracks, self.match_iou, self.max_misses = self._tracker.max_tracks, self._tracker.match_iou, self._tracker.max_misses
         self.motion = self._tracker.motion
 
-    def __call__(self, frames, to_host=False, events=None, timestamps=None):
-        """InstancePosePredictor's call; timestamps (B,) seconds of the frames, per stream, for the motion model (ignored without it)"""
-        if not self.motion:
-            return super().__call__(frames, to_host, events)
-        self._check(frames)                        # the frames' errors before the timestamps change anything
-        with torch.cuda.device(self.device):
-            self._tracker.stage_times(timestamps)
-        out = super().__call__(frames, to_host, events)
-        with torch.cuda.device(self.device):
-            self._tracker.staged()
-        return out
-
-    def reset(self, streams=None):
-        """forget the tracks of the given streams (default: all); their ids start again from 0"""
-        with torch.cuda.device(self.device):
-            self._tracker.reset(streams)
-
-    def tracks(self, to_host=False):
-        """the alive tracks (utils_multi.InstanceTracker.tracks): stream, slot, id, cls, misses, hits, rvec, R, t, rect; with motion
-        also R_filt, t_filt, velocity, pose_cov and filter_valid"""
-        with torch.cuda.device(self.device):
-            return self._tracker.tracks(to_host)
-
     def _head_buffers(self, c):
         super()._head_buffers(c)
         self._tracker.buffers(c)
@@ -187,13 +206,56 @@ class TrackingPosePredictor(InstancePosePredictor):
     def _solve(self, c, s):
         self._tracker.solve(c, s, c.P3, self._K32)
 
-    def _capture(self, c, warmup=2):
-        saved = self._tracker.snapshot()          # the warm-up runs advance the tracks: put them back before the first replay
-        super()._capture(c, warmup)
-        self._tracker.restore(saved)
-
     def _outputs(self, c):
         return dict(super()._outputs(c), track_id=c.track_id, warm=c.warm, **self._tracker.outputs(c))
+
+
+class WorldTrackingPosePredictor(_TrackedCalls, InstancePosePredictor):
+    """InstancePosePredictor(rig=...) whose world instances keep their identity across calls (utils_multi.WorldInstanceTracker,
+    rules: csrc/world_track_core.h).  rig: utils.camera_rig(...) of C cameras; batch (default C) a multiple of C, frame g C + c
+    being camera c of capture g, and each capture g its own stream.  After ssp_fuse_instances, in the same graph replay, each
+    world instance (in the fusion's emission order) takes the alive track of its class whose position lies nearest, strictly within
+    match_dist x the class's box diagonal (the largest distance between two of its 8 corners); unmatched tracks die after
+    max_misses + 1 captures in a row without a match, and unmatched instances take the lowest free slot of max_tracks and the
+    stream's next id.  The other arguments are InstancePosePredictor's with a rig (fuse = (gate, reproj_thresh, keypoint_sigma)).
+
+    Returns every output of InstancePosePredictor(rig=...), with its bits, plus track_id (B, M) int32 (each detection's world
+    instance's track, -1 for none) and world_track_id (G, M) int32 (-1 in empty and untracked world slots).  The per-row PnP and
+    the fusion stay cold: a track's prediction does not feed them.  The track state is one set of device arrays shared by every
+    frame size and source; reset(streams) zeroes some streams in place; the warm-up runs before a graph capture do not advance it.
+
+    motion="constant_velocity" runs TrackingPosePredictor's constant-velocity pose filter per track in world axes (a rig is static,
+    so the velocity is the object's own), fed by each instance's fused pose and world_cov; the match then compares each instance
+    with the track's predicted position.  The outputs add, per world slot, R_filt (G, M, 3, 3), t_filt (G, M, 3), pose_cov (G, M,
+    6, 6), velocity (G, M, 6) = (w rad/s, v mesh units/s) and reinit (G, M) bool; __call__ takes timestamps= (G,) seconds, one per
+    capture.  accel_sigma, init_velocity_sigma, gate and frame_dt are TrackingPosePredictor's, and not tuned on real data."""
+
+    def __init__(self, model, objects, rig, frame_size=(640, 480), shape=None, batch=None, conf_thresh=None, nms_thresh=0.4,
+                 max_instances=32, max_tracks=64, match_dist=0.5, max_misses=5, graph=True, max_graphs=4, motion=None,
+                 accel_sigma=(2.0, 1.0), init_velocity_sigma=(1.0, 0.5), gate=22.46, frame_dt=1 / 30, fuse=(40.0, 8.0, 2.0)):
+        if not isinstance(rig, CameraRig):
+            raise SspError("WorldTrackingPosePredictor tracks the world instances of a rig: rig must be a CameraRig (utils.camera_rig)")
+        check_track_args(max_tracks, 0.0, max_misses)
+        check_sigma("match_dist", match_dist)
+        check_motion_args(motion, 1.0, accel_sigma, init_velocity_sigma, gate, frame_dt)
+        super().__init__(model, objects, None, frame_size, shape, len(rig.K) if batch is None else batch, conf_thresh, nms_thresh,
+                         max_instances, graph, max_graphs, rig=rig, fuse=fuse)
+        self._tracker = WorldInstanceTracker(objects, rig, self.num_classes, self.batch // len(rig.K), max_tracks, match_dist, max_misses,
+                                             motion=motion, accel_sigma=accel_sigma, init_velocity_sigma=init_velocity_sigma, gate=gate,
+                                             frame_dt=frame_dt, device=self.device)
+        self.max_tracks, self.match_dist, self.max_misses = self._tracker.max_tracks, self._tracker.match_dist, self._tracker.max_misses
+        self.motion = self._tracker.motion
+
+    def _head_buffers(self, c):
+        super()._head_buffers(c)
+        self._tracker.buffers(c, self.max_instances)
+
+    def _tail(self, c, s, valid=None):
+        super()._tail(c, s, valid)
+        self._tracker.solve(c, s, c.fi)            # the world instances of ssp_fuse_instances, in the same stream
+
+    def _outputs(self, c):
+        return dict(super()._outputs(c), **self._tracker.outputs(c))
 
 
 def check_detect_args(nms_thresh, max_instances):
@@ -224,9 +286,10 @@ SIZE_KEYS = predict_multi.SIZE_KEYS + predict.SIZE_KEYS      # a multi-object .d
 
 def parse_args(argv=None):
     """the command line, checked before any model is built: raises SspError for a bad --object, --nms-thresh, --max-instances,
-    --match-iou, --max-misses, --max-tracks, --reproj-thresh, --dist, --keypoint-sigma, --fps, --depth-scale or --refine-iters, for
-    --track with --pnp consensus or --depth-dir, for --motion without --track, and for --rig with --track, --dist, --depth-dir, --pnp
-    consensus or an image count that is not whole captures (a.rig_cams is then the rig's CameraRig, else None)"""
+    --match-iou, --max-misses, --max-tracks, --match-dist, --reproj-thresh, --dist, --keypoint-sigma, --fps, --depth-scale or
+    --refine-iters, for --track with --pnp consensus or --depth-dir, for --motion without --track, for --match-dist without --rig,
+    and for --rig with --dist, --depth-dir, --pnp consensus or an image count that is not whole captures (a.rig_cams is then the
+    rig's CameraRig, else None)"""
     ap = argparse.ArgumentParser(prog="python -m singleshotpose_b200.predict_instances",
                                  description="6-D pose of every detected instance of the requested objects in each image")
     ap.add_argument("--datacfg", required=True, help=".data file: fx fy u0 v0 and width height (or im_width im_height); mesh")
@@ -254,10 +317,14 @@ def parse_args(argv=None):
                     help="associate the detections of several calibrated cameras (utils_host.read_rig: K, R, t[, dist] per camera) into "
                          "world instances: the images come in groups of C, image i is camera i %% C; adds the column world_index and the "
                          "per-world-instance rows capture " + " ".join(WORLD_KEYS))
+    ap.add_argument("--match-dist", type=float, default=None,
+                    help="--rig --track: a world instance matches a track of its class within this many box diagonals (default 0.5)")
     ap.add_argument("images", nargs="+")
     a = ap.parse_args(argv)
-    if a.rig is not None and a.track:
-        raise SspError("--track is not supported with --rig: world instances are not tracked over time yet")
+    if a.match_dist is not None:
+        if a.rig is None:
+            raise SspError("--match-dist is the radius of the world tracks: it needs --rig (one camera's tracks match by --match-iou)")
+        check_sigma("--match-dist", a.match_dist)
     check_pnp_args(a.pnp, a.reproj_thresh)
     check_depth_args(a)
     if a.track:
@@ -285,8 +352,16 @@ def _region_anchors(modelcfg):
     raise SspError("%s has no [region] block" % modelcfg)
 
 
+def check_inputs(a):
+    """SspError, before any model is built, for a --datacfg, --modelcfg, --weightfile or image that is not a file"""
+    for name, path in [("--datacfg", a.datacfg), ("--modelcfg", a.modelcfg), ("--weightfile", a.weightfile)] + [("image", p) for p in a.images]:
+        if not os.path.isfile(path):
+            raise SspError("%s %s: no such file" % (name, path))
+
+
 def main(argv=None):
     a = parse_args(argv)
+    check_inputs(a)
     mesh, K, size = read_camera(a.datacfg, SIZE_KEYS)
     dist = camera_dist(a) if a.rig_cams is None else None
     meshes = a.objects
@@ -329,10 +404,16 @@ def main(argv=None):
 def _main_rig(a, model, objects, size, rig):
     """the --rig command line: one call per capture of C images"""
     Cn = len(rig.K)
-    pred = InstancePosePredictor(model, objects, None, frame_size=size, batch=Cn, nms_thresh=a.nms_thresh, max_instances=a.max_instances,
-                                 rig=rig)
-    rows = {k: [] for k in ROW_KEYS + ("world_index",)}
-    world = {k: [] for k in WORLD_KEYS}
+    kw = dict(frame_size=size, batch=Cn, nms_thresh=a.nms_thresh, max_instances=a.max_instances, rig=rig)
+    motion = "constant_velocity" if a.motion else None
+    if a.track:
+        pred = WorldTrackingPosePredictor(model, objects, max_tracks=a.max_tracks, max_misses=a.max_misses,
+                                          match_dist=0.5 if a.match_dist is None else a.match_dist, motion=motion,
+                                          fuse=(40.0, 8.0, a.keypoint_sigma), frame_dt=1.0 / a.fps, **kw)
+    else:
+        pred = InstancePosePredictor(model, objects, None, **kw)
+    rows = {k: [] for k in ROW_KEYS + ("world_index",) + (("track_id",) if a.track else ())}
+    world = {k: [] for k in WORLD_KEYS + (("world_track_id",) if a.track else ()) + (MOTION_KEYS if motion else ())}
     image, capture = [], []
     for g, r in enumerate(predict_files(pred, a.images, None, Cn)):
         for b in range(Cn):

@@ -1,6 +1,12 @@
 """Multi-object decode -- drop-in for ``get_multi_region_boxes`` of reference multi_obj_pose_estimation/utils_multi.py:266-382.
 The dense per-(cell, anchor) arithmetic and the reference's sequential fallback maxima run on the GPU; the host only
-applies the confidence mask (one device->host copy).  The pose helpers are shared with utils.py."""
+applies the confidence mask (one device->host copy).  The pose helpers are shared with utils.py.
+
+Also the trackers: InstanceTracker follows the instances of B camera streams across frames (csrc/track_core.h, with the pose
+filter of csrc/pose_filter_core.h), and WorldInstanceTracker follows the fused world instances of a camera rig across captures
+(csrc/world_track_core.h).  Both keep their state in device arrays allocated once, share the stream plumbing of _TrackStreams
+(reset, snapshot / restore around graph capture, per-stream timestamps) and are issued inside the predictors' graph replay by
+predict_instances.TrackingPosePredictor and WorldTrackingPosePredictor."""
 from __future__ import annotations
 
 import ctypes as _ctypes
@@ -11,7 +17,8 @@ import torch
 from ._lib import CONSTANTS, call, ptr, stream_ptr, SspError
 from .utils import (pnp_batched, compute_projection, compute_transformation, calcAngularDistance, get_3D_corners,  # noqa: F401
                     get_camera_intrinsic, convert2cpu, convert2cpu_long, project_points_batched, adi_batched, mesh_diameter,
-                    check_pnp_args, object_table, pnp_truth_and_prediction, pnp_one, camera_distortion, distortion_tensor, check_sigma)
+                    check_pnp_args, object_table, pnp_truth_and_prediction, pnp_one, camera_distortion, distortion_tensor, check_sigma,
+                    CameraRig)
 from .utils_host import (makedirs, get_all_files, calc_pts_diameter, adi, get_2d_bb, corner_confidences, corner_confidence,  # noqa: F401
                          sigmoid, softmax, read_truths, read_truths_args, read_pose, load_class_names, image2torch, scale_bboxes,
                          file_lines, get_image_size, logging)
@@ -232,7 +239,76 @@ def rodrigues_batched(r):
     return torch.where(small[:, None, None], eye, R)
 
 
-class InstanceTracker:
+class _TrackStreams:
+    """The stream state the trackers share: each stream's slots live in device arrays allocated once (graphs bake their
+    addresses in), zeroed in place by reset(); with motion, the per-stream frame intervals go through a pinned host buffer that
+    the launches copy from (stage_times / staged), and each stream's last timestamp stays on the host.  A subclass sets
+    self.motion, self.frame_dt and self.device, calls _init_times(n streams) and lists its device arrays in _state()."""
+
+    def _init_times(self, streams):
+        self._streams = int(streams)
+        if self.motion:
+            self._dt = torch.zeros(streams, dtype=torch.float64, device=self.device)   # this frame's interval per stream, read by the replay
+            self._dt_pin = torch.zeros(streams, dtype=torch.float64).pin_memory()
+            self._dt_copied = torch.cuda.Event()      # the launches that last read _dt_pin have been enqueued before this
+            self._last_time = np.full(streams, np.nan)    # each stream's last timestamp (NaN: none since the start or a reset)
+
+    # ------------------------------------------------------------------ state
+    def reset(self, streams=None):
+        """forget every track of the given streams (default: all), in place: ids start again from 0; with motion, their filters
+        and last timestamps too (the next frame of such a stream has dt = 0)"""
+        sel = slice(None) if streams is None else np.asarray(streams, np.int64).reshape(-1)
+        idx = sel if streams is None else torch.as_tensor(sel, device=self.device)
+        for t in self._state():
+            t[idx] = 0
+        if self.motion:
+            self._last_time[sel] = np.nan
+
+    def snapshot(self):
+        saved = tuple(t.clone() for t in self._state())
+        return saved + (self._last_time.copy(),) if self.motion else saved
+
+    def restore(self, saved):
+        for t, s in zip(self._state(), saved):
+            t.copy_(s)
+        if self.motion:
+            self._last_time[:] = saved[-1]
+
+    def stage_times(self, timestamps=None):
+        """with motion: this frame's interval per stream into the pinned buffer the next launches copy from.  timestamps: one
+        per stream, seconds, or None for each stream's last timestamp + frame_dt (a stream's first frame is at 0); dt = 0 for a stream's first
+        frame.  SspError, before anything changes, for a timestamp that is not finite or not after the stream's last one."""
+        if not self.motion:
+            return
+        last = self._last_time
+        if timestamps is None:
+            now = np.where(np.isnan(last), 0.0, last + self.frame_dt)
+        else:
+            try:
+                now = np.asarray(timestamps, np.float64).reshape(-1)
+            except (TypeError, ValueError):
+                raise SspError("timestamps must be %d numbers (seconds), got %r" % (self._streams, timestamps))
+            if now.shape != (self._streams,) or not np.isfinite(now).all():
+                raise SspError("timestamps must be %d finite numbers (seconds), one per stream, got %r" % (self._streams, timestamps))
+            bad = ~np.isnan(last) & ~(now > last)
+            if bad.any():
+                b = int(np.nonzero(bad)[0][0])
+                raise SspError("stream %d: timestamp %r is not after the stream's last one, %r" % (b, float(now[b]), float(last[b])))
+        # the last frame's copy out of the pinned buffer has run.  The event is recorded after ALL of that frame's launches (the copy
+        # is a node inside the captured graph, where no host-visible event can follow it alone), so this waits until the previous
+        # frame has finished.  Host frames already wait for their own staging buffer this way; for device and JPEG frames it is a
+        # host synchronisation per frame that motion=None does not have.
+        self._dt_copied.synchronize()
+        self._dt_pin.numpy()[:] = np.where(np.isnan(last), 0.0, now - last)
+        self._last_time = now
+
+    def staged(self):
+        """after the launches of a frame are enqueued: the pinned interval buffer may be rewritten once they have run"""
+        if self.motion:
+            self._dt_copied.record()
+
+
+class InstanceTracker(_TrackStreams):
     """Stable track ids across the frames of B camera streams, and PnP warm-started from each track's last pose (rules:
     csrc/track_core.h).  Per frame: the instances of detect_instances; ssp_track_associate matches each to an alive track of its
     class (highest IoU of the corner rectangles > match_iou, in det_conf order), ages the unmatched tracks (a track dies after
@@ -295,69 +371,12 @@ class InstanceTracker:
         self.state_next_id = torch.zeros(B, dtype=torch.int32, device=dev)
         if self.motion:
             self.state_filter = torch.zeros(B, T, FILTER_DOUBLES, dtype=torch.float64, device=dev)
-            self._dt = torch.zeros(B, dtype=torch.float64, device=dev)        # this frame's interval per stream, read by the replay
-            self._dt_pin = torch.zeros(B, dtype=torch.float64).pin_memory()
-            self._dt_copied = torch.cuda.Event()      # the launches that last read _dt_pin have been enqueued before this
-            self._last_time = np.full(B, np.nan)      # each stream's last timestamp (NaN: none since the start or a reset)
+        self._init_times(B)
         self._bufs = None
 
-    # ------------------------------------------------------------------ state
     def _state(self):
         base = (self.state_tracks, self.state_rects, self.state_poses, self.state_next_id)
         return base + (self.state_filter,) if self.motion else base
-
-    def reset(self, streams=None):
-        """forget every track of the given streams (default: all), in place: ids start again from 0; with motion, their filters
-        and last timestamps too (the next frame of such a stream has dt = 0)"""
-        sel = slice(None) if streams is None else np.asarray(streams, np.int64).reshape(-1)
-        idx = sel if streams is None else torch.as_tensor(sel, device=self.device)
-        for t in self._state():
-            t[idx] = 0
-        if self.motion:
-            self._last_time[sel] = np.nan
-
-    def snapshot(self):
-        saved = tuple(t.clone() for t in self._state())
-        return saved + (self._last_time.copy(),) if self.motion else saved
-
-    def restore(self, saved):
-        for t, s in zip(self._state(), saved):
-            t.copy_(s)
-        if self.motion:
-            self._last_time[:] = saved[-1]
-
-    def stage_times(self, timestamps=None):
-        """with motion: this frame's interval per stream into the pinned buffer the next launches copy from.  timestamps: (B,)
-        seconds, or None for each stream's last timestamp + frame_dt (a stream's first frame is at 0); dt = 0 for a stream's first
-        frame.  SspError, before anything changes, for a timestamp that is not finite or not after the stream's last one."""
-        if not self.motion:
-            return
-        last = self._last_time
-        if timestamps is None:
-            now = np.where(np.isnan(last), 0.0, last + self.frame_dt)
-        else:
-            try:
-                now = np.asarray(timestamps, np.float64).reshape(-1)
-            except (TypeError, ValueError):
-                raise SspError("timestamps must be %d numbers (seconds), got %r" % (self.batch, timestamps))
-            if now.shape != (self.batch,) or not np.isfinite(now).all():
-                raise SspError("timestamps must be %d finite numbers (seconds), one per stream, got %r" % (self.batch, timestamps))
-            bad = ~np.isnan(last) & ~(now > last)
-            if bad.any():
-                b = int(np.nonzero(bad)[0][0])
-                raise SspError("stream %d: timestamp %r is not after the stream's last one, %r" % (b, float(now[b]), float(last[b])))
-        # the last frame's copy out of the pinned buffer has run.  The event is recorded after ALL of that frame's launches (the copy
-        # is a node inside the captured graph, where no host-visible event can follow it alone), so this waits until the previous
-        # frame has finished.  Host frames already wait for their own staging buffer this way; for device and JPEG frames it is a
-        # host synchronisation per frame that motion=None does not have.
-        self._dt_copied.synchronize()
-        self._dt_pin.numpy()[:] = np.where(np.isnan(last), 0.0, now - last)
-        self._last_time = now
-
-    def staged(self):
-        """after the launches of a frame are enqueued: the pinned interval buffer may be rewritten once they have run"""
-        if self.motion:
-            self._dt_copied.record()
 
     def tracks(self, to_host=False):
         """the alive tracks of every stream, ordered by (stream, slot): stream, slot, id, cls, misses, hits (n,) int32; rvec (n, 3),
@@ -473,6 +492,173 @@ class InstanceTracker:
         self.staged()
         return dict(count=c.count, kept=c.kept, cls=c.cls, track_id=c.track_id, warm=c.warm, conf=c.boxes[..., 2 * K],
                     cls_conf=c.boxes[..., 2 * K + 1], keypoints_px=c.kp, R=c.R, t=c.t, params=c.params, **self.outputs(c))
+
+
+# ------------------------------------------------------------------------------------------ tracking world instances over time
+FUSE_SINGULAR = CONSTANTS["SSP_FUSE_SINGULAR"]
+FUSED_KEYS = ("world_count", "world_cls", "R_world", "t_world", "world_cov", "fuse_status", "world_index")   # what the tracking reads
+
+
+def class_sizes(points):
+    """d_k (num_classes,) fp64 of an object table's points (num_classes, 9, 3) as the kernels read them (fp32): the largest
+    distance between two of each class's 8 box corners (0 for a class without an object)"""
+    c = np.asarray(points, np.float32).astype(np.float64)[:, 1:9]
+    return np.sqrt((((c[:, :, None] - c[:, None, :]) ** 2).sum(-1)).max((1, 2)))
+
+
+class WorldInstanceTracker(_TrackStreams):
+    """Stable ids, and with motion a pose filter, for the world instances of a rig of C calibrated cameras across captures (rules:
+    csrc/world_track_core.h).  Each of the `groups` captures of a call (rows g C .. g C + C - 1 of utils.fuse_instances_batched)
+    is its own stream.  Per capture: ssp_world_track_associate walks the world instances in the fusion's emission order and
+    matches each to the alive track of its class whose position lies nearest, strictly within match_dist x the class's box
+    diagonal (the largest distance between two of its 8 corners); it ages the unmatched tracks (a track dies after max_misses + 1
+    missed captures in a row) and gives the other instances the lowest free slot and the stream's next id.  ssp_world_track_commit
+    stores each track's fused world pose.  update(fused) is the eager surface; predict_instances.WorldTrackingPosePredictor
+    issues the same launches inside its graph replay, after ssp_fuse_instances.
+
+    Why a metric radius: the rig gives metric 3-D positions, two solid instances of one class cannot have centres much closer
+    than their size, and a radius scaled by the object means the same with and without motion.
+
+    objects: {class id: (3|4, 8) box corners}; rig: utils.camera_rig(...) (C cameras); groups: captures per call; max_tracks in
+    [1, 256] slots per stream, match_dist > 0, max_misses >= 0.  The state lives in device arrays allocated once (graphs bake their
+    addresses in): tracks (G, T, 5) int32 = alive, id, cls, misses, hits; poses (G, T, 12) fp64 = R (row-major), t of the track's
+    last fused world pose; next_id (G,) int32.  reset() zeroes them in place.
+
+    motion="constant_velocity" adds InstanceTracker's constant-velocity pose filter per track (csrc/pose_filter_core.h), fed by
+    each world instance's fused pose and its world_cov (the fusion's keypoint_sigma^2 (J^T J)^-1, unusable when fuse_status has the
+    singular bit).  The filter lives in world axes: a rig is static, so its velocity is the object's own.  Each capture, every alive
+    track's filter moves to the capture's time first and the match compares each instance with the predicted position; a
+    measurement with y^T S^-1 y > gate restarts the filter.  accel_sigma = (rad/s^2, mesh units/s^2), init_velocity_sigma = (rad/s,
+    mesh units/s), frame_dt: the capture interval in seconds when no timestamps are given; the defaults are not tuned on real data.
+    The filter state is one more device array, filter (G, T, 163) fp64.
+
+    Not done here: the per-row PnP and the fusion stay cold (a track's prediction does not feed them), dead tracks are not
+    re-identified, and one-view instances birth tracks as any other."""
+
+    def __init__(self, objects, rig, num_classes, groups, max_tracks=64, match_dist=0.5, max_misses=5, motion=None, accel_sigma=(2.0, 1.0),
+                 init_velocity_sigma=(1.0, 0.5), gate=22.46, frame_dt=1 / 30, device=None):
+        self.max_tracks, _iou, self.max_misses = check_track_args(max_tracks, 0.0, max_misses)
+        self.match_dist = check_sigma("match_dist", match_dist)
+        (self.motion, _sigma, self.accel_sigma, self.init_velocity_sigma, self.gate,
+         self.frame_dt) = check_motion_args(motion, 1.0, accel_sigma, init_velocity_sigma, gate, frame_dt)
+        if not isinstance(rig, CameraRig):
+            raise SspError("rig must be a CameraRig (utils.camera_rig)")
+        if isinstance(groups, bool) or not isinstance(groups, (int, np.integer)) or groups < 1:
+            raise SspError("groups must be an integer >= 1, got %r" % (groups,))
+        self.rig, self.views, self.groups, self.num_classes = rig, len(rig.K), int(groups), int(num_classes)
+        _classes, points, _K = object_table(objects if isinstance(objects, dict) else {0: objects}, num_classes, rig.K[0])
+        dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        self.device = dev
+        self.class_size = class_sizes(points)
+        self._size = torch.from_numpy(self.class_size).to(dev)
+        G, T = self.groups, self.max_tracks
+        self.state_tracks = torch.zeros(G, T, 5, dtype=torch.int32, device=dev)
+        self.state_poses = torch.zeros(G, T, 12, dtype=torch.float64, device=dev)
+        self.state_next_id = torch.zeros(G, dtype=torch.int32, device=dev)
+        if self.motion:
+            self.state_filter = torch.zeros(G, T, FILTER_DOUBLES, dtype=torch.float64, device=dev)
+        self._init_times(G)
+        self._bufs = None
+
+    def _state(self):
+        base = (self.state_tracks, self.state_poses, self.state_next_id)
+        return base + (self.state_filter,) if self.motion else base
+
+    def tracks(self, to_host=False):
+        """the alive tracks of every stream, ordered by (stream, slot): stream, slot, id, cls, misses, hits (n,) int32; R (n, 3, 3),
+        t (n, 3) fp64 = the track's last fused world pose.  With motion also the filter's R_filt (n, 3, 3), t_filt (n, 3), velocity
+        (n, 6) = (w rad/s, v mesh units/s, world axes) and pose_cov (n, 6, 6) at the last capture's time (a track that missed the
+        capture reports its prediction) and filter_valid (n,) bool."""
+        st = self.state_tracks
+        b, s = torch.nonzero(st[..., 0] != 0, as_tuple=True)
+        f, pose = st[b, s], self.state_poses[b, s]
+        out = dict(stream=b.int(), slot=s.int(), id=f[:, 1], cls=f[:, 2], misses=f[:, 3], hits=f[:, 4], R=pose[:, :9].reshape(-1, 3, 3),
+                   t=pose[:, 9:])
+        if self.motion:
+            fs = self.state_filter[b, s]
+            P = fs[:, 18:162].reshape(-1, 12, 12)
+            out.update(R_filt=fs[:, :9].reshape(-1, 3, 3), t_filt=fs[:, 9:12], velocity=fs[:, 12:18], pose_cov=P[:, :6, :6].contiguous(),
+                       filter_valid=fs[:, 162] == 1.0)
+        if to_host:
+            return {k: v.cpu().numpy() for k, v in out.items()}
+        return out
+
+    # ------------------------------------------------------------------ launches
+    def buffers(self, c, slots):
+        """the per-capture device buffers of the tracking launches, as attributes of c (G captures x `slots` world slots)"""
+        dev, G, M = self.device, self.groups, int(slots)
+        c.wslot = torch.empty(G, M, dtype=torch.int32, device=dev)
+        c.world_track_id = torch.empty(G, M, dtype=torch.int32, device=dev)
+        c.matched_i = torch.empty(G, M, dtype=torch.int32, device=dev)
+        c.track_id = torch.empty(G * self.views, M, dtype=torch.int32, device=dev)
+        if self.motion:
+            c.R_filt = torch.empty(G, M, 3, 3, dtype=torch.float64, device=dev)
+            c.t_filt = torch.empty(G, M, 3, dtype=torch.float64, device=dev)
+            c.pose_cov = torch.empty(G, M, 6, 6, dtype=torch.float64, device=dev)
+            c.velocity = torch.empty(G, M, 6, dtype=torch.float64, device=dev)
+            c.reinit_i = torch.empty(G, M, dtype=torch.int32, device=dev)
+            c.reinit = torch.empty(G, M, dtype=torch.bool, device=dev)
+
+    def outputs(self, c):
+        """track_id per detection, world_track_id per world slot and, with motion, the filter's outputs per world slot"""
+        out = dict(track_id=c.track_id, world_track_id=c.world_track_id)
+        if self.motion:
+            out.update(R_filt=c.R_filt, t_filt=c.t_filt, pose_cov=c.pose_cov, velocity=c.velocity, reinit=c.reinit)
+        return out
+
+    def solve(self, c, s, fused):
+        """associate and commit on ssp_fuse_instances' outputs (the dict fused, FUSED_KEYS) into the buffers of buffers(c)"""
+        G, T, M = self.groups, self.max_tracks, c.wslot.shape[1]
+        filt = dt = None
+        if self.motion:
+            self._dt.copy_(self._dt_pin, non_blocking=True)
+            filt, dt = self.state_filter, self._dt
+        call("ssp_world_track_associate", G, self.views, T, M, ptr(fused["world_count"]), ptr(fused["world_cls"]), ptr(fused["t_world"]),
+             ptr(fused["world_index"]), ptr(self._size), self.num_classes, self.match_dist, self.max_misses, ptr(self.state_tracks),
+             ptr(self.state_poses), ptr(filt), ptr(dt), self.accel_sigma[0], self.accel_sigma[1], ptr(self.state_next_id), ptr(c.wslot),
+             ptr(c.world_track_id), ptr(c.matched_i), ptr(c.track_id), s)
+        mo = [getattr(c, k, None) if self.motion else None for k in ("R_filt", "t_filt", "pose_cov", "velocity", "reinit_i")]
+        call("ssp_world_track_commit", G, T, M, ptr(fused["world_count"]), ptr(fused["R_world"]), ptr(fused["t_world"]), ptr(fused["world_cov"]),
+             ptr(fused["fuse_status"]), ptr(c.wslot), ptr(c.matched_i), ptr(self.state_tracks), ptr(self.state_poses), ptr(filt),
+             self.init_velocity_sigma[0], self.init_velocity_sigma[1], self.gate, *map(ptr, mo), s)
+        if self.motion:
+            torch.ne(c.reinit_i, 0, out=c.reinit)
+
+    def update(self, fused, timestamps=None):
+        """one capture of every stream from the dict of utils.fuse_instances_batched (or InstancePosePredictor(rig=...)'s outputs)
+        -> dict of device tensors: track_id (G C, M) int32 (each detection's world instance's id, -1 for none), world_track_id (G, M)
+        (-1 in empty and untracked world slots), matched (G, M) bool (an existing track took the instance).  With motion:
+        timestamps (G,) seconds of this capture per stream (stage_times), and per world slot with a track the filtered pose R_filt
+        (G, M, 3, 3), t_filt (G, M, 3), its covariance pose_cov (G, M, 6, 6) over (dth, dt_) in world axes, the velocity (G, M, 6)
+        and reinit (G, M) bool; zeros elsewhere.  Returned tensors are reused."""
+        missing = [k for k in FUSED_KEYS if k not in fused]
+        if missing:
+            raise SspError("fused lacks %s: pass the dict of utils.fuse_instances_batched" % ", ".join(missing))
+        G, Cn = self.groups, self.views
+        M = fused["world_cls"].shape[1] if fused["world_cls"].dim() == 2 else -1
+        want = dict(world_count=(G,), world_cls=(G, M), R_world=(G, M, 3, 3), t_world=(G, M, 3), world_cov=(G, M, 6, 6), fuse_status=(G, M),
+                    world_index=(G * Cn, M))
+        dtypes = dict(world_count=torch.int32, world_cls=torch.int32, fuse_status=torch.int32, world_index=torch.int32)
+        for k, shape in want.items():
+            v = fused[k]
+            if (not torch.is_tensor(v) or not v.is_cuda or tuple(v.shape) != shape or not v.is_contiguous()
+                    or v.dtype != dtypes.get(k, torch.float64)):
+                raise SspError("fused[%r] must be a contiguous CUDA %s tensor of shape %s for %d captures of %d cameras, got %s"
+                               % (k, dtypes.get(k, torch.float64), shape, G, Cn, getattr(v, "shape", type(v).__name__)))
+        if self._bufs is not None and self._bufs.wslot.shape[1] != M:
+            raise SspError("this tracker follows %d world slots per capture, got %d" % (self._bufs.wslot.shape[1], M))
+        self.stage_times(timestamps)
+        if self._bufs is None:
+            import types
+            self._bufs = types.SimpleNamespace()
+            self.buffers(self._bufs, M)
+            self._bufs.matched = torch.empty(G, M, dtype=torch.bool, device=self.device)
+        c = self._bufs
+        self.solve(c, stream_ptr(), fused)
+        self.staged()
+        torch.ne(c.matched_i, 0, out=c.matched)
+        return dict(self.outputs(c), matched=c.matched)
+
 
 
 # ------------------------------------------------------------------------------------------ batched evaluation tail
