@@ -437,6 +437,35 @@ int ssp_fuse_instances(const float* points3d_table, int num_classes, const float
                        double* t_world, double* world_cov, int* members, double* view_err, int* fuse_hyp, int* fuse_status,
                        int* world_index, float* corners_world, void* work, long long work_bytes, void* stream);
 
+/* ---- calibrating a camera rig from the object it sees (rules: csrc/calibrate_rig_core.h; csrc/multiview_rows.cu,
+ *      csrc/calibrate_rig.cu), fp64.  The cameras (`views` = C, 1..SSP_RIG_MAX_VIEWS: K3x3_f32, K3x3, dist8_or_null), the rows
+ *      b = g * C + c, points3d, points2d and valid are ssp_fuse_views'; the extrinsics are unknown.  Observation o = g * slots + s.
+ *  ssp_calibrate_rig: step 1 solves every (row, slot) with its camera into R_rows [rows][slots][9], t_rows [3] (the bits of
+ *      ssp_fuse_views' R_out, t_out).  Each camera pair scores up to 256 relative-pose hypotheses, one per co-observation, over all
+ *      its co-observations (both views carried across within gate px); a maximum spanning tree over the winners' agreement counts
+ *      (>= 3) rooted at camera `reference` gives the initial rig, whose world frame is the reference camera's (R = I, t = 0).  Then
+ *      at most 4 rounds of: ssp_fuse_views' fusion of every observation under the current rig, and a bundle adjustment (LM, at most
+ *      max_iter steps, Schur complement on the device) of the free cameras' extrinsics and the world poses of the observations fused
+ *      in >= 2 cameras (linked); the rounds stop when no linked view set changes, and the fusion runs once more under the final
+ *      rig.  Out per camera: R_cam [C][9], t_cam [C][3] (camera-from-world), cam_cov [C][36] (keypoint_sigma^2 times the camera's
+ *      block of the reduced system's inverse, left perturbation in the camera frame; zeros for the reference), cam_obs [C] (linked
+ *      observations it is fused in), cam_rmse [C] (RMS px of those views, -1 for none), tree_parent [C] (-1 for the root and
+ *      unconnected cameras), edge_agree [C] (the tree edge's agreement count) and cam_status [C] (SSP_CALIB_UNCONNECTED: no tree
+ *      path to the reference, zero extrinsics; SSP_CALIB_SINGULAR: cam_cov zeros).  Per observation: R_world [groups][slots][9],
+ *      t_world [3], views_out [C] bytes and view_err [C] as ssp_fuse_views writes them under the final rig, linked [groups][slots]
+ *      bytes.  Global: rounds, iterations (LM steps over all rounds), cost (the final sum of squared residuals).  work: DEVICE
+ *      scratch (8-B aligned) of at least the *bytes_out that ssp_calibrate_rig_work_bytes(groups, views, slots, bytes_out) writes.
+ *      SSP_ERR_ARG as ssp_fuse_views, and for a reference outside 0..views-1. ---- */
+#define SSP_CALIB_UNCONNECTED 1
+#define SSP_CALIB_SINGULAR 2
+int ssp_calibrate_rig_work_bytes(int groups, int views, int slots, long long* bytes_out);
+int ssp_calibrate_rig(const float* points3d, int points3d_shared, const float* points2d, const unsigned char* valid, int num_points, int groups,
+                      int views, int slots, const float* K3x3_f32, const double* K3x3, const double* dist8_or_null, int reference,
+                      double gate, double reproj_thresh, double keypoint_sigma, int max_iter, double* R_rows, double* t_rows,
+                      double* R_cam, double* t_cam, double* cam_cov, int* cam_obs, double* cam_rmse, int* tree_parent, int* edge_agree,
+                      int* cam_status, double* R_world, double* t_world, unsigned char* views_out, double* view_err,
+                      unsigned char* linked, int* rounds, int* iterations, double* cost, void* work, long long work_bytes, void* stream);
+
 /* ---- tracking the world instances of a rig over time (rules: csrc/world_track_core.h; csrc/world_track.cu), fp64.  Each capture g
  *      of ssp_fuse_instances (rows g * views .. g * views + views - 1, M = slots world slots) is its own stream with T = max_tracks
  *      (1..256) slots, state in DEVICE arrays the caller keeps between calls (zeros for a fresh start):

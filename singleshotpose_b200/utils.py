@@ -688,6 +688,86 @@ def fuse_instances_batched(points3D_table, keypoints_px, cls, count, rig, gate=4
     return o
 
 
+CALIB_STATUS = {"unconnected": 1, "singular": 2}                       # ssp_calibrate_rig's camera status bits (SSP_CALIB_*)
+
+
+def calibrate_work_bytes(groups, views, slots):
+    """bytes of device workspace ssp_calibrate_rig needs"""
+    import ctypes
+    out = ctypes.c_longlong(0)
+    call("ssp_calibrate_rig_work_bytes", int(groups), int(views), int(slots), ctypes.byref(out))
+    return out.value
+
+
+def check_calibrate_args(K, dist, reference, gate, reproj_thresh, keypoint_sigma, max_iter):
+    """-> (K (C, 3, 3) float64, dist (C, 8) float64 or None, reference, gate, reproj_thresh, keypoint_sigma, max_iter), checked as
+    camera_rig checks the intrinsics and as ssp_calibrate_rig checks the rest; SspError otherwise"""
+    K = np.asarray(K, np.float64)
+    if K.ndim != 3:
+        raise SspError("K must be (C, 3, 3), one per camera, got %s" % (K.shape,))
+    C = len(K)
+    rig = camera_rig(K, np.repeat(np.eye(3)[None], max(C, 0), 0), np.zeros((C, 3)), dist)      # the intrinsics' and dist's checks
+    gate, thr, sigma = check_fuse_args(gate, reproj_thresh, keypoint_sigma)
+    if not isinstance(reference, (int, np.integer)) or not 0 <= reference < C:
+        raise SspError("the reference camera must be one of 0..%d, got %r" % (C - 1, reference))
+    if not isinstance(max_iter, (int, np.integer)) or max_iter < 1:
+        raise SspError("max_iter must be an integer >= 1, got %r" % (max_iter,))
+    return rig.K, rig.dist, int(reference), gate, thr, sigma, int(max_iter)
+
+
+def calibrate_rig_batched(points_3D, keypoints_px, K, dist=None, valid=None, reference=0, gate=40.0, reproj_thresh=8.0, keypoint_sigma=2.0,
+                          max_iter=30):
+    """Calibrate the extrinsics of a rig of C cameras from the object they see, on the GPU (ssp_calibrate_rig, rule:
+    csrc/calibrate_rig_core.h).  K (C, 3, 3) each camera's intrinsics, dist as camera_rig takes it; keypoints_px (B, P, 2) or
+    (B, S, P, 2) raw pixels, row b = g C + c camera c's view of capture g; points_3D (P, 3) shared or one set per row (and slot);
+    valid (B,) or (B, S) bool, default all.  Each camera pair's relative pose comes from the consensus of its co-observations, a
+    maximum spanning tree rooted at camera `reference` gives the initial rig (its world frame is the reference camera's: R = I,
+    t = 0), and rounds of ssp_fuse_views' fusion and a bundle adjustment of the extrinsics and the fused world poses refine it.
+    -> dict: per camera R (C, 3, 3), t (C, 3) camera-from-world, cam_cov (C, 6, 6) (keypoint_sigma^2 times the marginal covariance
+    of (dth, dt_), the left perturbation in the camera frame), cam_obs (C,) (fused observations the camera is in), cam_rmse (C,)
+    (RMS px of those views), tree_parent (C,), edge_agree (C,), cam_status (C,) (CALIB_STATUS bits); per observation R_world
+    (G[, S], 3, 3), t_world (G[, S], 3), views (G[, S], C) bool, view_err (G[, S], C), linked (G[, S]) bool; per row R_rows, t_rows (the
+    per-view solve); rounds, iterations, cost; and rig, a CameraRig for PosePredictor(rig=...), or None when a camera is
+    unconnected.  Arrays are CUDA tensors, rig numpy."""
+    K, D, reference, gate, thr, sigma, max_iter = check_calibrate_args(K, dist, reference, gate, reproj_thresh, keypoint_sigma, max_iter)
+    dev = _dev()
+    uv = torch.as_tensor(np.asarray(keypoints_px, np.float32) if not torch.is_tensor(keypoints_px) else keypoints_px).to(dev, torch.float32)
+    slotted = uv.dim() == 4
+    uv = (uv if slotted else uv.unsqueeze(1)).contiguous()
+    if uv.dim() != 4 or uv.shape[-1] != 2:
+        raise SspError("keypoints_px must be (B, P, 2) or (B, S, P, 2), got %s" % (tuple(uv.shape),))
+    B, S, npts = uv.shape[:3]
+    C = len(K)
+    if B % C:
+        raise SspError("%d rows are not whole captures of the rig's %d cameras" % (B, C))
+    P3 = torch.as_tensor(np.asarray(points_3D, np.float32) if not torch.is_tensor(points_3D) else points_3D).to(dev, torch.float32).contiguous()
+    shared = P3.dim() == 2
+    if P3.shape[-2:] != (npts, 3) or (not shared and P3.numel() != B * S * npts * 3):
+        raise SspError("points_3D %s does not match keypoints_px %s" % (tuple(P3.shape), tuple(uv.shape)))
+    ok = torch.ones(B, S, dtype=torch.bool, device=dev) if valid is None else torch.as_tensor(valid).to(dev, torch.bool).reshape(B, S).contiguous()
+    to = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a, dt)).to(dev)
+    K32, K64, Dt = to(K, np.float32), to(K, np.float64), None if D is None else to(D, np.float64)
+    G = B // C
+    f64 = lambda *s: torch.empty(*s, dtype=torch.float64, device=dev)
+    i32 = lambda *s: torch.empty(*s, dtype=torch.int32, device=dev)
+    o = dict(R_rows=f64(B, S, 3, 3), t_rows=f64(B, S, 3), R=f64(C, 3, 3), t=f64(C, 3), cam_cov=f64(C, 6, 6), cam_obs=i32(C), cam_rmse=f64(C),
+             tree_parent=i32(C), edge_agree=i32(C), cam_status=i32(C), R_world=f64(G, S, 3, 3), t_world=f64(G, S, 3),
+             views=torch.empty(G, S, C, dtype=torch.bool, device=dev), view_err=f64(G, S, C),
+             linked=torch.empty(G, S, dtype=torch.bool, device=dev), rounds=i32(1), iterations=i32(1), cost=f64(1))
+    work = f64(max(calibrate_work_bytes(G, C, S), 8) // 8)
+    call("ssp_calibrate_rig", ptr(P3), 1 if shared else 0, ptr(uv), ptr(ok), npts, G, C, S, ptr(K32), ptr(K64), ptr(Dt), reference, gate, thr,
+         sigma, max_iter, *(ptr(v) for v in o.values()), ptr(work), work.numel() * 8, stream_ptr())
+    if not slotted:
+        for k in ("R_rows", "t_rows", "R_world", "t_world", "views", "view_err", "linked"):
+            o[k] = o[k][:, 0]
+    for k in ("rounds", "iterations"):
+        o[k] = int(o[k][0])
+    o["cost"] = float(o["cost"][0])
+    status = o["cam_status"].cpu().numpy()
+    o["rig"] = None if (status & CALIB_STATUS["unconnected"]).any() else camera_rig(K, o["R"].cpu().numpy(), o["t"].cpu().numpy(), D)
+    return o
+
+
 # ------------------------------------------------------------------------------------------ training-set creation
 RENDER_CHUNK_BYTES = 1 << 30           # device scratch of one ssp_render_masks launch; larger batches go in chunks
 

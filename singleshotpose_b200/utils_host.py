@@ -338,3 +338,15 @@ def read_rig(path):
         if missing:
             raise SspError("rig file %s has no %s" % (path, ", ".join(missing)))
         return camera_rig(z["K"], z["R"], z["t"], z["dist"] if "dist" in z.files else None)
+
+
+def write_rig(path, rig):
+    """write a utils.CameraRig to the .npz that read_rig reads back bit for bit: K, R, t and, for a rig with distortion, dist (C, 8)"""
+    from ._lib import SspError
+    from .utils import CameraRig
+    if not isinstance(rig, CameraRig):
+        raise SspError("write_rig takes a CameraRig (utils.camera_rig), got %s" % type(rig).__name__)
+    arrays = dict(K=np.asarray(rig.K, np.float64), R=np.asarray(rig.R, np.float64), t=np.asarray(rig.t, np.float64))
+    if rig.dist is not None:
+        arrays["dist"] = np.asarray(rig.dist, np.float64)
+    np.savez(path, **arrays)
