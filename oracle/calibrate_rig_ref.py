@@ -154,6 +154,7 @@ def calibrate_ref(K, dist, P, uv, valid, R_rows, t_rows, reference=0, gate=40.0,
                 w = sc[winner(sc)]
                 wins[(a, b)] = (w[0], w[1], w[2])
     Rc, tc, parent, edge, conn = initial_rig(C, reference, wins)
+    R_tree, t_tree = Rc.copy(), tc.copy()
     free = [c for c in range(C) if conn[c] and c != reference]
     keys, rounds, iters, cost, cov, singular = None, 0, 0, 0.0, np.zeros((C, 6, 6)), False
     while True:
@@ -187,4 +188,4 @@ def calibrate_ref(K, dist, P, uv, valid, R_rows, t_rows, reference=0, gate=40.0,
     status = np.array([(0 if conn[c] else UNCONNECTED) | (SINGULAR if singular and c in free else 0) for c in range(C)])
     return dict(R=Rc, t=tc, cam_cov=cov, cam_obs=cam_obs, cam_rmse=cam_rmse, tree_parent=parent, edge_agree=edge, cam_status=status,
                 R_world=np.array([f["R"] for f in fused]), t_world=np.array([f["t"] for f in fused]), views=views, view_err=view_err,
-                linked=linked, rounds=rounds, iterations=iters, cost=cost)
+                linked=linked, rounds=rounds, iterations=iters, cost=cost, R_tree=R_tree, t_tree=t_tree)
