@@ -408,6 +408,33 @@ int ssp_fuse_views(const float* points3d, int points3d_shared, const float* poin
                    double* view_err, int* fuse_hyp, int* fuse_status, float* corners_world, void* work, long long work_bytes,
                    void* stream);
 
+/* ---- refinement of a rig's world poses against every camera's registered depth frame: one point-to-plane ICP in world axes
+ *      (rules: csrc/refine_rig_core.h; csrc/refine_rig.cu), fp64, one thread-block cluster of min(views, 8) 256-thread CTAs per
+ *      problem, every iteration in one launch.  The rig is ssp_fuse_views' (`views` = C cameras, 1..SSP_RIG_MAX_VIEWS; K3x3 [C][9]
+ *      DEVICE fp64, the projection's K; dist8_or_null [C][8]; R_rig [C][9], t_rig [C][3] camera from world); depth [groups * C][H][W]
+ *      uint16, row b = g * C + c registered to camera c, depth_scale as ssp_refine_depth takes it.  model, offsets, diam, iters and
+ *      the gates are ssp_refine_depth's; cls [groups][slots] (DEVICE int) each problem's class; points3d_table [num_classes]
+ *      [num_points][3] (DEVICE fp32) the points drawn into corners_world_ref.  count_or_null: DEVICE int [groups] (slots at
+ *      m >= count[g] get zeros and status 0); fuse_status_or_null: DEVICE int [groups][slots], ssp_fuse_views' status.
+ *  ssp_refine_depth_rig: refines each world pose R_world [groups][slots][9], t_world [3] (world from object) against the pairs of
+ *      every camera at once: each camera pairs the model points under its camera pose exactly as ssp_refine_depth does, the terms
+ *      are taken in world axes and one solve per iteration updates the world pose (left perturbation, as world_cov).  Out: R_out,
+ *      t_out; points_out, rmse_out of the last iteration over every camera; view_points [groups][slots][C] and view_rmse [C] each
+ *      camera's pairs and RMS point-to-plane residual of the last iteration (0: no pairs); status_out: SSP_REFINE_FEW_POINTS (fewer
+ *      than SSP_REFINE_MIN_POINTS pairs in all), SSP_REFINE_SINGULAR, SSP_REFINE_BAD_POSE (a pose that is not finite, or a
+ *      fuse_status with SSP_FUSE_NO_VALID or SSP_FUSE_NO_VIEW); with a bit set the output pose is the input pose.
+ *      corners_world_ref [groups * C][slots][num_points][2]: the output pose in every row's camera, ssp_fuse_views' corners_world
+ *      arithmetic (zeros where the fusion has no pose).  With C = 1 and identity extrinsics the outputs are ssp_refine_depth's bit
+ *      for bit.  SSP_ERR_ARG as ssp_refine_depth, and for views outside 1..16, num_points outside 7..10 or a null required
+ *      pointer. ---- */
+int ssp_refine_depth_rig(const unsigned short* depth, int W, int H, double depth_scale, int views, const double* K3x3,
+                         const double* dist8_or_null, const double* R_rig, const double* t_rig, const double* model, const int* offsets,
+                         const double* diam, const float* points3d_table, int num_points, int num_classes, const int* cls, int groups,
+                         int slots, const int* count_or_null, const int* fuse_status_or_null, const double* R_world,
+                         const double* t_world, int iters, double gate_start, double gate_end, double* R_out, double* t_out,
+                         int* points_out, double* rmse_out, int* status_out, int* view_points, double* view_rmse,
+                         float* corners_world_ref, void* stream);
+
 /* ---- fusing every detected instance across the cameras of a rig (rules: csrc/multiview_instances_core.h; csrc/multiview_rows.cu,
  *      csrc/multiview_instances.cu), fp64.  The rig, the rows b = g * C + c and max_iter are ssp_fuse_views'; each row has `slots` = M
  *      detection slots (1..SSP_FUSE_MAX_SLOTS): points3d_table [num_classes][num_points][3] (DEVICE fp32, the PnP points of each class

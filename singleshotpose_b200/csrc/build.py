@@ -6,13 +6,13 @@ import subprocess
 import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-SOURCES = ["abi.cu", "conv_tc.cu", "conv_band.cu", "conv_bandt.cu", "wgrad_tc.cu", "conv_simt.cu", "l0_fused.cu", "elementwise.cu", "sgd_pack.cu", "region.cu", "region_multi.cu", "pnp.cu", "pnp_consensus.cu", "pnp_dist.cu", "track.cu", "pose_filter.cu", "refine_depth.cu", "multiview_rows.cu", "multiview.cu", "multiview_instances.cu", "calibrate_rig.cu", "world_track.cu", "augment.cu", "adds.cu", "jpeg.cu", "render.cu"]
+SOURCES = ["abi.cu", "conv_tc.cu", "conv_band.cu", "conv_bandt.cu", "wgrad_tc.cu", "conv_simt.cu", "l0_fused.cu", "elementwise.cu", "sgd_pack.cu", "region.cu", "region_multi.cu", "pnp.cu", "pnp_consensus.cu", "pnp_dist.cu", "track.cu", "pose_filter.cu", "refine_depth.cu", "refine_rig.cu", "multiview_rows.cu", "multiview.cu", "multiview_instances.cu", "calibrate_rig.cu", "world_track.cu", "augment.cu", "adds.cu", "jpeg.cu", "render.cu"]
 # augment.cu restates Pillow's float/double pixel arithmetic bit for bit: no multiply-add contraction there
 # pose_filter.cu: the fp64 filter arithmetic is rounded as the host harness (g++ -ffp-contract=off) rounds it
-# refine_depth.cu: likewise, so the refinement's sums equal the harness's bit for bit
+# refine_depth.cu, refine_rig.cu: likewise, so the refinements' sums equal the harness's bit for bit
 # multiview.cu, multiview_instances.cu: the fusion stages likewise (multiview_rows.cu keeps the contraction of pnp.cu, whose bits its
 # PnP reproduces); world_track.cu: the pose filter of the world tracks likewise; calibrate_rig.cu: the rig calibration likewise
-EXTRA = {"augment.cu": ["-fmad=false"], "pose_filter.cu": ["-fmad=false"], "refine_depth.cu": ["-fmad=false"], "multiview.cu": ["-fmad=false"],
+EXTRA = {"augment.cu": ["-fmad=false"], "pose_filter.cu": ["-fmad=false"], "refine_depth.cu": ["-fmad=false"], "refine_rig.cu": ["-fmad=false"], "multiview.cu": ["-fmad=false"],
          "multiview_instances.cu": ["-fmad=false"], "world_track.cu": ["-fmad=false"],
          "calibrate_rig.cu": ["-fmad=false"]}
 LIB = os.path.join(HERE, "libssp_b200.so")

@@ -28,7 +28,8 @@ Command line: python -m singleshotpose_b200.predict --datacfg cfg/ape.data --mod
               [--depth-dir DIR [--depth-scale 0.001 --refine-iters 10]]: refine each pose against DIR/<image stem>.png, a 16-bit
               depth PNG registered to the image, adding the columns R_ref t_ref corners_ref_px refine_points refine_rmse refine_status
               [--rig rig.npz]: the images come in groups of C calibrated cameras (image i is camera i % C; utils_host.read_rig), adding
-              the per-capture columns R_world t_world world_cov views view_err fuse_hyp fuse_status and the per-image corners_world_px
+              the per-capture columns R_world t_world world_cov views view_err fuse_hyp fuse_status and the per-image corners_world_px;
+              with --depth-dir too, the fused poses are refined against every camera's depth, adding the columns RIG_REFINE_KEYS
 """
 from __future__ import annotations
 
@@ -91,6 +92,8 @@ class _FramePredictor:
     every row with its own camera into c.R, c.t, c.corners and fuses each capture's valid views (the head's flags) into one world
     pose per slot; a detecting head's slots are instead associated across the views by one ssp_fuse_instances (rule:
     csrc/multiview_instances_core.h), which solves every row likewise and fuses each capture's detections into world instances.
+    With a rig and meshes (not a detecting head) _fuse is followed by _refine_rig: one ssp_refine_depth_rig (rule:
+    csrc/refine_rig_core.h) refines each capture's fused world poses against the depth frames of all its cameras.
     _tail runs the whole tail; every head calls it.
     A subclass supplies the rest: _head_buffers(chain) allocates its selection's static buffers, _head(chain, stream) launches
     the selection after the forward and then the tail, and _outputs(chain) names the returned tensors."""
@@ -115,7 +118,7 @@ class _FramePredictor:
         self.eng.materialize(dev)
         self.rig = rig
         if rig is not None:
-            check_rig_predictor(name, rig, K, dist_coeffs, pnp, meshes, self.batch)
+            check_rig_predictor(name, rig, K, dist_coeffs, pnp, meshes, self.batch, detects=slots is not None)
             self.fuse_gate, self.fuse_thresh, self.keypoint_sigma = check_fuse_args(*fuse)
             K = rig.K[0]                        # object_table's check only: each row is solved and projected with its camera's K
         self.classes, points, Km = object_table(objects, self.num_classes, K)
@@ -156,6 +159,8 @@ class _FramePredictor:
             self._model, self._offsets, self._diam = refine_model_table(meshes, self.num_classes, dev)
             if not self._detects:                  # slot q: class classes[q]
                 self._slot_cls = torch.from_numpy(np.tile(self.classes.astype(np.int32), (B, 1))).to(dev)
+            if rig is not None:                    # the drawn points of corners_world_ref, by class id
+                self._P3_table = torch.from_numpy(points.astype(np.float32)).to(dev)
         W, H = self.shape
         self.out_hw = self.eng.spatial(self.eng.layers[-1], H, W)               # raises for a shape off the pooling pyramid
         self._bufs = Buffers(self.eng, self.batch, H, W, False, split_k=True)
@@ -184,7 +189,17 @@ class _FramePredictor:
             c.inliers = torch.empty(B, S, K, dtype=torch.bool, device=dev)
             wb = consensus_work_bytes(K, len(self._subsets), B * S)
             c.pnp_work = torch.empty(max(wb, 8) // 8, dtype=torch.float64, device=dev)
-        if self._refines:
+        if self._refines and self.rig is not None:
+            G, Cn = B // len(self.rig.K), len(self.rig.K)
+            c.R_world_ref = torch.empty(G, S, 3, 3, dtype=torch.float64, device=dev)
+            c.t_world_ref = torch.empty(G, S, 3, dtype=torch.float64, device=dev)
+            c.ref_points = torch.empty(G, S, dtype=torch.int32, device=dev)
+            c.ref_rmse = torch.empty(G, S, dtype=torch.float64, device=dev)
+            c.ref_status = torch.empty(G, S, dtype=torch.int32, device=dev)
+            c.ref_view_points = torch.empty(G, S, Cn, dtype=torch.int32, device=dev)
+            c.ref_view_rmse = torch.empty(G, S, Cn, dtype=torch.float64, device=dev)
+            c.corners_world_ref = torch.empty(B, S, K, 2, dtype=torch.float32, device=dev)
+        elif self._refines:
             c.R_ref = torch.empty(B, S, 3, 3, dtype=torch.float64, device=dev)
             c.t_ref = torch.empty(B, S, 3, dtype=torch.float64, device=dev)
             c.corners_ref = torch.empty(B, S, K, 2, dtype=torch.float32, device=dev)
@@ -260,6 +275,19 @@ class _FramePredictor:
              self.refine_gate[0], self.refine_gate[1], ptr(c.R_ref), ptr(c.t_ref), ptr(c.ref_points), ptr(c.ref_rmse), ptr(c.ref_status), s)
         self._project(c, s, c.R_ref, c.t_ref, c.corners_ref)
 
+    def _refine_rig(self, c, s):
+        """with a rig and meshes: each capture's fused world poses c.R_world, c.t_world refined against the depth frames of all
+        its cameras at once (ssp_refine_depth_rig; row b of c.depth is camera b % C) into c.R_world_ref, c.t_world_ref, ...;
+        c.corners_world_ref the refined pose in each frame's camera"""
+        Wf, Hf = c.frame
+        _K32, K64, D, Rr, tr = self._rig
+        Cn = len(self.rig.K)
+        call("ssp_refine_depth_rig", ptr(c.depth), Wf, Hf, self.depth_scale, Cn, ptr(K64), ptr(D), ptr(Rr), ptr(tr), ptr(self._model),
+             ptr(self._offsets), ptr(self._diam), ptr(self._P3_table), self.num_keypoints, self.num_classes, ptr(self._slot_cls),
+             self.batch // Cn, self.num_slots, None, ptr(c.fuse_status), ptr(c.R_world), ptr(c.t_world), self.refine_iters,
+             self.refine_gate[0], self.refine_gate[1], ptr(c.R_world_ref), ptr(c.t_world_ref), ptr(c.ref_points), ptr(c.ref_rmse),
+             ptr(c.ref_status), ptr(c.ref_view_points), ptr(c.ref_view_rmse), ptr(c.corners_world_ref), s)
+
     def _fuse(self, c, s, valid):
         """with a rig: every row's PnP and projection with its camera into c.R, c.t, c.corners, and each capture's valid views
         (valid (B, S) bool) fused into c.R_world, c.t_world, ... (ssp_fuse_views)"""
@@ -288,6 +316,8 @@ class _FramePredictor:
             return
         if self.rig is not None:
             self._fuse(c, s, valid)
+            if self._refines:
+                self._refine_rig(c, s)
             return
         self._solve(c, s)
         self._project(c, s)
@@ -308,6 +338,10 @@ class _FramePredictor:
     def _refine_outputs(self, c):
         if not self._refines:
             return {}
+        if self.rig is not None:
+            return dict(R_world_ref=c.R_world_ref, t_world_ref=c.t_world_ref, refine_points=c.ref_points, refine_rmse=c.ref_rmse,
+                        refine_status=c.ref_status, refine_view_points=c.ref_view_points, refine_view_rmse=c.ref_view_rmse,
+                        corners_world_ref_px=c.corners_world_ref)
         return dict(R_ref=c.R_ref, t_ref=c.t_ref, corners_ref_px=c.corners_ref, refine_points=c.ref_points, refine_rmse=c.ref_rmse,
                     refine_status=c.ref_status)
 
@@ -505,7 +539,11 @@ class PosePredictor(_FramePredictor):
     part in the fusion when conf > conf_thresh (default the cfg's [net] conf_thresh).  The outputs add, per capture, R_world (G, 3, 3),
     t_world (G, 3) world-from-object, world_cov (G, 6, 6), views (G, C) bool, view_err (G, C), fuse_hyp (G,), fuse_status (G,)
     (utils.fuse_views_batched, fuse = (gate, reproj_thresh, keypoint_sigma)), and per frame corners_world_px (B, 9, 2), the fused
-    pose in the frame's camera.  Not with pnp="consensus" or a mesh."""
+    pose in the frame's camera.  Not with pnp="consensus".  With a rig and mesh= every call takes depth=(B, H, W), row b registered
+    to frame b's camera, and each capture's fused pose is refined against the depth of all its cameras at once
+    (utils.refine_depth_rig_batched): the outputs add, per capture, R_world_ref (G, 3, 3), t_world_ref (G, 3), refine_points,
+    refine_rmse, refine_status (G,), refine_view_points, refine_view_rmse (G, C), and per frame corners_world_ref_px (B, 9, 2);
+    there is no per-frame R_ref."""
 
     def __init__(self, model, corners3D, K, frame_size=(640, 480), shape=None, batch=1, graph=True, max_graphs=4, pnp="plain",
                  reproj_thresh=8.0, dist_coeffs=None, mesh=None, depth_scale=0.001, refine_iters=10, refine_gate=(0.5, 0.02), rig=None,
@@ -537,17 +575,18 @@ class PosePredictor(_FramePredictor):
         return dict(R=c.R[:, 0], t=c.t[:, 0], conf=c.conf, keypoints_px=c.kp[:, 0], corners_px=c.corners[:, 0], **one)
 
 
-def check_rig_predictor(name, rig, K, dist_coeffs, pnp, meshes, batch):
+def check_rig_predictor(name, rig, K, dist_coeffs, pnp, meshes, batch, detects=False):
     """SspError for what a predictor with a rig refuses: a rig that is not a utils.CameraRig, K or dist_coeffs given as well
-    (each camera brings its own), pnp="consensus", meshes, or a batch that is not whole captures.  A detecting head
-    is let through: its detections are associated across the views (ssp_fuse_instances)"""
+    (each camera brings its own), pnp="consensus", meshes on a detecting head (detects: its world instances are not refined), or
+    a batch that is not whole captures.  A detecting head is let through: its detections are associated across the views
+    (ssp_fuse_instances)"""
     if not isinstance(rig, CameraRig):
         raise SspError("rig must be a CameraRig (utils.camera_rig)")
     if K is not None or dist_coeffs is not None:
         raise SspError("%s with a rig takes K=None and no dist_coeffs: each camera of the rig brings its own" % name)
     if pnp != "plain":
         raise SspError("%s with a rig fuses the plain per-view solves: pnp=%r is not supported with a rig" % (name, pnp))
-    if meshes is not None:
+    if meshes is not None and detects:
         raise SspError("%s: depth refinement (mesh= / meshes=) is not supported with a rig" % name)
     if batch % len(rig.K):
         raise SspError("batch %d is not a multiple of the rig's %d cameras" % (batch, len(rig.K)))
@@ -557,6 +596,8 @@ def check_rig_predictor(name, rig, K, dist_coeffs, pnp, meshes, batch):
 FUSE_KEYS = ("R_world", "t_world", "world_cov", "views", "view_err", "fuse_hyp", "fuse_status", "corners_world_px")     # the --rig columns
 CONSENSUS_KEYS = {"plain": (), "consensus": ("inliers", "hyp")}          # the .npz columns each --pnp adds
 REFINE_KEYS = ("R_ref", "t_ref", "corners_ref_px", "refine_points", "refine_rmse", "refine_status")     # the --depth-dir columns
+RIG_REFINE_KEYS = ("R_world_ref", "t_world_ref", "refine_points", "refine_rmse", "refine_status", "refine_view_points", "refine_view_rmse",
+                   "corners_world_ref_px")                                # the --rig --depth-dir columns
 SIZE_KEYS = (("width", "height"),)                                      # the frame size entries of a single-object .data file
 
 
@@ -587,15 +628,21 @@ def add_rig_arg(ap):
                          "in groups of C, image i is camera i %% C; adds the columns " + " ".join(FUSE_KEYS))
 
 
-def check_rig_args(args):
-    """-> the --rig file's CameraRig, or None; SspError for --rig with --dist, --depth-dir or --pnp consensus, or an image count
-    that is not a multiple of the rig's cameras"""
+def check_rig_args(args, refines=True):
+    """-> the --rig file's CameraRig, or None; SspError for --rig with --dist or --pnp consensus, an image count that is not a
+    multiple of the rig's cameras, and with --depth-dir an image whose depth file DIR/<stem>.png does not exist (checked before
+    the .data file or the model is read); refines=False: --depth-dir itself is refused with --rig"""
     if args.rig is None:
         return None
     if args.dist is not None:
         raise SspError("--dist and --rig: each camera of the rig brings its own distortion coefficients (the rig's dist)")
-    if args.depth_dir is not None:
+    if args.depth_dir is not None and not refines:
         raise SspError("--depth-dir is not supported with --rig")
+    if args.depth_dir is not None:
+        for p in args.images:
+            path = os.path.join(args.depth_dir, os.path.splitext(os.path.basename(p))[0] + ".png")
+            if not os.path.isfile(path):
+                raise SspError("depth file %s does not exist" % path)
     if args.pnp != "plain":
         raise SspError("--pnp %s is not supported with --rig" % args.pnp)
     from .utils_host import read_rig
@@ -604,6 +651,13 @@ def check_rig_args(args):
         raise SspError("%d images are not whole captures of the rig's %d cameras: give the images in groups of %d"
                        % (len(args.images), len(rig.K), len(rig.K)))
     return rig
+
+
+def refine_keys(refine, rig):
+    """the .npz columns --depth-dir adds: REFINE_KEYS, or RIG_REFINE_KEYS with --rig"""
+    if not refine:
+        return ()
+    return RIG_REFINE_KEYS if rig is not None else REFINE_KEYS
 
 
 def check_depth_args(args):
@@ -738,7 +792,7 @@ def main(argv=None):
     refine = dict(mesh=read_mesh(mesh), **refine_kwargs(a)) if a.depth_dir is not None else {}
     cams = dict(K=K) if rig is None else dict(K=None, rig=rig, batch=len(rig.K))
     pred = PosePredictor(model, corners3D, frame_size=size, pnp=a.pnp, reproj_thresh=a.reproj_thresh, dist_coeffs=dist, **cams, **refine)
-    res = {k: [] for k in ("R", "t", "conf", "keypoints_px", "corners_px") + CONSENSUS_KEYS[a.pnp] + (REFINE_KEYS if refine else ())
+    res = {k: [] for k in ("R", "t", "conf", "keypoints_px", "corners_px") + CONSENSUS_KEYS[a.pnp] + refine_keys(refine, rig)
            + (FUSE_KEYS if rig is not None else ())}
     for r in predict_files(pred, a.images, a.depth_dir, pred.batch):
         for k in res:

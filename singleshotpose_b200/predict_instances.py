@@ -340,7 +340,7 @@ def parse_args(argv=None):
     a.objects = parse_objects(a.object) if a.object else None
     if a.dist is not None:
         camera_distortion(a.dist)
-    a.rig_cams = check_rig_args(a)
+    a.rig_cams = check_rig_args(a, refines=False)
     return a
 
 

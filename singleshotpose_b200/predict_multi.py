@@ -34,8 +34,8 @@ import numpy as np
 import torch
 
 from ._lib import SspError, call, ptr
-from .predict import (CONSENSUS_KEYS, FUSE_KEYS, REFINE_KEYS, _FramePredictor, add_depth_args, add_dist_arg, add_pnp_args, add_rig_arg, camera_dist,
-                      check_depth_args, check_rig_args, mesh_corners, predict_files, read_camera, read_mesh, refine_kwargs)
+from .predict import (CONSENSUS_KEYS, FUSE_KEYS, _FramePredictor, add_depth_args, add_dist_arg, add_pnp_args, add_rig_arg, camera_dist,
+                      check_depth_args, check_rig_args, mesh_corners, predict_files, read_camera, read_mesh, refine_keys, refine_kwargs)
 from .utils import check_pnp_args
 
 MAX_ENTRIES = 4096          # H*W*num_anchors the select kernel keeps in shared memory (eval_multi_core.h kMaxEntries)
@@ -60,7 +60,10 @@ class MultiPosePredictor(_FramePredictor):
     rig=utils.camera_rig(...) of C calibrated cameras (K=None, no dist_coeffs): frame g C + c is camera c of capture g, and each
     class's detected views are fused into one world pose, as predict.PosePredictor's rig= does; the outputs add R_world (G, Q, 3, 3),
     t_world (G, Q, 3), world_cov (G, Q, 6, 6), views (G, Q, C), view_err (G, Q, C), fuse_hyp, fuse_status (G, Q) and
-    corners_world_px (B, Q, 9, 2)."""
+    corners_world_px (B, Q, 9, 2).  With a rig and meshes= each class's fused pose is refined against the depth of all the
+    capture's cameras, as predict.PosePredictor's rig= with mesh= does, adding R_world_ref (G, Q, 3, 3), t_world_ref (G, Q, 3),
+    refine_points, refine_rmse, refine_status (G, Q), refine_view_points, refine_view_rmse (G, Q, C) and corners_world_ref_px
+    (B, Q, 9, 2)."""
 
     def __init__(self, model, objects, K, frame_size=(640, 480), shape=None, batch=1, conf_thresh=None, graph=True, max_graphs=4,
                  pnp="plain", reproj_thresh=8.0, dist_coeffs=None, meshes=None, depth_scale=0.001, refine_iters=10, refine_gate=(0.5, 0.02),
@@ -165,7 +168,7 @@ def main(argv=None):
     model.cuda().eval()
     cams = dict(K=K) if rig is None else dict(K=None, rig=rig, batch=len(rig.K))
     pred = MultiPosePredictor(model, objects, frame_size=size, pnp=a.pnp, reproj_thresh=a.reproj_thresh, dist_coeffs=dist, **cams, **refine)
-    res = {k: [] for k in OUTPUT_KEYS + CONSENSUS_KEYS[a.pnp] + (REFINE_KEYS if refine else ()) + (FUSE_KEYS if rig is not None else ())}
+    res = {k: [] for k in OUTPUT_KEYS + CONSENSUS_KEYS[a.pnp] + refine_keys(refine, rig) + (FUSE_KEYS if rig is not None else ())}
     for r in predict_files(pred, a.images, a.depth_dir, pred.batch):
         for k in res:
             res[k].extend(r[k])

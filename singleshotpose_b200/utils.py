@@ -480,6 +480,22 @@ def refine_model_table(meshes, num_classes, dev):
     return (torch.from_numpy(np.ascontiguousarray(model)).to(dev), torch.from_numpy(offsets).to(dev), torch.from_numpy(diam).to(dev))
 
 
+def _depth_tensor(depth, dev):
+    """(n, H, W) uint16 numpy array or CUDA tensor -> the device int16 tensor of its bits; SspError for another type or shape"""
+    if torch.is_tensor(depth):
+        if not depth.is_cuda or depth.dtype != torch.uint16:
+            raise SspError("depth given as a torch tensor must be a CUDA uint16 tensor, got %s %s" % (depth.device, depth.dtype))
+        D = depth.to(dev).view(torch.int16).contiguous()
+    else:
+        D = np.asarray(depth)
+        if D.dtype != np.uint16:
+            raise SspError("depth must be uint16, got %s" % D.dtype)
+        D = torch.from_numpy(np.ascontiguousarray(D).view(np.int16)).to(dev)
+    if D.dim() != 3:
+        raise SspError("depth must be (n, H, W), got %s" % (tuple(D.shape),))
+    return D
+
+
 def refine_depth_batched(depth, vertices, faces, K, R, t, depth_scale=0.001, iters=10, gate=(0.5, 0.02), dist_coeffs=None):
     """Refine n poses of one mesh against n registered depth frames on the GPU (ssp_refine_depth, rule: csrc/refine_depth_core.h):
     projective point-to-plane ICP of the mesh's vertices, with the outward normals of vertex_normals, against the depth pixel
@@ -493,17 +509,7 @@ def refine_depth_batched(depth, vertices, faces, K, R, t, depth_scale=0.001, ite
     depth_scale, iters, (s, e) = check_refine_args(depth_scale, iters, gate)
     k = camera_distortion(dist_coeffs)
     dev = _dev()
-    if torch.is_tensor(depth):
-        if not depth.is_cuda or depth.dtype != torch.uint16:
-            raise SspError("depth given as a torch tensor must be a CUDA uint16 tensor, got %s %s" % (depth.device, depth.dtype))
-        D = depth.to(dev).view(torch.int16).contiguous()
-    else:
-        D = np.asarray(depth)
-        if D.dtype != np.uint16:
-            raise SspError("depth must be uint16, got %s" % D.dtype)
-        D = torch.from_numpy(np.ascontiguousarray(D).view(np.int16)).to(dev)
-    if D.dim() != 3:
-        raise SspError("depth must be (n, H, W), got %s" % (tuple(D.shape),))
+    D = _depth_tensor(depth, dev)
     n, H, W = D.shape
     R, t = (torch.as_tensor(a).to(dev, torch.float64).contiguous() for a in (R, t))
     R, t = R.reshape(-1, 3, 3), t.reshape(-1, 3)
@@ -628,6 +634,54 @@ def fuse_views_batched(points_3D, keypoints_px, rig, valid=None, gate=40.0, repr
          ptr(o["views"]), ptr(o["view_err"]), ptr(o["fuse_hyp"]), ptr(o["fuse_status"]), ptr(o["corners_world_px"]), ptr(work),
          work.numel() * 8, stream_ptr())
     return o if slotted else {k: v[:, 0] for k, v in o.items()}
+
+
+def refine_depth_rig_batched(depth, vertices, faces, rig, R_world, t_world, depth_scale=0.001, iters=10, gate=(0.5, 0.02), fuse_status=None):
+    """Refine world poses of one mesh against the depth frames of every camera of a rig at once on the GPU (ssp_refine_depth_rig,
+    rule: csrc/refine_rig_core.h): each camera pairs the mesh's vertices with its own depth frame as refine_depth_batched does,
+    and one point-to-plane ICP over the pairs of all cameras solves for the world pose.  rig: camera_rig's CameraRig of C cameras;
+    depth (G C, H, W) uint16 numpy array or CUDA tensor, row g C + c registered to camera c (its K and coefficients); R_world
+    (G[, S], 3, 3), t_world (G[, S], 3) world from model (fuse_views_batched's); fuse_status (G[, S]) int or None: a pose whose
+    status has FUSE_STATUS no_valid or no_view is left as it is (bad_pose).  depth_scale, iters and gate as refine_depth_batched.
+    -> (R (G[, S], 3, 3), t (G[, S], 3), points (G[, S]) int32 pairs of the last iteration over all cameras, rmse (G[, S]) its RMS
+    point-to-plane residual, status (G[, S]) int32 REFINE_STATUS bits (with a bit set the pose is the input pose), view_points
+    (G[, S], C) int32 and view_rmse (G[, S], C) each camera's pairs and RMS residual of the last iteration), CUDA tensors."""
+    depth_scale, iters, (s, e) = check_refine_args(depth_scale, iters, gate)
+    if not isinstance(rig, CameraRig):
+        raise SspError("rig must be a CameraRig (utils.camera_rig)")
+    dev = _dev()
+    D = _depth_tensor(depth, dev)
+    B, H, W = D.shape
+    C = len(rig.K)
+    if B % C:
+        raise SspError("%d depth frames are not whole captures of the rig's %d cameras" % (B, C))
+    G = B // C
+    R, t = (torch.as_tensor(a).to(dev, torch.float64).contiguous() for a in (R_world, t_world))
+    if R.dim() < 3 or R.shape[-2:] != (3, 3) or R.shape[0] != G or t.shape != R.shape[:-1]:
+        raise SspError("refine_depth_rig_batched: %d captures but R_world %s, t_world %s: (G[, S], 3, 3) and (G[, S], 3)"
+                       % (G, tuple(R.shape), tuple(t.shape)))
+    lead = tuple(R.shape[:-2])
+    S = int(np.prod(lead[1:], dtype=np.int64)) if len(lead) > 1 else 1
+    fs = None
+    if fuse_status is not None:
+        fs = torch.as_tensor(fuse_status).to(dev, torch.int32).contiguous()
+        if tuple(fs.shape) != lead:
+            raise SspError("fuse_status must be %s, got %s" % (lead, tuple(fs.shape)))
+    model, offsets, diam = refine_model_table({0: (vertices, faces)}, 1, dev)
+    i32 = lambda *sh: torch.empty(*sh, dtype=torch.int32, device=dev)
+    f64 = lambda *sh: torch.empty(*sh, dtype=torch.float64, device=dev)
+    out = (torch.empty_like(R), torch.empty_like(t), i32(*lead), f64(*lead), i32(*lead), i32(*lead, C), f64(*lead, C))
+    if G == 0 or S == 0:
+        return out
+    _K32, K64, Dd, Rr, tr = rig_tensors(rig, dev)
+    V = np.asarray(vertices, np.float64)
+    box = np.concatenate([V.mean(0, keepdims=True), get_3D_corners(np.c_[V, np.ones((len(V), 1))].T)[:3].T])    # the drawn points
+    table = torch.from_numpy(box.astype(np.float32)).to(dev)
+    corners = torch.empty(B, S, 9, 2, dtype=torch.float32, device=dev)
+    cls = torch.zeros(G, S, dtype=torch.int32, device=dev)
+    call("ssp_refine_depth_rig", ptr(D), W, H, depth_scale, C, ptr(K64), ptr(Dd), ptr(Rr), ptr(tr), ptr(model), ptr(offsets), ptr(diam),
+         ptr(table), 9, 1, ptr(cls), G, S, None, ptr(fs), ptr(R), ptr(t), iters, s, e, *(ptr(o) for o in out), ptr(corners), stream_ptr())
+    return out
 
 
 def fuse_instances_work_bytes(groups, views, slots):
