@@ -435,6 +435,33 @@ int ssp_refine_depth_rig(const unsigned short* depth, int W, int H, double depth
                          int* points_out, double* rmse_out, int* status_out, int* view_points, double* view_rmse,
                          float* corners_world_ref, void* stream);
 
+/* ---- refinement of every world instance of a rig's capture against every camera's depth frame, each depth pixel owned by the
+ *      instance drawn in front of it (rules: csrc/refine_instances_core.h; csrc/refine_instances.cu), fp64.  The rig, depth,
+ *      depth_scale, model, offsets, diam, points3d_table, iters and the gates are ssp_refine_depth_rig's; the problems are the world
+ *      slots of ssp_fuse_instances: world_cls [groups][slots] (slots 1..SSP_FUSE_MAX_SLOTS; a class outside [0, num_classes) is an
+ *      empty slot), world_count_or_null [groups] (slots at w >= world_count[g] get zeros and status 0), fuse_status_or_null, R_world,
+ *      t_world.  faces [total][3] (DEVICE int32) class c's triangles at face_offsets[c] .. face_offsets[c + 1] - 1 (DEVICE int
+ *      [num_classes + 1]) as class-local vertex indices into its model rows (every index must lie in [0, its vertex count));
+ *      max_faces the largest face count of a class.
+ *  ssp_refine_instances_rig: per iteration, every non-empty slot with a usable input pose is drawn at its current pose (its input
+ *      pose once a status bit has stopped it) into one z-buffer of 64-bit keys (float depth << 32 | slot) per camera; each slot
+ *      then pairs as ssp_refine_depth_rig does, dropping a pair whose pixel another slot owns, and solves.  Out: ssp_refine_depth_rig's
+ *      outputs per slot, view_hidden [groups][slots][C] the pairs dropped for ownership in the last iteration that ran, and
+ *      instance_map [groups * C][H][W] int16: the slot drawn in front at each pixel under the output poses (-1: none).  A capture
+ *      whose only drawn slot is w gives ssp_refine_depth_rig's outputs for w bit for bit.  work: DEVICE scratch (8-B aligned) of at
+ *      least the *bytes_out that ssp_refine_instances_rig_work_bytes(groups, views, slots, W, H, bytes_out) writes: the owner
+ *      buffers (8 B per pixel per frame) and the pose state.  SSP_ERR_ARG as ssp_refine_depth_rig, and for slots outside 1..256,
+ *      max_faces < 0, a null pointer or a short workspace. ---- */
+int ssp_refine_instances_rig_work_bytes(int groups, int views, int slots, int W, int H, long long* bytes_out);
+int ssp_refine_instances_rig(const unsigned short* depth, int W, int H, double depth_scale, int views, const double* K3x3,
+                             const double* dist8_or_null, const double* R_rig, const double* t_rig, const double* model, const int* offsets,
+                             const double* diam, const int* faces, const int* face_offsets, int max_faces, const float* points3d_table,
+                             int num_points, int num_classes, const int* world_cls, int groups, int slots, const int* world_count_or_null,
+                             const int* fuse_status_or_null, const double* R_world, const double* t_world, int iters, double gate_start,
+                             double gate_end, double* R_out, double* t_out, int* points_out, double* rmse_out, int* status_out,
+                             int* view_points, double* view_rmse, int* view_hidden, float* corners_world_ref, short* instance_map,
+                             void* work, long long work_bytes, void* stream);
+
 /* ---- fusing every detected instance across the cameras of a rig (rules: csrc/multiview_instances_core.h; csrc/multiview_rows.cu,
  *      csrc/multiview_instances.cu), fp64.  The rig, the rows b = g * C + c and max_iter are ssp_fuse_views'; each row has `slots` = M
  *      detection slots (1..SSP_FUSE_MAX_SLOTS): points3d_table [num_classes][num_points][3] (DEVICE fp32, the PnP points of each class

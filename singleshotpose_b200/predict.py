@@ -43,8 +43,9 @@ import torch
 from ._lib import SspError, call, load, ptr, stream_ptr
 from .engine import Buffers
 from .image import BICUBIC
-from .utils import (CameraRig, camera_distortion, check_fuse_args, check_pnp_args, check_refine_args, consensus_subsets, consensus_work_bytes,
-                    distortion_tensor, fuse_instances_outputs, fuse_instances_work_bytes, fuse_work_bytes, inlier_bits, keypoint_bits, object_table, refine_model_table, rig_tensors)
+from .utils import (CameraRig, camera_distortion, check_fuse_args, check_instance_meshes, check_pnp_args, check_refine_args, consensus_subsets,
+                    consensus_work_bytes, distortion_tensor, fuse_instances_outputs, fuse_instances_work_bytes, fuse_work_bytes, inlier_bits,
+                    keypoint_bits, object_table, refine_face_table, refine_instances_work_bytes, refine_model_table, rig_tensors)
 
 
 class _Chain:
@@ -92,8 +93,10 @@ class _FramePredictor:
     every row with its own camera into c.R, c.t, c.corners and fuses each capture's valid views (the head's flags) into one world
     pose per slot; a detecting head's slots are instead associated across the views by one ssp_fuse_instances (rule:
     csrc/multiview_instances_core.h), which solves every row likewise and fuses each capture's detections into world instances.
-    With a rig and meshes (not a detecting head) _fuse is followed by _refine_rig: one ssp_refine_depth_rig (rule:
-    csrc/refine_rig_core.h) refines each capture's fused world poses against the depth frames of all its cameras.
+    With a rig and meshes _fuse is followed by _refine_rig: one ssp_refine_depth_rig (rule: csrc/refine_rig_core.h) refines each
+    capture's fused world poses against the depth frames of all its cameras; a detecting head's world instances are refined
+    together by _refine_instances instead: one ssp_refine_instances_rig (rule: csrc/refine_instances_core.h), in which each depth
+    pixel belongs to the instance drawn in front of it.
     _tail runs the whole tail; every head calls it.
     A subclass supplies the rest: _head_buffers(chain) allocates its selection's static buffers, _head(chain, stream) launches
     the selection after the forward and then the tail, and _outputs(chain) names the returned tensors."""
@@ -118,7 +121,7 @@ class _FramePredictor:
         self.eng.materialize(dev)
         self.rig = rig
         if rig is not None:
-            check_rig_predictor(name, rig, K, dist_coeffs, pnp, meshes, self.batch, detects=slots is not None)
+            check_rig_predictor(name, rig, K, dist_coeffs, pnp, meshes, self.batch, detects=slots is not None, num_classes=self.num_classes)
             self.fuse_gate, self.fuse_thresh, self.keypoint_sigma = check_fuse_args(*fuse)
             K = rig.K[0]                        # object_table's check only: each row is solved and projected with its camera's K
         self.classes, points, Km = object_table(objects, self.num_classes, K)
@@ -161,6 +164,9 @@ class _FramePredictor:
                 self._slot_cls = torch.from_numpy(np.tile(self.classes.astype(np.int32), (B, 1))).to(dev)
             if rig is not None:                    # the drawn points of corners_world_ref, by class id
                 self._P3_table = torch.from_numpy(points.astype(np.float32)).to(dev)
+            if rig is not None and self._detects:  # the faces the world instances are drawn with
+                self._faces, self._face_offsets, self._max_faces = refine_face_table(check_instance_meshes(meshes, self.num_classes),
+                                                                                     self.num_classes, dev)
         W, H = self.shape
         self.out_hw = self.eng.spatial(self.eng.layers[-1], H, W)               # raises for a shape off the pooling pyramid
         self._bufs = Buffers(self.eng, self.batch, H, W, False, split_k=True)
@@ -199,6 +205,11 @@ class _FramePredictor:
             c.ref_view_points = torch.empty(G, S, Cn, dtype=torch.int32, device=dev)
             c.ref_view_rmse = torch.empty(G, S, Cn, dtype=torch.float64, device=dev)
             c.corners_world_ref = torch.empty(B, S, K, 2, dtype=torch.float32, device=dev)
+            if self._detects:
+                Wf, Hf = c.frame
+                c.ref_view_hidden = torch.empty(G, S, Cn, dtype=torch.int32, device=dev)
+                c.instance_map = torch.empty(B, Hf, Wf, dtype=torch.int16, device=dev)
+                c.ref_work = torch.empty(max(refine_instances_work_bytes(G, Cn, S, Wf, Hf), 8) // 8, dtype=torch.float64, device=dev)
         elif self._refines:
             c.R_ref = torch.empty(B, S, 3, 3, dtype=torch.float64, device=dev)
             c.t_ref = torch.empty(B, S, 3, dtype=torch.float64, device=dev)
@@ -288,6 +299,22 @@ class _FramePredictor:
              self.refine_gate[0], self.refine_gate[1], ptr(c.R_world_ref), ptr(c.t_world_ref), ptr(c.ref_points), ptr(c.ref_rmse),
              ptr(c.ref_status), ptr(c.ref_view_points), ptr(c.ref_view_rmse), ptr(c.corners_world_ref), s)
 
+    def _refine_instances(self, c, s):
+        """with a rig, meshes and a detecting head: every world instance of each capture (c.fi) refined against the depth frames
+        of all its cameras, each depth pixel owned by the instance drawn in front of it (ssp_refine_instances_rig), into
+        c.R_world_ref, c.t_world_ref, ..., c.ref_view_hidden and c.instance_map"""
+        Wf, Hf = c.frame
+        _K32, K64, D, Rr, tr = self._rig
+        Cn = len(self.rig.K)
+        fi = c.fi
+        call("ssp_refine_instances_rig", ptr(c.depth), Wf, Hf, self.depth_scale, Cn, ptr(K64), ptr(D), ptr(Rr), ptr(tr), ptr(self._model),
+             ptr(self._offsets), ptr(self._diam), ptr(self._faces), ptr(self._face_offsets), self._max_faces, ptr(self._P3_table),
+             self.num_keypoints, self.num_classes, ptr(fi["world_cls"]), self.batch // Cn, self.num_slots, ptr(fi["world_count"]),
+             ptr(fi["fuse_status"]), ptr(fi["R_world"]), ptr(fi["t_world"]), self.refine_iters, self.refine_gate[0], self.refine_gate[1],
+             ptr(c.R_world_ref), ptr(c.t_world_ref), ptr(c.ref_points), ptr(c.ref_rmse), ptr(c.ref_status), ptr(c.ref_view_points),
+             ptr(c.ref_view_rmse), ptr(c.ref_view_hidden), ptr(c.corners_world_ref), ptr(c.instance_map), ptr(c.ref_work),
+             c.ref_work.numel() * 8, s)
+
     def _fuse(self, c, s, valid):
         """with a rig: every row's PnP and projection with its camera into c.R, c.t, c.corners, and each capture's valid views
         (valid (B, S) bool) fused into c.R_world, c.t_world, ... (ssp_fuse_views)"""
@@ -313,6 +340,8 @@ class _FramePredictor:
         the fusion of the views whose slots are valid (B, S) bool"""
         if self.rig is not None and self._detects:
             self._fuse_instances(c, s)
+            if self._refines:
+                self._refine_instances(c, s)
             return
         if self.rig is not None:
             self._fuse(c, s, valid)
@@ -339,9 +368,12 @@ class _FramePredictor:
         if not self._refines:
             return {}
         if self.rig is not None:
-            return dict(R_world_ref=c.R_world_ref, t_world_ref=c.t_world_ref, refine_points=c.ref_points, refine_rmse=c.ref_rmse,
-                        refine_status=c.ref_status, refine_view_points=c.ref_view_points, refine_view_rmse=c.ref_view_rmse,
-                        corners_world_ref_px=c.corners_world_ref)
+            out = dict(R_world_ref=c.R_world_ref, t_world_ref=c.t_world_ref, refine_points=c.ref_points, refine_rmse=c.ref_rmse,
+                       refine_status=c.ref_status, refine_view_points=c.ref_view_points, refine_view_rmse=c.ref_view_rmse,
+                       corners_world_ref_px=c.corners_world_ref)
+            if self._detects:
+                out.update(refine_view_hidden=c.ref_view_hidden, instance_map=c.instance_map)
+            return out
         return dict(R_ref=c.R_ref, t_ref=c.t_ref, corners_ref_px=c.corners_ref, refine_points=c.ref_points, refine_rmse=c.ref_rmse,
                     refine_status=c.ref_status)
 
@@ -575,11 +607,12 @@ class PosePredictor(_FramePredictor):
         return dict(R=c.R[:, 0], t=c.t[:, 0], conf=c.conf, keypoints_px=c.kp[:, 0], corners_px=c.corners[:, 0], **one)
 
 
-def check_rig_predictor(name, rig, K, dist_coeffs, pnp, meshes, batch, detects=False):
+def check_rig_predictor(name, rig, K, dist_coeffs, pnp, meshes, batch, detects=False, num_classes=None):
     """SspError for what a predictor with a rig refuses: a rig that is not a utils.CameraRig, K or dist_coeffs given as well
-    (each camera brings its own), pnp="consensus", meshes on a detecting head (detects: its world instances are not refined), or
-    a batch that is not whole captures.  A detecting head is let through: its detections are associated across the views
-    (ssp_fuse_instances)"""
+    (each camera brings its own), pnp="consensus", or a batch that is not whole captures; on a detecting head (detects), whose
+    detections are associated across the views (ssp_fuse_instances) and whose world instances are drawn to refine them against
+    depth, meshes that utils.check_instance_meshes refuses (a class id outside [0, num_classes), a face index outside its
+    vertices, a diameter that is not > 0 or no face of non-zero area)"""
     if not isinstance(rig, CameraRig):
         raise SspError("rig must be a CameraRig (utils.camera_rig)")
     if K is not None or dist_coeffs is not None:
@@ -587,7 +620,7 @@ def check_rig_predictor(name, rig, K, dist_coeffs, pnp, meshes, batch, detects=F
     if pnp != "plain":
         raise SspError("%s with a rig fuses the plain per-view solves: pnp=%r is not supported with a rig" % (name, pnp))
     if meshes is not None and detects:
-        raise SspError("%s: depth refinement (mesh= / meshes=) is not supported with a rig" % name)
+        check_instance_meshes(meshes, num_classes)
     if batch % len(rig.K):
         raise SspError("batch %d is not a multiple of the rig's %d cameras" % (batch, len(rig.K)))
 
@@ -628,16 +661,14 @@ def add_rig_arg(ap):
                          "in groups of C, image i is camera i %% C; adds the columns " + " ".join(FUSE_KEYS))
 
 
-def check_rig_args(args, refines=True):
+def check_rig_args(args):
     """-> the --rig file's CameraRig, or None; SspError for --rig with --dist or --pnp consensus, an image count that is not a
     multiple of the rig's cameras, and with --depth-dir an image whose depth file DIR/<stem>.png does not exist (checked before
-    the .data file or the model is read); refines=False: --depth-dir itself is refused with --rig"""
+    the .data file or the model is read)"""
     if args.rig is None:
         return None
     if args.dist is not None:
         raise SspError("--dist and --rig: each camera of the rig brings its own distortion coefficients (the rig's dist)")
-    if args.depth_dir is not None and not refines:
-        raise SspError("--depth-dir is not supported with --rig")
     if args.depth_dir is not None:
         for p in args.images:
             path = os.path.join(args.depth_dir, os.path.splitext(os.path.basename(p))[0] + ".png")

@@ -42,7 +42,10 @@ Command line: python -m singleshotpose_b200.predict_instances --datacfg cfg/occl
               [--rig rig.npz]: the images come in groups of C calibrated cameras (image i is camera i % C; utils_host.read_rig)
               and each capture's detections are associated into world instances, adding the per-detection column world_index and
               the per-world-instance rows capture world_cls R_world t_world world_cov members view_err fuse_hyp fuse_status
-              (not with --dist, --depth-dir or --pnp consensus)
+              (not with --dist or --pnp consensus)
+              [--rig rig.npz --depth-dir DIR [--depth-scale 0.001 --refine-iters 10]]: each capture's world instances are refined
+              together against every camera's DIR/<image stem>.png, each depth pixel owned by the instance drawn in front of it,
+              adding the per-world-instance columns RIG_REFINE_KEYS (not with --track)
               [--rig rig.npz --track [--match-dist 0.5 --max-misses 5 --max-tracks 64] [--motion cv --keypoint-sigma 2 --fps 30]]:
               the captures, in order, as one stream of tracked world instances, adding the per-detection column track_id, the
               per-world-instance column world_track_id and, with --motion, the per-world-instance columns R_filt t_filt velocity
@@ -69,6 +72,8 @@ OUTPUT_KEYS = ("count", "kept", "cls", "R", "t", "conf", "cls_conf", "keypoints_
 ROW_KEYS = ("cls", "R", "t", "conf", "cls_conf", "keypoints_px", "corners_px")
 MOTION_KEYS = ("R_filt", "t_filt", "velocity", "pose_cov")          # the --motion columns
 WORLD_KEYS = ("world_cls", "R_world", "t_world", "world_cov", "members", "view_err", "fuse_hyp", "fuse_status")   # --rig: per world instance
+RIG_REFINE_KEYS = ("R_world_ref", "t_world_ref", "refine_points", "refine_rmse", "refine_status", "refine_view_points", "refine_view_rmse",
+                   "refine_view_hidden")                                  # --rig --depth-dir: per world instance
 
 
 class InstancePosePredictor(_FramePredictor):
@@ -93,7 +98,15 @@ class InstancePosePredictor(_FramePredictor):
     distortion gives; the detections are then associated across the views into world instances (utils.fuse_instances_batched,
     fuse = (gate, reproj_thresh, keypoint_sigma)), adding per capture world_count (G,), unfused (G,), world_cls (G, M), R_world
     (G, M, 3, 3), t_world (G, M, 3), world_cov (G, M, 6, 6), members (G, M, C), view_err (G, M, C), fuse_hyp (G, M), fuse_status
-    (G, M), and per frame world_index (B, M) and corners_world_px (B, M, 9, 2).  Not with pnp="consensus" or meshes."""
+    (G, M), and per frame world_index (B, M) and corners_world_px (B, M, 9, 2).  Not with pnp="consensus".
+    With a rig and meshes every call takes depth=(B, H, W), row b registered to frame b's camera, and each capture's world
+    instances are refined together against the depth of all its cameras (utils.refine_instances_rig_batched): every instance is
+    drawn at its current pose, a depth pixel belongs to the instance drawn in front of it, and an instance pairs only with the
+    pixels no other instance owns.  The outputs add, per world slot, R_world_ref (G, M, 3, 3), t_world_ref (G, M, 3),
+    refine_points, refine_rmse, refine_status (G, M), refine_view_points, refine_view_rmse, refine_view_hidden (G, M, C) (the pairs
+    dropped because another instance owns their pixel), per frame corners_world_ref_px (B, M, 9, 2) and instance_map (B, H, W)
+    int16 (the world slot drawn in front at each pixel under the refined poses, -1 for none); every other output keeps its bits.
+    Each mesh needs a diameter > 0 and a face of non-zero area."""
 
     def __init__(self, model, objects, K, frame_size=(640, 480), shape=None, batch=1, conf_thresh=None, nms_thresh=0.4, max_instances=32,
                  graph=True, max_graphs=4, pnp="plain", reproj_thresh=8.0, dist_coeffs=None, meshes=None, depth_scale=0.001, refine_iters=10,
@@ -288,8 +301,8 @@ def parse_args(argv=None):
     """the command line, checked before any model is built: raises SspError for a bad --object, --nms-thresh, --max-instances,
     --match-iou, --max-misses, --max-tracks, --match-dist, --reproj-thresh, --dist, --keypoint-sigma, --fps, --depth-scale or
     --refine-iters, for --track with --pnp consensus or --depth-dir, for --motion without --track, for --match-dist without --rig,
-    and for --rig with --dist, --depth-dir, --pnp consensus or an image count that is not whole captures (a.rig_cams is then the
-    rig's CameraRig, else None)"""
+    for --rig with --dist, --pnp consensus or an image count that is not whole captures, and for --rig --depth-dir with a missing
+    depth file (a.rig_cams is then the rig's CameraRig, else None)"""
     ap = argparse.ArgumentParser(prog="python -m singleshotpose_b200.predict_instances",
                                  description="6-D pose of every detected instance of the requested objects in each image")
     ap.add_argument("--datacfg", required=True, help=".data file: fx fy u0 v0 and width height (or im_width im_height); mesh")
@@ -340,7 +353,7 @@ def parse_args(argv=None):
     a.objects = parse_objects(a.object) if a.object else None
     if a.dist is not None:
         camera_distortion(a.dist)
-    a.rig_cams = check_rig_args(a, refines=False)
+    a.rig_cams = check_rig_args(a)
     return a
 
 
@@ -381,7 +394,7 @@ def main(argv=None):
     motion = "constant_velocity" if a.motion else None
     rig = a.rig_cams
     if rig is not None:
-        return _main_rig(a, model, objects, size, rig)
+        return _main_rig(a, model, objects, size, rig, refine)
     if a.track:
         pred = TrackingPosePredictor(model, objects, K, frame_size=size, nms_thresh=a.nms_thresh, max_instances=a.max_instances,
                                      max_tracks=a.max_tracks, match_iou=a.match_iou, max_misses=a.max_misses, dist_coeffs=dist,
@@ -401,8 +414,9 @@ def main(argv=None):
     print("%d images -> %d detections -> %s" % (len(a.images), len(image), a.out))
 
 
-def _main_rig(a, model, objects, size, rig):
-    """the --rig command line: one call per capture of C images"""
+def _main_rig(a, model, objects, size, rig, refine):
+    """the --rig command line: one call per capture of C images; refine: the predictor's meshes and refinement keywords with
+    --depth-dir"""
     Cn = len(rig.K)
     kw = dict(frame_size=size, batch=Cn, nms_thresh=a.nms_thresh, max_instances=a.max_instances, rig=rig)
     motion = "constant_velocity" if a.motion else None
@@ -411,11 +425,12 @@ def _main_rig(a, model, objects, size, rig):
                                           match_dist=0.5 if a.match_dist is None else a.match_dist, motion=motion,
                                           fuse=(40.0, 8.0, a.keypoint_sigma), frame_dt=1.0 / a.fps, **kw)
     else:
-        pred = InstancePosePredictor(model, objects, None, **kw)
+        pred = InstancePosePredictor(model, objects, None, **kw, **refine)
     rows = {k: [] for k in ROW_KEYS + ("world_index",) + (("track_id",) if a.track else ())}
-    world = {k: [] for k in WORLD_KEYS + (("world_track_id",) if a.track else ()) + (MOTION_KEYS if motion else ())}
+    world = {k: [] for k in WORLD_KEYS + (("world_track_id",) if a.track else ()) + (MOTION_KEYS if motion else ())
+             + (RIG_REFINE_KEYS if refine else ())}
     image, capture = [], []
-    for g, r in enumerate(predict_files(pred, a.images, None, Cn)):
+    for g, r in enumerate(predict_files(pred, a.images, a.depth_dir, Cn)):
         for b in range(Cn):
             n = int(r["count"][b])
             image += [g * Cn + b] * n

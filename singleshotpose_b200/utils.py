@@ -684,6 +684,124 @@ def refine_depth_rig_batched(depth, vertices, faces, rig, R_world, t_world, dept
     return out
 
 
+def check_instance_meshes(meshes, num_classes):
+    """-> {class id: (vertices (Nv, 3) float64, faces (Nf, 3) int32)} of a {class id: (vertices, faces)} dict whose ids lie in
+    [0, num_classes); SspError, before any device work, for a mesh that is not (Nv, 3) vertices and (Nf, 3) integer faces, a face
+    index outside [0, Nv), a diameter that is not > 0 or no face of non-zero area (the refinement of world instances draws them)"""
+    if not isinstance(meshes, dict) or not meshes:
+        raise SspError("meshes must be a non-empty {class id: (vertices, faces)} dict")
+    out = {}
+    for c in sorted(meshes):
+        if isinstance(c, bool) or not isinstance(c, (int, np.integer)) or not 0 <= c < num_classes:
+            raise SspError("class id %r is not in [0, %d)" % (c, num_classes))
+        try:
+            V, F = meshes[c]
+            V, F = np.asarray(V, np.float64), np.asarray(F)
+        except (TypeError, ValueError):
+            raise SspError("the mesh of class %d must be (vertices, faces)" % c)
+        if V.ndim != 2 or V.shape[1] != 3 or not np.isfinite(V).all():
+            raise SspError("the vertices of class %d must be finite (Nv, 3), got %s" % (c, V.shape))
+        if F.ndim != 2 or F.shape[1] != 3 or not np.issubdtype(F.dtype, np.integer):
+            raise SspError("the faces of class %d must be (Nf, 3) integers, got %s %s" % (c, F.shape, F.dtype))
+        if F.size and (F.min() < 0 or F.max() >= len(V)):
+            raise SspError("a face index of class %d lies outside [0, %d)" % (c, len(V)))
+        if not len(V) or not (np.ptp(V, axis=0) > 0).any():
+            raise SspError("the mesh of class %d has no diameter > 0" % c)
+        if not np.cross(V[F[:, 1]] - V[F[:, 0]], V[F[:, 2]] - V[F[:, 0]]).any():
+            raise SspError("the mesh of class %d has no face of non-zero area to draw" % c)
+        out[int(c)] = (V, F.astype(np.int32))
+    return out
+
+
+def refine_face_table(meshes, num_classes, dev):
+    """checked meshes (check_instance_meshes) -> device (faces [total][3] int32 class-local vertex indices, face_offsets
+    [num_classes + 1] int32), and the largest face count of a class: the tables ssp_refine_instances_rig draws from"""
+    counts = np.zeros(num_classes, np.int64)
+    for c, (_V, F) in meshes.items():
+        counts[c] = len(F)
+    faces = np.concatenate([meshes[c][1] for c in sorted(meshes)]).astype(np.int32)
+    offsets = np.concatenate([[0], np.cumsum(counts)]).astype(np.int32)
+    return torch.from_numpy(np.ascontiguousarray(faces)).to(dev), torch.from_numpy(offsets).to(dev), int(counts.max())
+
+
+def mesh_box_table(meshes, num_classes):
+    """(num_classes, 9, 3) float32: each mesh's vertex centroid and its 8 box corners (get_3D_corners), zeros for a class without one"""
+    table = np.zeros((num_classes, 9, 3), np.float32)
+    for c, (V, _F) in meshes.items():
+        table[c] = np.concatenate([V.mean(0, keepdims=True), get_3D_corners(np.c_[V, np.ones((len(V), 1))].T)[:3].T])
+    return table
+
+
+def refine_instances_work_bytes(groups, views, slots, W, H):
+    """bytes of device workspace ssp_refine_instances_rig needs"""
+    import ctypes
+    out = ctypes.c_longlong(0)
+    call("ssp_refine_instances_rig_work_bytes", int(groups), int(views), int(slots), int(W), int(H), ctypes.byref(out))
+    return out.value
+
+
+def refine_instances_rig_batched(depth, meshes, rig, world_cls, R_world, t_world, world_count=None, fuse_status=None, depth_scale=0.001,
+                                 iters=10, gate=(0.5, 0.02)):
+    """Refine every world instance of each capture of a rig against the depth frames of all its cameras on the GPU
+    (ssp_refine_instances_rig, rule: csrc/refine_instances_core.h): per iteration every instance is drawn at its current pose into
+    a z-buffer per camera, a depth pixel belongs to the instance drawn in front of it, and each instance refines as
+    refine_depth_rig_batched does with the pixels no other instance owns.  Instances lying against and on top of each other (a
+    bin of parts) then do not pair with their neighbours' surfaces.
+    meshes {class id: (vertices, faces)}; rig: camera_rig's CameraRig of C cameras; depth (G C, H, W) uint16 numpy array or CUDA
+    tensor, row g C + c registered to camera c; world_cls (G, M) int (-1: an empty slot; a class without a mesh is never drawn and
+    stops with few_points), R_world (G, M, 3, 3), t_world (G, M, 3) world from model, world_count (G,) int or None (slots past it are empty), fuse_status (G, M) or None:
+    fuse_instances_batched's outputs feed it as they are.  depth_scale, iters and gate as refine_depth_batched.
+    -> (R (G, M, 3, 3), t (G, M, 3), points, rmse, status (G, M), view_points, view_rmse, view_hidden (G, M, C) the pairs each
+    camera dropped because another instance owns their pixel, corners_world_ref_px (G C, M, 9, 2) the mesh's centroid and box
+    corners under each output pose in each row's camera, instance_map (G C, H, W) int16: the slot drawn in front at each pixel
+    under the output poses, -1 for none), CUDA tensors.  REFINE_STATUS as refine_depth_rig_batched; empty slots get zeros."""
+    depth_scale, iters, (s, e) = check_refine_args(depth_scale, iters, gate)
+    if not isinstance(rig, CameraRig):
+        raise SspError("rig must be a CameraRig (utils.camera_rig)")
+    if not isinstance(meshes, dict) or not meshes:
+        raise SspError("meshes must be a non-empty {class id: (vertices, faces)} dict")
+    num_classes = max(int(c) + 1 if isinstance(c, (int, np.integer)) and not isinstance(c, bool) else 1 for c in meshes)
+    meshes = check_instance_meshes(meshes, num_classes)
+    shape = lambda a: tuple(a.shape) if torch.is_tensor(a) else np.shape(a)
+    if len(shape(depth)) != 3:
+        raise SspError("depth must be (G C, H, W), got %s" % (shape(depth),))
+    B, H, W = shape(depth)
+    C = len(rig.K)
+    if B % C:
+        raise SspError("%d depth frames are not whole captures of the rig's %d cameras" % (B, C))
+    G = B // C
+    sc = shape(world_cls)
+    if len(sc) != 2 or sc[0] != G or shape(R_world) != (*sc, 3, 3) or shape(t_world) != (*sc, 3):
+        raise SspError("refine_instances_rig_batched: %d captures but world_cls %s, R_world %s, t_world %s: (G, M), (G, M, 3, 3), (G, M, 3)"
+                       % (G, sc, shape(R_world), shape(t_world)))
+    M = sc[1]
+    if not 1 <= M <= CONSTANTS["SSP_FUSE_MAX_SLOTS"]:
+        raise SspError("refine_instances_rig_batched takes 1..%d world slots, got %d" % (CONSTANTS["SSP_FUSE_MAX_SLOTS"], M))
+    if (world_count is not None and shape(world_count) != (G,)) or (fuse_status is not None and shape(fuse_status) != (G, M)):
+        raise SspError("world_count must be (%d,) and fuse_status (%d, %d)" % (G, G, M))
+    dev = _dev()
+    D = _depth_tensor(depth, dev)
+    t32 = lambda a, dt: (a if torch.is_tensor(a) else torch.as_tensor(np.asarray(a))).to(dev, dt).contiguous()
+    cls, R, t = t32(world_cls, torch.int32), t32(R_world, torch.float64), t32(t_world, torch.float64)
+    cnt = None if world_count is None else t32(world_count, torch.int32)
+    fs = None if fuse_status is None else t32(fuse_status, torch.int32)
+    model, offsets, diam = refine_model_table(meshes, num_classes, dev)
+    faces, foff, max_faces = refine_face_table(meshes, num_classes, dev)
+    table = torch.from_numpy(mesh_box_table(meshes, num_classes)).to(dev)
+    i32 = lambda *sh: torch.empty(*sh, dtype=torch.int32, device=dev)
+    f64 = lambda *sh: torch.empty(*sh, dtype=torch.float64, device=dev)
+    out = (f64(G, M, 3, 3), f64(G, M, 3), i32(G, M), f64(G, M), i32(G, M), i32(G, M, C), f64(G, M, C), i32(G, M, C),
+           torch.empty(B, M, 9, 2, dtype=torch.float32, device=dev), torch.empty(B, H, W, dtype=torch.int16, device=dev))
+    if G == 0:
+        return out
+    _K32, K64, Dd, Rr, tr = rig_tensors(rig, dev)
+    work = torch.empty(max(refine_instances_work_bytes(G, C, M, W, H), 8) // 8, dtype=torch.float64, device=dev)
+    call("ssp_refine_instances_rig", ptr(D), W, H, depth_scale, C, ptr(K64), ptr(Dd), ptr(Rr), ptr(tr), ptr(model), ptr(offsets), ptr(diam),
+         ptr(faces), ptr(foff), max_faces, ptr(table), 9, num_classes, ptr(cls), G, M, ptr(cnt), ptr(fs), ptr(R), ptr(t), iters, s, e,
+         *(ptr(o) for o in out), ptr(work), work.numel() * 8, stream_ptr())
+    return out
+
+
 def fuse_instances_work_bytes(groups, views, slots):
     """bytes of device workspace ssp_fuse_instances needs"""
     import ctypes
