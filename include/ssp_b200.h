@@ -520,6 +520,41 @@ int ssp_calibrate_rig(const float* points3d, int points3d_shared, const float* p
                       int* cam_status, double* R_world, double* t_world, unsigned char* views_out, double* view_err,
                       unsigned char* linked, int* rounds, int* iterations, double* cost, void* work, long long work_bytes, void* stream);
 
+/* ---- calibrating an RGB-D rig against depth: a point-to-plane bundle adjustment of the extrinsics and the observations' world
+ *      poses (rules: csrc/calibrate_rig_depth_core.h; csrc/calibrate_rig_depth.cu), fp64, the second stage after ssp_calibrate_rig.
+ *      The cameras (`views` = C, 2..SSP_RIG_MAX_VIEWS; K3x3 [C][9] DEVICE fp64, dist8_or_null [C][8]) with ssp_calibrate_rig's
+ *      reference, cam_status_in [C] (DEVICE int), R_cam_in [C][9], t_cam_in [C][3] (camera-from-world; the reference R = I, t = 0);
+ *      observation o = g * slots + s with ssp_calibrate_rig's R_world_in [O][9], t_world_in [O][3], obs_views [O][C] and linked [O]
+ *      (DEVICE bytes).  One mesh for every observation: model [num_vertices][6] (DEVICE fp64 vertices and outward normals) and its
+ *      diameter diam; depth [groups * C][H][W] uint16, row g * C + c camera c's frame of capture g, depth_scale, iters and the
+ *      gates as ssp_refine_depth_rig takes them.
+ *  ssp_calibrate_rig_depth: iters Gauss-Newton steps, with no accept test, of the free cameras' extrinsics (connected, not the
+ *      reference) and the linked observations' world poses.  Each active view pairs the mesh with its depth as ssp_refine_depth_rig
+ *      does; the reduced system over the free cameras is solved by a Cholesky factorisation.  Out per camera: R_cam, t_cam,
+ *      cam_cov [C][36] (the RMS residual squared times the camera's block of the last reduced system's inverse: a lower bound, the
+ *      pairs taken as independent; zeros for the reference, held and unconnected cameras), cam_points [C], cam_rmse [C] (its pairs
+ *      and RMS point-to-plane residual in the last iteration), cam_status [C] (SSP_CALIB_DEPTH_UNCONNECTED passed through;
+ *      SSP_CALIB_DEPTH_FEW_POINTS: held, fewer than SSP_REFINE_MIN_POINTS pairs, its extrinsics kept; SSP_CALIB_DEPTH_SINGULAR).
+ *      Per observation: R_world, t_world, obs_points, obs_rmse of its last iteration, obs_status (SSP_REFINE_FEW_POINTS or
+ *      SSP_REFINE_SINGULAR stop it, with the input pose; an observation that is not linked keeps its pose with zeros).  Global:
+ *      status [1] (SSP_CALIB_DEPTH_SINGULAR: the reduced system could not be factored; every output pose is then its input) and
+ *      iter_rmse [iters] (the RMS residual over every active pair before each iteration's update, 0 for iterations not run).
+ *      work: DEVICE scratch (8-B aligned) of at least the *bytes_out that ssp_calibrate_rig_depth_work_bytes(groups, views, slots,
+ *      bytes_out) writes.  SSP_ERR_ARG as ssp_refine_depth_rig and ssp_calibrate_rig, and for views < 2, num_vertices < 1 or a
+ *      diameter not > 0 and finite. ---- */
+#define SSP_CALIB_DEPTH_UNCONNECTED 1
+#define SSP_CALIB_DEPTH_FEW_POINTS 2
+#define SSP_CALIB_DEPTH_SINGULAR 4
+int ssp_calibrate_rig_depth_work_bytes(int groups, int views, int slots, long long* bytes_out);
+int ssp_calibrate_rig_depth(const unsigned short* depth, int W, int H, double depth_scale, int views, const double* K3x3,
+                            const double* dist8_or_null, int reference, const int* cam_status_in, const double* R_cam_in,
+                            const double* t_cam_in, const double* model, int num_vertices, double diam, int groups, int slots,
+                            const unsigned char* obs_views, const unsigned char* linked, const double* R_world_in,
+                            const double* t_world_in, int iters, double gate_start, double gate_end, double* R_cam, double* t_cam,
+                            double* cam_cov, int* cam_points, double* cam_rmse, int* cam_status, double* R_world, double* t_world,
+                            int* obs_points, double* obs_rmse, int* obs_status, int* status, double* iter_rmse, void* work,
+                            long long work_bytes, void* stream);
+
 /* ---- tracking the world instances of a rig over time (rules: csrc/world_track_core.h; csrc/world_track.cu), fp64.  Each capture g
  *      of ssp_fuse_instances (rows g * views .. g * views + views - 1, M = slots world slots) is its own stream with T = max_tracks
  *      (1..256) slots, state in DEVICE arrays the caller keeps between calls (zeros for a fresh start):

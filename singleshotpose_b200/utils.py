@@ -940,6 +940,81 @@ def calibrate_rig_batched(points_3D, keypoints_px, K, dist=None, valid=None, ref
     return o
 
 
+CALIB_DEPTH_STATUS = {"unconnected": 1, "few_points": 2, "singular": 4}  # ssp_calibrate_rig_depth's bits (SSP_CALIB_DEPTH_*)
+CALIB_KEYS = ("R", "t", "cam_status", "R_world", "t_world", "views", "linked")   # what the depth stage reads of calibrate_rig_batched
+
+
+def calibrate_depth_work_bytes(groups, views, slots):
+    """bytes of device workspace ssp_calibrate_rig_depth needs"""
+    import ctypes
+    out = ctypes.c_longlong(0)
+    call("ssp_calibrate_rig_depth_work_bytes", int(groups), int(views), int(slots), ctypes.byref(out))
+    return out.value
+
+
+def calibrate_rig_depth_batched(depth, vertices, faces, K, calib, dist=None, reference=0, depth_scale=0.001, iters=10, gate=(0.5, 0.02)):
+    """Calibrate an RGB-D rig against depth on the GPU (ssp_calibrate_rig_depth, rule: csrc/calibrate_rig_depth_core.h): the
+    second stage after calibrate_rig_batched.  A Gauss-Newton bundle adjustment of the free cameras' extrinsics (connected, not
+    the reference) and the linked observations' world poses, whose residuals are the point-to-plane residuals of the mesh's
+    vertices against every camera's depth, paired as refine_depth_rig_batched pairs them, over `iters` fixed iterations with the
+    gate shrinking from gate[0] to gate[1] times the mesh's diameter.
+    calib: calibrate_rig_batched's dict as it comes back, called with the same K, dist and reference.  depth (G C, H, W) uint16
+    numpy array or CUDA tensor, row g C + c camera c's frame of capture g (its K and coefficients); vertices, faces: the mesh of
+    the object the rig saw.
+    -> dict of CUDA tensors: per camera R (C, 3, 3), t (C, 3), cam_cov (C, 6, 6) (the RMS residual squared times the camera's
+    block of the last reduced system's inverse, left perturbation in the camera frame; it takes the pairs as independent, so it is
+    a lower bound on the true covariance; zeros for the reference, held and unconnected cameras), cam_points (C,), cam_rmse (C,)
+    (pairs and RMS point-to-plane residual in mesh units in the last iteration), cam_status (C,) CALIB_DEPTH_STATUS bits; per
+    observation R_world (G[, S], 3, 3), t_world, obs_points, obs_rmse, obs_status (REFINE_STATUS few_points / singular: the input
+    pose is kept); status (int, CALIB_DEPTH_STATUS singular: every pose is its input) and iter_rmse (iters,); and rig, a CameraRig,
+    or None when a camera is unconnected or the status is set."""
+    depth_scale, iters, (s, e) = check_refine_args(depth_scale, iters, gate)
+    K, D, reference = check_calibrate_args(K, dist, reference, 40.0, 8.0, 2.0, 1)[:3]
+    C = len(K)
+    if C < 2:
+        raise SspError("a rig to calibrate has 2..%d cameras, got %d" % (CONSTANTS["SSP_RIG_MAX_VIEWS"], C))
+    if not isinstance(calib, dict) or any(k not in calib for k in CALIB_KEYS):
+        missing = [k for k in CALIB_KEYS if not isinstance(calib, dict) or k not in calib]
+        raise SspError("calib must be calibrate_rig_batched's dict: it has no %s" % ", ".join(missing))
+    V = np.asarray(vertices, np.float64)
+    if V.ndim != 2 or V.shape[1] != 3 or len(V) == 0:
+        raise SspError("the mesh needs (Nv, 3) vertices with Nv >= 1, got %s" % (V.shape,))
+    if not (np.isfinite(V).all() and np.ptp(V, axis=0).max() > 0):
+        raise SspError("the mesh has diameter 0 (or a vertex that is not finite): the gate is a fraction of the diameter")
+    shape = lambda k: tuple(calib[k].shape) if torch.is_tensor(calib[k]) else np.shape(calib[k])
+    lead = shape("R_world")[:-2]
+    if (len(lead) not in (1, 2) or shape("R_world")[-2:] != (3, 3) or shape("t_world") != lead + (3,) or shape("views") != lead + (C,)
+            or shape("linked") != lead or shape("R") != (C, 3, 3) or shape("t") != (C, 3) or shape("cam_status") != (C,)):
+        raise SspError("calib's shapes disagree with %d cameras: %s" % (C, ", ".join("%s %s" % (k, shape(k)) for k in CALIB_KEYS)))
+    G, S = lead[0], (lead[1] if len(lead) > 1 else 1)
+    dshape = tuple(depth.shape) if torch.is_tensor(depth) else np.shape(depth)
+    if len(dshape) != 3 or dshape[0] != G * C:
+        raise SspError("depth %s for %d captures of %d cameras: (G C, H, W), row g C + c camera c's frame of capture g" % (dshape, G, C))
+    dev = _dev()
+    Dt = _depth_tensor(depth, dev)
+    _B, H, W = Dt.shape
+    diam = mesh_diameter(V)
+    dv = lambda k, dt: torch.as_tensor(calib[k]).to(dev, dt).contiguous()
+    Rw, tw, Rc, tc = (dv(k, torch.float64) for k in ("R_world", "t_world", "R", "t"))
+    views, linked, st_in = dv("views", torch.uint8), dv("linked", torch.uint8), dv("cam_status", torch.int32)
+    model = refine_model_table({0: (vertices, faces)}, 1, dev)[0]
+    to = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a, dt)).to(dev)
+    K64, Dd = to(K, np.float64), None if D is None else to(D, np.float64)
+    f64 = lambda *sh: torch.empty(*sh, dtype=torch.float64, device=dev)
+    i32 = lambda *sh: torch.empty(*sh, dtype=torch.int32, device=dev)
+    o = dict(R=f64(C, 3, 3), t=f64(C, 3), cam_cov=f64(C, 6, 6), cam_points=i32(C), cam_rmse=f64(C), cam_status=i32(C), R_world=f64(*lead, 3, 3),
+             t_world=f64(*lead, 3), obs_points=i32(*lead), obs_rmse=f64(*lead), obs_status=i32(*lead), status=i32(1), iter_rmse=f64(iters))
+    work = f64(max(calibrate_depth_work_bytes(G, C, S), 8) // 8)
+    call("ssp_calibrate_rig_depth", ptr(Dt), W, H, depth_scale, C, ptr(K64), ptr(Dd), reference, ptr(st_in), ptr(Rc), ptr(tc), ptr(model),
+         len(V), diam, G, S, ptr(views), ptr(linked), ptr(Rw), ptr(tw), iters, s, e, *(ptr(v) for v in o.values()), ptr(work),
+         work.numel() * 8, stream_ptr())
+    o["status"] = int(o["status"][0])
+    cam_status = o["cam_status"].cpu().numpy()
+    bad = o["status"] or (cam_status & CALIB_DEPTH_STATUS["unconnected"]).any()
+    o["rig"] = None if bad else camera_rig(K, o["R"].cpu().numpy(), o["t"].cpu().numpy(), D)
+    return o
+
+
 # ------------------------------------------------------------------------------------------ training-set creation
 RENDER_CHUNK_BYTES = 1 << 30           # device scratch of one ssp_render_masks launch; larger batches go in chunks
 
