@@ -294,8 +294,9 @@ def _route(z, kind):
 
 def _check_inference(eng, B, N, H, W):
     """every layer of an inference forward (fused epilogue, split-K or conv + bn_apply) from the planes the engine kept: the
-    destination planes hi + lo against leaky(scale conv(x_hi, w_hi) + shift) in fp64, routed (direct, pool, reorg, concat offset),
-    with the folded scale / shift the kernels read; y against conv(x_hi, w_hi) where the layer wrote it (and the head's bias)"""
+    destination planes hi + lo against leaky(scale conv(x, w) + shift) in fp64, routed (direct, pool, reorg, concat offset),
+    with the folded scale / shift the kernels read; y against conv(x, w) where the layer wrote it (and the head's bias).  x, w are
+    the operand values the forward reads: x_hi, w_hi in fast mode, x_hi + x_lo, w_hi + w_lo in exact mode"""
     mods = eng.conv_modules()
     for L in eng.layers:
         conv, bn = mods[L.index]
@@ -308,7 +309,11 @@ def _check_inference(eng, B, N, H, W):
         else:
             idx = _idx(N, h, w)
             A = _nchw(B.x_hi[i], idx, N, h, w, L.cin)
-            Wf = eng.w_hi[i][:, :K].double().view(L.cout, k, k, L.cin).permute(0, 3, 1, 2)
+            Wf = eng.w_hi[i][:, :K].double()
+            if not eng.fast:
+                A = A + _nchw(B.x_lo[i], idx, N, h, w, L.cin)
+                Wf = Wf + eng.w_lo[i][:, :K].double()
+            Wf = Wf.view(L.cout, k, k, L.cin).permute(0, 3, 1, 2)
         ref = F.conv2d(A, Wf, None if L.bn else conv.bias.detach().double(), padding=(k - 1) // 2)
         del A
         tol = 2e-5 + 5e-9 * K                     # the suite's tensor-core bound
